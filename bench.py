@@ -52,7 +52,7 @@ def read_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback"  # H100 SXM data sheet (700 W)
 
 
 class ClockSampler:
@@ -74,6 +74,7 @@ class ClockSampler:
         self._nv = None
         self._h = None
         self.max_mhz = None
+        self.name = self.power_limit_w = None  # the card and its power limit are part of every number measured on it
         self.source = "unavailable"
         try:
             import pynvml as nv
@@ -82,6 +83,9 @@ class ClockSampler:
             self._nv = nv
             self._h = nv.nvmlDeviceGetHandleByIndex(self._physical_index(nv, index))
             self.max_mhz = float(nv.nvmlDeviceGetMaxClockInfo(self._h, nv.NVML_CLOCK_SM))
+            name = nv.nvmlDeviceGetName(self._h)
+            self.name = name.decode() if isinstance(name, bytes) else name
+            self.power_limit_w = nv.nvmlDeviceGetPowerManagementLimit(self._h) / 1000.0
             self.source = "nvml"
         except Exception as exc:  # no NVML: nvidia-smi polling (slow, ~50 ms per query)
             self._nv = None
@@ -119,11 +123,12 @@ class ClockSampler:
             ["nvidia-smi", f"--id={self.index}",
              "--query-gpu=clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap", "--format=csv,noheader,nounits"],
+             "clocks_event_reasons.sw_power_cap,power.limit,name", "--format=csv,noheader,nounits"],
             capture_output=True, text=True, timeout=5,
         ).stdout.strip()
         f = [x.strip() for x in out.split(",")]
         self.max_mhz = float(f[1])
+        self.power_limit_w, self.name = float(f[7]), f[8]
         return float(f[0]), float(f[2]), [k for i, k in enumerate(self.NAMES) if f[3 + i] == "Active"]
 
     def sample_now(self, sync=True):
@@ -155,7 +160,8 @@ class ClockSampler:
 
     def summary(self):
         if not self.samples:
-            return {"sm_mhz": None, "sm_max_mhz": self.max_mhz, "reasons": [f"no sample ({self.source})"]}
+            return {"sm_mhz": None, "sm_max_mhz": self.max_mhz, "reasons": [f"no sample ({self.source})"],
+                    "gpu": self.name, "power_limit_w": self.power_limit_w}
         t0 = self._t0 if self._t0 is not None else -1e30
         t1 = self._t1 if self._t1 is not None else 1e30
         inside = [x for x in self.samples if t0 <= x[0] <= t1]
@@ -164,6 +170,8 @@ class ClockSampler:
         return {
             "sm_mhz": float(np.median([x[1] for x in used])),
             "sm_max_mhz": self.max_mhz,
+            "gpu": self.name,
+            "power_limit_w": self.power_limit_w,
             "reasons": reasons,
             "power_w": float(np.max([x[2] for x in used])),
             "samples_in_timed_region": len(inside),
@@ -344,7 +352,11 @@ def main():
     ap.add_argument("--envs-per-gpu", type=int, default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-other-workloads", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (rank 0's envs)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.workload == "plumbing"):
+        ap.error("--dump-outputs covers the servos, pendulum and mpc workloads of the GPU implementation")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -374,8 +386,7 @@ def main():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         # The rollout all-gather runs on NCCL's own stream while the next rollout simulates. The step kernel
         # occupies every SM (255 registers x 224 threads leave no room for a second block), so the collective's
-        # CTAs only get SMs when a simulation block retires. Measured on 2 GPUs (tools/run_2gpu_variants.sh): a
-        # high-priority NCCL stream or fewer CTAs (NCCL_MAX_CTAS) make it worse, the default is best.
+        # CTAs only get SMs when a simulation block retires. UPKIE_BENCH_NCCL_PRIORITY=1 tries a high-priority stream.
         pg_options = None
         if os.environ.get("UPKIE_BENCH_NCCL_PRIORITY", "0") == "1":
             pg_options = dist.ProcessGroupNCCL.Options(is_high_priority_stream=True)
@@ -437,7 +448,7 @@ def main():
             # sources); null when no capture of this build / workload exists
             "traffic": side.get("dram_bytes"),
             "traffic_source": side.get("source"),
-            "peak_kind": f"{peaks_kind} (MEASURED_PEAKS.json hbm_gbs)" if peaks_kind == "measured" else "fallback 6650 GB/s",
+            "peak_kind": f"{peaks_kind} (MEASURED_PEAKS.json hbm_gbs)" if peaks_kind == "measured" else "H100 SXM data sheet 3350 GB/s",
             "algorithmic_bytes_per_unit": b_alg,
             "kernel_ms": kernel_ms,
             "kernel_ms_statistic": "median over the timed steps of the CUDA-event interval around each launch",
@@ -450,12 +461,11 @@ def main():
         sm_mhz = clocks.get("sm_mhz") or clocks.get("sm_max_mhz")
         instr = side.get("instr_per_env_step")
         if sm_mhz and instr:
-            sched_cycles = 148 * 4 * sm_mhz * 1e6  # issue slots per second
+            sms = torch.cuda.get_device_properties(dev).multi_processor_count
+            sched_cycles = sms * 4 * sm_mhz * 1e6  # issue slots per second
             ipc = instr * (n_per_gpu / 32.0) / (kernel_ms * 1e-3) / sched_cycles
             line["roofline"]["fp32_issue"] = {
                 "ipc_per_scheduler": ipc, "peak_ipc": 1.0, "frac": ipc,
-                # tools/micro/ffma2_bench.cu on this pool: three-register scalar FFMA saturates at 0.59 inst/cycle/scheduler
-                "measured_scalar_ffma_ceiling_ipc": 0.59,
                 "instr_per_env_step": instr,
                 "fp_instr_share": side.get("fp_instr_share"),
                 "sm_mhz_used": sm_mhz,
@@ -476,6 +486,28 @@ def main():
     print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(path, outputs):
+    """``outputs``: name -> device tensor whose first axis is the env / robot index. Written as float32 (float64
+    stays float64); when the arrays exceed DUMP_MAX_BYTES, the same seeded subset of rows is kept in every array and
+    its indices go to ``index.npy``."""
+    arrays = {}
+    for name, t in outputs.items():
+        a = t.detach().cpu().numpy()
+        arrays[name] = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+    n = len(next(iter(arrays.values())))
+    row_bytes = sum(a.nbytes for a in arrays.values()) / n
+    if row_bytes * n > DUMP_MAX_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(n, int(DUMP_MAX_BYTES // (row_bytes + 8)), replace=False))
+        arrays = {name: a[keep] for name, a in arrays.items()}
+        arrays["index"] = keep.astype(np.float64)
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, f"{name}.npy"), a)
 
 
 def ncu_sidecar(workload, config, n_per_gpu, regime):
@@ -558,10 +590,11 @@ def other_workloads(torch, dev, model):
         acts = [((torch.rand((n, 1), device=dev, generator=gen) * 2 - 1) * 3.0).contiguous() for _ in range(8)]
         ms, med = timed(lambda i: env.sim.step_pendulum(acts[i % 8]))
         out["pendulum_4096"] = {"metric": "env-steps/sec", "value": n / (ms * 1e-3), "ms_per_step": ms,
-                                "kernel_ms_median": med, "workload": "BASELINE configs[1]"}
+                                "kernel_ms_median": med, "steps": 200, "workload": "BASELINE configs[1]"}
         gms = timed_graph(lambda i: env.sim.step_pendulum(acts[i % 8]))
         if gms:
-            out["pendulum_4096"].update({"graph_replay_ms_per_step": gms, "graph_replay_value": n / (gms * 1e-3)})
+            out["pendulum_4096"].update({"graph_replay_ms_per_step": gms, "graph_replay_value": n / (gms * 1e-3),
+                                         "graph_replay_steps": 48 * 8})
         env.close()
         for H in (16, 50):
             cfg = _abi.default_mpc_config()
@@ -572,11 +605,12 @@ def other_workloads(torch, dev, model):
             vt, contact = U(-1, 1), torch.ones(n, dtype=torch.uint8, device=dev)
             ms, med = timed(lambda i: mpc.step_tensors(xs[i % 8], vt, contact, 0.005))
             out[f"mpc_4096_h{H}"] = {"metric": "qp-solves/sec", "value": n / (ms * 1e-3), "ms_per_step": ms,
-                                     "kernel_ms_median": med,
+                                     "kernel_ms_median": med, "steps": 200,
                                      "workload": "BASELINE configs[3]" + (" at the reference's default horizon" if H == 50 else "")}
             gms = timed_graph(lambda i: mpc.step_tensors(xs[i % 8], vt, contact, 0.005))
             if gms:
-                out[f"mpc_4096_h{H}"].update({"graph_replay_ms_per_step": gms, "graph_replay_value": n / (gms * 1e-3)})
+                out[f"mpc_4096_h{H}"].update({"graph_replay_ms_per_step": gms, "graph_replay_value": n / (gms * 1e-3),
+                                              "graph_replay_steps": 48 * 8})
     except Exception as exc:  # secondary lines must never take the headline down
         out["error"] = repr(exc)
     out["servos_65536_exact_mode"] = exact_mode_line()
@@ -593,7 +627,7 @@ def body_contacts_line():
                             "--no-cpu-baseline", "--no-other-workloads"], env=env, capture_output=True, text=True, timeout=300)
         j = json.loads(r.stdout.strip().splitlines()[-1])
         return {"metric": "env-steps/sec", "value": j["value"], "ms_per_step": j["ms_per_step"],
-                "kernel_ms_median": j["roofline"]["kernel_ms"],
+                "kernel_ms_median": j["roofline"]["kernel_ms"], "steps": j["steps"], "warmup": j["warmup"],
                 "workload": "headline workload with body_contacts = 1: ~1/3 of the robots sit on their torso box and never "
                             "reach the 0.15 m reset height; every warp solves its rows in general_contact_solve()"}
     except Exception as exc:
@@ -615,7 +649,7 @@ def exact_mode_line():
                             "--no-cpu-baseline", "--no-other-workloads"], env=env, capture_output=True, text=True, timeout=300)
         j = json.loads(r.stdout.strip().splitlines()[-1])
         return {"metric": "env-steps/sec", "value": j["value"], "ms_per_step": j["ms_per_step"],
-                "kernel_ms_median": j["roofline"]["kernel_ms"],
+                "kernel_ms_median": j["roofline"]["kernel_ms"], "steps": j["steps"], "warmup": j["warmup"],
                 "workload": "headline workload, exact arithmetic: no fast-math, full 126 B records"}
     except Exception as exc:
         return {"error": repr(exc)}
@@ -676,9 +710,6 @@ def bench_env(args, torch, dist, dev, rank, world, model, K, W):
 
     # two buffers: the gather of rollout r (NVLink) overlaps the simulation of r + 1. "peer": symmetric-memory
     # buffers, every rank pushes its slot to the peers with the copy engines (no SM); "nccl": all_gather_into_tensor
-    # Measured (tools/run_2gpu_variants.sh, tools/run_8gpu.sh): 2 GPUs peer 96 % vs nccl 84 % weak-scaling efficiency;
-    # 8 GPUs nccl 64 %, the first (unstaggered, one-stream) peer push collapsed there -> nccl stays the default
-    # beyond 2 GPUs until the staggered push is validated at 8.
     # Transport of the rollout records (UPKIE_BENCH_GATHER overrides): "multicast" - the step kernel's row stores go
     # to the NVSwitch multicast address of a symmetric-memory buffer (multimem.st), one store reaches every GPU, the
     # only collective left is a barrier per rollout; "peerstore" - same kernel storing each row into every peer's
@@ -708,8 +739,6 @@ def bench_env(args, torch, dist, dev, rank, world, model, K, W):
     counters = {"gathers": 0}
     pending = {"push": None}
     # UPKIE_BENCH_PUSH=now: the immediate in-kernel transports (rows leave at the END of the launch that produced them)
-    # Default "now" since the second session of round 2: measured best at 2 and at 4 GPUs with the final kernels
-    # (profiles/r02_multigpu.md, last section: 20-step run at N = 4: now 2.15e9, deferred 2.05e9, kernel 1.84e9 env-steps/s)
     push_mode = os.environ.get("UPKIE_BENCH_PUSH", "now")  # now | deferred | kernel
     deferred = push_mode == "deferred"
 
@@ -807,6 +836,14 @@ def bench_env(args, torch, dist, dev, rank, world, model, K, W):
         clk.mark_end()
         if profiling:
             torch.cuda.profiler.stop()
+        if args.dump_outputs and rank == 0:
+            # every transport leaves this rank's rows of a step in its local slot of the rollout buffer
+            k_last = Wa + K - 1
+            buf = rollouts[(k_last // T_roll) % 2]
+            t = k_last % buf.T
+            names = ("obs", "reward", "terminated", "truncated")
+            views = (buf.obs, buf.reward, buf.terminated, buf.truncated)
+            dump_outputs(args.dump_outputs, {name: v[t] for name, v in zip(names, views) if v is not None})
         if world > 1:
             dist.barrier()
     gathers = counters["gathers"]
@@ -829,7 +866,6 @@ def bench_env(args, torch, dist, dev, rank, world, model, K, W):
     # e2e through the public VectorEnv API with HOST buffers (H2D + kernel + D2H per step)
     # this step's inputs live in pinned host memory (4 rotating buffers), outputs land in pinned memory
     host_acts = [a.cpu().pin_memory().numpy() for a in acts[:4]]
-    Ke = max(100, min(K, 400))
     for k in range(12):  # warm-up: first-touch of the handle's pinned staging buffers, streams, events
         env.step(host_acts[k % 4])
     torch.cuda.synchronize()
@@ -837,9 +873,9 @@ def bench_env(args, torch, dist, dev, rank, world, model, K, W):
         dist.barrier()
     if profiling_e2e:
         torch.cuda.profiler.start()
-    step_s = np.empty(Ke)
+    step_s = np.empty(K)
     t0 = time.perf_counter()
-    for k in range(Ke):
+    for k in range(K):
         ts = time.perf_counter()
         env.step(host_acts[k % 4])  # returns when the step's results are in host memory
         step_s[k] = time.perf_counter() - ts
@@ -851,13 +887,13 @@ def bench_env(args, torch, dist, dev, rank, world, model, K, W):
     if world > 1:
         dist.all_reduce(te, op=dist.ReduceOp.MAX)
     e2e = {
-        "value": n * world * Ke / float(te[0].item()),
+        "value": n * world * K / float(te[0].item()),
         "unit": "env-steps/s",
         "h2d_bytes_per_step": n * act_bytes,
         # servos: position/velocity/torque rows (72 B) + terminated; temperature, voltage, reward and truncated
         # are constants of the reference that the env fills once on the host (DESIGN.md, host path)
         "d2h_bytes_per_step": n * ((72 if servos else obs_bytes) + 1),
-        "steps": Ke,
+        "steps": K,
         "warmup": 12,
         "median_ms_per_step": 1e3 * float(te[1].item()),
         "value_from_median_step": n * world / float(te[1].item()),
@@ -900,7 +936,7 @@ def bench_env(args, torch, dist, dev, rank, world, model, K, W):
         "body_contact_rows": int(getattr(env.config, "body_contacts", 0)) != 0,
         "parallelism": f"env-index sharded x{world}" + transport,
         "l2": f"{N_ACTION_BUFFERS} rotating action buffers ({N_ACTION_BUFFERS * n * act_bytes / 1e6:.0f} MB"
-              " vs 126 MB L2); robot state stays resident by design",
+              f" vs {torch.cuda.get_device_properties(dev).L2_cache_size / 1e6:.0f} MB L2); robot state stays resident by design",
     }
     if world > 1:
         config["gather"] = {
@@ -991,22 +1027,23 @@ def bench_mpc(args, torch, dev, rank, world, K, W):
         clk.mark_begin()
         events[0].record()
         for k in range(K):
-            mpc.step_tensors(xs[k % N_ACTION_BUFFERS], vt, contact, 0.005)
+            v_cmd = mpc.step_tensors(xs[k % N_ACTION_BUFFERS], vt, contact, 0.005)
             events[k + 1].record()
         clk.sample_now()
         torch.cuda.synchronize()
         clk.mark_end()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"commanded_velocity": v_cmd})
     total_ms = events[0].elapsed_time(events[K])
     per_step = np.array([events[k].elapsed_time(events[k + 1]) for k in range(K)])
     xh = [x.cpu().numpy() for x in xs[:4]]
     vth, ch = vt.cpu().numpy(), contact.cpu().numpy()
-    Ke = max(10, min(K, 400))
     t0 = time.perf_counter()
-    for k in range(Ke):
+    for k in range(K):
         mpc.step(xh[k % 4], vth, ch, 0.005)
     e2e_s = time.perf_counter() - t0
-    e2e = {"value": n * Ke / e2e_s, "unit": "qp-solves/s", "h2d_bytes_per_step": n * (16 + 4 + 1),
-           "d2h_bytes_per_step": n * 4, "steps": Ke, "api": "BatchedMPCBalancer.step(numpy) -> numpy"}
+    e2e = {"value": n * K / e2e_s, "unit": "qp-solves/s", "h2d_bytes_per_step": n * (16 + 4 + 1),
+           "d2h_bytes_per_step": n * 4, "steps": K, "api": "BatchedMPCBalancer.step(numpy) -> numpy"}
     config = {"workload": "MPC balancer 4096 robots x horizon-16 box-QP per 5 ms tick (BASELINE configs[3])",
               "robots": n, "horizon": 16, "l2": "working set < L2 by nature (4096 x 157 B)"}
     return n * K, total_ms, float(np.median(per_step)), e2e, K, clk.summary(), config, n

@@ -1,6 +1,6 @@
 /* SPDX-License-Identifier: Apache-2.0
  *
- * upkie_b200.h -- C ABI of the B200-native vectorised Upkie simulation and
+ * upkie_b200.h -- C ABI of the H100-native vectorised Upkie simulation and
  * balance-control path (libupkie_b200.so).
  *
  * This is the drop-in boundary of SURVEY.md section 8(b). The reference has no
@@ -214,7 +214,7 @@ typedef struct UpkieSimConfig {
    * this struct). Was: PGS sweeps stop early once every impulse of a warp changed by less than
    * pgs_tolerance * |impulse| + 1e-9 in one sweep (Bullet: m_leastSquaresResidualThreshold-style
    * exit); 0 = always run pgs_iterations sweeps. Default 1e-5: ~50 ulp of the fp32 impulses, the converged
-   * contact impulses then differ from 50 full sweeps by < 1e-6 m/s on velocities (profiles/r01_variants.md) */
+   * contact impulses then differed from 50 full sweeps by < 1e-6 m/s on velocities */
   double pgs_tolerance;
   /* Bullet's SOLVER_USE_WARMSTARTING: normal contact impulses start each substep at
    * warmstarting_factor x the previous substep's value while the contact persists (Bullet: 0.85), friction rows
@@ -228,7 +228,7 @@ typedef struct UpkieSimConfig {
    * the packed ten-row solver (four limit slots + six contact rows); 3 (default) = rows on, the ten-row solver for
    * the warps that hold a robot on a bound and the six-row contact solver for the others; 1 = the scalar reference
    * implementation of the rows, which exists in the HOST build of the kernel arithmetic only (tests): on the device
-   * it is an alias of 3 (measured 18x slower than the plain kernel on a B200, DESIGN.md section 3).
+   * it is an alias of 3 (many times slower than the plain kernel, DESIGN.md section 3).
    * Same results to round-off in all three. */
   int32_t joint_limits;
   int32_t reserved_joint_limits; /* keeps the doubles below 8-byte aligned without implicit padding */
@@ -271,7 +271,7 @@ typedef struct UpkieSimConfig {
    * (normals, then frictions). At most UPKIE_MAX_BODY_CONTACTS points (the deepest) are active per robot. Needs
    * joint_limits != 0. Handles with body_contacts = 1 run their own kernel instantiations (step_*_body.cu); there a
    * warp that holds no such point runs the packed solvers, one that does solves ALL rows of its 32 robots in a general
-   * scalar solver - measured ~50x the packed cost for that warp and substep on a B200 (DESIGN.md section 3), which is
+   * scalar solver - many times the packed cost for that warp and substep (DESIGN.md section 3), which is
    * why the default is 0 = off (a fallen robot's torso passes through the floor, as in round 1) for batched handles:
    * RL workloads reset fallen robots anyway. B200Backend, the single-env drop-in for PyBulletBackend, turns it on. */
   int32_t body_contacts;
@@ -435,7 +435,7 @@ int upkie_b200_step_servos_peers(void* handle, const float* action, float* const
  * sends the rows of an EARLIER step - read from src_obs / src_terminated, this rank's local slot of that step - to
  * every GPU: to the multicast addresses mc_obs / mc_terminated when n_peers == 0, else into the n_peers buffers
  * peer_obs[p] / peer_terminated[p]. The remote stores then drain under the ~0.1 ms of simulation instead of holding up
- * the completion of the launch (measured at 8 GPUs: the immediate form costs 8 % of kernel time at 20-step runs).
+ * the completion of the launch.
  * src_obs == NULL: nothing to send (first step). upkie_b200_push_rows sends a slot on its own (last step of a
  * rollout, before the ranks' barrier). Alignment as above; n_envs a multiple of 32. */
 typedef struct UpkiePush {

@@ -19,6 +19,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_spine_runs.json")
+OUT_SIDE_BY_SIDE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "ref_spine_side_by_side.npz")
 sys.path.insert(0, ROOT)
 
 
@@ -63,6 +64,12 @@ def main():
                                    "columns": "left wheel velocity, feedforward; right wheel velocity, feedforward; "
                                               "left_hip kp_scale, kd_scale; right_knee kp_scale", "out": rows})
         print("controllers", freq, "final left wheel velocity", rows[-1][0])
+    # stream 7 at 500 Hz: every output column of both pipelines (test_reference_library_side_by_side), in binary
+    freq = 500
+    ref = O.RefSpine(A.default_observer_config(model, float(freq)), A.default_wheel_balancer_config(float(freq)), freq)
+    obs = np.array([ref.observers_step(r) for r in inputs.observer_inputs(A, 7)])
+    ctl = np.array([ref.controllers_step(obs3, target, act).reshape(-1) for obs3, target, act in inputs.controller_inputs(7)])
+    np.savez(OUT_SIDE_BY_SIDE, spine_frequency=freq, stream=7, observers=obs, controllers=ctl)
     with open(OUT, "w") as f:
         json.dump(out, f)
     print("wrote", OUT, os.path.getsize(OUT) // 1024, "KB")

@@ -2,7 +2,7 @@
 """ctypes wrapper of tests/hostsim/libhostsim.so (TEST INFRASTRUCTURE).
 
 Runs the kernels' per-robot arithmetic (upkie_b200/csrc/sim_core.cuh and
-mpc_core.cuh, the exact __host__ __device__ code the sm_100a kernels inline) on
+mpc_core.cuh, the exact __host__ __device__ code the sm_90a kernels inline) on
 the CPU so that `pytest -m "not gpu"` can check the fp32 formulation against the
 fp64 oracle without a GPU. The product never loads this library.
 """
@@ -72,7 +72,7 @@ class HostSim:
     """fp32 kernel arithmetic, one robot after the other, on the CPU."""
 
     def __init__(self, model, config, n, scalar_legs=False):
-        """``scalar_legs=False``: ``step_servos`` / ``step_gyropod`` run the substep the kernels run (f32x2-paired
+        """``scalar_legs=False``: ``step_servos`` / ``step_gyropod`` run the substep the kernels run (paired
         legs, sim_pair.cuh); ``True``: the scalar-leg variant of sim_core.cuh (``UPKIE_PAIRED_LEGS=0`` builds)."""
         self.n = n
         self._m = model.to_struct()

@@ -1,6 +1,6 @@
 # SPDX-License-Identifier: Apache-2.0
 """The kernels' per-robot arithmetic (sim_core.cuh / sim_pair.cuh / mpc_core.cuh compiled for the
-host, fp32: `HostSim` steps with the same f32x2-paired substep functions the device runs) against the fp64 oracle. Runs without a GPU; the `-m gpu` tests repeat
+host, fp32: `HostSim` steps with the same paired-leg substep functions the device runs) against the fp64 oracle. Runs without a GPU; the `-m gpu` tests repeat
 the comparisons through the C ABI on the device.
 
 Tolerances (DESIGN.md "Parity"): the fp32 common-frame formulation carries ~1e-5
@@ -110,7 +110,7 @@ def test_fp32_error_budget_against_textbook_fp32(model, oracle_lib):
     hs.set_state(st)
     o64.set_state(st.astype(np.float64))
     o32.set_state(st.astype(np.float64))
-    hp = HostSim(model, cfg, n)  # the paired (f32x2) substep the device runs, reached through the extras entry point
+    hp = HostSim(model, cfg, n)  # the paired-leg substep the device runs, reached through the extras entry point
     hp.set_state(st)
     hp.step_servos_ext(act, np.zeros((n, 7, 3), dtype=np.float32))
     hs.step_servos(act)  # the same substep through the plain entry point

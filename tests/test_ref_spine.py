@@ -4,10 +4,8 @@ wheel_balancer controllers (WheelStopper -> WheelBalancer), compiled unmodified 
 Eigen / palimpsest / spdlog headers (oracle/Makefile `ref`, oracle/ref_spine_shim.cpp), versus the oracle's
 restatement and the kernels' arithmetic.
 
-* tests/golden/ref_spine_runs.json holds that library's outputs on the seeded inputs of
-  tests/golden/ref_spine_inputs.py: the comparison runs everywhere, reference tree or not;
-* where oracle/_ref/libupkie_ref_spine.so exists (the build container, and the GPU box through the snapshot) the
-  library itself is driven side by side with the oracle on fresh random inputs.
+tests/golden/ref_spine_runs.json holds that library's outputs on the seeded inputs of tests/golden/ref_spine_inputs.py
+(tests/golden/make_ref_spine_golden.py writes it), so the comparison runs without the reference tree.
 Rows a14 and f2 of SURVEY.md section 8."""
 import ctypes as C
 import json
@@ -108,20 +106,20 @@ def test_kernel_arithmetic_matches_the_reference_cpp(golden, model, stream):
 
 
 def test_reference_library_side_by_side(model, oracle_lib):
-    """Direct comparison with the compiled reference where oracle/_ref/ exists (fresh inputs, not the golden ones)."""
-    O = oracle_lib
-    if not os.path.exists(O.REF_SPINE_PATH):
-        pytest.skip("oracle/_ref/libupkie_ref_spine.so not built (reference tree absent)")
-    freq = 500
+    """Every output column of both reference pipelines at 500 Hz on a third input stream
+    (tests/golden/ref_spine_side_by_side.npz, written by make_ref_spine_golden.py from the compiled reference library)
+    against the oracle."""
+    g = np.load(os.path.join(os.path.dirname(__file__), "golden", "ref_spine_side_by_side.npz"))
+    freq = int(g["spine_frequency"])
     ocfg = A.default_observer_config(model, float(freq))
     wcfg = A.default_wheel_balancer_config(float(freq))
-    ref = O.RefSpine(ocfg, wcfg, freq)
     oo = OracleObservers(oracle_lib, ocfg, 1)
     ob = OracleBalancer(oracle_lib, wcfg, 1)
-    rows = inputs.observer_inputs(A, 7)
+    rows = inputs.observer_inputs(A, int(g["stream"]))
+    theirs = g["observers"]
     for k in range(inputs.N_STEPS):
-        assert np.allclose(oo.step(rows[k:k + 1])[0], ref.observers_step(rows[k]), rtol=1e-12, atol=1e-12), k
-    for k, (obs3, target, act) in enumerate(inputs.controller_inputs(7)):
+        assert np.allclose(oo.step(rows[k:k + 1])[0], theirs[k], rtol=1e-12, atol=1e-12), k
+    theirs = g["controllers"]
+    for k, (obs3, target, act) in enumerate(inputs.controller_inputs(int(g["stream"]))):
         mine, _ = ob.step(obs3.reshape(1, 3), None if target is None else target.reshape(1, 2), act.reshape(1, 6, 6))
-        theirs = ref.controllers_step(obs3, target, act)
-        assert np.allclose(mine.reshape(6, 6), theirs, rtol=1e-12, atol=1e-12, equal_nan=True), k
+        assert np.allclose(mine.reshape(-1), theirs[k], rtol=1e-12, atol=1e-12, equal_nan=True), k

@@ -2,9 +2,8 @@
 """GPU tests of the joint-limit rows on the device (k_step<.., NOISE=2, ..>: config.joint_limits = 1 -> 3 on the
 device, 2, 3) against the oracle, the Backend contact query, and the parity-audit recorder.
 
-Written at the end of round 1 (hence the file name: it sorted last so that its first run on a B200 could not mask the
-tests that had already been green there); green on the B200 since the first GPU call of round 2
-(profiles/r02_variants.md). The CPU build of the same kernel code agrees with the oracle
+Written at the end of round 1 (hence the file name: it sorted last so that its first run on a GPU could not mask the
+tests that had already been green there). The CPU build of the same kernel code agrees with the oracle
 (tests/test_kernel_arithmetic_cpu.py::test_joint_limit_rows)."""
 import numpy as np
 import pytest

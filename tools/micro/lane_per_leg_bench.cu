@@ -1,13 +1,13 @@
 // Microbenchmark (round 2, VERDICT item 3 "measure, don't estimate"): the articulated-body passes 1-2 of one substep
-// - the largest packed-f32x2 stretch of k_step (20 % of its instructions) - in the two thread mappings:
-//   A  lane = robot: base_inertia_bias + legs_pass12 (both legs packed into FFMA2 / FMUL2 / FADD2, sim_pair.cuh), what
+// - the largest paired-leg stretch of k_step - in the two thread mappings:
+//   A  lane = robot: base_inertia_bias + legs_pass12 (both legs as pairs, sim_pair.cuh), what
 //      the kernels run;
 //   B  lane = leg: two adjacent lanes per robot, each runs base_inertia_bias (redundantly) and the scalar leg_pass12 of
 //      sim_core.cuh on its own leg, then the two halves of the base's articulated inertia / bias force (27 words) are
 //      combined with __shfl_xor. OPTIMISTIC for B: every lane uses the compile-time constants of the left leg (a real
 //      lane-per-leg kernel would select its leg's constants at run time: one more instruction per constant operand).
 // Both run `REPS` dependent repetitions per launch (a tick has 5 substeps) and fold every output into a checksum.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 --use_fast_math -o lane_per_leg_bench lane_per_leg_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 --use_fast_math -o lane_per_leg_bench lane_per_leg_bench.cu
 //   python -c "...write /tmp/pgs_model.bin (UpkieModel + UpkieSimConfig), see tools/r02/body_gate_stats.cpp" ; ./lane_per_leg_bench
 #include <cstdio>
 #include <cstring>

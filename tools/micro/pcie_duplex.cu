@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: Apache-2.0
 // Developer microbenchmark: what the host<->device leg of one env step can reach on this box.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pcie_duplex pcie_duplex.cu && ./pcie_duplex
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pcie_duplex pcie_duplex.cu && ./pcie_duplex
 // Measures pinned H2D (9.4 MB = 65536 x 144 B) and D2H (8.3 MB = 65536 x 126 B) alone, concurrently on two streams
 // (full duplex), chunked, and through zero-copy (SM loads/stores on mapped pinned memory).
 #include <chrono>
@@ -125,7 +125,9 @@ int main() {
   float4 *zha; float2* zho;
   CK(cudaHostGetDevicePointer(&zha, ha, 0));
   CK(cudaHostGetDevicePointer(&zho, ho, 0));
-  for (int grid : {148, 296, 592, 1184}) {
+  int sms = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+  for (int grid : {sms, 2 * sms, 4 * sms, 8 * sms}) {
     t = wall_ms([&] { zc_read<<<grid, 256, 0, s1>>>(zha, reinterpret_cast<float4*>(da), ab / 16); cudaStreamSynchronize(s1); }, R);
     printf("zero-copy read 9.4 MB, grid %d x 256: %.4f ms (%.1f GB/s)\n", grid, t, ab / t / 1e6);
     t = wall_ms([&] { zc_read<<<grid, 256, 0, s1>>>(reinterpret_cast<const float4*>(dob), reinterpret_cast<float4*>(ho), ob / 16); cudaStreamSynchronize(s1); }, R);
@@ -142,8 +144,8 @@ int main() {
   for (int block : {128, 64}) {
     for (long long delay : {0LL, 35000LL, 70000LL}) {  // cycles at ~1.9 GHz: 0, ~18 us, ~37 us
       for (int mode : {1, 2, 3}) {
-        t = wall_ms([&] { zc_pipeline<<<148, block, 2 * (block / 32) * 4608, s1>>>(zha, reinterpret_cast<float4*>(zho), n, delay, mode); cudaStreamSynchronize(s1); }, R);
-        printf("zc_pipeline 148 x %d, delay %lld cycles, %s: %.4f ms\n", block, delay, mode == 1 ? "read only" : mode == 2 ? "write only" : "read+write", t);
+        t = wall_ms([&] { zc_pipeline<<<sms, block, 2 * (block / 32) * 4608, s1>>>(zha, reinterpret_cast<float4*>(zho), n, delay, mode); cudaStreamSynchronize(s1); }, R);
+        printf("zc_pipeline %d x %d, delay %lld cycles, %s: %.4f ms\n", sms, block, delay, mode == 1 ? "read only" : mode == 2 ? "write only" : "read+write", t);
       }
     }
   }

@@ -9,7 +9,7 @@ backend interface (``reset(init_state) -> observation``, ``step(action) -> obser
 ``upkie/envs/backends/backend.py:11-50``), so the same seeded action sequence is fed to each and the spine
 observations are compared tick by tick.
 
-    # on a B200 box
+    # on a GPU machine
     python tools/parity_audit.py record --backend b200 --scenario stand --ticks 400 --out b200.mpack
     # on a machine with `pip install upkie pybullet upkie_description`
     python tools/parity_audit.py record --backend pybullet --scenario stand --ticks 400 --out bullet.mpack

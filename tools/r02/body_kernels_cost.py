@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 # SPDX-License-Identifier: Apache-2.0
 """What the body-contact kernel family (NOISE = 4) costs when no torso touches the floor: 4 096 pendulum envs with
-body_contacts off / on, device time per tick from a CUDA-graph replay (run on a B200; prints two lines)."""
+body_contacts off / on, device time per tick from a CUDA-graph replay (run on a GPU; prints two lines)."""
 import os
 import sys
 

@@ -44,8 +44,7 @@ def build():
             if KERNEL in l and "Function properties" in l:
                 info = " | ".join(x.strip() for x in lines[i + 1:i + 3])
         objs = [os.path.join(OBJ, os.path.splitext(s)[0] + ".o") for s in b.SOURCES if not s.startswith(UNIT)] + [obj]
-        rc = subprocess.call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o",
-                              os.path.join(OUT, f"lib_{name}.so")] + objs)
+        rc = subprocess.call(["nvcc"] + b.GENCODE + ["-shared", "-o", os.path.join(OUT, f"lib_{name}.so")] + objs)
         print(f"{name:16s} rc={p.returncode}/{rc} {info}")
 
 

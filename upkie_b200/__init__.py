@@ -1,5 +1,5 @@
 # SPDX-License-Identifier: Apache-2.0
-"""upkie_b200 -- B200-native vectorised Upkie simulation and balance control.
+"""upkie_b200 -- H100-native vectorised Upkie simulation and balance control.
 
 Drop-in for the reference's env-step hot path (``UpkieServos`` /
 ``UpkieGyropod`` / ``UpkiePendulum`` / ``UpkieBaseVelocity`` on the PyBullet

@@ -1,7 +1,7 @@
 # SPDX-License-Identifier: Apache-2.0
 """ctypes loader of ``libupkie_b200.so`` (the C ABI of ``include/upkie_b200.h``).
 
-The library is built in-tree by ``upkie_b200.build.build()`` (nvcc, sm_100a). There
+The library is built in-tree by ``upkie_b200.build.build()`` (nvcc, sm_90a). There
 is no fallback: if the shared object is missing, or no CUDA device is present
 when a handle is created, the product path raises.
 """
@@ -87,7 +87,7 @@ def lib():
             raise MissingOptionalDependency(
                 f"{LIB_PATH} not found: build it with "
                 "`python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). upkie_b200 has no CPU fallback."
+                "(nvcc, sm_90a). upkie_b200 has no CPU fallback."
             )
         L = C.CDLL(LIB_PATH)
         for name, (restype, argtypes) in SYMBOLS.items():

@@ -38,7 +38,7 @@ except Exception:  # pragma: no cover - the reference is not installed in this i
 
 
 class B200Backend(_Base):
-    """Backend using the sm_100a simulation kernels (one robot)."""
+    """Backend using the sm_90a simulation kernels (one robot)."""
 
     def __init__(
         self,

@@ -1,5 +1,5 @@
 # SPDX-License-Identifier: Apache-2.0
-"""In-tree build of ``libupkie_b200.so`` with nvcc for sm_100a."""
+"""In-tree build of ``libupkie_b200.so`` with nvcc for sm_90a (H100)."""
 
 import os
 import subprocess
@@ -16,11 +16,11 @@ DEPS = SOURCES + [
     "observers.cuh", "observers_core.cuh", "controllers.cuh", "controllers_core.cuh", "../../include/upkie_b200.h",
 ]
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + [
     "-lineinfo", "-O3", "-std=c++17",
-    # approximate division / sqrt / sincos (<= 2 ulp, arguments range-reduced in the code) and FTZ:
-    # -19% kernel time; the parity tolerances already absorb fp32 round-off of that size
+    # approximate division / sqrt / sincos (<= 2 ulp, arguments range-reduced in the code) and FTZ; the parity
+    # tolerances already absorb fp32 round-off of that size (bench.py's exact_mode line times the library without it)
     "--use_fast_math",
     "-Xcompiler", "-fPIC",
 ]
@@ -78,7 +78,7 @@ def build_exact(force: bool = False) -> str:
     failed = [src for src, p in zip(EXACT_SOURCES, procs) if p.wait() != 0]
     if failed:
         raise RuntimeError(f"nvcc (exact build) failed on {failed}")
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", EXACT_LIB_PATH] + objs)
+    subprocess.check_call([nvcc] + GENCODE + ["-shared", "-o", EXACT_LIB_PATH] + objs)
     return EXACT_LIB_PATH
 
 
@@ -98,5 +98,5 @@ def build(force: bool = False, verbose: bool = False) -> str:
     failed = [src for src, p in zip(SOURCES, procs) if p.wait() != 0]
     if failed:
         raise RuntimeError(f"nvcc failed on {failed}")
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB_PATH] + objs)
+    subprocess.check_call([nvcc] + GENCODE + ["-shared", "-o", LIB_PATH] + objs)
     return LIB_PATH

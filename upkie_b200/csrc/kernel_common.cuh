@@ -6,8 +6,7 @@
 //   step_device.cu  TILE=0  per-thread action loads / observation stores (device buffers)
 //   step_host.cu    TILE=1  per-warp shared-memory tile with coalesced 16 B accesses, the variant whose
 //                           warps read actions from and write observations to mapped pinned HOST memory
-// Keeping them apart leaves the register allocation of the device-buffer kernel untouched (the tile
-// costs it 8 % when both paths live in one kernel, profiles/r01_variants.md).
+// Keeping them apart leaves the register allocation of the device-buffer kernel untouched by the tile path.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -16,7 +15,7 @@
 
 namespace upkie_b200 {
 
-// build-time tuning knobs (tools/variants.py explores them; defaults are the measured best)
+// build-time tuning knobs (tools/variants.py explores them)
 #ifndef UPKIE_MAX_THREADS
 #define UPKIE_MAX_THREADS 256
 #endif

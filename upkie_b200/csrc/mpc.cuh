@@ -145,7 +145,7 @@ inline int mpc_create_impl(const UpkieMpcConfig& c, int n, int device, void** ou
   h->n = n;
   h->device = device;
   // 5 N floats of gains per robot in shared memory; keep blocks small so that
-  // several fit per SM (227 KB) and the grid covers all 148 SMs at N = 4096
+  // several fit per SM (227 KB) and N = 4096 spreads over 128 of the H100's 132 SMs
   h->block = 32;
   h->smem = (size_t(5) * h->M.N * h->block + size_t(h->M.N) * kMpcTabRow) * sizeof(float);
   cudaError_t e = cudaSetDevice(device);

@@ -92,7 +92,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   for (int j = 0; j < UPKIE_NJ; ++j) {
     const double ax = m.joint_axis[j][0], ay = m.joint_axis[j][1], az = m.joint_axis[j][2];
     if (std::fabs(ax) > 1e-9 || std::fabs(az) > 1e-9 || std::fabs(std::fabs(ay) - 1.0) > 1e-9) {
-      err = "model: the sm_100a kernels specialise on joint axes along +-y of the base frame (Upkie, Cookie)";
+      err = "model: the kernels specialise on joint axes along +-y of the base frame (Upkie, Cookie)";
       return UPKIE_B200_EMODEL;
     }
     P.sgn[j] = ay > 0 ? 1.f : -1.f;

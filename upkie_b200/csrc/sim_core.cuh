@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: Apache-2.0
 //
-// sim_core.cuh -- per-robot simulation arithmetic of the sm_100a kernels.
+// sim_core.cuh -- per-robot simulation arithmetic of the sm_90a kernels.
 //
 // One CUDA thread advances one robot (lane = robot): the path is bound by fp32
 // issue rate, not by HBM (DESIGN.md "Roofline"), so the layout keeps all 32
@@ -37,10 +37,10 @@
 namespace upkie_b200 {
 
 #ifndef UPKIE_PAIRED_LEGS
-#define UPKIE_PAIRED_LEGS 1  // left/right leg arithmetic packed into f32x2 instructions (sim_pair.cuh)
+#define UPKIE_PAIRED_LEGS 1  // left/right leg arithmetic on (left, right) pairs (sim_pair.cuh)
 #endif
 
-// (left leg, right leg) pair; maps onto one 64-bit register pair / one FFMA2 operand
+// (left leg, right leg) pair; maps onto one 64-bit register pair
 struct alignas(8) f2 {
   float x, y;
 };
@@ -560,8 +560,8 @@ constexpr int kPhaseSyncs = 6;
 // r_k = rhs_k + sum_l G_kl lam_l is kept up to date for every row, so a row update is clamp(r_k) and the change
 // delta = lam_k' - lam_k is pushed into all six residuals with independent FMAs (r_m += G_mk delta). Same
 // iterates as the textbook sweep that re-sums each row, but the dependent chain per row is clamp -> delta -> one
-// FMA instead of a six-term sum (the solver is latency-bound: ~1.75 warps per scheduler), and the six updates
-// pair into three f32x2 FMAs in the paired build (sim_pair.cuh).
+// FMA instead of a six-term sum (the solver is latency-bound), and the six updates pair into three fma2 calls in the
+// paired build (sim_pair.cuh).
 //
 // Exit rule (Bullet's, btSequentialImpulseConstraintSolver::solveGroupCacheFriendlyIterations): after every sweep the
 // largest squared velocity-level change of a row, (delta_k * dinv_k)^2 with dinv_k = 1 / jacDiagABInv_k, is compared with
@@ -1132,7 +1132,7 @@ UPKIE_HD uint32_t state_sanity(const RobotState& S) {
 }
 
 // Host-side test entry (tests/hostsim): one env tick from a servo action. SCALAR_LEGS = false runs the substep the
-// kernels run (substep(): the f32x2-paired legs unless UPKIE_PAIRED_LEGS is 0), true the scalar-leg variant.
+// kernels run (substep(): the paired legs unless UPKIE_PAIRED_LEGS is 0), true the scalar-leg variant.
 template <bool SCALAR_LEGS = false, typename AnyFn>
 UPKIE_HD uint32_t step_servo_action(const SimParams& P, RobotState& S, float a[UPKIE_ACT_DIM], const float* eps, float mu,
                                     AnyFn warp_any, float* body_rec = nullptr) {

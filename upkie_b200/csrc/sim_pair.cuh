@@ -1,17 +1,14 @@
 // SPDX-License-Identifier: Apache-2.0
 //
-// sim_pair.cuh -- the physics substep with the LEFT and RIGHT leg packed into the
-// two lanes of sm_100a's f32x2 instructions (FFMA2 / FMUL2 / FADD2).
+// sim_pair.cuh -- the physics substep with the LEFT and RIGHT leg carried as
+// (left, right) pairs.
 //
-// Why: the step kernel is bound by the scalar fp32 pipe (profiles/r01_variants.md:
-// three-register scalar FFMA saturates at 0.59 inst/cycle/scheduler on B200, FFMA2
-// moves two FMAs per lane per instruction at the same issue cost). The two legs of
-// the robot run the same arithmetic on different data, so every per-leg scalar of
-// sim_core.cuh becomes an f2 = (left, right). SASS provides for free most of what the
-// pairing needs (not the negation of a register pair, see neg2): broadcast of a scalar register to both lanes
-// (`R.F32`), lane swap (`R.F32x2.LO_HI`, used for the cross-leg impulse responses)
-// and 64-bit constant-bank operands (the per-leg model constants are stored as
-// adjacent pairs in SimParams).
+// The two legs of the robot run the same arithmetic on different data, so every
+// per-leg scalar of sim_core.cuh becomes an f2 = (left, right) and the per-leg model
+// constants are stored as adjacent pairs in SimParams. On sm_90 each pair operation
+// is two scalar instructions with explicit rounding (fma2 / mul2 / add2 below): the
+// hot paths carry pre-negated copies (noz, ninvD, negated LDL factors, p' = -p in
+// the up-pass) so that every update is one fused multiply-add per lane.
 //
 // Included by sim_core.cuh; same mathematics as the scalar functions there, which
 // remain available with -DUPKIE_PAIRED_LEGS=0.
@@ -25,25 +22,12 @@ UPKIE_HD f2 mk2(float a, float b) { f2 r; r.x = a; r.y = b; return r; }
 UPKIE_HD f2 bc2(float a) { return mk2(a, a); }          // broadcast
 UPKIE_HD f2 swp2(f2 v) { return mk2(v.y, v.x); }       // lane swap (free: .LO_HI operand modifier)
 #if defined(__CUDA_ARCH__)
-// FFMA2 / FMUL2 / FADD2 take no negate modifier on a packed register operand (checked in SASS: a scalar
-// negation of each lane costs two FADDs), so a packed negation is ONE multiply by (-1, -1) -- exact -- and the
-// hot paths below carry pre-negated copies instead (noz, ninvD, negated LDL factors, p' = -p in the up-pass).
-UPKIE_HD f2 neg2(f2 v) {
-  const float2 r = __fmul2_rn(make_float2(v.x, v.y), make_float2(-1.f, -1.f));
-  return mk2(r.x, r.y);
-}
-UPKIE_HD f2 fma2(f2 a, f2 b, f2 c) {
-  const float2 r = __ffma2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y), make_float2(c.x, c.y));
-  return mk2(r.x, r.y);
-}
-UPKIE_HD f2 mul2(f2 a, f2 b) {
-  const float2 r = __fmul2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  return mk2(r.x, r.y);
-}
-UPKIE_HD f2 add2(f2 a, f2 b) {
-  const float2 r = __fadd2_rn(make_float2(a.x, a.y), make_float2(b.x, b.y));
-  return mk2(r.x, r.y);
-}
+// sm_90 has no packed f32x2 arithmetic: each lane is one scalar instruction with round-to-nearest intrinsics, which the
+// compiler may neither contract nor reassociate, so the results match a packed (FFMA2 / FMUL2 / FADD2) build bit for bit.
+UPKIE_HD f2 neg2(f2 v) { return mk2(-v.x, -v.y); }
+UPKIE_HD f2 fma2(f2 a, f2 b, f2 c) { return mk2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+UPKIE_HD f2 mul2(f2 a, f2 b) { return mk2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+UPKIE_HD f2 add2(f2 a, f2 b) { return mk2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 #else
 UPKIE_HD f2 neg2(f2 v) { return mk2(-v.x, -v.y); }
 UPKIE_HD f2 fma2(f2 a, f2 b, f2 c) { return mk2(a.x * b.x + c.x, a.y * b.y + c.y); }
@@ -608,10 +592,9 @@ UPKIE_HD void legs_impulse_up_general(const SimParams& P, const LegCache2& lc, c
   for (int i = 0; i < 6; ++i) nptop[i] = q[i];
 }
 
-// Round-2 A/B on a B200 (profiles/r02_variants.md): two rewrites that cut ~280 instructions per substep out of this
-// function - closed-form up-passes for the joint-limit directions, the Delassus matrix stored as paired columns and
-// scaled in place - measured SLOWER (0.1423 / 0.1484 ms against 0.1403 ms per 65 536-env tick): they lengthen live
-// ranges in a kernel that already spills, and ptxas' schedule matters more than the instruction count here. Kept as is.
+// Two rewrites that cut ~280 instructions per substep out of this function - closed-form up-passes for the joint-limit
+// directions, the Delassus matrix stored as paired columns and scaled in place - were measured slower: they lengthen
+// live ranges in a kernel that already spills, and ptxas' schedule matters more than the instruction count here.
 template <typename AnyFn, typename SyncFn>
 UPKIE_HD void contact_solve_ten_rows(const SimParams& P, RobotState& S, const LegCache2& lc, const float IA0[21],
                                      const float nIA0[21], const float R[9], const float zb[3], float inv_n,
@@ -815,7 +798,7 @@ UPKIE_HD void contact_solve_ten_rows(const SimParams& P, RobotState& S, const Le
 #endif
   };
 #ifndef UPKIE_SWEEPS_PER_TRIP
-#define UPKIE_SWEEPS_PER_TRIP 2  // measured on a B200, 65 536-env torque workload: 1 -> 0.1465, 2 -> 0.1384, 4 -> 0.1419 ms per tick
+#define UPKIE_SWEEPS_PER_TRIP 2  // sweeps between two warp votes on the exit test
 #endif
   for (int it = 0; it < P.pgs_iterations; it += UPKIE_SWEEPS_PER_TRIP) {
     after_sweep(sweep(false), it);  // even iteration: the non-contact rows are walked backwards
@@ -1286,7 +1269,7 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
   lim.n = 0;
   // limits: 0 no joint-limit rows, 1 scalar slow path for the robots that have one, 2 packed ten-row solver for all
   // The scalar slow path exists in the HOST build only (the CPU test-suite's independent second implementation of the
-  // limit rows): on a B200 it measured 18x the plain kernel on the torque workload (profiles/r02_limits.md) and its
+  // limit rows): on the device the whole warp would wait for the lanes that take it, and its
   // dynamically indexed local arrays cost every NOISE=2 kernel a 2 KB stack frame. On the device 1 aliases to 3.
   // body-ground contacts: a warp that holds a robot with a collision point near the ground solves all rows of its
   // robots in general_contact_solve() instead of the packed solvers (warp-uniform choice)
@@ -1496,7 +1479,7 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
 #pragma unroll
       for (int p = 0; p < 3; ++p) r2[p] = fma2(Gc[l][p], bc2(lam[l]), r2[p]);
     // One sweep = six row updates in Bullet's order: clamp the row's residual, push the change into all six
-    // residuals (three FFMA2), keep the largest velocity-level change of the sweep. A lane whose sweep stayed at or
+    // residuals (three paired FMAs), keep the largest velocity-level change of the sweep. A lane whose sweep stayed at or
     // below Bullet's residual threshold is frozen (its later updates are no-ops) until the warp's last lane is done.
     bool frozen = false;
     auto sweep = [&]() -> float {

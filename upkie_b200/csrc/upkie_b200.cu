@@ -1,6 +1,6 @@
 // SPDX-License-Identifier: Apache-2.0
 //
-// upkie_b200.cu -- sm_100a kernels and the C ABI of include/upkie_b200.h.
+// upkie_b200.cu -- sm_90a kernels and the C ABI of include/upkie_b200.h.
 //
 // Kernels (one thread = one robot, state struct-of-arrays, model in the kernel
 // parameter constant bank):
@@ -65,8 +65,8 @@ struct Handle {
   int autoreset = AUTORESET_DISABLED;
   uint64_t seed = 0, env_offset = 0;
   int block = UPKIE_DEFAULT_BLOCK;
-  int num_sms = 148;
-  int host_chunks = 2;           // chunks of the pipelined host-buffer step (measured best of 2..16, tools/e2e_parts.py)
+  int num_sms = 0;               // cudaDevAttrMultiProcessorCount, read at create
+  int host_chunks = 2;           // chunks of the pipelined host-buffer step (tools/e2e_parts.py sweeps 2..16)
   uint64_t step_launches = 0;    // step kernels launched (upkie_b200_launch_count)
   int host_block = 128;          // zero-copy step: persistent blocks of 4 warps, one per SM: ~3.5 tiles per block at
   int host_blocks_per_sm = 1;    // 65536 envs, so PCIe reads of tile k+1 overlap the compute of tile k
@@ -219,11 +219,11 @@ __global__ void k_init_state(const __grid_constant__ SimParams P, int n, int n_p
   (void)n;
 }
 
-// Block size per launch. Two measured effects (profiles/r01_variants.md): (1) the warps of a block run the
-// substep body in lock-step (one barrier per substep) and share its instruction fetches, so large blocks win
-// (256 > 128 > 64); (2) with 255 registers/thread one 256-thread block fills an SM, so 65 536 envs = 256 blocks
-// = 1.73 waves left 25 % of the SM-time idle. Pick the number of waves k first, then the block size (multiple of
-// 32) that makes the grid k * num_sms blocks: every SM gets the same number of equally sized blocks.
+// Block size per launch. (1) The warps of a block run the substep body in lock-step (one barrier per substep) and
+// share its instruction fetches, so larger blocks fetch less per warp; (2) with 255 registers/thread one 256-thread
+// block fills an SM, so a fixed block size leaves a partial last wave (65 536 envs in 256-thread blocks on 132 SMs:
+// 1.94 waves). Pick the number of waves k first, then the block size (multiple of 32) that makes the grid
+// k * num_sms blocks: every SM gets the same number of equally sized blocks.
 int pick_block(const Handle* h, int cnt) {
   if (h->block > 0) return h->block;
   const int per_wave = h->num_sms * UPKIE_MAX_THREADS;
@@ -329,8 +329,8 @@ T* mapped(T* p) {
 // pinned (mapped) buffers one of three pipelines runs, `zero_copy` selecting it:
 //   2 (default, servos)  hybrid: the copy engine streams the action rows in, chunk by chunk on one stream; each
 //                        chunk's TILE=1 kernel waits for its rows only and writes observations / flags straight
-//                        to host memory. Copy-engine reads overlap SM writes on the link, SM reads do not
-//                        (63 GB/s combined, tools/micro/pcie_duplex.cu).
+//                        to host memory. Copy-engine reads overlap SM writes on the link, SM reads and writes
+//                        share it (tools/micro/pcie_duplex.cu measures both).
 //   1                    one persistent TILE=1 launch reading actions from and writing observations to host memory.
 //   0                    H2D copy -> TILE=0 kernel -> D2H copies per chunk on rotating streams.
 // `compact` (servos): observation rows [6][3] = position, velocity, torque (TILE=1 kernels).

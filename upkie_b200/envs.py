@@ -1,5 +1,5 @@
 # SPDX-License-Identifier: Apache-2.0
-"""Vectorised Upkie environments on the sm_100a kernels.
+"""Vectorised Upkie environments on the sm_90a kernels.
 
 ``B200VectorEnv`` is a ``gymnasium.vector.VectorEnv`` whose
 ``single_action_space`` / ``single_observation_space`` are identical to the

@@ -129,7 +129,7 @@ class PeerRolloutBuffer(RolloutBuffer):
 
     Why not NCCL's all-gather here: the step kernel occupies every SM (255 registers x 224 threads leave no
     room for another block), so a collective implemented as SM kernels only advances when simulation blocks
-    retire and slows the simulation it is meant to overlap (2 GPUs: 74-89 % weak-scaling efficiency). Copy
+    retire and slows the simulation it is meant to overlap. Copy
     engines need no SM.
     """
 

@@ -4,7 +4,7 @@
 ``UpkieSim`` owns a ``libupkie_b200`` handle and exposes the flat fast path of
 SURVEY.md section 8(b): ``step_servos(action[N, 6, 6]) -> obs[N, 6, 5], reward[N],
 terminated[N], truncated[N]`` over PyTorch CUDA tensors (PyTorch is used for
-device memory and streams only; all arithmetic happens in the sm_100a kernels).
+device memory and streams only; all arithmetic happens in the sm_90a kernels).
 """
 
 import ctypes as C

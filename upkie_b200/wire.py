@@ -1,6 +1,6 @@
 # SPDX-License-Identifier: Apache-2.0
-"""Wire format of the reference's agent <-> spine mailbox, for replaying B200 trajectories against a real spine
-(or a spine log against the B200 simulator).
+"""Wire format of the reference's agent <-> spine mailbox, for replaying GPU trajectories against a real spine
+(or a spine log against the GPU simulator).
 
 The reference exchanges msgpack dictionaries through a POSIX shared-memory mailbox laid out as
 ``[request: u32][size: u32][payload]`` in native byte order (``upkie/envs/backends/spine/spine_interface.py:108-169``,
