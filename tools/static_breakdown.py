@@ -7,6 +7,8 @@ belongs to (needs the library built with -lineinfo, which build.py does). Develo
     python tools/static_breakdown.py [kernel-substring] --ncu reports/prof.ncu-rep
         # adds DYNAMIC columns from an `ncu --set full --import-source on` capture of the SAME build: warp
         # instructions executed and sampled stall reasons per bucket (joined by instruction index)
+    python tools/static_breakdown.py [kernel-substring] --lib build/ab_step/base/upkie_b200/libupkie_b200.so
+        # another build of the library, e.g. the base revision that tools/ab_step.py builds
 
 The "substep:" buckets (and `servo_substep`) are inside the `nb_substeps` loop; the PGS bucket holds two inlined
 copies of the six-row sweep, each run once per pair of sweeps.
@@ -93,10 +95,15 @@ def main():
         k = args.index("--ncu")
         rep = args[k + 1]
         del args[k:k + 2]
+    lib = LIB
+    if "--lib" in args:
+        k = args.index("--lib")
+        lib = args[k + 1]
+        del args[k:k + 2]
     want = args[0] if args else "k_stepILi0ELi1ELi2ELi1E"
     dyn = ncu_rows(rep) if rep else None
     with tempfile.TemporaryDirectory() as tmp:
-        subprocess.run(["cuobjdump", "-xelf", "all", LIB], cwd=tmp, check=True, stdout=subprocess.DEVNULL)
+        subprocess.run(["cuobjdump", "-xelf", "all", lib], cwd=tmp, check=True, stdout=subprocess.DEVNULL)
         text = None
         for cubin in sorted(os.listdir(tmp)):
             dis = subprocess.run(["nvdisasm", "--print-line-info-inline", os.path.join(tmp, cubin)],
@@ -109,7 +116,7 @@ def main():
                 print(f"kernel {m.group(1)[:90]}... in {cubin}")
                 break
         if text is None:
-            raise SystemExit(f"no kernel matching {want!r} in {LIB}")
+            raise SystemExit(f"no kernel matching {want!r} in {lib}")
     starts = {}
 
     def func_of(fn, ln):

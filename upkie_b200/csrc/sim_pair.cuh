@@ -6,9 +6,10 @@
 // The two legs of the robot run the same arithmetic on different data, so every
 // per-leg scalar of sim_core.cuh becomes an f2 = (left, right) and the per-leg model
 // constants are stored as adjacent pairs in SimParams. On sm_90 each pair operation
-// is two scalar instructions with explicit rounding (fma2 / mul2 / add2 below): the
-// hot paths carry pre-negated copies (noz, ninvD, negated LDL factors, p' = -p in
-// the up-pass) so that every update is one fused multiply-add per lane.
+// is two scalar instructions with explicit rounding (fma2 / mul2 / add2 below). A
+// negated operand (neg2) costs nothing there: FFMA and FMUL negate their inputs, and
+// fma(-a, b, c) rounds exactly as fma(na, b, c) with na = -a, so no negated copies
+// are kept in registers.
 //
 // Included by sim_core.cuh; same mathematics as the scalar functions there, which
 // remain available with -DUPKIE_PAIRED_LEGS=0.
@@ -43,28 +44,27 @@ UPKIE_HD void cross3_2(const f2 a[3], const f2 b[3], f2 c[3]) {
 }
 
 // S^T x for S = s * [0 1 0 | -oz 0 ox], both legs
-UPKIE_HD f2 sdot2(f2 s, f2 ox, f2 noz, const f2 x[6]) { return mul2(s, fma2(ox, x[5], fma2(noz, x[3], x[1]))); }
+UPKIE_HD f2 sdot2(f2 s, f2 ox, f2 oz, const f2 x[6]) { return mul2(s, fma2(ox, x[5], fma2(neg2(oz), x[3], x[1]))); }
 
 struct LegCache2 {
-  f2 ox[3], oz[3], noz[3];  // joint origins (x, z) in the base frame, and -z
+  f2 ox[3], oz[3];  // joint origins (x, z) in the base frame
   f2 U[3][6];
-  f2 invD[3], ninvD[3];     // 1 / D and -1 / D
+  f2 invD[3];       // 1 / D
 };
 
-// two right-hand sides at once against the scalar LDL^T factors of ldl6(); nA = -A (negated once per substep,
-// the packed FMA has no negate modifier)
-UPKIE_HD void ldl6_solve2(const float A[21], const float nA[21], f2 x[6]) {
+// two right-hand sides at once against the scalar LDL^T factors of ldl6()
+UPKIE_HD void ldl6_solve2(const float A[21], f2 x[6]) {
 #pragma unroll
   for (int i = 1; i < 6; ++i) {
 #pragma unroll
-    for (int k = 0; k < i; ++k) x[i] = fma2(bc2(nA[SI(k, i)]), x[k], x[i]);
+    for (int k = 0; k < i; ++k) x[i] = fma2(bc2(-A[SI(k, i)]), x[k], x[i]);
   }
 #pragma unroll
   for (int i = 0; i < 6; ++i) x[i] = mul2(x[i], bc2(A[SI(i, i)]));
 #pragma unroll
   for (int i = 4; i >= 0; --i) {
 #pragma unroll
-    for (int k = i + 1; k < 6; ++k) x[i] = fma2(bc2(nA[SI(i, k)]), x[k], x[i]);
+    for (int k = i + 1; k < 6; ++k) x[i] = fma2(bc2(-A[SI(i, k)]), x[k], x[i]);
   }
 }
 
@@ -93,7 +93,6 @@ UPKIE_HD void legs_pass12(const SimParams& P, const float q[6], const float qd[6
       oz = oz_n;
       lc.ox[k] = ox;
       lc.oz[k] = oz;
-      lc.noz[k] = neg2(oz);
       phi = fma2(s, mk2(q[k], q[k + 3]), phi);
       if (k < 2 || !P.wheel_symmetric) {
         float sx, cx, sy, cy;
@@ -106,7 +105,7 @@ UPKIE_HD void legs_pass12(const SimParams& P, const float q[6], const float qd[6
       sphi[k] = sp;
       const f2 w = mul2(s, mk2(qd[k], qd[k + 3]));
       Vc[1] = add2(Vc[1], w);
-      Vc[3] = fma2(lc.noz[k], w, Vc[3]);
+      Vc[3] = fma2(neg2(oz), w, Vc[3]);
       Vc[5] = fma2(ox, w, Vc[5]);
 #pragma unroll
       for (int i = 0; i < 6; ++i) V[k][i] = Vc[i];
@@ -116,7 +115,7 @@ UPKIE_HD void legs_pass12(const SimParams& P, const float q[6], const float qd[6
 #pragma unroll
   for (int k = 2; k >= 0; --k) {
     const f2 s = P.sgn2[k];
-    const f2 ox = lc.ox[k], oz = lc.oz[k], noz = lc.noz[k];
+    const f2 ox = lc.ox[k], oz = lc.oz[k];
     const f2 scale = eps ? mk2(1.f + eps[k], 1.f + eps[k + 3]) : bc2(1.f);
     const f2 m = mul2(P.mass2[k], scale);
     f2 C[3], Ib[6];
@@ -229,7 +228,6 @@ UPKIE_HD void legs_pass12(const SimParams& P, const float q[6], const float qd[6
       U[1] = mul2(s, Iyy);
       invD = mul2(free2, mk2(1.f / Iyy.x, 1.f / Iyy.y));
       u = sub2(mk2(tau[k], tau[k + 3]), mul2(s, spin_damp));
-      lc.ninvD[k] = neg2(invD);
       // Ia = IA - U U^T / D: the rotor stops resisting rotation about its own axis; pa = pA + Ia c + S u
       IA[SI(1, 1)] = fma2(neg2(free2), Iyy, IA[SI(1, 1)]);
 #pragma unroll
@@ -244,16 +242,14 @@ UPKIE_HD void legs_pass12(const SimParams& P, const float q[6], const float qd[6
       p[1] = fma2(mul2(s, free2), u, p[1]);
     } else {
 #pragma unroll
-      for (int r = 0; r < 6; ++r) U[r] = mul2(s, fma2(ox, IA[SI(r, 5)], fma2(noz, IA[SI(r, 3)], IA[SI(r, 1)])));
-      const f2 D = sdot2(s, ox, noz, U);
+      for (int r = 0; r < 6; ++r) U[r] = mul2(s, fma2(ox, IA[SI(r, 5)], fma2(neg2(oz), IA[SI(r, 3)], IA[SI(r, 1)])));
+      const f2 D = sdot2(s, ox, oz, U);
       invD = mul2(free2, mk2(1.f / D.x, 1.f / D.y));
-      u = sub2(mk2(tau[k], tau[k + 3]), sdot2(s, ox, noz, pA));
+      u = sub2(mk2(tau[k], tau[k + 3]), sdot2(s, ox, oz, pA));
       // Ia = IA - U U^T / D ; pa = pA + Ia c + U u / D
-      const f2 ninvD = neg2(invD);
-      lc.ninvD[k] = ninvD;
       f2 nUd[6];
 #pragma unroll
-      for (int r = 0; r < 6; ++r) nUd[r] = mul2(U[r], ninvD);
+      for (int r = 0; r < 6; ++r) nUd[r] = mul2(U[r], neg2(invD));
 #pragma unroll
       for (int r = 0; r < 6; ++r) {
 #pragma unroll
@@ -295,12 +291,12 @@ UPKIE_HD void legs_pass3(const SimParams& P, const LegCache2& lc, const f2 cc[3]
       a[i] = add2(a[i], cc[k][i]);
       dot = fma2(lc.U[k][i], a[i], dot);
     }
-    const f2 dd = fma2(dot, lc.ninvD[k], mul2(uu[k], lc.invD[k]));  // (u - U.a) / D
+    const f2 dd = fma2(dot, neg2(lc.invD[k]), mul2(uu[k], lc.invD[k]));  // (u - U.a) / D
     qdd[k] = dd.x;
     qdd[k + 3] = dd.y;
     const f2 w = mul2(P.sgn2[k], dd);
     a[1] = add2(a[1], w);
-    a[3] = fma2(lc.noz[k], w, a[3]);
+    a[3] = fma2(neg2(lc.oz[k]), w, a[3]);
     a[5] = fma2(lc.ox[k], w, a[5]);
   }
 }
@@ -314,9 +310,9 @@ UPKIE_HD void legs_impulse_up(const SimParams& P, const LegCache2& lc, const f2 
   for (int i = 0; i < 6; ++i) q[i] = f[i];
 #pragma unroll
   for (int k = 2; k >= 0; --k) {
-    const f2 u = sdot2(P.sgn2[k], lc.ox[k], lc.noz[k], q);
+    const f2 u = sdot2(P.sgn2[k], lc.ox[k], lc.oz[k], q);
     uu[k] = u;
-    const f2 nud = mul2(u, lc.ninvD[k]);
+    const f2 nud = mul2(u, neg2(lc.invD[k]));
 #pragma unroll
     for (int i = 0; i < 6; ++i) q[i] = fma2(lc.U[k][i], nud, q[i]);
   }
@@ -338,12 +334,11 @@ UPKIE_HD void legs_impulse_down(const SimParams& P, const LegCache2& lc, const f
 #pragma unroll
     for (int i = 0; i < 6; ++i) dot = fma2(SWAP ? swp2(lc.U[k][i]) : lc.U[k][i], aw[i], dot);
     const f2 invD = SWAP ? swp2(lc.invD[k]) : lc.invD[k];
-    const f2 ninvD = SWAP ? swp2(lc.ninvD[k]) : lc.ninvD[k];
-    const f2 dd = SWAP ? mul2(dot, ninvD) : fma2(dot, ninvD, mul2(uu[k], invD));
+    const f2 dd = SWAP ? mul2(dot, neg2(invD)) : fma2(dot, neg2(invD), mul2(uu[k], invD));
     dqd[k] = dd;
     const f2 w = mul2(SWAP ? swp2(P.sgn2[k]) : P.sgn2[k], dd);
     aw[1] = add2(aw[1], w);
-    aw[3] = fma2(SWAP ? swp2(lc.noz[k]) : lc.noz[k], w, aw[3]);
+    aw[3] = fma2(neg2(SWAP ? swp2(lc.oz[k]) : lc.oz[k]), w, aw[3]);
     aw[5] = fma2(SWAP ? swp2(lc.ox[k]) : lc.ox[k], w, aw[5]);
   }
 }
@@ -580,11 +575,11 @@ UPKIE_HD void legs_impulse_up_general(const SimParams& P, const LegCache2& lc, c
   for (int i = 0; i < 6; ++i) q[i] = f ? f[i] : bc2(0.f);
 #pragma unroll
   for (int k = 2; k >= 0; --k) {
-    f2 u = sdot2(P.sgn2[k], lc.ox[k], lc.noz[k], q);  // zero above the level a joint impulse enters at
+    f2 u = sdot2(P.sgn2[k], lc.ox[k], lc.oz[k], q);  // zero above the level a joint impulse enters at
     if (k == 1) u = add2(u, gk);
     if (k == 0) u = add2(u, gh);
     uu[k] = u;
-    const f2 nud = mul2(u, lc.ninvD[k]);
+    const f2 nud = mul2(u, neg2(lc.invD[k]));
 #pragma unroll
     for (int i = 0; i < 6; ++i) q[i] = fma2(lc.U[k][i], nud, q[i]);
   }
@@ -597,7 +592,7 @@ UPKIE_HD void legs_impulse_up_general(const SimParams& P, const LegCache2& lc, c
 // live ranges in a kernel that already spills, and ptxas' schedule matters more than the instruction count here.
 template <typename AnyFn, typename SyncFn>
 UPKIE_HD void contact_solve_ten_rows(const SimParams& P, RobotState& S, const LegCache2& lc, const float IA0[21],
-                                     const float nIA0[21], const float R[9], const float zb[3], float inv_n,
+                                     const float R[9], const float zb[3], float inv_n,
                                      const f2 Pc[3], const f2& dist, bool actL, bool actR, float mu, AnyFn warp_any,
                                      SyncFn phase_sync) {
   // limit slots: dir = +1 at the lower bound, -1 at the upper one, 0 when the joint is inside its range
@@ -651,7 +646,7 @@ UPKIE_HD void contact_solve_ten_rows(const SimParams& P, RobotState& S, const Le
     for (int k = 0; k < 3; ++k) {
       const f2 w = mul2(P.sgn2[k], mk2(S.qd[k], S.qd[k + 3]));
       Vw[1] = add2(Vw[1], w);
-      Vw[3] = fma2(lc.noz[k], w, Vw[3]);
+      Vw[3] = fma2(neg2(lc.oz[k]), w, Vw[3]);
       Vw[5] = fma2(lc.ox[k], w, Vw[5]);
     }
   }
@@ -666,7 +661,7 @@ UPKIE_HD void contact_solve_ten_rows(const SimParams& P, RobotState& S, const Le
       f2 da0[6];
 #pragma unroll
       for (int i = 0; i < 6; ++i) da0[i] = pt_[d][i];
-      ldl6_solve2(IA0, nIA0, da0);
+      ldl6_solve2(IA0, da0);
 #pragma unroll
       for (int e = 0; e <= d; ++e) {
         f2 wo = bc2(0.f), wc = bc2(0.f);
@@ -1224,9 +1219,6 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
   legs_pass12(P, S.q, S.qd, tau, V0, eps, lc, cc, uu, IA0, pA0, locked);
   phase_sync();  // 1
   ldl6(IA0);
-  float nIA0[21];  // negated factors for the packed solves (ldl6_solve2)
-#pragma unroll
-  for (int i = 0; i < 21; ++i) nIA0[i] = -IA0[i];
   float a0[6];
 #pragma unroll
   for (int i = 0; i < 6; ++i) a0[i] = wext ? wext[i] - pA0[i] : -pA0[i];
@@ -1335,7 +1327,7 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
   } else
 #endif
   if (ten_rows) {
-    contact_solve_ten_rows(P, S, lc, IA0, nIA0, R, zb, inv_n, Pc, dist, inL, inR, mu, warp_any, phase_sync);
+    contact_solve_ten_rows(P, S, lc, IA0, R, zb, inv_n, Pc, dist, inL, inR, mu, warp_any, phase_sync);
   } else if (!warp_any(actL || actR)) {
     S.lam_n[0] = 0.f;
     S.lam_n[1] = 0.f;
@@ -1373,7 +1365,7 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
       for (int k = 0; k < 3; ++k) {
         const f2 w = mul2(P.sgn2[k], mk2(S.qd[k], S.qd[k + 3]));
         Vw[1] = add2(Vw[1], w);
-        Vw[3] = fma2(lc.noz[k], w, Vw[3]);
+        Vw[3] = fma2(neg2(lc.oz[k]), w, Vw[3]);
         Vw[5] = fma2(lc.ox[k], w, Vw[5]);
       }
     }
@@ -1393,7 +1385,7 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
         f2 da0[6];
 #pragma unroll
         for (int i = 0; i < 6; ++i) da0[i] = pt_[d][i];
-        ldl6_solve2(IA0, nIA0, da0);  // a0(d) = -IA0^-1 ptop(d); lane x: left column, lane y: right column
+        ldl6_solve2(IA0, da0);  // a0(d) = -IA0^-1 ptop(d); lane x: left column, lane y: right column
 #pragma unroll
         for (int e = 0; e <= d; ++e) {
           f2 wo = bc2(0.f), wc = bc2(0.f);

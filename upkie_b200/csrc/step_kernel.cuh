@@ -172,8 +172,11 @@ __device__ __forceinline__ void step_env(
         if (resetting && sub == 2) spine_assemble_observation(S, L);
         spine_cycle(P, S, L, a, resetting, eps, mu, WarpAny(), PhaseSync(), P.joint_limits >= 1 ? P.joint_limits : 1, br);
       } else {
+        // NOISE >= 2: the device's two limit modes (1 and 0 alias to 3 there, see physics_substep_paired), spelled as
+        // a choice between two nonzero constants so that the compiler drops servo_substep's limits == 0 branches, a
+        // second and third inlined copy of the substep that these kernels never run
         servo_substep(P, S, a, resetting, eps, mu, WarpAny(), PhaseSync(), NOISE ? &nz : nullptr, sub,
-                      (NOISE && ext) ? &xf : nullptr, NOISE >= 2 ? (P.joint_limits >= 1 ? P.joint_limits : 1) : 0, br);
+                      (NOISE && ext) ? &xf : nullptr, NOISE >= 2 ? (P.joint_limits == 2 ? 2 : 3) : 0, br);
       }
     } else {
 #pragma unroll
