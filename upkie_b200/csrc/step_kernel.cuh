@@ -449,10 +449,20 @@ cudaError_t launch_step_mode(const StepArgs& a) {
   const int aligned =
       ((reinterpret_cast<uintptr_t>(a.action) | reinterpret_cast<uintptr_t>(a.obs)) & 15) == 0 && (a.i0 % 32) == 0;
   const int coalesce = (aligned ? 1 : 0) | ((TILE && a.compact_obs) ? 2 : 0);  // bit 0 tile path, bit 1 compact rows
-#define LAUNCH_N(AR, NZ)                                                                                         \
-  k_step<MODE, AR, NZ, TILE><<<grid, a.block, smem, a.stream>>>(                                                 \
-      *a.P, a.i0, a.i0 + a.cnt, a.n_pad, a.state, a.action, a.obs, a.reward, a.terminated, a.truncated, a.eps,   \
-      a.mu, a.err, a.done_prev, a.episode, a.tick, a.seed, a.env_offset, a.ext, a.ext_local, coalesce, a.peers, a.lag)
+  // a 256-thread block's two tile buffers take 72 KB: above 48 KB of dynamic shared memory a kernel must opt in (per
+  // device, so on every launch)
+#define LAUNCH_N(AR, NZ)                                                                                          \
+  do {                                                                                                            \
+    if (smem > 48 * 1024) {                                                                                       \
+      const cudaError_t e = cudaFuncSetAttribute(k_step<MODE, AR, NZ, TILE>,                                      \
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));         \
+      if (e != cudaSuccess) return e;                                                                             \
+    }                                                                                                             \
+    k_step<MODE, AR, NZ, TILE><<<grid, a.block, smem, a.stream>>>(                                                \
+        *a.P, a.i0, a.i0 + a.cnt, a.n_pad, a.state, a.action, a.obs, a.reward, a.terminated, a.truncated, a.eps,  \
+        a.mu, a.err, a.done_prev, a.episode, a.tick, a.seed, a.env_offset, a.ext, a.ext_local, coalesce, a.peers, \
+        a.lag);                                                                                                   \
+  } while (0)
 #if UPKIE_STEP_SPINE_TU
 #define LAUNCH(AR) LAUNCH_N(AR, 3)
 #elif UPKIE_STEP_BODY_TU
