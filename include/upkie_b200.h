@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define UPKIE_B200_ABI_VERSION 6
+#define UPKIE_B200_ABI_VERSION 7
 
 #define UPKIE_NJ 6 /* actuated joints */
 #define UPKIE_NB 7 /* moving bodies: base lump + 2 x (upper leg, lower leg, wheel) */
@@ -287,6 +287,16 @@ typedef struct UpkieSimConfig {
    * sweep. Default 1e-7; 0 = always pgs_iterations sweeps. Evaluated per robot after every sweep: a robot that has
    * met the threshold keeps its impulses while the other robots of its warp finish. */
   double solver_residual_threshold;
+  /* Episode time limit (ABI 7), per env, with the semantics of Gymnasium's TimeLimit wrapper: 0 (default) = none,
+   * truncated is always 0. T > 0: every env counts the agent steps since its last reset (upkie_b200_reset, masked or
+   * not, and either fused auto-reset set the count to 0; the next-step auto-reset's own step is not counted) and a
+   * step returns truncated = 1 once that count reaches T, independently of terminated (both can be 1). The fused
+   * auto-reset fires on terminated | truncated; with auto-reset disabled truncated stays 1 until the env is reset.
+   * The counts are kept only while a limit is set: when upkie_b200_set_config turns a limit on or changes it, every
+   * env's count is set to 0, so episodes are timed from that call. upkie_b200_get_elapsed / set_elapsed read and
+   * restore them. The in-kernel rollout transports (multicast, peers, push) reject a limit. */
+  int32_t max_episode_steps;
+  int32_t reserved_max_episode_steps;
 } UpkieSimConfig;
 
 /* Spine-mode lag record of one env (upkie_b200_get_lag / set_lag, [N][UPKIE_LAG_DIM] floats): the two latest
@@ -376,7 +386,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config);
  * at t+1, which returns its reset observation and ignores its action),
  * 2 = same-step (re-initialised inside the terminating call, which returns the
  * reset observation together with terminated = 1). Initial states are drawn on
- * the device as in upkie_b200_reset(init_state = NULL). */
+ * the device as in upkie_b200_reset(init_state = NULL). With a time limit
+ * (UpkieSimConfig.max_episode_steps) an env resets on terminated | truncated;
+ * in same-step mode upkie_b200_step / upkie_b200_step_host can also return the
+ * observation the resetting envs reached before their reset (final_obs). */
 int upkie_b200_set_autoreset(void* handle, int mode, uint64_t seed, uint64_t env_offset);
 
 /* Per-env domain randomisation; either pointer may be NULL (= nominal).
@@ -460,8 +473,10 @@ int upkie_b200_push_rows(void* handle, const UpkiePush* push, void* stream);
  * pageable buffers go through pinned staging in pipelined chunks (H2D copy ->
  * kernel -> D2H copy on rotating streams).
  * `reward` and `truncated` may be NULL here and in the device-buffer calls: the
- * reference returns constants for them (0.0, upkie_env.py:230; False,
- * upkie_env.py:197) and a caller that knows it saves the bytes. */
+ * reference returns a constant reward (0.0, upkie_env.py:230) and leaves
+ * truncation to a TimeLimit wrapper (False, upkie_env.py:197,232). truncated
+ * is 0 for every env unless the configuration sets max_episode_steps, so a
+ * caller without a limit that knows it saves the bytes. */
 int upkie_b200_step_servos_host(void* handle, const float* action, float* obs,
                                 float* reward, uint8_t* terminated,
                                 uint8_t* truncated);
@@ -470,11 +485,36 @@ int upkie_b200_step_gyropod_host(void* handle, const float* action, int act_dim,
                                  uint8_t* truncated);
 /* UpkieServos step that transports only what changes: obs[N][6][3] = position,
  * velocity, torque per joint. Temperature (42.0) and voltage (18.0) are
- * constants of the simulator (pybullet_backend.py:471-472), reward and
- * truncated constants of the env (upkie_env.py:197,230): the caller fills them
- * once. 72 + 1 B per env over PCIe instead of 126 B. */
+ * constants of the simulator (pybullet_backend.py:471-472), reward a constant
+ * of the env (upkie_env.py:230): the caller fills them once. truncated is not
+ * returned: it is 0 without a time limit; with max_episode_steps set, use
+ * upkie_b200_step_host with compact = 1. 72 + 1 B per env over PCIe instead
+ * of 126 B. */
 int upkie_b200_step_servos_host_compact(void* handle, const float* action,
                                         float* obs, uint8_t* terminated);
+
+/* General form of the step calls above: outputs in one struct, so that the compact servo rows can come with
+ * `truncated`, and any step with the observations of its same-step auto-resets.
+ * act_dim: 36 = UpkieServos (obs [N][6][5], or [N][6][3] with compact = 1), 2 = UpkieGyropod (obs [N][6]),
+ * 1 = UpkiePendulum (obs [N][4]). reward, truncated and final_obs may be NULL.
+ * final_obs (same-step auto-reset only; ignored in the other modes): every env that resets in this step first
+ * stores there, at its own row, the observation it would have returned without the reset (layout of `obs`; spine
+ * mode: the rows its spine assembled before the reset). The rows of the other envs are left untouched: mask them
+ * with terminated | truncated (Gymnasium's info["final_obs"] / info["_final_obs"]). */
+typedef struct UpkieStepOutputs {
+  float* obs;
+  float* reward;
+  uint8_t* terminated;
+  uint8_t* truncated;
+  float* final_obs;
+  int32_t compact;  /* UpkieServos: 1 = compact rows [6][3] (position, velocity, torque) */
+  int32_t reserved;
+} UpkieStepOutputs;
+/* device buffers, asynchronous on `stream` */
+int upkie_b200_step(void* handle, int act_dim, const float* action, const UpkieStepOutputs* out, void* stream);
+/* host buffers, synchronous, as upkie_b200_step_servos_host: final_obs, when given, is stored into by the kernel
+ * itself (through its mapped alias when it is pinned, else through a pinned copy of the caller's rows) */
+int upkie_b200_step_host(void* handle, int act_dim, const float* action, const UpkieStepOutputs* out);
 
 /* Replaces PyBulletBackend.get_spine_observation without side effects: returns
  * the observation assembled by the last reset/step. out[N][UPKIE_SPINE_DIM]. */
@@ -507,6 +547,11 @@ int upkie_b200_get_counters(void* handle, uint32_t* episode /* [N] */, uint32_t*
                             uint8_t* pending_reset /* [N] */, uint32_t* error_flags /* [N] */, void* stream);
 int upkie_b200_set_counters(void* handle, const uint32_t* episode, const uint32_t* tick,
                             const uint8_t* pending_reset, const uint32_t* error_flags, void* stream);
+/* Checkpoint / resume of the time-limit counts (UpkieSimConfig.max_episode_steps): agent steps since each env's
+ * last reset, elapsed[N] (device pointer). The steps count them only while a limit is set. An env whose next-step
+ * auto-reset is pending holds 0xffffffff: its reset step adds 1 and is thus not counted. */
+int upkie_b200_get_elapsed(void* handle, uint32_t* elapsed, void* stream);
+int upkie_b200_set_elapsed(void* handle, const uint32_t* elapsed, void* stream);
 
 /* Replaces PyBulletBackend.set_external_forces (pybullet_backend.py:603-625):
  * force[N][UPKIE_NB][3] (device pointer, newtons) acts at the centre of mass of

@@ -2,16 +2,16 @@
 """Before / after comparison of the step kernel library (developer tool).
 
     python tools/ab_step.py build [REV]   # no GPU needed: extracts REV (default HEAD) into build/ab_step/base,
-                                          # builds its library there, and builds the working tree's library
-    python tools/ab_step.py run [OUT]     # on the GPU: times both libraries with bench.py, alternating, and
+                                          # builds its libraries there, and builds the working tree's
+    python tools/ab_step.py run [OUT]     # on the GPU: times both revisions with bench.py, alternating, and
                                           # compares their outputs; writes OUT (default build/ab_step/out)
 
-`run` loads each library into the working tree's Python package through UPKIE_B200_LIB, so REV must have the same
-C ABI (include/upkie_b200.h) as the working tree. It runs, in this order:
+`run` times each revision with its own checkout: the old one runs build/ab_step/base/bench.py with its own Python
+package and libraries (cwd build/ab_step/base), the new one the working tree's. So the two may differ in their C ABI
+(include/upkie_b200.h). It runs, in this order:
   - bench.py --no-cpu-baseline --no-other-workloads, old / new alternating, ROUNDS times each (the headline);
-  - bench.py --no-cpu-baseline --dump-outputs once per library (same seeds): obs / terminated compared with
-    numpy.array_equal, and the secondary workloads of that run (exact mode uses the working tree's exact library
-    in both runs);
+  - bench.py --no-cpu-baseline --dump-outputs once per revision (same seeds): obs / terminated compared with
+    numpy.array_equal, and the secondary workloads of that run (exact mode: each revision's own exact library);
 and prints one JSON summary line with the card's name and power limit.
 """
 import json
@@ -23,8 +23,8 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BASE = os.path.join(ROOT, "build", "ab_step", "base")
-LIBS = {"old": os.path.join(BASE, "upkie_b200", "libupkie_b200.so"),
-        "new": os.path.join(ROOT, "upkie_b200", "libupkie_b200.so")}
+TREES = {"old": BASE, "new": ROOT}
+LIBS = {name: os.path.join(tree, "upkie_b200", "libupkie_b200.so") for name, tree in TREES.items()}
 ROUNDS = 5
 
 
@@ -34,7 +34,8 @@ def build():
     os.makedirs(BASE)
     archive = subprocess.run(["git", "-C", ROOT, "archive", rev], check=True, capture_output=True).stdout
     subprocess.run(["tar", "-x", "-C", BASE], input=archive, check=True)
-    build_lib = "import sys; sys.path.insert(0, '.'); from upkie_b200 import build; print(build.build(force=True))"
+    build_lib = ("import sys; sys.path.insert(0, '.'); from upkie_b200 import build; "
+                 "print(build.build(force=True), build.build_exact(force=True))")
     procs = [subprocess.Popen([sys.executable, "-c", build_lib], cwd=d) for d in (BASE, ROOT)]
     if any(p.wait() for p in procs):
         raise SystemExit("ab_step: library build failed")
@@ -43,12 +44,12 @@ def build():
                                text=True).stdout)
 
 
-def bench(lib, extra):
-    env = dict(os.environ, UPKIE_B200_LIB=lib)
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--no-cpu-baseline"] + extra,
-                       env=env, capture_output=True, text=True, cwd=ROOT)
+def bench(tree, extra):
+    env = {k: v for k, v in os.environ.items() if k != "UPKIE_B200_LIB"}
+    r = subprocess.run([sys.executable, os.path.join(tree, "bench.py"), "--gpus", "1", "--no-cpu-baseline"] + extra,
+                       env=env, capture_output=True, text=True, cwd=tree)
     if r.returncode != 0:
-        raise SystemExit(f"bench.py failed with {lib}:\n{r.stdout[-2000:]}\n{r.stderr[-4000:]}")
+        raise SystemExit(f"bench.py failed in {tree}:\n{r.stdout[-2000:]}\n{r.stderr[-4000:]}")
     return json.loads(r.stdout.strip().splitlines()[-1])
 
 
@@ -61,7 +62,8 @@ def card():
 def run():
     import numpy as np
 
-    out = sys.argv[2] if len(sys.argv) > 2 else os.path.join(ROOT, "build", "ab_step", "out")
+    # absolute: the old revision's bench.py runs with its own checkout as working directory
+    out = os.path.abspath(sys.argv[2] if len(sys.argv) > 2 else os.path.join(ROOT, "build", "ab_step", "out"))
     os.makedirs(out, exist_ok=True)
     for name, lib in LIBS.items():
         if not os.path.exists(lib):
@@ -70,8 +72,8 @@ def run():
     summary = {"card": card(), "base_rev": open(rev_file).read().strip() if os.path.exists(rev_file) else None}
     head = {name: [] for name in LIBS}
     for _ in range(ROUNDS):
-        for name, lib in LIBS.items():
-            j = bench(lib, ["--no-other-workloads"])
+        for name, tree in TREES.items():
+            j = bench(tree, ["--no-other-workloads"])
             head[name].append({"ms_per_step": j["ms_per_step"], "kernel_ms": j["roofline"]["kernel_ms"],
                                "sm_mhz": j["clocks"].get("sm_mhz"), "power_limit_w": j["clocks"].get("power_limit_w")})
             print(name, json.dumps(head[name][-1]), flush=True)
@@ -83,8 +85,8 @@ def run():
     old_ms = summary["headline"]["old"]["ms_per_step_median"]
     summary["headline"]["speedup"] = old_ms / summary["headline"]["new"]["ms_per_step_median"]
     full = {}
-    for name, lib in LIBS.items():
-        j = bench(lib, ["--dump-outputs", os.path.join(out, name)])
+    for name, tree in TREES.items():
+        j = bench(tree, ["--dump-outputs", os.path.join(out, name)])
         full[name] = j
         with open(os.path.join(out, f"bench_{name}.json"), "w") as f:
             json.dump(j, f)

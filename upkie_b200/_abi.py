@@ -12,7 +12,7 @@ import ctypes as C
 
 import numpy as np
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 LAG_REPLY1, LAG_REPLY2, LAG_IMU, LAG_OBS_REPLY, LAG_OBS_IMU, LAG_OBS_BASE, LAG_OBS_CONTACT, LAG_DIM = 0, 18, 36, 49, 67, 80, 90, 91  # spine-mode lag record (include/upkie_b200.h)
 
 NJ = 6
@@ -144,6 +144,8 @@ class UpkieSimConfig(C.Structure):
         ("body_contact_erp", C.c_double),
         ("body_friction", C.c_double),
         ("solver_residual_threshold", C.c_double),
+        ("max_episode_steps", C.c_int32),
+        ("reserved_max_episode_steps", C.c_int32),
     ]
 
 
@@ -294,6 +296,8 @@ def default_sim_config(frequency: float = 200.0) -> UpkieSimConfig:
     c.body_contact_erp = 0.2  # btContactSolverInfo::m_erp2
     c.body_friction = 0.5  # URDF importer default lateral friction of a link without <contact>
     c.solver_residual_threshold = 1e-7  # PyBullet's solverResidualThreshold default (Bullet's m_leastSquaresResidualThreshold)
+    c.max_episode_steps = 0  # no time limit (include/upkie_b200.h: max_episode_steps)
+    c.reserved_max_episode_steps = 0
     return c
 
 
@@ -308,6 +312,20 @@ class UpkiePush(C.Structure):
         ("peer_obs", C.c_void_p * 8),
         ("peer_terminated", C.c_void_p * 8),
         ("n_peers", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class UpkieStepOutputs(C.Structure):
+    """``UpkieStepOutputs`` of include/upkie_b200.h: the output buffers of ``upkie_b200_step`` / ``_step_host``."""
+
+    _fields_ = [
+        ("obs", C.c_void_p),
+        ("reward", C.c_void_p),
+        ("terminated", C.c_void_p),
+        ("truncated", C.c_void_p),
+        ("final_obs", C.c_void_p),
+        ("compact", C.c_int32),
         ("reserved", C.c_int32),
     ]
 

@@ -48,6 +48,8 @@ SYMBOLS = {
     "upkie_b200_step_servos_host": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_step_gyropod_host": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp]),
     "upkie_b200_step_servos_host_compact": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_step": (C.c_int, [_vp, C.c_int, _vp, C.POINTER(_abi.UpkieStepOutputs), _vp]),
+    "upkie_b200_step_host": (C.c_int, [_vp, C.c_int, _vp, C.POINTER(_abi.UpkieStepOutputs)]),
     "upkie_b200_spine_obs": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_reset_obs": (C.c_int, [_vp, C.c_int, _vp, _vp]),
     "upkie_b200_get_state": (C.c_int, [_vp, _vp, _vp]),
@@ -58,6 +60,8 @@ SYMBOLS = {
     "upkie_b200_error_flags": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_get_counters": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_set_counters": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    "upkie_b200_get_elapsed": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_elapsed": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_set_external_forces": (C.c_int, [_vp, _vp, C.c_uint32, _vp]),
     "upkie_b200_default_wheel_balancer_config": (C.c_int, [_vp]),
     "upkie_b200_wheel_balancer_create": (C.c_int, [_vp, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),

@@ -62,6 +62,8 @@ inline void default_sim_config(UpkieSimConfig* c) {
   c->body_contact_erp = 0.2;  // btContactSolverInfo::m_erp2
   c->body_friction = 0.5;     // URDF importer default lateral friction of a link without <contact>
   c->solver_residual_threshold = 1e-7;  // PyBullet: getSolverInfo().m_leastSquaresResidualThreshold = 1e-7
+  c->max_episode_steps = 0;  // no time limit (the reference leaves it to a TimeLimit wrapper, upkie_env.py:232)
+  c->reserved_max_episode_steps = 0;
 }
 
 inline void default_mpc_config(UpkieMpcConfig* c) {
@@ -243,6 +245,13 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
     P.init_angvel[k] = float(c.init_angular_velocity[k]);
     P.init_linvel[k] = float(c.init_linear_velocity[k]);
   }
+  if (c.max_episode_steps < 0) {
+    err = "config: max_episode_steps must be >= 0 (0 = no time limit)";
+    return UPKIE_B200_EINVAL;
+  }
+  P.max_episode_steps = c.max_episode_steps;
+  P.elapsed = nullptr;
+  P.final_obs = nullptr;
   return 0;
 }
 

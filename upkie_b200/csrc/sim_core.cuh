@@ -115,6 +115,12 @@ struct SimParams {
   // substep to (upkie_b200_get_body_contacts); null in the host build and when the handle has no body contacts
   float* body_rec;
   int body_rec_stride;
+  // episode time limit (config.max_episode_steps, 0 = none): elapsed[n] counts each env's agent steps since its last
+  // reset (the handle's buffer; null in the host build), final_obs receives the rows of the same-step auto-resets'
+  // terminal observations (set per launch, null = not requested)
+  int max_episode_steps;
+  uint32_t* elapsed;
+  float* final_obs;
 };
 
 // per-robot state in registers

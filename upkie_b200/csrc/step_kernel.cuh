@@ -41,6 +41,39 @@ __device__ __forceinline__ void mc_store_u32(uint32_t* addr, uint32_t v) {
   asm volatile("multimem.st.relaxed.sys.global.b32 [%0], %1;" ::"l"(addr), "r"(v) : "memory");
 }
 
+// The observation row env `i` would return if it did not reset in this step, stored at its row of P.final_obs before
+// the same-step auto-reset overwrites the state. Same layout as the step's own rows: servos [6][5] or compact [6][3]
+// (spine mode: the rows the spine assembled), gyropod o6, pendulum [4]. Per-thread stores: only resetting lanes write.
+template <int MODE, bool SPINE>
+__device__ __forceinline__ void store_final_obs(const SimParams& P, const RobotState& S, const SpineLag& L,
+                                                const float* o6, const NoiseCtx* nz, bool compact, int i) {
+  if (MODE == MODE_SERVOS) {
+    float tq[6];
+    measured_torques(P, S, nz, tq);
+    const int dim = compact ? 18 : UPKIE_OBS_DIM;
+    float* o = P.final_obs + size_t(i) * dim;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+      const float q = SPINE ? L.obs_rep[3 * j] : S.q[j];
+      const float qd = SPINE ? L.obs_rep[3 * j + 1] : S.qd[j];
+      const float t = SPINE ? L.obs_rep[3 * j + 2] : tq[j];
+      if (compact) {
+        o[3 * j] = q; o[3 * j + 1] = qd; o[3 * j + 2] = t;
+      } else {
+        o[5 * j] = q; o[5 * j + 1] = qd; o[5 * j + 2] = t;
+        o[5 * j + 3] = SPINE ? 20.0f : 42.0f;  // BulletInterface.cpp:70 / pybullet_backend.py:471
+        o[5 * j + 4] = 18.0f;                  // pybullet_backend.py:472
+      }
+    }
+  } else if (MODE == MODE_GYROPOD) {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) P.final_obs[size_t(i) * 6 + k] = o6[k];
+  } else {
+    float* o = P.final_obs + size_t(i) * 4;
+    o[0] = o6[1]; o[1] = o6[0]; o[2] = o6[4]; o[3] = o6[3];  // upkie_pendulum.py:17
+  }
+}
+
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE=1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), and it is reused to transpose the observation rows on the way out.
@@ -205,8 +238,23 @@ __device__ __forceinline__ void step_env(
   }
   if (resetting) term = false;
 
+  // Episode time limit (config.max_episode_steps): a uniform branch, no counter traffic without a limit. Every step
+  // adds 1 to the env's count elapsed[i]; the step of a next-step auto-reset is not counted: a lane that will reset
+  // at the next step leaves 0xffffffff, which that step's +1 turns into 0. The in-kernel transports (TILE=2) do not
+  // carry `truncated`: the host rejects a limit there. Same-step mode needs the flag before its reset; the other
+  // modes count in a block of their own after the stores of the tick (below).
+  const bool timed = TILE != 2 && P.max_episode_steps > 0;
+  bool trunc = false;
+  uint32_t elapsed = 0;
+  if (AUTORESET == AUTORESET_SAME_STEP && timed) {
+    elapsed = P.elapsed[i] + 1u;
+    trunc = elapsed >= uint32_t(P.max_episode_steps);
+  }
+
   if (AUTORESET == AUTORESET_SAME_STEP) {
-    if (term) {
+    if (term || trunc) {
+      if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, NOISE ? &nz : nullptr, TILE && compact, i);
+      elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
       float init[UPKIE_INIT_DIM];
@@ -331,9 +379,18 @@ __device__ __forceinline__ void step_env(
   if (!live) return;
   if (reward) reward[i] = 0.0f;  // upkie_env.py:230
   if (TILE != 2) terminated[i] = term ? 1 : 0;
-  if (truncated) truncated[i] = 0;
+  if (truncated) truncated[i] = trunc ? 1 : 0;
+  if (AUTORESET == AUTORESET_SAME_STEP && timed) P.elapsed[i] = elapsed;
   if (e) err[i] |= e;
   if (AUTORESET == AUTORESET_NEXT_STEP) done_prev[i] = term ? 1 : 0;
+  if (AUTORESET != AUTORESET_SAME_STEP && timed) {
+    uint32_t el = P.elapsed[i] + 1u;
+    const bool tr = el >= uint32_t(P.max_episode_steps);
+    if (AUTORESET == AUTORESET_NEXT_STEP && (term || tr)) el = 0xffffffffu;  // reset pending: the next step is not counted
+    P.elapsed[i] = el;
+    if (truncated) truncated[i] = tr ? 1 : 0;
+    if (AUTORESET == AUTORESET_NEXT_STEP && tr) done_prev[i] = 1;
+  }
 }
 
 // Deferred rollout transport: send the warp's 32 compact rows (and `terminated` bytes) of an EARLIER step, read from

@@ -58,6 +58,7 @@ struct Handle {
   uint8_t* done_prev = nullptr;  // [n]
   uint32_t* episode = nullptr;   // [n]
   uint32_t* tick = nullptr;      // [n] env ticks since create: counter of the noise generator
+  uint32_t* elapsed = nullptr;   // [n] agent steps since the env's last reset (config.max_episode_steps)
   float* ext = nullptr;          // [7 * 3][n_pad] external forces, null = none
   float* lag = nullptr;          // [UPKIE_LAG_DIM][n_pad] spine-mode lag records (config.spine_mode), else null
   float* body_rec = nullptr;     // [UPKIE_BODY_REC_DIM][n_pad] body-ground contacts of the last substep (config.body_contacts)
@@ -76,6 +77,7 @@ struct Handle {
   uint8_t *h_term = nullptr, *h_trunc = nullptr;
   float *d_act = nullptr, *d_obs = nullptr, *d_rew = nullptr;
   uint8_t *d_term = nullptr, *d_trunc = nullptr;
+  float* h_fin = nullptr;        // pinned copy of a pageable final_obs buffer (allocated on first use)
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -131,6 +133,7 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
   store_state(state, n_pad, i, S);
   err[i] = 0;
   done_prev[i] = 0;
+  P.elapsed[i] = 0;
 }
 
 __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ state,
@@ -237,13 +240,25 @@ int pick_block(const Handle* h, int cnt) {
 
 // envs [i0, i0 + cnt): all buffers are indexed by the env index of the handle. `tile` selects the
 // shared-memory-tile instantiation (host buffers), see kernel_common.cuh.
+// `final_obs`: rows of the same-step auto-resets' terminal observations (null = not requested): it travels in a copy of
+// the parameter block made for this launch only.
 int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float* obs, float* reward, uint8_t* term,
                uint8_t* trunc, cudaStream_t s, bool tile = false, bool persistent = true, bool compact = false,
-               bool multicast = false, const PeerPtrs* peers = nullptr) {
+               bool multicast = false, const PeerPtrs* peers = nullptr, float* final_obs = nullptr) {
+  if (multicast && h->P.max_episode_steps > 0)
+    return fail(UPKIE_B200_EINVAL, "max_episode_steps has no in-kernel rollout transport: it does not carry truncated "
+                                   "(use upkie_b200_step with compact rows)");
   StepArgs a;
   std::memset(&a.peers, 0, sizeof(a.peers));
   if (peers) a.peers = *peers;
-  a.P = &h->P;
+  SimParams P_launch;
+  if (final_obs && h->autoreset == AUTORESET_SAME_STEP) {
+    P_launch = h->P;
+    P_launch.final_obs = final_obs;
+    a.P = &P_launch;
+  } else {
+    a.P = &h->P;
+  }
   a.mode = mode;
   a.autoreset = h->autoreset;
   a.noise = h->P.joint_limits ? 2 : ((h->P.any_ctrl_noise || h->P.any_meas_noise || h->ext) ? 1 : 0);  // "extras" kernels
@@ -339,8 +354,11 @@ T* mapped(T* p) {
 //   1                    one persistent TILE=1 launch reading actions from and writing observations to host memory.
 //   0                    H2D copy -> TILE=0 kernel -> D2H copies per chunk on rotating streams.
 // `compact` (servos): observation rows [6][3] = position, velocity, torque (TILE=1 kernels).
+// `final_obs` (same-step auto-reset): its rows are sparse, so in every pipeline the kernel stores them straight into
+// host memory through the mapped alias; a pageable buffer goes through a pinned copy of the caller's rows, so that
+// the rows of the envs that do not reset keep their values.
 int step_host(Handle* h, int mode, const float* action, float* obs, float* reward, uint8_t* term, uint8_t* trunc,
-              bool compact = false) {
+              bool compact = false, float* final_obs = nullptr) {
   if (!action || !obs || !term) return fail(UPKIE_B200_EINVAL, "step_host: null buffer");
   int rc = ensure_staging(h);
   if (rc) return rc;
@@ -357,6 +375,13 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
   float* dst_rew = reward ? (pin_out ? reward : h->h_rew) : nullptr;
   uint8_t* dst_term = pin_out ? term : h->h_term;
   uint8_t* dst_trunc = trunc ? (pin_out ? trunc : h->h_trunc) : nullptr;
+  if (h->autoreset != AUTORESET_SAME_STEP) final_obs = nullptr;
+  const bool fin_staged = final_obs && !mapped(final_obs);
+  if (fin_staged) {
+    if (!h->h_fin) CUDA_TRY(cudaMallocHost(&h->h_fin, n * UPKIE_OBS_DIM * sizeof(float)));
+    std::memcpy(h->h_fin, final_obs, n * obs_dim * sizeof(float));
+  }
+  float* fin = final_obs ? mapped(fin_staged ? h->h_fin : final_obs) : nullptr;
 
   // Order the private (non-blocking) streams after whatever the caller enqueued on the default stream - reset(),
   // set_state(), set_counters() through PyTorch's default current stream: without this a step_*_host() right after
@@ -401,14 +426,14 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
       cudaStream_t sk = h->host_streams[1 + (c % h->host_kernel_streams)];
       CUDA_TRY(cudaStreamWaitEvent(sk, h->host_events[c], 0));
       rc = step_range(h, mode, start[c], chunk_count(c), h->d_act, mapped(dst_obs), mapped(dst_rew), mapped(dst_term),
-                      mapped(dst_trunc), sk, /*tile=*/true, /*persistent=*/false, compact);
+                      mapped(dst_trunc), sk, /*tile=*/true, /*persistent=*/false, compact, false, nullptr, fin);
       if (rc) return rc;
     }
     for (int k = 0; k < h->host_kernel_streams; ++k) CUDA_TRY(cudaStreamSynchronize(h->host_streams[1 + k]));
   } else if (pipeline == 1) {
     cudaStream_t s = h->host_streams[0];
     rc = step_range(h, mode, 0, h->n, mapped(src_act), mapped(dst_obs), mapped(dst_rew), mapped(dst_term),
-                    mapped(dst_trunc), s, /*tile=*/true, /*persistent=*/true, compact);
+                    mapped(dst_trunc), s, /*tile=*/true, /*persistent=*/true, compact, false, nullptr, fin);
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(s));
   } else {
@@ -420,7 +445,7 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
                                size_t(cnt) * act_dim * sizeof(float), cudaMemcpyHostToDevice, s));
       // compact rows exist in the TILE=1 kernels only; device staging buffers either way
       rc = step_range(h, mode, i0, cnt, h->d_act, h->d_obs, h->d_rew, h->d_term, h->d_trunc, s, /*tile=*/compact,
-                      /*persistent=*/false, compact);
+                      /*persistent=*/false, compact, false, nullptr, fin);
       if (rc) return rc;
       CUDA_TRY(cudaMemcpyAsync(dst_obs + size_t(i0) * obs_dim, h->d_obs + size_t(i0) * obs_dim,
                                size_t(cnt) * obs_dim * sizeof(float), cudaMemcpyDeviceToHost, s));
@@ -436,6 +461,7 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
     std::memcpy(term, h->h_term, n);
     if (trunc) std::memcpy(trunc, h->h_trunc, n);
   }
+  if (fin_staged) std::memcpy(final_obs, h->h_fin, n * obs_dim * sizeof(float));
   return UPKIE_B200_OK;
 }
 
@@ -531,6 +557,9 @@ int upkie_b200_create(const UpkieModel* model, const UpkieSimConfig* config, int
   }
   if (e == cudaSuccess) e = cudaMalloc(&h->tick, size_t(n_envs) * sizeof(uint32_t));
   if (e == cudaSuccess) e = cudaMemset(h->tick, 0, size_t(n_envs) * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&h->elapsed, size_t(n_envs) * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMemset(h->elapsed, 0, size_t(n_envs) * sizeof(uint32_t));
+  h->P.elapsed = h->elapsed;
   if (e == cudaSuccess) {
     k_init_state<<<(h->n_pad + 127) / 128, 128>>>(h->P, h->n, h->n_pad, h->state);
     e = cudaGetLastError();
@@ -550,8 +579,8 @@ void upkie_b200_destroy(void* handle) {
   if (!h) return;
   cudaSetDevice(h->device);
   cudaFree(h->state); cudaFree(h->eps); cudaFree(h->mu); cudaFree(h->err); cudaFree(h->done_prev); cudaFree(h->episode);
-  cudaFree(h->tick); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
-  cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
+  cudaFree(h->tick); cudaFree(h->elapsed); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
+  cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
     if (h->host_streams[k]) cudaStreamDestroy(h->host_streams[k]);
@@ -582,6 +611,15 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   }
   P.body_rec = P.body_contacts ? h->body_rec : nullptr;
   P.body_rec_stride = h->n_pad;
+  P.elapsed = h->elapsed;
+  if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
+    // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
+    // were kept against another limit; steps enqueued before the call finish first.
+    CUDA_TRY(cudaSetDevice(h->device));
+    CUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaMemset(h->elapsed, 0, size_t(h->n) * sizeof(uint32_t)));
+    CUDA_TRY(cudaDeviceSynchronize());
+  }
   // kernels read the parameter block by value at launch: steps already enqueued keep the old one
   h->P = P;
   return UPKIE_B200_OK;
@@ -764,6 +802,38 @@ int upkie_b200_step_servos_host_compact(void* handle, const float* action, float
   return step_host(h, MODE_SERVOS, action, obs, nullptr, terminated, nullptr, /*compact=*/true);
 }
 
+namespace {
+int step_mode_of(int act_dim) {
+  return act_dim == UPKIE_ACT_DIM ? MODE_SERVOS : (act_dim == 2 ? MODE_GYROPOD : (act_dim == 1 ? MODE_PENDULUM : -1));
+}
+}  // namespace
+
+int upkie_b200_step(void* handle, int act_dim, const float* action, const UpkieStepOutputs* out, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  const int mode = step_mode_of(act_dim);
+  if (mode < 0) return fail(UPKIE_B200_EINVAL, "step: act_dim must be 36 (servos), 2 (gyropod) or 1 (pendulum)");
+  if (!out || !action || !out->obs || !out->terminated) return fail(UPKIE_B200_EINVAL, "step: null buffer");
+  const bool compact = out->compact != 0;
+  if (compact && mode != MODE_SERVOS) return fail(UPKIE_B200_EINVAL, "step: compact rows exist for servos only");
+  CUDA_TRY(cudaSetDevice(h->device));
+  // compact rows: the TILE=1 kernels on device buffers, as upkie_b200_step_servos_compact
+  return step_range(h, mode, 0, h->n, action, out->obs, out->reward, out->terminated, out->truncated,
+                    static_cast<cudaStream_t>(stream), /*tile=*/compact, /*persistent=*/false, compact, false, nullptr,
+                    out->final_obs);
+}
+
+int upkie_b200_step_host(void* handle, int act_dim, const float* action, const UpkieStepOutputs* out) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  const int mode = step_mode_of(act_dim);
+  if (mode < 0) return fail(UPKIE_B200_EINVAL, "step_host: act_dim must be 36 (servos), 2 (gyropod) or 1 (pendulum)");
+  if (!out) return fail(UPKIE_B200_EINVAL, "step_host: null outputs");
+  const bool compact = out->compact != 0;
+  if (compact && mode != MODE_SERVOS) return fail(UPKIE_B200_EINVAL, "step_host: compact rows exist for servos only");
+  return step_host(h, mode, action, out->obs, out->reward, out->terminated, out->truncated, compact, out->final_obs);
+}
+
 int upkie_b200_step_gyropod_host(void* handle, const float* action, int act_dim, float* obs, float* reward,
                                  uint8_t* terminated, uint8_t* truncated) {
   Handle* h = as_handle(handle);
@@ -917,6 +987,24 @@ int upkie_b200_set_counters(void* handle, const uint32_t* episode, const uint32_
   if (tick) CUDA_TRY(cudaMemcpyAsync(h->tick, tick, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   if (pending_reset) CUDA_TRY(cudaMemcpyAsync(h->done_prev, pending_reset, n, cudaMemcpyDeviceToDevice, s));
   if (error_flags) CUDA_TRY(cudaMemcpyAsync(h->err, error_flags, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_elapsed(void* handle, uint32_t* elapsed, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !elapsed) return fail(UPKIE_B200_EINVAL, "get_elapsed: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaMemcpyAsync(elapsed, h->elapsed, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+                           static_cast<cudaStream_t>(stream)));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_elapsed(void* handle, const uint32_t* elapsed, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !elapsed) return fail(UPKIE_B200_EINVAL, "set_elapsed: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaMemcpyAsync(h->elapsed, elapsed, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+                           static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 

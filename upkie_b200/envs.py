@@ -13,6 +13,10 @@ with the reference's reset semantics (seeded NumPy sampling of the initial
 state, ``upkie/envs/upkie_env.py:162-194``), ``reward == 0.0`` and
 ``truncated == False`` (``upkie_env.py:230-232``), fall termination for the
 wheeled-inverted-pendulum wrappers (``upkie_gyropod.py:333-352``).
+
+``max_episode_steps=T`` adds the time limit of Gymnasium's ``TimeLimit`` wrapper
+per env inside the step kernel (``truncated`` once an env has run T steps since
+its last reset), which the fused auto-reset honours.
 """
 
 from typing import Any, Dict, Optional, Tuple, Union
@@ -211,6 +215,14 @@ def spine_row_to_dict(r: np.ndarray) -> dict:
     }
 
 
+def _check_max_episode_steps(value) -> int:
+    if value is None:
+        return 0
+    if int(value) != value or value < 0 or value > 0x7FFFFFFF:
+        raise UpkieException(f"max_episode_steps must be an integer in [0, 2**31), got {value!r} (0 = no time limit)")
+    return int(value)
+
+
 def make_config(
     frequency: float = 200.0,
     nb_substeps: Optional[int] = None,
@@ -227,11 +239,14 @@ def make_config(
     joint_limits: Union[bool, int] = True,
     spine_mode: bool = False,
     body_contacts: bool = False,
+    max_episode_steps: int = 0,
 ) -> _abi.UpkieSimConfig:
     """Split of the keyword arguments the reference's factories forward to the
-    backend, the servo env and the wrappers (``upkie/envs/entry_points.py:41-61,99-109``)."""
+    backend, the servo env and the wrappers (``upkie/envs/entry_points.py:41-61,99-109``).
+    ``max_episode_steps``: per-env time limit in agent steps, 0 = none (include/upkie_b200.h)."""
     if frequency is None:
         raise UpkieException("This environment needs a loop frequency")
+    max_episode_steps = _check_max_episode_steps(max_episode_steps)
     cfg = _abi.default_sim_config(frequency)
     if nb_substeps is not None:
         cfg.nb_substeps = int(nb_substeps)
@@ -260,13 +275,26 @@ def make_config(
     cfg.leg_gain_scale = leg_gain_scale
     cfg.max_ground_velocity = max_ground_velocity
     cfg.max_yaw_velocity = max_yaw_velocity
+    cfg.max_episode_steps = max_episode_steps
     if init_state is not None:
         init_state.apply_to_config(cfg)
     return cfg
 
 
 class B200VectorEnv(VectorEnv):
-    """N Upkie environments stepped by one kernel launch per ``step()``."""
+    """N Upkie environments stepped by one kernel launch per ``step()``.
+
+    ``max_episode_steps=T`` (0 = none) is Gymnasium's ``TimeLimit`` per env, kept by the step kernel: ``truncated[i]``
+    is 1 once env ``i`` has run T steps since its last reset, independently of ``terminated``. The auto-reset fires on
+    ``terminated | truncated``; with ``autoreset_mode="disabled"`` an env stays truncated until it is reset.
+
+    With ``autoreset_mode="same_step"``, a step in which some env reset adds ``info["final_obs"]``, the observation
+    each resetting env reached before its reset, and ``info["_final_obs"]``, the bool mask of those envs
+    (``terminated | truncated``). Unlike ``SyncVectorEnv``'s per-env object array, ``final_obs`` is dense batched
+    storage with the observation's structure (servo dictionary of arrays, array, or CUDA tensor from
+    ``step_tensors``): rows outside the mask hold stale values. ``copy=True`` copies it as it copies the
+    observation. ``info["final_info"]`` (the terminal step's spine observation) is not provided.
+    """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
 
@@ -298,7 +326,9 @@ class B200VectorEnv(VectorEnv):
         copy: bool = True,
         spine_mode: bool = False,
         body_contacts: bool = False,
+        max_episode_steps: int = 0,
     ):
+        max_episode_steps = _check_max_episode_steps(max_episode_steps)
         if env_type not in ENV_TYPES:
             raise UpkieException(f"env_type must be one of {ENV_TYPES}")
         if autoreset_mode not in _AUTORESET:
@@ -323,8 +353,12 @@ class B200VectorEnv(VectorEnv):
             config = make_config(
                 frequency, nb_substeps, torque_control_kp, torque_control_kd, joint_properties, max_gain_scale,
                 fall_pitch, leg_gain_scale, max_ground_velocity, max_yaw_velocity, self.init_state, noise_seed,
-                joint_limits, spine_mode, body_contacts,
+                joint_limits, spine_mode, body_contacts, max_episode_steps,
             )
+        elif max_episode_steps:
+            # an explicit limit overrides the one of the given configuration (a copy: the caller's struct is untouched)
+            config = _abi.UpkieSimConfig.from_buffer_copy(config)
+            config.max_episode_steps = max_episode_steps
         self.config = config
         if self.config.spine_mode and env_type != "servos":
             raise UpkieException("spine_mode is available for env_type='servos' (the wrappers of a spine read observer "
@@ -510,31 +544,70 @@ class B200VectorEnv(VectorEnv):
                 if isinstance(action, dict)
                 else np.ascontiguousarray(np.asarray(action, dtype=np.float32).reshape(n, 6, 6))
             )
-            obs18, term = self.sim.step_servos_host_compact(a)
             hb = self.sim._host_buffers()
+            fin = None
+            if self._host_general_step():
+                obs18, term, trunc, fin = self.sim.step_host(a, 36, compact=True, final_obs=self._same_step())
+            else:
+                obs18, term, trunc = *self.sim.step_servos_host_compact(a), hb["trunc"]
             info = {"spine_observation": SpineObservations(self.sim)}
             if self.copy:
                 obs18 = obs18.copy()
+                self._add_final_obs(info, term, trunc, fin, lambda f: self._servo_obs_dict(f.copy(), cache=False))
                 return (self._servo_obs_dict(obs18, cache=False), hb["rew"].copy(), term.view(np.bool_).copy(),
-                        hb["trunc"].view(np.bool_).copy(), info)
-            return self._servo_obs_dict(obs18), hb["rew"], term.view(np.bool_), hb["trunc"].view(np.bool_), info
+                        trunc.view(np.bool_).copy(), info)
+            self._add_final_obs(info, term, trunc, fin, lambda f: self._servo_obs_dict(f, cache=False))
+            return self._servo_obs_dict(obs18), hb["rew"], term.view(np.bool_), trunc.view(np.bool_), info
         else:
             d = 2 if self.env_type == "gyropod" else 1
             a = np.ascontiguousarray(np.asarray(action, dtype=np.float32).reshape(n, d))
-            obs, rew, term, trunc = self.sim.step_gyropod_host(a)
+            fin = None
+            if self._host_general_step():
+                obs, term, trunc, fin = self.sim.step_host(a, d, final_obs=self._same_step())
+                rew = self.sim._host_buffers()["rew"]
+            else:
+                obs, rew, term, trunc = self.sim.step_gyropod_host(a)
         info = {"spine_observation": SpineObservations(self.sim)}
         if self.copy:
+            self._add_final_obs(info, term, trunc, fin, np.copy)
             return obs.copy(), rew.copy(), term.view(np.bool_).copy(), trunc.view(np.bool_).copy(), info
         # views of the handle's pinned output buffers: valid until the next step()
+        self._add_final_obs(info, term, trunc, fin, lambda f: f)
         return self._format_obs(obs), rew, term.view(np.bool_), trunc.view(np.bool_), info
+
+    def _same_step(self) -> bool:
+        return self.autoreset_mode == "same_step"
+
+    def _host_general_step(self) -> bool:
+        """Host path through ``upkie_b200_step_host`` (``truncated`` from the kernel, final observations) when a time
+        limit or the same-step auto-reset needs it; otherwise the calls that leave ``truncated`` on the host."""
+        return self.config.max_episode_steps > 0 or self._same_step()
+
+    @staticmethod
+    def _add_final_obs(info: dict, term, trunc, fin, fmt) -> None:
+        """``info["final_obs"]`` / ``info["_final_obs"]`` when some env reset in this step (same-step mode)."""
+        if fin is None:
+            return
+        if isinstance(term, torch.Tensor):
+            mask = (term | trunc).bool()
+            if not bool(mask.any()):
+                return
+        else:
+            mask = (term | trunc).view(np.bool_)
+            if not mask.any():
+                return
+        info["final_obs"] = fmt(fin)
+        info["_final_obs"] = mask
 
     def step_tensors(self, action: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor, dict]:
         """Zero-copy fast path: CUDA tensors in, CUDA tensors out
-        (``action[N, 6, 6]`` / ``[N, 2]`` / ``[N, 1]``)."""
+        (``action[N, 6, 6]`` / ``[N, 2]`` / ``[N, 1]``). In same-step mode ``info["final_obs"]`` is a CUDA tensor of
+        the observation's shape and ``info["_final_obs"]`` a CUDA bool tensor."""
+        fin = self._device_final_obs() if self._same_step() else None
         if self.env_type == "servos":
-            obs, rew, term, trunc = self.sim.step_servos(action)
+            obs, rew, term, trunc = self.sim.step_servos(action, final_obs=fin)
         elif self.env_type == "gyropod":
-            obs, rew, term, trunc = self.sim.step_gyropod(action)
+            obs, rew, term, trunc = self.sim.step_gyropod(action, final_obs=fin)
         elif self.env_type == "base_velocity":
             # UpkieBaseVelocity.step (upkie_base_velocity.py:164-202): the MPC turns the commanded linear
             # velocity into a ground velocity from the LAST spine observation, the gyropod env is stepped,
@@ -546,5 +619,16 @@ class B200VectorEnv(VectorEnv):
                 self.sim.spine_obs,
             )
         else:
-            obs, rew, term, trunc = self.sim.step_pendulum(action)
-        return obs, rew, term, trunc, {"spine_observation": SpineObservations(self.sim)}
+            obs, rew, term, trunc = self.sim.step_pendulum(action, final_obs=fin)
+        info = {"spine_observation": SpineObservations(self.sim)}
+        # same-step mode: one host synchronisation per step decides whether some env reset
+        self._add_final_obs(info, term, trunc, fin, lambda f: f)
+        return obs, rew, term, trunc, info
+
+    def _device_final_obs(self) -> torch.Tensor:
+        """Device final-observation rows of the same-step auto-reset, in the observation's layout (reused)."""
+        fin = getattr(self, "_final_obs_tensor", None)
+        if fin is None:
+            shape = {"servos": (self.num_envs, 6, 5), "gyropod": (self.num_envs, 6), "pendulum": (self.num_envs, 4)}
+            fin = self._final_obs_tensor = torch.zeros(shape[self.env_type], dtype=torch.float32, device=self.sim.device)
+        return fin

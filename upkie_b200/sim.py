@@ -25,6 +25,13 @@ def _ptr(t: Optional[torch.Tensor]):
     return C.c_void_p(t.data_ptr()) if t is not None else None
 
 
+def _addr(x) -> Optional[int]:
+    """Address of a tensor or ndarray for an ``UpkieStepOutputs`` field (None stays NULL)."""
+    if x is None:
+        return None
+    return x.data_ptr() if isinstance(x, torch.Tensor) else x.ctypes.data
+
+
 class UpkieSim:
     """N independent robots on one CUDA device.
 
@@ -155,10 +162,26 @@ class UpkieSim:
             self._check_tensor(truncated, (self.n,), torch.uint8, "truncated")
         return obs, reward, terminated, truncated
 
+    def _step(self, act_dim: int, action, obs, reward, terminated, truncated, final_obs, compact: bool = False):
+        """``upkie_b200_step``: the general device-buffer step (``truncated`` with compact rows, ``final_obs``)."""
+        out = _abi.UpkieStepOutputs(_addr(obs), _addr(reward), _addr(terminated), _addr(truncated), _addr(final_obs),
+                                    1 if compact else 0, 0)
+        check(lib().upkie_b200_step(self._h, int(act_dim), _ptr(action), C.byref(out), self._stream()))
+
+    def _check_final_obs(self, final_obs: Optional[torch.Tensor], shape):
+        if final_obs is not None:
+            self._check_tensor(final_obs, shape, name="final_obs")
+
     def step_servos(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, reward=None, terminated=None,
-                    truncated=None):
+                    truncated=None, final_obs: Optional[torch.Tensor] = None):
+        """``final_obs[N, 6, 5]`` (same-step auto-reset): the envs that reset in this step first store there the
+        observation they reached; the other rows are left untouched (mask with ``terminated | truncated``)."""
         self._check_tensor(action, (self.n, 6, 6), name="action")
         obs, reward, terminated, truncated = self._outputs(obs, self.obs_servos, reward, terminated, truncated)
+        if final_obs is not None:
+            self._check_final_obs(final_obs, (self.n, 6, 5))
+            self._step(36, action, obs, reward, terminated, truncated, final_obs)
+            return obs, reward, terminated, truncated
         check(
             lib().upkie_b200_step_servos(
                 self._h, _ptr(action), _ptr(obs), _ptr(reward), _ptr(terminated), _ptr(truncated), self._stream(),
@@ -182,6 +205,26 @@ class UpkieSim:
             self._check_tensor(terminated, (self.n,), torch.uint8, "terminated")
         check(lib().upkie_b200_step_servos_compact(self._h, _ptr(action), _ptr(obs), _ptr(terminated), self._stream()))
         return obs, terminated
+
+    def step_servos_compact_truncated(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, terminated=None,
+                                      truncated=None, final_obs: Optional[torch.Tensor] = None):
+        """``step_servos_compact`` that also returns ``truncated`` (the episode time limit, ``max_episode_steps``)
+        and, in same-step auto-reset mode, fills the compact rows ``final_obs[N, 6, 3]`` of the envs that reset.
+        Returns ``(obs, terminated, truncated)``."""
+        self._check_tensor(action, (self.n, 6, 6), name="action")
+        if obs is None:
+            if getattr(self, "obs_servos_compact", None) is None:
+                self.obs_servos_compact = torch.empty((self.n, 6, 3), dtype=torch.float32, device=self.device)
+            obs = self.obs_servos_compact
+        elif obs.numel() != self.n * 18 or obs.dtype != torch.float32 or not obs.is_contiguous() or obs.data_ptr() % 16:
+            raise UpkieRuntimeError("obs: expected contiguous 16-byte aligned float32 [N, 6, 3]")
+        terminated = self.terminated if terminated is None else terminated
+        truncated = self.truncated if truncated is None else truncated
+        for name, t in (("terminated", terminated), ("truncated", truncated)):
+            self._check_tensor(t, (self.n,), torch.uint8, name)
+        self._check_final_obs(final_obs, (self.n, 6, 3))
+        self._step(36, action, obs, None, terminated, truncated, final_obs, compact=True)
+        return obs, terminated, truncated
 
     def step_servos_multicast(self, action: torch.Tensor, obs_mc_ptr: int, terminated_mc_ptr: int) -> None:
         """Compact rows and ``terminated`` go to NVSwitch multicast addresses (``PeerRolloutBuffer.multicast_slot``): every GPU of the node receives them."""
@@ -213,9 +256,13 @@ class UpkieSim:
         check(lib().upkie_b200_push_rows(self._h, C.byref(push), self._stream()))
 
     def step_gyropod(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, reward=None, terminated=None,
-                     truncated=None):
+                     truncated=None, final_obs: Optional[torch.Tensor] = None):
         self._check_tensor(action, (self.n, 2), name="action")
         obs, reward, terminated, truncated = self._outputs(obs, self.obs_gyropod, reward, terminated, truncated)
+        if final_obs is not None:
+            self._check_final_obs(final_obs, (self.n, 6))
+            self._step(2, action, obs, reward, terminated, truncated, final_obs)
+            return obs, reward, terminated, truncated
         check(
             lib().upkie_b200_step_gyropod(
                 self._h, _ptr(action), 2, _ptr(obs), _ptr(reward), _ptr(terminated), _ptr(truncated), self._stream(),
@@ -224,9 +271,13 @@ class UpkieSim:
         return obs, reward, terminated, truncated
 
     def step_pendulum(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, reward=None, terminated=None,
-                      truncated=None):
+                      truncated=None, final_obs: Optional[torch.Tensor] = None):
         self._check_tensor(action, (self.n, 1), name="action")
         obs, reward, terminated, truncated = self._outputs(obs, self.obs_pendulum, reward, terminated, truncated)
+        if final_obs is not None:
+            self._check_final_obs(final_obs, (self.n, 4))
+            self._step(1, action, obs, reward, terminated, truncated, final_obs)
+            return obs, reward, terminated, truncated
         check(
             lib().upkie_b200_step_gyropod(
                 self._h, _ptr(action), 1, _ptr(obs), _ptr(reward), _ptr(terminated), _ptr(truncated), self._stream(),
@@ -254,10 +305,23 @@ class UpkieSim:
                 "rew": pinned((self.n,), torch.float32),
                 "term": pinned((self.n,), torch.uint8),
                 "trunc": pinned((self.n,), torch.uint8),
+                "trunc_dev": pinned((self.n,), torch.uint8),  # truncated as the kernel writes it (time limit set)
             }
             self._hb["rew"][:] = 0.0  # upkie_env.py:230
             self._hb["trunc"][:] = 0  # upkie_env.py:197
         return self._hb
+
+    def _limited(self) -> bool:
+        return self.config.max_episode_steps > 0
+
+    def _host_final_obs(self, dim: int) -> np.ndarray:
+        """Pinned final-observation rows of the same-step auto-reset (allocated on first use)."""
+        hb = self._host_buffers()
+        key = f"fin{dim}"
+        if key not in hb:
+            shape = {30: (self.n, 6, 5), 18: (self.n, 6, 3)}.get(dim, (self.n, dim))
+            hb[key] = torch.zeros(shape, dtype=torch.float32, pin_memory=True).numpy()
+        return hb[key]
 
     def host_action_buffer(self, act_dim: int = 36) -> np.ndarray:
         """Pinned ``[N, 6, 6]`` / ``[N, 2]`` / ``[N, 1]`` action array to fill in place."""
@@ -272,9 +336,12 @@ class UpkieSim:
             a = np.ascontiguousarray(action, dtype=np.float32)
         if a.size != self.n * 36:
             raise UpkieRuntimeError(f"action: expected {self.n * 36} float32 values, got {a.size}")
-        obs, rew, term, trunc = hb["obs30"], hb["rew"], hb["term"], hb["trunc"]
-        # reward and truncated are constants of the reference (upkie_env.py:197,230): not transported
-        check(lib().upkie_b200_step_servos_host(self._h, a.ctypes.data, obs.ctypes.data, None, term.ctypes.data, None))
+        obs, rew, term = hb["obs30"], hb["rew"], hb["term"]
+        # reward is a constant of the reference (upkie_env.py:230), and so is truncated without a time limit
+        # (upkie_env.py:197): not transported then
+        trunc = hb["trunc_dev"] if self._limited() else hb["trunc"]
+        check(lib().upkie_b200_step_servos_host(self._h, a.ctypes.data, obs.ctypes.data, None, term.ctypes.data,
+                                                trunc.ctypes.data if self._limited() else None))
         return obs, rew, term, trunc
 
     def step_servos_host_compact(self, action: np.ndarray):
@@ -298,11 +365,32 @@ class UpkieSim:
         if act_dim not in (1, 2) or a.size != self.n * act_dim:
             raise UpkieRuntimeError("action: expected shape [N, 1] (pendulum) or [N, 2] (gyropod)")
         obs = hb["obs6"] if act_dim == 2 else hb["obs4"]
-        rew, term, trunc = hb["rew"], hb["term"], hb["trunc"]
+        rew, term = hb["rew"], hb["term"]
+        trunc = hb["trunc_dev"] if self._limited() else hb["trunc"]
         check(
-            lib().upkie_b200_step_gyropod_host(self._h, a.ctypes.data, act_dim, obs.ctypes.data, None, term.ctypes.data, None)
+            lib().upkie_b200_step_gyropod_host(self._h, a.ctypes.data, act_dim, obs.ctypes.data, None, term.ctypes.data,
+                                               trunc.ctypes.data if self._limited() else None)
         )
         return obs, rew, term, trunc
+
+    def step_host(self, action: np.ndarray, act_dim: int, compact: bool = False, final_obs: bool = False):
+        """``upkie_b200_step_host``: host arrays, ``truncated`` written by the kernel on every path. ``act_dim`` 36
+        (servos, ``compact`` = rows ``[N, 6, 3]``), 2 (gyropod) or 1 (pendulum). ``final_obs=True`` (same-step
+        auto-reset): the envs that reset in this step also store the observation they reached into a pinned buffer
+        of the observation's layout; its other rows keep their values. Returns ``(obs, terminated, truncated,
+        final_obs or None)``: pinned arrays that the next ``*_host`` call overwrites."""
+        hb = self._host_buffers()
+        a = action
+        if a.dtype != np.float32 or not a.flags["C_CONTIGUOUS"]:
+            a = np.ascontiguousarray(action, dtype=np.float32)
+        if act_dim not in (36, 2, 1) or a.size != self.n * act_dim or (compact and act_dim != 36):
+            raise UpkieRuntimeError(f"action: expected {self.n} rows of {act_dim} float32 values (act_dim 36, 2 or 1)")
+        dim = {36: 18 if compact else 30, 2: 6, 1: 4}[act_dim]
+        obs, term, trunc = hb[f"obs{dim}"], hb["term"], hb["trunc_dev"]
+        fin = self._host_final_obs(dim) if final_obs else None
+        out = _abi.UpkieStepOutputs(_addr(obs), None, _addr(term), _addr(trunc), _addr(fin), 1 if compact else 0, 0)
+        check(lib().upkie_b200_step_host(self._h, int(act_dim), a.ctypes.data, C.byref(out)))
+        return obs, term, trunc, fin
 
     @property
     def launches(self) -> int:
@@ -356,7 +444,7 @@ class UpkieSim:
     # checkpoint / resume ------------------------------------------------------------------
     def state_dict(self) -> dict:
         """Everything a handle needs to continue bit for bit (``torch.save``-able): robot state, episode / tick
-        counters, pending auto-resets, error flags, randomisation, external forces, auto-reset keys. The model and
+        counters, time-limit counts, pending auto-resets, error flags, randomisation, external forces, auto-reset keys. The model and
         the configuration are construction arguments and are not included."""
         i32, u8 = torch.int32, torch.uint8
         episode = torch.empty(self.n, dtype=i32, device=self.device)
@@ -364,11 +452,14 @@ class UpkieSim:
         pending = torch.empty(self.n, dtype=u8, device=self.device)
         flags = torch.empty(self.n, dtype=i32, device=self.device)
         check(lib().upkie_b200_get_counters(self._h, _ptr(episode), _ptr(tick), _ptr(pending), _ptr(flags), self._stream()))
+        elapsed = torch.empty(self.n, dtype=i32, device=self.device)
+        check(lib().upkie_b200_get_elapsed(self._h, _ptr(elapsed), self._stream()))
         friction, eps = getattr(self, "_randomization", (None, None))
         force, local_mask = getattr(self, "_external", (None, 0))
         return {
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
+            "elapsed": elapsed,  # steps since each env's last reset (the time limit's counts)
             "friction": friction, "inertia_eps": eps, "external_force": force, "external_local_mask": local_mask,
             "autoreset": getattr(self, "_autoreset", (AUTORESET_DISABLED, 0, 0)),
         }
@@ -381,6 +472,10 @@ class UpkieSim:
         check(lib().upkie_b200_set_counters(
             self._h, _ptr(sd["episode"].to(dev)), _ptr(sd["tick"].to(dev)), _ptr(sd["pending_reset"].to(dev)),
             _ptr(sd["error_flags"].to(dev)), self._stream()))
+        # a checkpoint written before the time limit existed restores zero counts
+        elapsed = sd.get("elapsed")
+        elapsed = torch.zeros(self.n, dtype=torch.int32, device=dev) if elapsed is None else elapsed.to(dev).contiguous()
+        check(lib().upkie_b200_set_elapsed(self._h, _ptr(elapsed), self._stream()))
         torch.cuda.current_stream(dev).synchronize()
         self.set_randomization(None if sd["friction"] is None else sd["friction"].to(dev),
                                None if sd["inertia_eps"] is None else sd["inertia_eps"].to(dev))
