@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define UPKIE_B200_ABI_VERSION 7
+#define UPKIE_B200_ABI_VERSION 8
 
 #define UPKIE_NJ 6 /* actuated joints */
 #define UPKIE_NB 7 /* moving bodies: base lump + 2 x (upper leg, lower leg, wheel) */
@@ -311,6 +311,21 @@ typedef struct UpkieSimConfig {
 #define UPKIE_LAG_OBS_CONTACT 90
 #define UPKIE_LAG_DIM 91
 
+/* Per-env parameter table (upkie_b200_set_env_params / get_env_params, [N][UPKIE_EP_DIM] floats): one row per env
+ * that overrides, for that env, the UpkieSimConfig fields of the same meaning, wherever the kernels read them. What N
+ * reference envs built with different PyBulletBackend(torque_control_kp=..., torque_control_kd=...,
+ * joint_properties={joint: JointProperties(...)}) arguments and different spine ImuUncertainty hold. */
+#define UPKIE_EP_KP 0             /* torque_control_kp (pybullet_backend.py:65, used at :528) */
+#define UPKIE_EP_KD 1             /* torque_control_kd (pybullet_backend.py:64, used at :529) */
+#define UPKIE_EP_FRICTION 2       /* [6] JointProperties.friction (joint_properties.py:24-40, pybullet_backend.py:538-543) */
+#define UPKIE_EP_CTRL_NOISE 8     /* [6] JointProperties.torque_control_noise (pybullet_backend.py:545-552) */
+#define UPKIE_EP_MEAS_NOISE 14    /* [6] JointProperties.torque_measurement_noise (pybullet_backend.py:461-466) */
+#define UPKIE_EP_IMU_ACC_BIAS 20  /* [3] ImuUncertainty accelerometer_bias (ImuUncertainty.h:29-69) */
+#define UPKIE_EP_IMU_ACC_NOISE 23 /* ImuUncertainty accelerometer_noise */
+#define UPKIE_EP_IMU_GYRO_BIAS 24 /* [3] ImuUncertainty gyroscope_bias */
+#define UPKIE_EP_IMU_GYRO_NOISE 27 /* ImuUncertainty gyroscope_noise */
+#define UPKIE_EP_DIM 28
+
 /* MPCBalancer parameters (upkie/controllers/mpc_balancer.py:168-181) */
 typedef struct UpkieMpcConfig {
   double fall_pitch;              /* 1.0 */
@@ -391,6 +406,21 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config);
  * in same-step mode upkie_b200_step / upkie_b200_step_host can also return the
  * observation the resetting envs reached before their reset (final_obs). */
 int upkie_b200_set_autoreset(void* handle, int mode, uint64_t seed, uint64_t env_offset);
+
+/* Per-env actuator and IMU parameters (ABI 8): rows[N][UPKIE_EP_DIM] (device pointer, layout UPKIE_EP_*) replace,
+ * env by env, the config's torque_control_kp / kd, joint_friction, torque_control_noise, torque_measurement_noise and
+ * imu_* fields, wherever the kernels use them: the torque law of every substep (spine mode: kp and kd only, the C++
+ * spine has no joint friction or torque noise, BulletInterface.cpp:329-352), the torque measurement noise of the
+ * observations and the ImuUncertainty of upkie_b200_spine_obs. noise_seed still comes from the config; noise is drawn
+ * with the same keys as without a table, so an env draws the same numbers whatever its batch holds.
+ * Every value must be finite, gains, friction and noise standard deviations >= 0 (biases may be negative); otherwise
+ * UPKIE_B200_EINVAL and the previous table stays. NULL drops the table: every env runs the config's values again.
+ * upkie_b200_set_config keeps the table. Waits for the device (not a hot-path call); takes effect for launches
+ * enqueued after it. The in-kernel rollout transports (multicast, peers, push) reject a handle with a table. */
+int upkie_b200_set_env_params(void* handle, const float* rows, void* stream);
+/* The parameters in force, rows[N][UPKIE_EP_DIM] (device pointer): the table, or without one the config's values
+ * (as floats) in every row. */
+int upkie_b200_get_env_params(void* handle, float* rows, void* stream);
 
 /* Per-env domain randomisation; either pointer may be NULL (= nominal).
  * friction[N]: combined floor friction (extension, SURVEY 8d config 3).

@@ -12,7 +12,7 @@ import ctypes as C
 
 import numpy as np
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 LAG_REPLY1, LAG_REPLY2, LAG_IMU, LAG_OBS_REPLY, LAG_OBS_IMU, LAG_OBS_BASE, LAG_OBS_CONTACT, LAG_DIM = 0, 18, 36, 49, 67, 80, 90, 91  # spine-mode lag record (include/upkie_b200.h)
 
 NJ = 6
@@ -55,6 +55,10 @@ ST_PREV_IMU_VEL, ST_TORQUE, ST_LEG_TARGET, ST_YAW, ST_YAW_VEL, ST_CONTACT = 25, 
 ST_IMU_ACC = 41
 ST_CONTACT_IMPULSE = 44
 ST_FRICTION_IMPULSE = 46  # rolling / lateral friction impulses of the last substep, left wheel then right wheel
+# per-env parameter table (upkie_b200_set_env_params): row offsets, UPKIE_EP_* of include/upkie_b200.h
+EP_KP, EP_KD, EP_FRICTION, EP_CTRL_NOISE, EP_MEAS_NOISE = 0, 1, 2, 8, 14
+EP_IMU_ACC_BIAS, EP_IMU_ACC_NOISE, EP_IMU_GYRO_BIAS, EP_IMU_GYRO_NOISE = 20, 23, 24, 27
+EP_DIM = 28
 # spine observation offsets
 SP_BASE_ANGVEL, SP_BASE_LINVEL, SP_PITCH, SP_ROT = 0, 3, 6, 7
 SP_IMU_QUAT, SP_IMU_ANGVEL, SP_IMU_LINACC, SP_IMU_RAWACC = 16, 20, 23, 26
@@ -357,3 +361,18 @@ def struct_to_dict(s: C.Structure) -> dict:
         else:
             out[name] = v
     return out
+
+
+def config_env_params(c: "UpkieSimConfig") -> np.ndarray:
+    """The row ``[EP_DIM]`` float32 of the per-env parameter table that holds a configuration's own values: what every
+    env runs without a table (``upkie_b200_get_env_params``)."""
+    r = np.empty(EP_DIM, dtype=np.float64)
+    r[EP_KP], r[EP_KD] = c.torque_control_kp, c.torque_control_kd
+    r[EP_FRICTION : EP_FRICTION + NJ] = list(c.joint_friction)
+    r[EP_CTRL_NOISE : EP_CTRL_NOISE + NJ] = list(c.torque_control_noise)
+    r[EP_MEAS_NOISE : EP_MEAS_NOISE + NJ] = list(c.torque_measurement_noise)
+    r[EP_IMU_ACC_BIAS : EP_IMU_ACC_BIAS + 3] = list(c.imu_accelerometer_bias)
+    r[EP_IMU_ACC_NOISE] = c.imu_accelerometer_noise
+    r[EP_IMU_GYRO_BIAS : EP_IMU_GYRO_BIAS + 3] = list(c.imu_gyroscope_bias)
+    r[EP_IMU_GYRO_NOISE] = c.imu_gyroscope_noise
+    return r.astype(np.float32)  # the kernels' fp32 values of the double fields (round to nearest, as params.h)

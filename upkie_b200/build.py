@@ -10,7 +10,7 @@ LIB_PATH = os.path.join(_HERE, "libupkie_b200.so")
 # compiled in parallel, then linked
 SOURCES = ["upkie_b200.cu", "step_device.cu", "step_host.cu", "step_multicast.cu", "step_device_limits.cu",
            "step_host_limits.cu", "step_multicast_limits.cu", "step_device_spine.cu", "step_host_spine.cu",
-           "step_device_body.cu", "step_host_body.cu"]
+           "step_device_body.cu", "step_host_body.cu", "step_device_table.cu", "step_host_table.cu"]
 DEPS = SOURCES + [
     "sim_core.cuh", "sim_pair.cuh", "kernel_common.cuh", "step_kernel.cuh", "params.h", "mpc.cuh", "mpc_core.cuh",
     "observers.cuh", "observers_core.cuh", "controllers.cuh", "controllers_core.cuh", "../../include/upkie_b200.h",

@@ -9,4 +9,5 @@ cudaError_t launch_step_multicast(const StepArgs&) { return cudaErrorNotSupporte
 cudaError_t launch_push_rows(const PeerPtrs&, int, cudaStream_t) { return cudaErrorNotSupported; }
 cudaError_t launch_step_device_spine(const StepArgs&) { return cudaErrorNotSupported; }
 cudaError_t launch_step_device_body(const StepArgs&) { return cudaErrorNotSupported; }
+cudaError_t launch_step_device_table(const StepArgs&) { return cudaErrorNotSupported; }
 }  // namespace upkie_b200

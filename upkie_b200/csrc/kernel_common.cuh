@@ -84,7 +84,7 @@ struct PeerPtrs {
 // One launch of the env-step kernel over the envs [i0, i0 + cnt) of a handle.
 struct StepArgs {
   const SimParams* P;
-  int mode, autoreset, noise;  // noise: 1 = the "extras" instantiation (torque noise models, external forces), 2 = extras + joint-limit rows, 3 = 2 + spine timing, 4 = 2 + body-ground contact rows
+  int mode, autoreset, noise;  // noise: 1 = the "extras" instantiation (torque noise models, external forces), 2 = extras + joint-limit rows, 3 = 2 + spine timing, 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table
   int i0, cnt, n_pad, block;
   int compact_obs;      // TILE=1, servos: observation rows [6][3] (position, velocity, torque) instead of [6][5]
   int grid;             // TILE=1: number of persistent blocks (0 = one block per tile)
@@ -119,5 +119,7 @@ cudaError_t launch_step_device_body(const StepArgs& a);  // step_device_body.cu:
 cudaError_t launch_step_host_body(const StepArgs& a);    // step_host_body.cu: NOISE=4, TILE=1
 cudaError_t launch_step_device_spine(const StepArgs& a);  // step_device_spine.cu: NOISE=3 (spine timing), TILE=0
 cudaError_t launch_step_host_spine(const StepArgs& a);    // step_host_spine.cu: NOISE=3, TILE=1
+cudaError_t launch_step_device_table(const StepArgs& a);  // step_device_table.cu: NOISE=5 (limits + per-env table), TILE=0
+cudaError_t launch_step_host_table(const StepArgs& a);    // step_host_table.cu: NOISE=5, TILE=1
 
 }  // namespace upkie_b200

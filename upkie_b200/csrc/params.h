@@ -252,7 +252,55 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.max_episode_steps = c.max_episode_steps;
   P.elapsed = nullptr;
   P.final_obs = nullptr;
+  P.env_params = nullptr;
+  P.env_params_stride = 0;
   return 0;
+}
+
+// ---- per-env parameter table (upkie_b200_set_env_params) ----------------------------------------------------------
+// What a row of the table (or the config) holds besides plain values: bad input, and which noise models some env needs
+constexpr uint32_t kEpInvalid = 1u, kEpCtrlNoise = 2u, kEpMeasNoise = 4u, kEpImuUncertainty = 8u;
+
+UPKIE_HD uint32_t env_row_flags(const float* r) {
+  uint32_t f = 0;
+  for (int k = 0; k < UPKIE_EP_DIM; ++k) {
+    const bool bias = (k >= UPKIE_EP_IMU_ACC_BIAS && k < UPKIE_EP_IMU_ACC_BIAS + 3) ||
+                      (k >= UPKIE_EP_IMU_GYRO_BIAS && k < UPKIE_EP_IMU_GYRO_BIAS + 3);
+    if (!(fabsf(r[k]) <= 3.402823466e38f)) f |= kEpInvalid;  // NaN or infinite
+    if (!bias && !(r[k] >= 0.f)) f |= kEpInvalid;           // gains, friction, standard deviations
+    if (bias && r[k] != 0.f) f |= kEpImuUncertainty;
+  }
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    // the reference's thresholds: noise is drawn only when sigma > 1e-10 (pybullet_backend.py:464,548)
+    if (r[UPKIE_EP_CTRL_NOISE + j] > 1e-10f) f |= kEpCtrlNoise;
+    if (r[UPKIE_EP_MEAS_NOISE + j] > 1e-10f) f |= kEpMeasNoise;
+  }
+  if (r[UPKIE_EP_IMU_ACC_NOISE] > 0.f || r[UPKIE_EP_IMU_GYRO_NOISE] > 0.f) f |= kEpImuUncertainty;
+  return f;
+}
+
+// the config's value of column k (what every env runs without a table)
+UPKIE_HD float config_env_param(const SimParams& P, int k) {
+  if (k == UPKIE_EP_KP) return P.kp;
+  if (k == UPKIE_EP_KD) return P.kd;
+  if (k < UPKIE_EP_CTRL_NOISE) return P.joint_friction[k - UPKIE_EP_FRICTION];
+  if (k < UPKIE_EP_MEAS_NOISE) return P.ctrl_noise[k - UPKIE_EP_CTRL_NOISE];
+  if (k < UPKIE_EP_IMU_ACC_BIAS) return P.meas_noise[k - UPKIE_EP_MEAS_NOISE];
+  if (k < UPKIE_EP_IMU_ACC_NOISE) return P.imu_acc_bias[k - UPKIE_EP_IMU_ACC_BIAS];
+  if (k == UPKIE_EP_IMU_ACC_NOISE) return P.imu_acc_noise;
+  if (k < UPKIE_EP_IMU_GYRO_NOISE) return P.imu_gyro_bias[k - UPKIE_EP_IMU_GYRO_BIAS];
+  return P.imu_gyro_noise;
+}
+
+// the "some env has this noise" flags of a parameter block as env_row_flags bits, and back
+inline uint32_t noise_flags(const SimParams& P) {
+  return (P.any_ctrl_noise ? kEpCtrlNoise : 0u) | (P.any_meas_noise ? kEpMeasNoise : 0u) |
+         (P.any_imu_uncertainty ? kEpImuUncertainty : 0u);
+}
+inline void set_noise_flags(SimParams& P, uint32_t f) {
+  P.any_ctrl_noise = (f & kEpCtrlNoise) ? 1 : 0;
+  P.any_meas_noise = (f & kEpMeasNoise) ? 1 : 0;
+  P.any_imu_uncertainty = (f & kEpImuUncertainty) ? 1 : 0;
 }
 
 // AoS state row <-> registers

@@ -5,7 +5,7 @@
 //       articulated-body dynamics, wheel-ground contact solve, semi-implicit integration), observation,
 //       termination; optional fused auto-reset; optional torque noise models.
 //       NOISE: 0 plain, 1 "extras" (noise models, external forces), 2 extras + joint-limit rows, 3 = 2 + spine timing
-//       (+ body-ground contact rows), 4 = 2 + body-ground contact rows.
+//       (+ body-ground contact rows), 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table.
 // Included by step_device.cu (TILE=0), step_host.cu (TILE=1), step_multicast.cu (TILE=2) and the two *_limits.cu
 // units (NOISE=2), see kernel_common.cuh.
 #pragma once
@@ -22,6 +22,9 @@
 #endif
 #ifndef UPKIE_STEP_BODY_TU
 #define UPKIE_STEP_BODY_TU 0  // 1 in step_*_body.cu: the NOISE=4 instantiations (extras + limits + body-ground contact rows)
+#endif
+#ifndef UPKIE_STEP_TABLE_TU
+#define UPKIE_STEP_TABLE_TU 0  // 1 in step_*_table.cu: the NOISE=5 instantiations (extras + limits + per-env parameter table)
 #endif
 #ifndef UPKIE_ACTION_IN_TILE
 #define UPKIE_ACTION_IN_TILE 0  // build-time experiment (tools/variants.py)
@@ -46,10 +49,10 @@ __device__ __forceinline__ void mc_store_u32(uint32_t* addr, uint32_t v) {
 // (spine mode: the rows the spine assembled), gyropod o6, pendulum [4]. Per-thread stores: only resetting lanes write.
 template <int MODE, bool SPINE>
 __device__ __forceinline__ void store_final_obs(const SimParams& P, const RobotState& S, const SpineLag& L,
-                                                const float* o6, const NoiseCtx* nz, bool compact, int i) {
+                                                const float* o6, const NoiseCtx* nz, bool compact, int i, int env_col) {
   if (MODE == MODE_SERVOS) {
     float tq[6];
-    measured_torques(P, S, nz, tq);
+    measured_torques(P, S, nz, tq, env_col);
     const int dim = compact ? 18 : UPKIE_OBS_DIM;
     float* o = P.final_obs + size_t(i) * dim;
 #pragma unroll
@@ -144,6 +147,10 @@ __device__ __forceinline__ void step_env(
   }
   // external forces ride on the NOISE ("extras") instantiations so the plain kernels stay untouched
   const ExtForces xf{ext ? ext + i : nullptr, size_t(n_pad), ext_local};
+  // this robot's column of the per-env parameter table. The NOISE=2 kernels (the headline's family) never run with a
+  // table, the host picks the NOISE=5 copy of them then: -1 compiles the table reads out of them, so that their
+  // register allocation is the one they have without the feature
+  const int env_col = NOISE == 2 ? -1 : i;
   int nsub = P.nb_substeps;
   // spine mode (config.spine_mode, UpkieServos, the NOISE=2 kernels): every substep is one cycle of the Bullet spine
   // (NOISE = 3: its own instantiations, step_*_spine.cu, so that the other kernels do not carry the lag record)
@@ -198,18 +205,19 @@ __device__ __forceinline__ void step_env(
     }
 #endif
     if (sub < nsub) {
-      // the body-ground contacts of the tick's last substep go to the handle's record (NOISE >= 3 kernels)
-      const BodyRecOut br{(NOISE >= 3 && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
+      // the body-ground contacts of the tick's last substep go to the handle's record (NOISE = 3, 4 kernels)
+      const BodyRecOut br{((NOISE == 3 || NOISE == 4) && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
                           size_t(P.body_rec_stride)};
       if (spine) {
         if (resetting && sub == 2) spine_assemble_observation(S, L);
-        spine_cycle(P, S, L, a, resetting, eps, mu, WarpAny(), PhaseSync(), P.joint_limits >= 1 ? P.joint_limits : 1, br);
+        spine_cycle(P, S, L, a, resetting, eps, mu, WarpAny(), PhaseSync(), P.joint_limits >= 1 ? P.joint_limits : 1, br,
+                    i);
       } else {
         // NOISE >= 2: the device's two limit modes (1 and 0 alias to 3 there, see physics_substep_paired), spelled as
         // a choice between two nonzero constants so that the compiler drops servo_substep's limits == 0 branches, a
         // second and third inlined copy of the substep that these kernels never run
         servo_substep(P, S, a, resetting, eps, mu, WarpAny(), PhaseSync(), NOISE ? &nz : nullptr, sub,
-                      (NOISE && ext) ? &xf : nullptr, NOISE >= 2 ? (P.joint_limits == 2 ? 2 : 3) : 0, br);
+                      (NOISE && ext) ? &xf : nullptr, NOISE >= 2 ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col);
       }
     } else {
 #pragma unroll
@@ -253,13 +261,14 @@ __device__ __forceinline__ void step_env(
 
   if (AUTORESET == AUTORESET_SAME_STEP) {
     if (term || trunc) {
-      if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, NOISE ? &nz : nullptr, TILE && compact, i);
+      if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, NOISE ? &nz : nullptr, TILE && compact, i, env_col);
       elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
       float init[UPKIE_INIT_DIM];
       sample_init_state(P, seed, env_offset + uint64_t(i), uint64_t(ep), init);
-      const BodyRecOut br{(NOISE >= 3 && P.body_rec && live) ? P.body_rec + i : nullptr, size_t(P.body_rec_stride)};
+      const BodyRecOut br{((NOISE == 3 || NOISE == 4) && P.body_rec && live) ? P.body_rec + i : nullptr,
+                          size_t(P.body_rec_stride)};
       if (spine) reset_robot_spine(P, S, L, init, eps, mu, WarpAny(), P.joint_limits, br);
       else reset_robot(P, S, init, eps, mu, WarpAny(), NOISE >= 2 ? P.joint_limits : 0, br);
       if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
@@ -276,7 +285,7 @@ __device__ __forceinline__ void step_env(
   if (MODE == MODE_SERVOS) {
     float o[UPKIE_OBS_DIM];
     float tq[6];
-    measured_torques(P, S, NOISE ? &nz : nullptr, tq);
+    measured_torques(P, S, NOISE ? &nz : nullptr, tq, env_col);
 #pragma unroll
     for (int j = 0; j < 6; ++j) {
       o[j * 5 + 0] = S.q[j]; o[j * 5 + 1] = S.qd[j]; o[j * 5 + 2] = tq[j];
@@ -526,6 +535,8 @@ cudaError_t launch_step_mode(const StepArgs& a) {
 #define LAUNCH(AR) LAUNCH_N(AR, 4)
 #elif UPKIE_STEP_LIMITS_TU
 #define LAUNCH(AR) LAUNCH_N(AR, 2)
+#elif UPKIE_STEP_TABLE_TU
+#define LAUNCH(AR) LAUNCH_N(AR, 5)
 #else
 #define LAUNCH(AR)                \
   do {                            \

@@ -62,6 +62,10 @@ struct Handle {
   float* ext = nullptr;          // [7 * 3][n_pad] external forces, null = none
   float* lag = nullptr;          // [UPKIE_LAG_DIM][n_pad] spine-mode lag records (config.spine_mode), else null
   float* body_rec = nullptr;     // [UPKIE_BODY_REC_DIM][n_pad] body-ground contacts of the last substep (config.body_contacts)
+  float* env_params = nullptr;   // [UPKIE_EP_DIM][n_pad] per-env parameter table (upkie_b200_set_env_params), else null
+  uint32_t env_param_flags = 0;  // env_row_flags of the table, OR-ed over its rows
+  uint32_t config_flags = 0;     // noise_flags of the config (restored when the table is dropped)
+  uint32_t* ep_check = nullptr;  // [1] device word of the table validation
   uint32_t ext_local = 0;
   int autoreset = AUTORESET_DISABLED;
   uint64_t seed = 0, env_offset = 0;
@@ -154,10 +158,10 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
     RobotState S;
     load_state(state, n_pad, i, S);
     float tq[6];
-    measured_torques(P, S, &nz, tq);
+    measured_torques(P, S, &nz, tq, i);
     spine_observation(P, S, o, tq);
   }
-  apply_imu_uncertainty(P, nz, o);
+  apply_imu_uncertainty(P, nz, o, i);
 #pragma unroll
   for (int k = 0; k < UPKIE_SPINE_DIM; ++k) out[size_t(i) * UPKIE_SPINE_DIM + k] = o[k];
 }
@@ -180,7 +184,7 @@ __global__ void k_reset_obs(const __grid_constant__ SimParams P, int n, int n_pa
   if (obs_dim == UPKIE_OBS_DIM) {
     float tq[6];
     const NoiseCtx nz{env_offset + uint64_t(i), tick[i]};
-    measured_torques(P, S, &nz, tq);
+    measured_torques(P, S, &nz, tq, i);
     for (int j = 0; j < 6; ++j) {
       float* o = out + size_t(i) * UPKIE_OBS_DIM + j * 5;
       o[0] = S.q[j]; o[1] = S.qd[j]; o[2] = tq[j]; o[3] = 42.0f; o[4] = 18.0f;
@@ -207,6 +211,23 @@ __global__ void k_set_state(int n, int n_pad, float* __restrict__ state, const f
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   for (int k = 0; k < UPKIE_STATE_DIM; ++k) state[size_t(k) * n_pad + i] = in[size_t(i) * UPKIE_STATE_DIM + k];
+}
+// per-env parameter table: validation of the caller's rows [n][UPKIE_EP_DIM] (env_row_flags OR-ed into *flags), and
+// the rows <-> struct-of-arrays transposes; without a table the rows read back the config's values
+__global__ void k_env_params_check(int n, const float* __restrict__ rows, uint32_t* __restrict__ flags) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t f = env_row_flags(rows + size_t(i) * UPKIE_EP_DIM);
+  if (f) atomicOr(flags, f);
+}
+__global__ void k_env_params_copy(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict__ table,
+                                  float* __restrict__ rows, int to_rows) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  for (int k = 0; k < UPKIE_EP_DIM; ++k) {
+    if (!to_rows) table[size_t(k) * n_pad + i] = rows[size_t(i) * UPKIE_EP_DIM + k];
+    else rows[size_t(i) * UPKIE_EP_DIM + k] = table ? table[size_t(k) * n_pad + i] : config_env_param(P, k);
+  }
 }
 __global__ void k_set_ext(int n, int n_pad, float* __restrict__ ext, const float* __restrict__ in) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -245,6 +266,9 @@ int pick_block(const Handle* h, int cnt) {
 int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float* obs, float* reward, uint8_t* term,
                uint8_t* trunc, cudaStream_t s, bool tile = false, bool persistent = true, bool compact = false,
                bool multicast = false, const PeerPtrs* peers = nullptr, float* final_obs = nullptr) {
+  if (multicast && h->P.env_params)
+    return fail(UPKIE_B200_EINVAL, "the per-env parameter table has no in-kernel rollout transport (use upkie_b200_step "
+                                   "with compact rows)");
   if (multicast && h->P.max_episode_steps > 0)
     return fail(UPKIE_B200_EINVAL, "max_episode_steps has no in-kernel rollout transport: it does not carry truncated "
                                    "(use upkie_b200_step with compact rows)");
@@ -262,6 +286,7 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   a.mode = mode;
   a.autoreset = h->autoreset;
   a.noise = h->P.joint_limits ? 2 : ((h->P.any_ctrl_noise || h->P.any_meas_noise || h->ext) ? 1 : 0);  // "extras" kernels
+  if (a.noise == 2 && h->P.env_params) a.noise = 5;  // the NOISE=2 kernels carry no table reads (step_*_table.cu)
   if (h->P.body_contacts) {  // the model's collision points hold contact rows: the NOISE=4 kernels (step_*_body.cu)
     if (multicast) return fail(UPKIE_B200_EINVAL, "body_contacts has no in-kernel rollout transport (use upkie_b200_step_servos_compact)");
     a.noise = 4;
@@ -501,6 +526,7 @@ int upkie_b200_create(const UpkieModel* model, const UpkieSimConfig* config, int
   if (rc) { delete h; return fail(rc, err); }
   h->magic = kMagic;
   h->model = *model;
+  h->config_flags = noise_flags(h->P);
   h->n = n_envs;
   h->n_pad = (n_envs + 31) / 32 * 32;
   h->device = device;
@@ -580,6 +606,7 @@ void upkie_b200_destroy(void* handle) {
   cudaSetDevice(h->device);
   cudaFree(h->state); cudaFree(h->eps); cudaFree(h->mu); cudaFree(h->err); cudaFree(h->done_prev); cudaFree(h->episode);
   cudaFree(h->tick); cudaFree(h->elapsed); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
+  cudaFree(h->env_params); cudaFree(h->ep_check);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -612,6 +639,13 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.body_rec = P.body_contacts ? h->body_rec : nullptr;
   P.body_rec_stride = h->n_pad;
   P.elapsed = h->elapsed;
+  // the per-env parameter table stays: its values and its noise flags override the config's
+  const uint32_t config_flags = noise_flags(P);
+  if (h->env_params) {
+    P.env_params = h->env_params;
+    P.env_params_stride = h->n_pad;
+    set_noise_flags(P, h->env_param_flags);
+  }
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -622,6 +656,60 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   }
   // kernels read the parameter block by value at launch: steps already enqueued keep the old one
   h->P = P;
+  h->config_flags = config_flags;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_env_params(void* handle, const float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (!rows) {
+    if (h->env_params) {
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may still read the table
+      cudaFree(h->env_params);
+      h->env_params = nullptr;
+    }
+    h->P.env_params = nullptr;
+    h->P.env_params_stride = 0;
+    set_noise_flags(h->P, h->config_flags);
+    return UPKIE_B200_OK;
+  }
+  // validate first: a rejected table leaves the previous one (or none) in force
+  if (!h->ep_check) CUDA_TRY(cudaMalloc(&h->ep_check, sizeof(uint32_t)));
+  CUDA_TRY(cudaMemsetAsync(h->ep_check, 0, sizeof(uint32_t), s));
+  k_env_params_check<<<(h->n + 127) / 128, 128, 0, s>>>(h->n, rows, h->ep_check);
+  CUDA_TRY(cudaGetLastError());
+  uint32_t flags = 0;
+  CUDA_TRY(cudaMemcpyAsync(&flags, h->ep_check, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  if (flags & kEpInvalid)
+    return fail(UPKIE_B200_EINVAL, "set_env_params: every value must be finite, and gains, friction and noise standard "
+                                   "deviations >= 0");
+  const size_t bytes = size_t(UPKIE_EP_DIM) * h->n_pad * sizeof(float);
+  if (!h->env_params) {
+    CUDA_TRY(cudaMalloc(&h->env_params, bytes));
+    CUDA_TRY(cudaMemsetAsync(h->env_params, 0, bytes, s));
+  }
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight on other streams may still read the previous table
+  k_env_params_copy<<<(h->n + 127) / 128, 128, 0, s>>>(h->P, h->n, h->n_pad, h->env_params, const_cast<float*>(rows), 0);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(s));
+  h->env_param_flags = flags;
+  h->P.env_params = h->env_params;
+  h->P.env_params_stride = h->n_pad;
+  set_noise_flags(h->P, flags);
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_env_params(void* handle, float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !rows) return fail(UPKIE_B200_EINVAL, "get_env_params: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  k_env_params_copy<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad,
+                                                                                        h->env_params, rows, 1);
+  CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
 

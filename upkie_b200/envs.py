@@ -19,7 +19,7 @@ per env inside the step kernel (``truncated`` once an env has run T steps since
 its last reset), which the fused auto-reset honours.
 """
 
-from typing import Any, Dict, Optional, Tuple, Union
+from typing import Any, Dict, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
@@ -281,6 +281,77 @@ def make_config(
     return cfg
 
 
+_JOINT_PROPERTY_COLUMNS = (
+    ("friction", _abi.EP_FRICTION),
+    ("torque_control_noise", _abi.EP_CTRL_NOISE),
+    ("torque_measurement_noise", _abi.EP_MEAS_NOISE),
+)
+
+
+def _per_env(value) -> bool:
+    return np.ndim(value) != 0
+
+
+def needs_env_params(torque_control_kp=None, torque_control_kd=None, joint_properties=None) -> bool:
+    """Whether these ``B200VectorEnv`` arguments differ between envs: ``[N]`` arrays, ``JointProperties`` with
+    array fields, or a sequence of per-env ``joint_properties`` dicts. All-scalar arguments fit in the config."""
+    if _per_env(torque_control_kp) or _per_env(torque_control_kd):
+        return True
+    if joint_properties is None:
+        return False
+    if not isinstance(joint_properties, dict):
+        return True
+    return any(_per_env(getattr(props, f, 0.0)) for props in joint_properties.values() for f, _ in _JOINT_PROPERTY_COLUMNS)
+
+
+def env_params_table(num_envs: int, base: np.ndarray, torque_control_kp=None, torque_control_kd=None,
+                     joint_properties=None) -> np.ndarray:
+    """Per-env parameter table ``[N, EP_DIM]`` float32 (``UpkieSim.set_env_params``) from the reference's constructor
+    arguments (``PyBulletBackend(torque_control_kp, torque_control_kd, joint_properties)``, ``pybullet_backend.py:55-65``).
+    ``base``: a configuration's row (``_abi.config_env_params``) or a table ``[N, EP_DIM]``; it fills every column the
+    arguments do not give (None = not given). Gains take a float or an ``[N]`` array. ``joint_properties`` takes
+    ``{joint: JointProperties}`` whose fields are floats or ``[N]`` arrays, or a sequence of N such dicts, one per env.
+    Raises ``UpkieException`` on a wrong length, a non-finite or a negative value."""
+    n = int(num_envs)
+    table = np.empty((n, _abi.EP_DIM), dtype=np.float32)  # C order, as the C ABI reads it
+    table[:] = np.asarray(base, dtype=np.float32)
+
+    def column(value, name):
+        v = np.asarray(value, dtype=np.float64)
+        if v.ndim > 1 or (v.ndim == 1 and v.shape[0] != n):
+            raise UpkieException(f"{name}: expected a float or an array of {n} values, got shape {v.shape}")
+        if not np.all(np.isfinite(v)) or np.any(v < 0.0):
+            raise UpkieException(f"{name}: values must be finite and >= 0")
+        return np.broadcast_to(v, (n,)).astype(np.float32)
+
+    if torque_control_kp is not None:
+        table[:, _abi.EP_KP] = column(torque_control_kp, "torque_control_kp")
+    if torque_control_kd is not None:
+        table[:, _abi.EP_KD] = column(torque_control_kd, "torque_control_kd")
+    if joint_properties is None:
+        return table
+    if isinstance(joint_properties, dict):
+        per_joint = [(None, joint_properties)]
+    else:
+        if len(joint_properties) != n:
+            raise UpkieException(f"joint_properties: expected one dict per env ({n}), got {len(joint_properties)}")
+        per_joint = list(enumerate(joint_properties))
+    for env, props_of in per_joint:
+        for j, name in enumerate(_abi.JOINT_NAMES):
+            props = (props_of or {}).get(name)
+            if props is None:
+                continue
+            for field, col in _JOINT_PROPERTY_COLUMNS:
+                value = getattr(props, field, 0.0)
+                if env is None:
+                    table[:, col + j] = column(value, f"joint_properties[{name!r}].{field}")
+                elif _per_env(value):
+                    raise UpkieException(f"joint_properties[{env}][{name!r}].{field}: a per-env dict takes floats")
+                else:
+                    table[env, col + j] = column(value, f"joint_properties[{env}][{name!r}].{field}")[0]
+    return table
+
+
 class B200VectorEnv(VectorEnv):
     """N Upkie environments stepped by one kernel launch per ``step()``.
 
@@ -294,6 +365,12 @@ class B200VectorEnv(VectorEnv):
     storage with the observation's structure (servo dictionary of arrays, array, or CUDA tensor from
     ``step_tensors``): rows outside the mask hold stale values. ``copy=True`` copies it as it copies the
     observation. ``info["final_info"]`` (the terminal step's spine observation) is not provided.
+
+    Domain randomisation of the actuators: ``torque_control_kp`` / ``torque_control_kd`` take a float or an ``[N]``
+    array, ``joint_properties`` a ``{joint: JointProperties}`` dict whose fields are floats or ``[N]`` arrays, or a
+    sequence of N such dicts (one per env, as N reference envs would be built). Per-env values go to the handle's
+    parameter table (``UpkieSim.set_env_params``, which also takes per-env IMU uncertainty); all-scalar arguments
+    build none. ``set_joint_properties`` changes them between episodes.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -313,9 +390,9 @@ class B200VectorEnv(VectorEnv):
         max_ground_velocity: float = 3.0,
         max_yaw_velocity: float = 1.0,
         nb_substeps: Optional[int] = None,
-        torque_control_kp: float = 20.0,
-        torque_control_kd: float = 1.0,
-        joint_properties: Optional[dict] = None,
+        torque_control_kp: Union[float, np.ndarray] = 20.0,
+        torque_control_kd: Union[float, np.ndarray] = 1.0,
+        joint_properties: Optional[Union[dict, Sequence[dict]]] = None,
         inertia_variation: float = 0.0,
         env_offset: int = 0,
         config: Optional[_abi.UpkieSimConfig] = None,
@@ -349,9 +426,14 @@ class B200VectorEnv(VectorEnv):
         self.env_offset = int(env_offset)
         self.autoreset_mode = autoreset_mode
         self.metadata = dict(self.metadata, autoreset_mode=autoreset_mode)
+        per_env = needs_env_params(torque_control_kp, torque_control_kd, joint_properties)
         if config is None:
+            # per-env arguments go to the parameter table below; the config keeps the scalar ones
             config = make_config(
-                frequency, nb_substeps, torque_control_kp, torque_control_kd, joint_properties, max_gain_scale,
+                frequency, nb_substeps,
+                20.0 if _per_env(torque_control_kp) else torque_control_kp,
+                1.0 if _per_env(torque_control_kd) else torque_control_kd,
+                None if per_env else joint_properties, max_gain_scale,
                 fall_pitch, leg_gain_scale, max_ground_velocity, max_yaw_velocity, self.init_state, noise_seed,
                 joint_limits, spine_mode, body_contacts, max_episode_steps,
             )
@@ -360,6 +442,9 @@ class B200VectorEnv(VectorEnv):
             config = _abi.UpkieSimConfig.from_buffer_copy(config)
             config.max_episode_steps = max_episode_steps
         self.config = config
+        # validated before any device is touched
+        env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
+                                      torque_control_kd, joint_properties) if per_env else None
         if self.config.spine_mode and env_type != "servos":
             raise UpkieException("spine_mode is available for env_type='servos' (the wrappers of a spine read observer "
                                  "outputs: feed info['spine_observation'] to upkie_b200.observers.ObserverPipeline)")
@@ -384,6 +469,8 @@ class B200VectorEnv(VectorEnv):
         self.observation_space = batch_space(self.single_observation_space, self.num_envs)
 
         self.sim = UpkieSim(self.num_envs, model=self.model, config=self.config, device=device)
+        if env_params is not None:
+            self.sim.set_env_params(torch.from_numpy(env_params).to(self.sim.device))
         self._seed = 0
         self.mpc_balancer = None
         if env_type == "base_velocity":
@@ -412,6 +499,13 @@ class B200VectorEnv(VectorEnv):
         rng = np.random.default_rng(seed)
         eps = rng.uniform(-inertia_variation, inertia_variation, size=(self.num_envs, 6)).astype(np.float32)
         self.sim.set_randomization(inertia_eps=torch.from_numpy(eps).to(self.sim.device))
+
+    def set_joint_properties(self, joint_properties=None, torque_control_kp=None, torque_control_kd=None) -> None:
+        """Re-randomise the actuators between episodes, with the constructor's argument forms; what is not given
+        (None) keeps its current per-env values. Takes effect from the next step."""
+        base = self.sim.get_env_params().cpu().numpy()
+        table = env_params_table(self.num_envs, base, torque_control_kp, torque_control_kd, joint_properties)
+        self.sim.set_env_params(torch.from_numpy(table).to(self.sim.device))
 
     def update_init_rand(self, **kwargs) -> None:
         """``UpkieEnv.update_init_rand`` (``upkie_env.py:244-251``)."""

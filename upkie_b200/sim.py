@@ -117,6 +117,24 @@ class UpkieSim:
         torch.cuda.current_stream(self.device).synchronize()
         self._randomization = (None if friction is None else friction.clone(), None if inertia_eps is None else inertia_eps.clone())
 
+    def set_env_params(self, rows: Optional[torch.Tensor] = None) -> None:
+        """Per-env actuator and IMU parameters ``rows[N, EP_DIM]`` (layout ``_abi.EP_*``): env ``i`` runs
+        ``torque_control_kp`` / ``kd``, joint friction, torque control / measurement noise and IMU uncertainty of row
+        ``i`` instead of the config's, from the next step on. What N reference envs built with different
+        ``PyBulletBackend`` arguments hold. ``None`` drops the table (every env runs the config's values again).
+        Values must be finite, gains, friction and noise standard deviations >= 0; otherwise the call raises and the
+        previous table stays."""
+        if rows is not None:
+            self._check_tensor(rows, (self.n, _abi.EP_DIM), name="env_params")
+        check(lib().upkie_b200_set_env_params(self._h, _ptr(rows), self._stream()))
+        self._env_params = None if rows is None else rows.clone()
+
+    def get_env_params(self) -> torch.Tensor:
+        """The parameters in force, ``[N, EP_DIM]``: the table, or without one the config's values in every row."""
+        out = torch.empty((self.n, _abi.EP_DIM), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_env_params(self._h, _ptr(out), self._stream()))
+        return out
+
     def set_external_forces(self, force: Optional[torch.Tensor] = None, local_mask: int = 0) -> None:
         """``force[N, 7, 3]`` newtons at the centres of mass of the 7 bodies, applied on every substep of
         the following steps until overwritten; ``None`` clears. Bit ``b`` of ``local_mask``: the force on
@@ -444,7 +462,7 @@ class UpkieSim:
     # checkpoint / resume ------------------------------------------------------------------
     def state_dict(self) -> dict:
         """Everything a handle needs to continue bit for bit (``torch.save``-able): robot state, episode / tick
-        counters, time-limit counts, pending auto-resets, error flags, randomisation, external forces, auto-reset keys. The model and
+        counters, time-limit counts, pending auto-resets, error flags, randomisation, per-env parameter table, external forces, auto-reset keys. The model and
         the configuration are construction arguments and are not included."""
         i32, u8 = torch.int32, torch.uint8
         episode = torch.empty(self.n, dtype=i32, device=self.device)
@@ -461,6 +479,7 @@ class UpkieSim:
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
             "elapsed": elapsed,  # steps since each env's last reset (the time limit's counts)
             "friction": friction, "inertia_eps": eps, "external_force": force, "external_local_mask": local_mask,
+            "env_params": getattr(self, "_env_params", None),  # per-env parameter table, None = the config's values
             "autoreset": getattr(self, "_autoreset", (AUTORESET_DISABLED, 0, 0)),
         }
 
@@ -481,6 +500,9 @@ class UpkieSim:
                                None if sd["inertia_eps"] is None else sd["inertia_eps"].to(dev))
         self.set_external_forces(None if sd["external_force"] is None else sd["external_force"].to(dev),
                                  sd["external_local_mask"])
+        # a checkpoint written before the per-env parameter table existed loads as "no table"
+        env_params = sd.get("env_params")
+        self.set_env_params(None if env_params is None else env_params.to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
