@@ -613,6 +613,40 @@ int upkie_b200_mpc_step(void* mpc, const float* x0, const float* v_target,
 /* Full optimal input sequence of the last solve, plan[N][nb_timesteps]. */
 int upkie_b200_mpc_plan(void* mpc, float* plan, void* stream);
 
+/* ---- UpkieBaseVelocity epilogue ---------------------------------------------
+ * An addition to ABI 8: a new entry point and a new struct, no existing layout or signature changed, so a caller
+ * built against an earlier ABI-8 header keeps working with this library.
+ * Replaces the end of UpkieBaseVelocity.step (upkie/envs/upkie_base_velocity.py:194-202: dead reckoning of the
+ * commanded linear velocity along the post-step yaw, observation [x, y, yaw]) and, for the envs that reset in this
+ * tick, UpkieBaseVelocity.reset (upkie_base_velocity.py:137-162: MPCBalancer.reset, x = y = 0, observation
+ * [0, 0, 0]). One launch per tick, after the tick's gyropod step (upkie_b200_step_gyropod / upkie_b200_step with
+ * act_dim 2) and upkie_b200_spine_obs, on the stream of those calls; `mpc` is the balancer whose upkie_b200_mpc_step
+ * produced the ground velocity of that step. Which envs reset is read on the device: every reset the step kernels
+ * sample (both fused auto-resets) counts an episode of the sim handle, which keeps a copy of the counters as of its
+ * last post step (upkie_b200_reset with init_state = NULL and upkie_b200_set_counters update that copy too). An
+ * explicit upkie_b200_reset from host rows cancels a pending next-step reset and is not seen here: the caller resets
+ * x, y and the balancer of those envs itself.
+ * Per env i, by autoreset_mode (must equal the sim handle's, upkie_b200_set_autoreset):
+ *  - no reset in this tick (always in mode 0): xy[i] += v cos(yaw) dt, v sin(yaw) dt with v = action[i][0] and
+ *    yaw = gyropod_obs[i][2], each product and sum rounded to nearest fp32 (no FMA) with the IEEE cosf / sinf;
+ *    obs[i] = [x, y, yaw];
+ *  - reset, mode 2 (same step): final_obs[i] = [x, y, yaw] as above with the pre-reset yaw gyropod_final_obs[i][2];
+ *  - reset, modes 1 and 2: xy[i] = 0, obs[i] = [0, 0, 0], commanded_velocity[i] = 0 and the mpc handle's warm start
+ *    of env i is dropped (upkie_b200_mpc_reset for that env). Rows of final_obs of the other envs are left untouched.
+ * Device buffers; gyropod_final_obs and final_obs are read / written in mode 2 only (may be NULL otherwise). */
+typedef struct UpkieBaseVelocityPost {
+  const float* action;             /* [N][2] the agent's action: commanded linear velocity, yaw velocity */
+  const float* gyropod_obs;        /* [N][6] observation of this tick's gyropod step */
+  const float* gyropod_final_obs;  /* [N][6] final-observation rows of that step (mode 2) */
+  float* xy;                       /* [N][2] dead-reckoned position, read and updated in place */
+  float* commanded_velocity;       /* [N] MPCBalancer.commanded_velocity of `mpc`, zeroed for the envs that reset */
+  float* obs;                      /* [N][3] out: [x, y, yaw] */
+  float* final_obs;                /* [N][3] out (mode 2): [x, y, yaw] the resetting envs reached */
+  float dt;                        /* agent period (the fp32 value the dead reckoning multiplies by) */
+  int32_t autoreset_mode;          /* 0 disabled, 1 next step, 2 same step */
+} UpkieBaseVelocityPost;
+int upkie_b200_base_velocity_post(void* handle, void* mpc, const UpkieBaseVelocityPost* args, void* stream);
+
 /* ---- observer pipeline handle --------------------------------------------
  * Replaces the spine's BaseOrientation -> FloorContact -> WheelOdometry observers
  * (upkie/cpp/observers/, spines/common/observers.h:23-44) for N robots: one call

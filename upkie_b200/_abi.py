@@ -334,6 +334,22 @@ class UpkieStepOutputs(C.Structure):
     ]
 
 
+class UpkieBaseVelocityPost(C.Structure):
+    """``UpkieBaseVelocityPost`` of include/upkie_b200.h: the buffers of ``upkie_b200_base_velocity_post``."""
+
+    _fields_ = [
+        ("action", C.c_void_p),
+        ("gyropod_obs", C.c_void_p),
+        ("gyropod_final_obs", C.c_void_p),
+        ("xy", C.c_void_p),
+        ("commanded_velocity", C.c_void_p),
+        ("obs", C.c_void_p),
+        ("final_obs", C.c_void_p),
+        ("dt", C.c_float),
+        ("autoreset_mode", C.c_int32),
+    ]
+
+
 def default_mpc_config() -> UpkieMpcConfig:
     """``MPCBalancer.__init__`` defaults (``mpc_balancer.py:168-181``)."""
     c = UpkieMpcConfig()

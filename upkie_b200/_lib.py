@@ -77,6 +77,7 @@ SYMBOLS = {
     "upkie_b200_mpc_reset": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_mpc_step": (C.c_int, [_vp, _vp, _vp, _vp, C.c_float, _vp, _vp, _vp, _vp]),
     "upkie_b200_mpc_plan": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_base_velocity_post": (C.c_int, [_vp, _vp, C.POINTER(_abi.UpkieBaseVelocityPost), _vp]),
     "upkie_b200_default_observer_config": (C.c_int, [C.POINTER(_abi.UpkieModel), C.POINTER(_abi.UpkieObserverConfig)]),
     "upkie_b200_observers_create": (C.c_int, [C.POINTER(_abi.UpkieObserverConfig), C.c_int, C.c_int, C.POINTER(_vp)]),
     "upkie_b200_observers_destroy": (None, [_vp]),

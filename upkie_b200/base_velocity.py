@@ -1,16 +1,19 @@
 # SPDX-License-Identifier: Apache-2.0
 """``UpkieBaseVelocity`` glue (``upkie/envs/upkie_base_velocity.py:164-202``) as device-agnostic tensor code.
 
-The env is an MPC balancer in front of the gyropod env plus dead reckoning. The three heavy pieces (MPC solve,
-gyropod step, spine observation) are passed in as callables: ``B200VectorEnv`` binds the CUDA kernels, the CPU tests
-bind the oracle -- the SAME ordering logic runs in both, and is pinned on golden runs of the reference's own class
-(``tests/test_base_velocity_golden.py``).
+The env is an MPC balancer in front of the gyropod env plus dead reckoning. ``base_velocity_tick`` states the
+reference's ordering with the three heavy pieces (MPC solve, gyropod step, spine observation) passed in as
+callables; the CPU tests bind the oracle and pin it on golden runs of the reference's own class
+(``tests/test_base_velocity_golden.py``). ``B200VectorEnv`` runs the same ordering on the GPU with its epilogue (dead
+reckoning, observation, and the auto-resets' ``UpkieBaseVelocity.reset``) in one kernel, ``base_velocity_post``.
 """
-from typing import Callable, Tuple
+import ctypes as C
+from typing import Callable, Optional, Tuple
 
 import torch
 
 from . import _abi
+from ._lib import check, lib
 
 
 def mpc_inputs_from_spine(spine_obs: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
@@ -54,3 +57,34 @@ def base_velocity_tick(
     xy[:, 1] += linear_velocity * torch.sin(yaw) * dt
     obs = torch.cat([xy, yaw[:, None]], dim=1)
     return obs, rew, term, trunc, new_spine
+
+
+def _addr(t: Optional[torch.Tensor]):
+    return None if t is None else t.data_ptr()
+
+
+def base_velocity_post(sim, mpc_balancer, action: torch.Tensor, gyro_obs: torch.Tensor, xy: torch.Tensor, dt: float,
+                       obs: torch.Tensor, autoreset_mode: int, gyro_final_obs: Optional[torch.Tensor] = None,
+                       final_obs: Optional[torch.Tensor] = None) -> None:
+    """``upkie_b200_base_velocity_post`` (``k_base_velocity_post``): the end of ``base_velocity_tick`` in one launch,
+    after ``sim``'s gyropod step and spine observation. Envs that did not reset in this tick dead-reckon ``xy`` (in
+    place) with the commanded linear velocity ``action[:, 0]`` along the post-step yaw ``gyro_obs[:, 2]`` and return
+    ``[x, y, yaw]`` in ``obs[N, 3]``, with the bits of ``base_velocity_tick``'s torch arithmetic. Envs that a fused
+    auto-reset of this tick re-initialised get ``UpkieBaseVelocity.reset`` (``upkie_base_velocity.py:137-162``):
+    ``x = y = 0``, observation ``[0, 0, 0]``, ``mpc_balancer.commanded_velocity`` 0 and no warm start; in same-step mode
+    (``autoreset_mode`` 2) they first store the ``[x, y, yaw]`` they reached, with the pre-reset yaw
+    ``gyro_final_obs[:, 2]``, into ``final_obs[N, 3]`` (other rows untouched)."""
+    n = sim.n
+    sim._check_tensor(action, (n, 2), name="action")
+    sim._check_tensor(gyro_obs, (n, 6), name="gyro_obs")
+    sim._check_tensor(xy, (n, 2), name="xy")
+    sim._check_tensor(obs, (n, 3), name="obs")
+    sim._check_tensor(mpc_balancer.commanded_velocity, (n,), name="commanded_velocity")
+    if gyro_final_obs is not None:
+        sim._check_tensor(gyro_final_obs, (n, 6), name="gyro_final_obs")
+    if final_obs is not None:
+        sim._check_tensor(final_obs, (n, 3), name="final_obs")
+    args = _abi.UpkieBaseVelocityPost(
+        _addr(action), _addr(gyro_obs), _addr(gyro_final_obs), _addr(xy), _addr(mpc_balancer.commanded_velocity),
+        _addr(obs), _addr(final_obs), float(dt), int(autoreset_mode))
+    check(lib().upkie_b200_base_velocity_post(sim._h, mpc_balancer._h, C.byref(args), sim._stream()))

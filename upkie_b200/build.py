@@ -10,8 +10,8 @@ LIB_PATH = os.path.join(_HERE, "libupkie_b200.so")
 # compiled in parallel, then linked
 SOURCES = ["upkie_b200.cu", "step_device.cu", "step_host.cu", "step_multicast.cu", "step_device_limits.cu",
            "step_host_limits.cu", "step_multicast_limits.cu", "step_device_spine.cu", "step_host_spine.cu",
-           "step_device_body.cu", "step_host_body.cu", "step_device_table.cu", "step_host_table.cu"]
-DEPS = SOURCES + [
+           "step_device_body.cu", "step_host_body.cu", "step_device_table.cu", "step_host_table.cu", "base_velocity.cu"]
+DEPS = SOURCES + ["base_velocity.cuh", "base_velocity_core.cuh",
     "sim_core.cuh", "sim_pair.cuh", "kernel_common.cuh", "step_kernel.cuh", "params.h", "mpc.cuh", "mpc_core.cuh",
     "observers.cuh", "observers_core.cuh", "controllers.cuh", "controllers_core.cuh", "../../include/upkie_b200.h",
 ]
@@ -24,6 +24,13 @@ NVCC_FLAGS = GENCODE + [
     "--use_fast_math",
     "-Xcompiler", "-fPIC",
 ]
+# translation units built without --use_fast_math: the base-velocity epilogue reproduces torch's IEEE cos / sin and
+# unfused fp32 products bit for bit (csrc/base_velocity_core.cuh)
+IEEE_SOURCES = {"base_velocity.cu"}
+
+
+def _flags(src: str, flags: list) -> list:
+    return [f for f in flags if f != "--use_fast_math"] if src in IEEE_SOURCES else flags
 
 
 def source_hash() -> str:
@@ -53,7 +60,7 @@ def is_stale() -> bool:
 # tests/test_gpu_exact_mode.py and bench.py's `exact_mode` line: what the one shortcut of the timed kernel (fast-math)
 # costs in accuracy and buys in time.
 EXACT_LIB_PATH = os.path.join(_HERE, "libupkie_b200_exact.so")
-EXACT_SOURCES = ["upkie_b200.cu", "step_device.cu", "step_device_limits.cu", "exact_stubs.cu"]
+EXACT_SOURCES = ["upkie_b200.cu", "step_device.cu", "step_device_limits.cu", "exact_stubs.cu", "base_velocity.cu"]
 EXACT_FLAGS = [f for f in NVCC_FLAGS if f != "--use_fast_math"] + ["-DUPKIE_EXACT_BUILD=1"]
 
 
@@ -94,7 +101,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     for src in SOURCES:
         obj = os.path.join(objdir, os.path.splitext(src)[0] + ".o")
         objs.append(obj)
-        procs.append(subprocess.Popen([nvcc] + flags + ["-c", "-o", obj, os.path.join(CSRC, src)]))
+        procs.append(subprocess.Popen([nvcc] + _flags(src, flags) + ["-c", "-o", obj, os.path.join(CSRC, src)]))
     failed = [src for src, p in zip(SOURCES, procs) if p.wait() != 0]
     if failed:
         raise RuntimeError(f"nvcc failed on {failed}")

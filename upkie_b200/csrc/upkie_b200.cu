@@ -10,7 +10,7 @@
 //                  fused auto-reset.
 //   k_reset        masked reset: set state, one physics substep, observe.
 //   k_spine_obs / k_reset_obs / k_get_state / k_set_state   layout helpers.
-// MPC kernels live in mpc.cuh.
+// MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
 // CUDA device and fails with UPKIE_B200_ECUDA otherwise.
@@ -24,6 +24,7 @@
 #include <string>
 
 #include "mpc.cuh"
+#include "base_velocity.cuh"
 #include "controllers.cuh"
 #include "observers.cuh"
 #include "kernel_common.cuh"
@@ -57,6 +58,7 @@ struct Handle {
   uint32_t* err = nullptr;     // [n]
   uint8_t* done_prev = nullptr;  // [n]
   uint32_t* episode = nullptr;   // [n]
+  uint32_t* bv_episode = nullptr;  // [n] episode as of the last upkie_b200_base_velocity_post: which envs reset since
   uint32_t* tick = nullptr;      // [n] env ticks since create: counter of the noise generator
   uint32_t* elapsed = nullptr;   // [n] agent steps since the env's last reset (config.max_episode_steps)
   float* ext = nullptr;          // [7 * 3][n_pad] external forces, null = none
@@ -571,6 +573,8 @@ int upkie_b200_create(const UpkieModel* model, const UpkieSimConfig* config, int
   if (e == cudaSuccess) e = cudaMemset(h->err, 0, size_t(n_envs) * sizeof(uint32_t));
   if (e == cudaSuccess) e = cudaMemset(h->done_prev, 0, size_t(n_envs));
   if (e == cudaSuccess) e = cudaMemset(h->episode, 0, size_t(n_envs) * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMalloc(&h->bv_episode, size_t(n_envs) * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaMemset(h->bv_episode, 0, size_t(n_envs) * sizeof(uint32_t));
   if (e == cudaSuccess && h->P.spine_mode) {
     e = cudaMalloc(&h->lag, size_t(UPKIE_LAG_DIM) * h->n_pad * sizeof(float));
     if (e == cudaSuccess) e = cudaMemset(h->lag, 0, size_t(UPKIE_LAG_DIM) * h->n_pad * sizeof(float));
@@ -605,6 +609,7 @@ void upkie_b200_destroy(void* handle) {
   if (!h) return;
   cudaSetDevice(h->device);
   cudaFree(h->state); cudaFree(h->eps); cudaFree(h->mu); cudaFree(h->err); cudaFree(h->done_prev); cudaFree(h->episode);
+  cudaFree(h->bv_episode);
   cudaFree(h->tick); cudaFree(h->elapsed); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
   cudaFree(h->env_params); cudaFree(h->ep_check);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
@@ -758,6 +763,9 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
   k_reset<<<grid, rblock, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
                                     h->done_prev, h->episode, seed, env_offset, h->lag);
   CUDA_TRY(cudaGetLastError());
+  // a reset sampled on the device counts an episode: it is not one the base-velocity post step has to carry out
+  if (!init_state)
+    CUDA_TRY(cudaMemcpyAsync(h->bv_episode, h->episode, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   return UPKIE_B200_OK;
 }
 
@@ -1071,7 +1079,11 @@ int upkie_b200_set_counters(void* handle, const uint32_t* episode, const uint32_
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t n = size_t(h->n);
-  if (episode) CUDA_TRY(cudaMemcpyAsync(h->episode, episode, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  if (episode) {
+    CUDA_TRY(cudaMemcpyAsync(h->episode, episode, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+    // restored counters are not resets for the base-velocity post step
+    CUDA_TRY(cudaMemcpyAsync(h->bv_episode, episode, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  }
   if (tick) CUDA_TRY(cudaMemcpyAsync(h->tick, tick, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   if (pending_reset) CUDA_TRY(cudaMemcpyAsync(h->done_prev, pending_reset, n, cudaMemcpyDeviceToDevice, s));
   if (error_flags) CUDA_TRY(cudaMemcpyAsync(h->err, error_flags, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
@@ -1121,6 +1133,47 @@ int upkie_b200_mpc_plan(void* mpc, float* plan, void* stream) {
   std::string err;
   int rc = mpc_plan_impl(mpc, plan, static_cast<cudaStream_t>(stream), err);
   return rc ? fail(rc, err) : UPKIE_B200_OK;
+}
+
+// ---- UpkieBaseVelocity epilogue -------------------------------------------------------------
+
+int upkie_b200_base_velocity_post(void* handle, void* mpc, const UpkieBaseVelocityPost* args, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "base_velocity_post: invalid sim handle");
+  MpcHandle* m = as_mpc(mpc);
+  if (!m) return fail(UPKIE_B200_EINVAL, "base_velocity_post: invalid mpc handle");
+  if (!args) return fail(UPKIE_B200_EINVAL, "base_velocity_post: null arguments");
+  if (m->n != h->n || m->device != h->device)
+    return fail(UPKIE_B200_EINVAL, "base_velocity_post: the mpc handle must hold as many robots as the sim handle has "
+                                   "envs, on the same device");
+  const UpkieBaseVelocityPost& a = *args;
+  if (!a.action || !a.gyropod_obs || !a.xy || !a.commanded_velocity || !a.obs)
+    return fail(UPKIE_B200_EINVAL, "base_velocity_post: null buffer");
+  if (!(a.dt > 0.f) || !std::isfinite(a.dt)) return fail(UPKIE_B200_EINVAL, "base_velocity_post: dt must be > 0 and finite");
+  if (a.autoreset_mode != h->autoreset)
+    return fail(UPKIE_B200_EINVAL, "base_velocity_post: autoreset_mode differs from the sim handle's "
+                                   "(upkie_b200_set_autoreset)");
+  const bool same_step = a.autoreset_mode == AUTORESET_SAME_STEP;
+  if (same_step && (!a.gyropod_final_obs || !a.final_obs))
+    return fail(UPKIE_B200_EINVAL, "base_velocity_post: same-step mode needs gyropod_final_obs and final_obs");
+  BaseVelocityPostArgs k;
+  k.n = h->n;
+  k.detect_resets = a.autoreset_mode != AUTORESET_DISABLED;
+  k.same_step = same_step;
+  k.dt = a.dt;
+  k.action = a.action;
+  k.gyro_obs = a.gyropod_obs;
+  k.gyro_final_obs = same_step ? a.gyropod_final_obs : nullptr;
+  k.episode = h->episode;
+  k.seen_episode = h->bv_episode;
+  k.xy = a.xy;
+  k.v_cmd = a.commanded_velocity;
+  k.active = m->active;
+  k.obs = a.obs;
+  k.final_obs = same_step ? a.final_obs : nullptr;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(launch_base_velocity_post(k, static_cast<cudaStream_t>(stream)));
+  return UPKIE_B200_OK;
 }
 
 // ---- observer pipeline --------------------------------------------------------------------

@@ -25,7 +25,7 @@ import numpy as np
 import torch
 
 from . import _abi
-from .base_velocity import base_velocity_tick
+from .base_velocity import base_velocity_post
 from .exceptions import UpkieException, UpkieRuntimeError
 from .gym_compat import VectorEnv, batch_space, spaces
 from .model import Model, default_model
@@ -363,7 +363,9 @@ class B200VectorEnv(VectorEnv):
     each resetting env reached before its reset, and ``info["_final_obs"]``, the bool mask of those envs
     (``terminated | truncated``). Unlike ``SyncVectorEnv``'s per-env object array, ``final_obs`` is dense batched
     storage with the observation's structure (servo dictionary of arrays, array, or CUDA tensor from
-    ``step_tensors``): rows outside the mask hold stale values. ``copy=True`` copies it as it copies the
+    ``step_tensors``): rows outside the mask hold stale values. ``base_velocity`` envs (``UpkieBaseVelocity``) take all three
+    modes: their ``final_obs`` is the ``[x, y, yaw]`` an env reached, and a reset (fused or through ``reset_mask``)
+    also zeroes that env's ``x, y`` and drops its MPC balancer's state. ``copy=True`` copies it as it copies the
     observation. ``info["final_info"]`` (the terminal step's spine observation) is not provided.
 
     Domain randomisation of the actuators: ``torque_control_kp`` / ``torque_control_kd`` take a float or an ``[N]``
@@ -458,8 +460,6 @@ class B200VectorEnv(VectorEnv):
                 max_ground_velocity, max_yaw_velocity
             )
         elif env_type == "base_velocity":
-            if autoreset_mode != "disabled":
-                raise UpkieException("base_velocity envs support autoreset_mode='disabled' only")
             self.single_action_space, self.single_observation_space = make_base_velocity_spaces(
                 max_ground_velocity, max_yaw_velocity
             )
@@ -483,6 +483,7 @@ class B200VectorEnv(VectorEnv):
             )
             self._xy = torch.zeros((self.num_envs, 2), dtype=torch.float32, device=self.sim.device)
             self._spine = None
+            self._bv_obs = None  # the observation the last step / reset returned (device), None = zeros
         self.sim.set_autoreset(_AUTORESET[autoreset_mode], self._seed, self.env_offset)
         self.inertia_variation = inertia_variation
         if abs(inertia_variation) > 1e-10:
@@ -613,11 +614,21 @@ class B200VectorEnv(VectorEnv):
         )
         info = {"spine_observation": SpineObservations(self.sim)}
         if self.env_type == "base_velocity":
-            # UpkieBaseVelocity.reset (upkie_base_velocity.py:138-162): MPC reset, x = y = 0, zero observation
-            self.mpc_balancer.reset()
-            self._xy.zero_()
+            # UpkieBaseVelocity.reset (upkie_base_velocity.py:137-162) of the reset envs: MPC reset, x = y = 0, zero
+            # observation; the other envs keep their state and their last observation
+            if mask is None:
+                self.mpc_balancer.reset()
+                self._xy.zero_()
+                obs = torch.zeros((n, 3), dtype=torch.float32, device=dev)
+            else:
+                m = torch.from_numpy(mask).to(dev)
+                self.mpc_balancer.reset(m)
+                self._xy.masked_fill_(m.bool()[:, None], 0.0)
+                obs = torch.zeros((n, 3), dtype=torch.float32, device=dev) if self._bv_obs is None else self._bv_obs.clone()
+                obs.masked_fill_(m.bool()[:, None], 0.0)
             self._spine = self.sim.spine_obs()
-            return np.zeros((n, 3), dtype=np.float32), info
+            self._bv_obs = obs
+            return obs.cpu().numpy(), info
         obs = self.sim.reset_obs(self._obs_dim()).cpu().numpy()
         return self._format_obs(obs), info
 
@@ -631,6 +642,9 @@ class B200VectorEnv(VectorEnv):
         if self.env_type == "base_velocity":
             a = torch.from_numpy(np.ascontiguousarray(np.asarray(action, dtype=np.float32).reshape(n, 2))).to(self.sim.device)
             obs, rew, term, trunc, info = self.step_tensors(a)
+            if "final_obs" in info:  # host copies, as the other env types' host path returns them
+                info["final_obs"] = info["final_obs"].cpu().numpy()
+                info["_final_obs"] = info["_final_obs"].cpu().numpy()
             return obs.cpu().numpy(), rew.cpu().numpy(), term.cpu().numpy().view(np.bool_), trunc.cpu().numpy().view(np.bool_), info
         if self.env_type == "servos":
             a = (
@@ -703,15 +717,7 @@ class B200VectorEnv(VectorEnv):
         elif self.env_type == "gyropod":
             obs, rew, term, trunc = self.sim.step_gyropod(action, final_obs=fin)
         elif self.env_type == "base_velocity":
-            # UpkieBaseVelocity.step (upkie_base_velocity.py:164-202): the MPC turns the commanded linear
-            # velocity into a ground velocity from the LAST spine observation, the gyropod env is stepped,
-            # (x, y) dead-reckon the commanded velocity along the post-step yaw
-            if self._spine is None:
-                self._spine = self.sim.spine_obs()
-            obs, rew, term, trunc, self._spine = base_velocity_tick(
-                action, self._spine, self._xy, self.dt, self.mpc_balancer.step_spine, self.sim.step_gyropod,
-                self.sim.spine_obs,
-            )
+            obs, rew, term, trunc = self._base_velocity_step(action, fin)
         else:
             obs, rew, term, trunc = self.sim.step_pendulum(action, final_obs=fin)
         info = {"spine_observation": SpineObservations(self.sim)}
@@ -719,10 +725,38 @@ class B200VectorEnv(VectorEnv):
         self._add_final_obs(info, term, trunc, fin, lambda f: f)
         return obs, rew, term, trunc, info
 
+    def _base_velocity_step(self, action: torch.Tensor, fin: Optional[torch.Tensor]):
+        """``UpkieBaseVelocity.step`` (``upkie_base_velocity.py:164-202``) in ``base_velocity_tick``'s order: the MPC
+        turns the commanded linear velocity into a ground velocity from the LAST spine observation, the gyropod env
+        is stepped (with its fused auto-reset), then one ``base_velocity_post`` launch dead-reckons (x, y) along the
+        post-step yaw and carries out ``UpkieBaseVelocity.reset`` for the envs that reset in this tick. In next-step
+        mode the MPC of a reset step runs on the terminal spine observation; the reset discards its result."""
+        n = self.num_envs
+        action = action.contiguous()
+        self.sim._check_tensor(action, (n, 2), name="action")
+        if self._spine is None:
+            self._spine = self.sim.spine_obs()
+        linear_velocity = action[:, 0].contiguous()
+        ground_velocity = self.mpc_balancer.step_spine(linear_velocity, self._spine, self.dt)
+        gyro_action = torch.stack([ground_velocity, action[:, 1]], dim=1).contiguous()
+        fin6 = None
+        if fin is not None:
+            fin6 = getattr(self, "_gyro_final_obs", None)
+            if fin6 is None:
+                fin6 = self._gyro_final_obs = torch.zeros((n, 6), dtype=torch.float32, device=self.sim.device)
+        obs6, rew, term, trunc = self.sim.step_gyropod(gyro_action, final_obs=fin6)
+        self._spine = self.sim.spine_obs()  # after a same-step reset: the reset's spine observation
+        obs = torch.empty((n, 3), dtype=torch.float32, device=self.sim.device)  # a new tensor per step, as before
+        base_velocity_post(self.sim, self.mpc_balancer, action, obs6, self._xy, self.dt, obs,
+                           _AUTORESET[self.autoreset_mode], fin6, fin)
+        self._bv_obs = obs
+        return obs, rew, term, trunc
+
     def _device_final_obs(self) -> torch.Tensor:
         """Device final-observation rows of the same-step auto-reset, in the observation's layout (reused)."""
         fin = getattr(self, "_final_obs_tensor", None)
         if fin is None:
-            shape = {"servos": (self.num_envs, 6, 5), "gyropod": (self.num_envs, 6), "pendulum": (self.num_envs, 4)}
+            shape = {"servos": (self.num_envs, 6, 5), "gyropod": (self.num_envs, 6), "pendulum": (self.num_envs, 4),
+                     "base_velocity": (self.num_envs, 3)}
             fin = self._final_obs_tensor = torch.zeros(shape[self.env_type], dtype=torch.float32, device=self.sim.device)
         return fin
