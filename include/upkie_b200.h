@@ -530,15 +530,19 @@ int upkie_b200_step_servos_host_compact(void* handle, const float* action,
  * final_obs (same-step auto-reset only; ignored in the other modes): every env that resets in this step first
  * stores there, at its own row, the observation it would have returned without the reset (layout of `obs`; spine
  * mode: the rows its spine assembled before the reset). The rows of the other envs are left untouched: mask them
- * with terminated | truncated (Gymnasium's info["final_obs"] / info["_final_obs"]). */
+ * with terminated | truncated (Gymnasium's info["final_obs"] / info["_final_obs"]).
+ * final_state (same-step auto-reset only; ignored in the other modes): 1 = every env that resets in this step also
+ * stashes its pre-reset state in the handle, from which upkie_b200_final_spine_obs computes the spine observation of
+ * the terminal step. The stash stays in device memory, for host buffers too. The field was a reserved pad (0) before:
+ * the struct's layout is unchanged, and so is the ABI version. The in-kernel rollout transports have no such flag. */
 typedef struct UpkieStepOutputs {
   float* obs;
   float* reward;
   uint8_t* terminated;
   uint8_t* truncated;
   float* final_obs;
-  int32_t compact;  /* UpkieServos: 1 = compact rows [6][3] (position, velocity, torque) */
-  int32_t reserved;
+  int32_t compact;      /* UpkieServos: 1 = compact rows [6][3] (position, velocity, torque) */
+  int32_t final_state;  /* 1 = stash the pre-reset states of this step's same-step auto-resets */
 } UpkieStepOutputs;
 /* device buffers, asynchronous on `stream` */
 int upkie_b200_step(void* handle, int act_dim, const float* action, const UpkieStepOutputs* out, void* stream);
@@ -549,6 +553,17 @@ int upkie_b200_step_host(void* handle, int act_dim, const float* action, const U
 /* Replaces PyBulletBackend.get_spine_observation without side effects: returns
  * the observation assembled by the last reset/step. out[N][UPKIE_SPINE_DIM]. */
 int upkie_b200_spine_obs(void* handle, float* out, void* stream);
+/* Spine observation of the terminal step of a same-step auto-reset (Gymnasium's info["final_info"]): for every env that
+ * reset in the last step, out[i] (device buffer [N][UPKIE_SPINE_DIM]) receives exactly what upkie_b200_spine_obs would
+ * have returned after that step had the env not reset: the post-step state's observation with the same torque
+ * measurement noise and IMU uncertainty (same noise keys, same row of the per-env parameter table), in spine mode the
+ * observation of the pre-reset lag record. The rows of the other envs are left untouched. Needs the last call that
+ * advanced or reset the simulator to be an upkie_b200_step / upkie_b200_step_host in same-step mode with
+ * final_state = 1; otherwise (a step without the flag, any other step call, upkie_b200_reset, set_state, set_lag,
+ * set_counters, set_elapsed, set_config, set_env_params, set_autoreset) it returns UPKIE_B200_EINVAL. The handle knows
+ * which envs stashed in that step: each step with the flag has a number, which a resetting env writes to its column of
+ * the stash. An addition to ABI 8: no existing layout, constant or signature changed. */
+int upkie_b200_final_spine_obs(void* handle, float* out, void* stream);
 
 /* Gyropod observation after a reset (upkie_gyropod.py:216-244): obs[N][obs_dim],
  * obs_dim 6 (gyropod) or 4 (pendulum); servo observation obs[N][6][5] for

@@ -330,7 +330,7 @@ class UpkieStepOutputs(C.Structure):
         ("truncated", C.c_void_p),
         ("final_obs", C.c_void_p),
         ("compact", C.c_int32),
-        ("reserved", C.c_int32),
+        ("final_state", C.c_int32),  # 1 = stash the same-step auto-resets' pre-reset states (final_spine_obs)
     ]
 
 

@@ -53,6 +53,7 @@ SYMBOLS = {
     "upkie_b200_step": (C.c_int, [_vp, C.c_int, _vp, C.POINTER(_abi.UpkieStepOutputs), _vp]),
     "upkie_b200_step_host": (C.c_int, [_vp, C.c_int, _vp, C.POINTER(_abi.UpkieStepOutputs)]),
     "upkie_b200_spine_obs": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_final_spine_obs": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_reset_obs": (C.c_int, [_vp, C.c_int, _vp, _vp]),
     "upkie_b200_get_state": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_get_lag": (C.c_int, [_vp, _vp, _vp]),

@@ -62,6 +62,12 @@ __device__ __forceinline__ void store_state(float* __restrict__ st, int n_pad, i
   for (int k = 0; k < UPKIE_STATE_DIM; ++k) st[size_t(k) * n_pad + i] = r[k];
 }
 
+// Stash of the same-step auto-reset's pre-reset states (SimParams.final_state, upkie_b200_final_spine_obs), rows of
+// n_pad floats: the step number that last wrote the env's column (uint32 bits), the state (store_state layout), and in
+// spine mode the lag record (lag_to_row layout)
+constexpr int kFinalMarkRow = 0, kFinalStateRow = 1, kFinalLagRow = 1 + UPKIE_STATE_DIM;
+constexpr int kFinalRows = kFinalLagRow, kFinalRowsSpine = kFinalLagRow + UPKIE_LAG_DIM;
+
 // TILE=2 (rollout rows leave the GPU from inside the step kernel): n = 0 -> `obs` / `terminated` are NVSwitch multicast
 // addresses (multimem.st, the switch replicates the store into every GPU's buffer); n > 0 -> plain stores into the n
 // peer buffers listed here (peer-mapped symmetric memory over NVLink; the list includes this rank's own buffer).

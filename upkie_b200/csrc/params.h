@@ -254,6 +254,8 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.final_obs = nullptr;
   P.env_params = nullptr;
   P.env_params_stride = 0;
+  P.final_gen = 0;
+  P.final_state = nullptr;
   return 0;
 }
 

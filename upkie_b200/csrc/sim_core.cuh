@@ -126,6 +126,12 @@ struct SimParams {
   // any_* flags above say whether SOME env of the table has that noise.
   const float* env_params;
   int env_params_stride;
+  // same-step auto-reset, terminal spine observation (UpkieStepOutputs.final_state; set per launch, null = not
+  // requested): a resetting env stashes its pre-reset state in the handle's buffer final_state (rows kFinal* of
+  // kernel_common.cuh, n_pad floats each) and marks its column with final_gen, the number of the step.
+  // Appended after every other field, so that their offsets stay where the kernels read them.
+  uint32_t final_gen;
+  float* final_state;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the

@@ -77,6 +77,22 @@ __device__ __forceinline__ void store_final_obs(const SimParams& P, const RobotS
   }
 }
 
+// The pre-reset state of env `i`, stashed before the same-step auto-reset overwrites it (upkie_b200_final_spine_obs
+// turns it into the spine observation the env would have returned, k_final_spine_obs): the step's number in the mark
+// row, the state, and in spine mode the lag record. Per-thread stores on the reset branch only.
+template <bool SPINE>
+__device__ __forceinline__ void store_final_state(const SimParams& P, const RobotState& S, const SpineLag& L, int n_pad,
+                                                  int i) {
+  reinterpret_cast<uint32_t*>(P.final_state + size_t(kFinalMarkRow) * n_pad)[i] = P.final_gen;
+  store_state(P.final_state + size_t(kFinalStateRow) * n_pad, n_pad, i, S);
+  if (SPINE) {
+    float lr[UPKIE_LAG_DIM];
+    lag_to_row(L, lr);
+#pragma unroll
+    for (int k = 0; k < UPKIE_LAG_DIM; ++k) P.final_state[size_t(kFinalLagRow + k) * n_pad + i] = lr[k];
+  }
+}
+
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE=1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), and it is reused to transpose the observation rows on the way out.
@@ -262,6 +278,9 @@ __device__ __forceinline__ void step_env(
   if (AUTORESET == AUTORESET_SAME_STEP) {
     if (term || trunc) {
       if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, NOISE ? &nz : nullptr, TILE && compact, i, env_col);
+      // neither the reset below nor the rest of the tick writes tick[i] (written above, before the physics) or the
+      // parameter table, so the stash and those give the rows k_spine_obs would have returned without the reset
+      if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
       elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;

@@ -10,6 +10,7 @@
 //                  fused auto-reset.
 //   k_reset        masked reset: set state, one physics substep, observe.
 //   k_spine_obs / k_reset_obs / k_get_state / k_set_state   layout helpers.
+//   k_final_spine_obs   spine observations of the same-step auto-resets' terminal step, from the step kernel's stash.
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -84,6 +85,12 @@ struct Handle {
   float *d_act = nullptr, *d_obs = nullptr, *d_rew = nullptr;
   uint8_t *d_term = nullptr, *d_trunc = nullptr;
   float* h_fin = nullptr;        // pinned copy of a pageable final_obs buffer (allocated on first use)
+  // same-step terminal spine observations (UpkieStepOutputs.final_state, upkie_b200_final_spine_obs): the stash
+  // [kFinalRows or kFinalRowsSpine][n_pad] (allocated on the first request), the number of the last step that asked for
+  // it, and whether that step is the last call that advanced or reset the simulator
+  float* final_state = nullptr;
+  uint32_t final_gen = 0;
+  bool final_valid = false;
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -159,6 +166,36 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
   } else {
     RobotState S;
     load_state(state, n_pad, i, S);
+    float tq[6];
+    measured_torques(P, S, &nz, tq, i);
+    spine_observation(P, S, o, tq);
+  }
+  apply_imu_uncertainty(P, nz, o, i);
+#pragma unroll
+  for (int k = 0; k < UPKIE_SPINE_DIM; ++k) out[size_t(i) * UPKIE_SPINE_DIM + k] = o[k];
+}
+
+// The spine observation rows of the envs that reset in step `gen` (same-step auto-reset), from the states they stashed
+// before the reset (store_final_state): k_spine_obs's device functions in its order, with the same noise keys (tick[i],
+// which the reset leaves alone) and the same column of the parameter table. The rows of the other envs are left as
+// they are.
+__global__ void k_final_spine_obs(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ stash,
+                                  uint32_t gen, const uint32_t* __restrict__ tick, uint64_t env_offset,
+                                  float* __restrict__ out, int spine) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  if (reinterpret_cast<const uint32_t*>(stash + size_t(kFinalMarkRow) * n_pad)[i] != gen) return;
+  float o[UPKIE_SPINE_DIM];
+  const NoiseCtx nz{env_offset + uint64_t(i), tick[i]};
+  if (spine) {
+    float lr[UPKIE_LAG_DIM];
+    for (int k = 0; k < UPKIE_LAG_DIM; ++k) lr[k] = stash[size_t(kFinalLagRow + k) * n_pad + i];
+    SpineLag L;
+    lag_from_row(lr, L);
+    spine_observation_from_lag(P, L, o);
+  } else {
+    RobotState S;
+    load_state(stash + size_t(kFinalStateRow) * n_pad, n_pad, i, S);
     float tq[6];
     measured_torques(P, S, &nz, tq, i);
     spine_observation(P, S, o, tq);
@@ -264,10 +301,15 @@ int pick_block(const Handle* h, int cnt) {
 // envs [i0, i0 + cnt): all buffers are indexed by the env index of the handle. `tile` selects the
 // shared-memory-tile instantiation (host buffers), see kernel_common.cuh.
 // `final_obs`: rows of the same-step auto-resets' terminal observations (null = not requested): it travels in a copy of
-// the parameter block made for this launch only.
+// the parameter block made for this launch only, as does the stash of the pre-reset states when `final_state` is set
+// (prepare_final_state allocated it and numbered the step).
 int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float* obs, float* reward, uint8_t* term,
                uint8_t* trunc, cudaStream_t s, bool tile = false, bool persistent = true, bool compact = false,
-               bool multicast = false, const PeerPtrs* peers = nullptr, float* final_obs = nullptr) {
+               bool multicast = false, const PeerPtrs* peers = nullptr, float* final_obs = nullptr,
+               bool final_state = false) {
+  h->final_valid = false;  // the simulator moves on: the caller marks the stash valid once the whole step is enqueued
+  if (multicast && final_state)
+    return fail(UPKIE_B200_EINVAL, "final_state has no in-kernel rollout transport (use upkie_b200_step)");
   if (multicast && h->P.env_params)
     return fail(UPKIE_B200_EINVAL, "the per-env parameter table has no in-kernel rollout transport (use upkie_b200_step "
                                    "with compact rows)");
@@ -278,9 +320,14 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   std::memset(&a.peers, 0, sizeof(a.peers));
   if (peers) a.peers = *peers;
   SimParams P_launch;
-  if (final_obs && h->autoreset == AUTORESET_SAME_STEP) {
+  const bool stash = final_state && h->final_state && h->autoreset == AUTORESET_SAME_STEP;
+  if ((final_obs || stash) && h->autoreset == AUTORESET_SAME_STEP) {
     P_launch = h->P;
     P_launch.final_obs = final_obs;
+    if (stash) {
+      P_launch.final_state = h->final_state;
+      P_launch.final_gen = h->final_gen;
+    }
     a.P = &P_launch;
   } else {
     a.P = &h->P;
@@ -330,6 +377,23 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   a.stream = s;
   CUDA_TRY(multicast ? launch_step_multicast(a) : (tile ? launch_step_host(a) : launch_step_device(a)));
   h->step_launches += 1;
+  return UPKIE_B200_OK;
+}
+
+// UpkieStepOutputs.final_state: whether this step stashes the pre-reset states (same-step mode only; the flag is
+// ignored in the other modes). The stash is allocated on the first request, so that a handle that never asks holds no
+// memory for it, and each such step gets a new number: the mark a resetting env leaves in its column of the stash.
+int prepare_final_state(Handle* h, int32_t flag, bool& stash) {
+  stash = flag != 0 && h->autoreset == AUTORESET_SAME_STEP;
+  if (!stash) return UPKIE_B200_OK;
+  if (!h->final_state) {
+    const size_t bytes = size_t(h->lag ? kFinalRowsSpine : kFinalRows) * h->n_pad * sizeof(float);
+    CUDA_TRY(cudaSetDevice(h->device));
+    CUDA_TRY(cudaMalloc(&h->final_state, bytes));
+    CUDA_TRY(cudaMemset(h->final_state, 0, bytes));
+    CUDA_TRY(cudaDeviceSynchronize());  // the marks are 0 before any stream's step reads them
+  }
+  if (++h->final_gen == 0) h->final_gen = 1;  // 0 is the mark of a column that no step has written
   return UPKIE_B200_OK;
 }
 
@@ -385,7 +449,7 @@ T* mapped(T* p) {
 // host memory through the mapped alias; a pageable buffer goes through a pinned copy of the caller's rows, so that
 // the rows of the envs that do not reset keep their values.
 int step_host(Handle* h, int mode, const float* action, float* obs, float* reward, uint8_t* term, uint8_t* trunc,
-              bool compact = false, float* final_obs = nullptr) {
+              bool compact = false, float* final_obs = nullptr, bool final_state = false) {
   if (!action || !obs || !term) return fail(UPKIE_B200_EINVAL, "step_host: null buffer");
   int rc = ensure_staging(h);
   if (rc) return rc;
@@ -453,14 +517,15 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
       cudaStream_t sk = h->host_streams[1 + (c % h->host_kernel_streams)];
       CUDA_TRY(cudaStreamWaitEvent(sk, h->host_events[c], 0));
       rc = step_range(h, mode, start[c], chunk_count(c), h->d_act, mapped(dst_obs), mapped(dst_rew), mapped(dst_term),
-                      mapped(dst_trunc), sk, /*tile=*/true, /*persistent=*/false, compact, false, nullptr, fin);
+                      mapped(dst_trunc), sk, /*tile=*/true, /*persistent=*/false, compact, false, nullptr, fin,
+                      final_state);
       if (rc) return rc;
     }
     for (int k = 0; k < h->host_kernel_streams; ++k) CUDA_TRY(cudaStreamSynchronize(h->host_streams[1 + k]));
   } else if (pipeline == 1) {
     cudaStream_t s = h->host_streams[0];
     rc = step_range(h, mode, 0, h->n, mapped(src_act), mapped(dst_obs), mapped(dst_rew), mapped(dst_term),
-                    mapped(dst_trunc), s, /*tile=*/true, /*persistent=*/true, compact, false, nullptr, fin);
+                    mapped(dst_trunc), s, /*tile=*/true, /*persistent=*/true, compact, false, nullptr, fin, final_state);
     if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(s));
   } else {
@@ -472,7 +537,7 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
                                size_t(cnt) * act_dim * sizeof(float), cudaMemcpyHostToDevice, s));
       // compact rows exist in the TILE=1 kernels only; device staging buffers either way
       rc = step_range(h, mode, i0, cnt, h->d_act, h->d_obs, h->d_rew, h->d_term, h->d_trunc, s, /*tile=*/compact,
-                      /*persistent=*/false, compact, false, nullptr, fin);
+                      /*persistent=*/false, compact, false, nullptr, fin, final_state);
       if (rc) return rc;
       CUDA_TRY(cudaMemcpyAsync(dst_obs + size_t(i0) * obs_dim, h->d_obs + size_t(i0) * obs_dim,
                                size_t(cnt) * obs_dim * sizeof(float), cudaMemcpyDeviceToHost, s));
@@ -611,7 +676,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->state); cudaFree(h->eps); cudaFree(h->mu); cudaFree(h->err); cudaFree(h->done_prev); cudaFree(h->episode);
   cudaFree(h->bv_episode);
   cudaFree(h->tick); cudaFree(h->elapsed); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
-  cudaFree(h->env_params); cudaFree(h->ep_check);
+  cudaFree(h->env_params); cudaFree(h->ep_check); cudaFree(h->final_state);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -630,6 +695,7 @@ int upkie_b200_num_envs(void* handle) {
 int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   Handle* h = as_handle(handle);
   if (!h || !config) return fail(UPKIE_B200_EINVAL, "set_config: invalid argument");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   SimParams P;
   std::memset(&P, 0, sizeof(P));
   std::string err;
@@ -668,6 +734,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
 int upkie_b200_set_env_params(void* handle, const float* rows, void* stream) {
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaSetDevice(h->device));
   if (!rows) {
@@ -722,6 +789,7 @@ int upkie_b200_set_autoreset(void* handle, int mode, uint64_t seed, uint64_t env
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
   if (mode < 0 || mode > 2) return fail(UPKIE_B200_EINVAL, "set_autoreset: mode must be 0 (disabled), 1 (next step) or 2 (same step)");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   h->autoreset = mode;
   h->seed = seed;
   h->env_offset = env_offset;
@@ -756,6 +824,7 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
                      void* stream) {
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int rblock = 128;
@@ -913,10 +982,15 @@ int upkie_b200_step(void* handle, int act_dim, const float* action, const UpkieS
   const bool compact = out->compact != 0;
   if (compact && mode != MODE_SERVOS) return fail(UPKIE_B200_EINVAL, "step: compact rows exist for servos only");
   CUDA_TRY(cudaSetDevice(h->device));
+  bool stash = false;
+  int rc = prepare_final_state(h, out->final_state, stash);
+  if (rc) return rc;
   // compact rows: the TILE=1 kernels on device buffers, as upkie_b200_step_servos_compact
-  return step_range(h, mode, 0, h->n, action, out->obs, out->reward, out->terminated, out->truncated,
-                    static_cast<cudaStream_t>(stream), /*tile=*/compact, /*persistent=*/false, compact, false, nullptr,
-                    out->final_obs);
+  rc = step_range(h, mode, 0, h->n, action, out->obs, out->reward, out->terminated, out->truncated,
+                  static_cast<cudaStream_t>(stream), /*tile=*/compact, /*persistent=*/false, compact, false, nullptr,
+                  out->final_obs, stash);
+  h->final_valid = rc == UPKIE_B200_OK && stash;
+  return rc;
 }
 
 int upkie_b200_step_host(void* handle, int act_dim, const float* action, const UpkieStepOutputs* out) {
@@ -927,7 +1001,12 @@ int upkie_b200_step_host(void* handle, int act_dim, const float* action, const U
   if (!out) return fail(UPKIE_B200_EINVAL, "step_host: null outputs");
   const bool compact = out->compact != 0;
   if (compact && mode != MODE_SERVOS) return fail(UPKIE_B200_EINVAL, "step_host: compact rows exist for servos only");
-  return step_host(h, mode, action, out->obs, out->reward, out->terminated, out->truncated, compact, out->final_obs);
+  bool stash = false;
+  int rc = prepare_final_state(h, out->final_state, stash);
+  if (rc) return rc;
+  rc = step_host(h, mode, action, out->obs, out->reward, out->terminated, out->truncated, compact, out->final_obs, stash);
+  h->final_valid = rc == UPKIE_B200_OK && stash;
+  return rc;
 }
 
 int upkie_b200_step_gyropod_host(void* handle, const float* action, int act_dim, float* obs, float* reward,
@@ -943,6 +1022,19 @@ int upkie_b200_spine_obs(void* handle, float* out, void* stream) {
   if (!h || !out) return fail(UPKIE_B200_EINVAL, "spine_obs: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
   k_spine_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, h->state, h->tick, h->env_offset, out, h->lag);
+  CUDA_TRY(cudaGetLastError());
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_final_spine_obs(void* handle, float* out, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !out) return fail(UPKIE_B200_EINVAL, "final_spine_obs: invalid argument");
+  if (!h->final_valid)
+    return fail(UPKIE_B200_EINVAL, "final_spine_obs: the last call that advanced or reset the simulator was not a "
+                                   "same-step auto-reset step with final_state = 1");
+  CUDA_TRY(cudaSetDevice(h->device));
+  k_final_spine_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
+      h->P, h->n, h->n_pad, h->final_state, h->final_gen, h->tick, h->env_offset, out, h->lag ? 1 : 0);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -969,6 +1061,7 @@ int upkie_b200_get_state(void* handle, float* state, void* stream) {
 int upkie_b200_set_state(void* handle, const float* state, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !state) return fail(UPKIE_B200_EINVAL, "set_state: invalid argument");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
   k_set_state<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->state, state);
   CUDA_TRY(cudaGetLastError());
@@ -1013,6 +1106,7 @@ int upkie_b200_set_lag(void* handle, const float* lag_rows, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !lag_rows) return fail(UPKIE_B200_EINVAL, "set_lag: invalid argument");
   if (!h->lag) return fail(UPKIE_B200_EINVAL, "set_lag: the handle was not created with spine_mode");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
   k_lag_copy<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->lag, const_cast<float*>(lag_rows), 0);
   CUDA_TRY(cudaGetLastError());
@@ -1076,6 +1170,7 @@ int upkie_b200_set_counters(void* handle, const uint32_t* episode, const uint32_
                             const uint32_t* error_flags, void* stream) {
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "set_counters: invalid handle");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t n = size_t(h->n);
@@ -1102,6 +1197,7 @@ int upkie_b200_get_elapsed(void* handle, uint32_t* elapsed, void* stream) {
 int upkie_b200_set_elapsed(void* handle, const uint32_t* elapsed, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !elapsed) return fail(UPKIE_B200_EINVAL, "set_elapsed: invalid argument");
+  h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaMemcpyAsync(h->elapsed, elapsed, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
                            static_cast<cudaStream_t>(stream)));

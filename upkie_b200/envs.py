@@ -161,23 +161,36 @@ class SpineObservations:
     """Lazy ``info["spine_observation"]``: fetched from the device on first use.
 
     ``obs[i]`` returns the reference's nested dictionary for env ``i``
-    (``pybullet_backend.py:325-331``); ``obs.array`` the flat ``[N, 62]`` array.
+    (``pybullet_backend.py:325-331``); ``obs.array`` the flat ``[N, 62]`` array,
+    ``obs.tensor`` the same rows as a CUDA tensor (no host copy).
     """
+
+    _key = "info['spine_observation']"
 
     def __init__(self, sim: UpkieSim):
         self._sim = sim
+        self._tensor = None
         self._array = None
         self._stamp = sim.launches  # step kernels launched so far: identifies the tick this object belongs to
+
+    def _fetch(self) -> torch.Tensor:
+        return self._sim.spine_obs()
+
+    @property
+    def tensor(self) -> torch.Tensor:
+        if self._tensor is None:
+            if self._sim.launches != self._stamp:
+                # the simulator has moved on: fetching now would silently return a LATER tick's observation
+                raise UpkieRuntimeError(
+                    f"{self._key} is fetched lazily and the simulator has been stepped since this step: "
+                    "read it (e.g. `.array`) before calling step() again")
+            self._tensor = self._fetch()
+        return self._tensor
 
     @property
     def array(self) -> np.ndarray:
         if self._array is None:
-            if self._sim.launches != self._stamp:
-                # the simulator has moved on: fetching now would silently return a LATER tick's observation
-                raise UpkieRuntimeError(
-                    "info['spine_observation'] is fetched lazily and the simulator has been stepped since this step: "
-                    "read it (e.g. `.array`) before calling step() again")
-            self._array = self._sim.spine_obs().cpu().numpy()
+            self._array = self.tensor.cpu().numpy()
         return self._array
 
     def __len__(self):
@@ -185,6 +198,18 @@ class SpineObservations:
 
     def __getitem__(self, i: int) -> dict:
         return spine_row_to_dict(self.array[i])
+
+
+class FinalSpineObservations(SpineObservations):
+    """Lazy ``info["final_info"]["spine_observation"]`` of a same-step auto-reset step: the spine observation of the
+    terminal step, row ``i`` for each env ``i`` that reset (``info["_final_info"]``), computed from the state the env
+    stashed before its reset (``UpkieSim.final_spine_obs``). Same access as ``SpineObservations``; rows outside the
+    mask are stale."""
+
+    _key = "info['final_info']['spine_observation']"
+
+    def _fetch(self) -> torch.Tensor:
+        return self._sim.final_spine_obs()
 
 
 def spine_row_to_dict(r: np.ndarray) -> dict:
@@ -366,7 +391,11 @@ class B200VectorEnv(VectorEnv):
     ``step_tensors``): rows outside the mask hold stale values. ``base_velocity`` envs (``UpkieBaseVelocity``) take all three
     modes: their ``final_obs`` is the ``[x, y, yaw]`` an env reached, and a reset (fused or through ``reset_mask``)
     also zeroes that env's ``x, y`` and drops its MPC balancer's state. ``copy=True`` copies it as it copies the
-    observation. ``info["final_info"]`` (the terminal step's spine observation) is not provided.
+    observation. The same step adds the terminal step's info in Gymnasium's layout: ``info["final_info"] =
+    {"spine_observation": ..., "_spine_observation": mask}`` and ``info["_final_info"] = mask``. Its
+    ``spine_observation`` is a lazy ``FinalSpineObservations``, the same kind of object as ``info["spine_observation"]``
+    (``[i]`` the reference's dictionary, ``.array``, ``.tensor``): for each env that reset, the spine observation the
+    step led to before the reset, which reward and termination wrappers read. Read it before the next ``step()``.
 
     Domain randomisation of the actuators: ``torque_control_kp`` / ``torque_control_kd`` take a float or an ``[N]``
     array, ``joint_properties`` a ``{joint: JointProperties}`` dict whose fields are floats or ``[N]`` arrays, or a
@@ -645,6 +674,9 @@ class B200VectorEnv(VectorEnv):
             if "final_obs" in info:  # host copies, as the other env types' host path returns them
                 info["final_obs"] = info["final_obs"].cpu().numpy()
                 info["_final_obs"] = info["_final_obs"].cpu().numpy()
+                info["_final_info"] = info["_final_info"].cpu().numpy()
+                fi = info["final_info"]
+                fi["_spine_observation"] = fi["_spine_observation"].cpu().numpy()
             return obs.cpu().numpy(), rew.cpu().numpy(), term.cpu().numpy().view(np.bool_), trunc.cpu().numpy().view(np.bool_), info
         if self.env_type == "servos":
             a = (
@@ -655,7 +687,8 @@ class B200VectorEnv(VectorEnv):
             hb = self.sim._host_buffers()
             fin = None
             if self._host_general_step():
-                obs18, term, trunc, fin = self.sim.step_host(a, 36, compact=True, final_obs=self._same_step())
+                obs18, term, trunc, fin = self.sim.step_host(a, 36, compact=True, final_obs=self._same_step(),
+                                                             final_state=self._same_step())
             else:
                 obs18, term, trunc = *self.sim.step_servos_host_compact(a), hb["trunc"]
             info = {"spine_observation": SpineObservations(self.sim)}
@@ -671,7 +704,7 @@ class B200VectorEnv(VectorEnv):
             a = np.ascontiguousarray(np.asarray(action, dtype=np.float32).reshape(n, d))
             fin = None
             if self._host_general_step():
-                obs, term, trunc, fin = self.sim.step_host(a, d, final_obs=self._same_step())
+                obs, term, trunc, fin = self.sim.step_host(a, d, final_obs=self._same_step(), final_state=self._same_step())
                 rew = self.sim._host_buffers()["rew"]
             else:
                 obs, rew, term, trunc = self.sim.step_gyropod_host(a)
@@ -691,35 +724,41 @@ class B200VectorEnv(VectorEnv):
         limit or the same-step auto-reset needs it; otherwise the calls that leave ``truncated`` on the host."""
         return self.config.max_episode_steps > 0 or self._same_step()
 
-    @staticmethod
-    def _add_final_obs(info: dict, term, trunc, fin, fmt) -> None:
-        """``info["final_obs"]`` / ``info["_final_obs"]`` when some env reset in this step (same-step mode)."""
+    def _add_final_obs(self, info: dict, term, trunc, fin, fmt) -> None:
+        """``info["final_obs"]`` / ``info["_final_obs"]`` and ``info["final_info"]`` / ``info["_final_info"]`` when
+        some env reset in this step (same-step mode, whose steps stash the pre-reset states)."""
         if fin is None:
             return
         if isinstance(term, torch.Tensor):
             mask = (term | trunc).bool()
             if not bool(mask.any()):
                 return
+            copy = torch.clone
         else:
             mask = (term | trunc).view(np.bool_)
             if not mask.any():
                 return
+            copy = np.copy
         info["final_obs"] = fmt(fin)
         info["_final_obs"] = mask
+        # Gymnasium 1.x SyncVectorEnv._add_info layout: a dict of the terminal infos, each key with its `_key` mask
+        info["final_info"] = {"spine_observation": FinalSpineObservations(self.sim), "_spine_observation": copy(mask)}
+        info["_final_info"] = copy(mask)
 
     def step_tensors(self, action: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor, dict]:
         """Zero-copy fast path: CUDA tensors in, CUDA tensors out
         (``action[N, 6, 6]`` / ``[N, 2]`` / ``[N, 1]``). In same-step mode ``info["final_obs"]`` is a CUDA tensor of
         the observation's shape and ``info["_final_obs"]`` a CUDA bool tensor."""
-        fin = self._device_final_obs() if self._same_step() else None
+        same = self._same_step()
+        fin = self._device_final_obs() if same else None
         if self.env_type == "servos":
-            obs, rew, term, trunc = self.sim.step_servos(action, final_obs=fin)
+            obs, rew, term, trunc = self.sim.step_servos(action, final_obs=fin, final_state=same)
         elif self.env_type == "gyropod":
-            obs, rew, term, trunc = self.sim.step_gyropod(action, final_obs=fin)
+            obs, rew, term, trunc = self.sim.step_gyropod(action, final_obs=fin, final_state=same)
         elif self.env_type == "base_velocity":
             obs, rew, term, trunc = self._base_velocity_step(action, fin)
         else:
-            obs, rew, term, trunc = self.sim.step_pendulum(action, final_obs=fin)
+            obs, rew, term, trunc = self.sim.step_pendulum(action, final_obs=fin, final_state=same)
         info = {"spine_observation": SpineObservations(self.sim)}
         # same-step mode: one host synchronisation per step decides whether some env reset
         self._add_final_obs(info, term, trunc, fin, lambda f: f)
@@ -744,7 +783,8 @@ class B200VectorEnv(VectorEnv):
             fin6 = getattr(self, "_gyro_final_obs", None)
             if fin6 is None:
                 fin6 = self._gyro_final_obs = torch.zeros((n, 6), dtype=torch.float32, device=self.sim.device)
-        obs6, rew, term, trunc = self.sim.step_gyropod(gyro_action, final_obs=fin6)
+        # same-step mode: the resetting envs also stash their terminal state (info["final_info"])
+        obs6, rew, term, trunc = self.sim.step_gyropod(gyro_action, final_obs=fin6, final_state=fin is not None)
         self._spine = self.sim.spine_obs()  # after a same-step reset: the reset's spine observation
         obs = torch.empty((n, 3), dtype=torch.float32, device=self.sim.device)  # a new tensor per step, as before
         base_velocity_post(self.sim, self.mpc_balancer, action, obs6, self._xy, self.dt, obs,

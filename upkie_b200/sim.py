@@ -180,10 +180,12 @@ class UpkieSim:
             self._check_tensor(truncated, (self.n,), torch.uint8, "truncated")
         return obs, reward, terminated, truncated
 
-    def _step(self, act_dim: int, action, obs, reward, terminated, truncated, final_obs, compact: bool = False):
-        """``upkie_b200_step``: the general device-buffer step (``truncated`` with compact rows, ``final_obs``)."""
+    def _step(self, act_dim: int, action, obs, reward, terminated, truncated, final_obs, compact: bool = False,
+              final_state: bool = False):
+        """``upkie_b200_step``: the general device-buffer step (``truncated`` with compact rows, ``final_obs``,
+        ``final_state``)."""
         out = _abi.UpkieStepOutputs(_addr(obs), _addr(reward), _addr(terminated), _addr(truncated), _addr(final_obs),
-                                    1 if compact else 0, 0)
+                                    1 if compact else 0, 1 if final_state else 0)
         check(lib().upkie_b200_step(self._h, int(act_dim), _ptr(action), C.byref(out), self._stream()))
 
     def _check_final_obs(self, final_obs: Optional[torch.Tensor], shape):
@@ -191,14 +193,16 @@ class UpkieSim:
             self._check_tensor(final_obs, shape, name="final_obs")
 
     def step_servos(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, reward=None, terminated=None,
-                    truncated=None, final_obs: Optional[torch.Tensor] = None):
+                    truncated=None, final_obs: Optional[torch.Tensor] = None, final_state: bool = False):
         """``final_obs[N, 6, 5]`` (same-step auto-reset): the envs that reset in this step first store there the
-        observation they reached; the other rows are left untouched (mask with ``terminated | truncated``)."""
+        observation they reached; the other rows are left untouched (mask with ``terminated | truncated``).
+        ``final_state=True`` (same-step auto-reset): they also stash their pre-reset state, whose spine observation
+        ``final_spine_obs()`` returns until the simulator moves on."""
         self._check_tensor(action, (self.n, 6, 6), name="action")
         obs, reward, terminated, truncated = self._outputs(obs, self.obs_servos, reward, terminated, truncated)
-        if final_obs is not None:
+        if final_obs is not None or final_state:
             self._check_final_obs(final_obs, (self.n, 6, 5))
-            self._step(36, action, obs, reward, terminated, truncated, final_obs)
+            self._step(36, action, obs, reward, terminated, truncated, final_obs, final_state=final_state)
             return obs, reward, terminated, truncated
         check(
             lib().upkie_b200_step_servos(
@@ -225,7 +229,8 @@ class UpkieSim:
         return obs, terminated
 
     def step_servos_compact_truncated(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, terminated=None,
-                                      truncated=None, final_obs: Optional[torch.Tensor] = None):
+                                      truncated=None, final_obs: Optional[torch.Tensor] = None,
+                                      final_state: bool = False):
         """``step_servos_compact`` that also returns ``truncated`` (the episode time limit, ``max_episode_steps``)
         and, in same-step auto-reset mode, fills the compact rows ``final_obs[N, 6, 3]`` of the envs that reset.
         Returns ``(obs, terminated, truncated)``."""
@@ -241,7 +246,7 @@ class UpkieSim:
         for name, t in (("terminated", terminated), ("truncated", truncated)):
             self._check_tensor(t, (self.n,), torch.uint8, name)
         self._check_final_obs(final_obs, (self.n, 6, 3))
-        self._step(36, action, obs, None, terminated, truncated, final_obs, compact=True)
+        self._step(36, action, obs, None, terminated, truncated, final_obs, compact=True, final_state=final_state)
         return obs, terminated, truncated
 
     def step_servos_multicast(self, action: torch.Tensor, obs_mc_ptr: int, terminated_mc_ptr: int) -> None:
@@ -274,12 +279,12 @@ class UpkieSim:
         check(lib().upkie_b200_push_rows(self._h, C.byref(push), self._stream()))
 
     def step_gyropod(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, reward=None, terminated=None,
-                     truncated=None, final_obs: Optional[torch.Tensor] = None):
+                     truncated=None, final_obs: Optional[torch.Tensor] = None, final_state: bool = False):
         self._check_tensor(action, (self.n, 2), name="action")
         obs, reward, terminated, truncated = self._outputs(obs, self.obs_gyropod, reward, terminated, truncated)
-        if final_obs is not None:
+        if final_obs is not None or final_state:
             self._check_final_obs(final_obs, (self.n, 6))
-            self._step(2, action, obs, reward, terminated, truncated, final_obs)
+            self._step(2, action, obs, reward, terminated, truncated, final_obs, final_state=final_state)
             return obs, reward, terminated, truncated
         check(
             lib().upkie_b200_step_gyropod(
@@ -289,12 +294,12 @@ class UpkieSim:
         return obs, reward, terminated, truncated
 
     def step_pendulum(self, action: torch.Tensor, obs: Optional[torch.Tensor] = None, reward=None, terminated=None,
-                      truncated=None, final_obs: Optional[torch.Tensor] = None):
+                      truncated=None, final_obs: Optional[torch.Tensor] = None, final_state: bool = False):
         self._check_tensor(action, (self.n, 1), name="action")
         obs, reward, terminated, truncated = self._outputs(obs, self.obs_pendulum, reward, terminated, truncated)
-        if final_obs is not None:
+        if final_obs is not None or final_state:
             self._check_final_obs(final_obs, (self.n, 4))
-            self._step(1, action, obs, reward, terminated, truncated, final_obs)
+            self._step(1, action, obs, reward, terminated, truncated, final_obs, final_state=final_state)
             return obs, reward, terminated, truncated
         check(
             lib().upkie_b200_step_gyropod(
@@ -391,12 +396,14 @@ class UpkieSim:
         )
         return obs, rew, term, trunc
 
-    def step_host(self, action: np.ndarray, act_dim: int, compact: bool = False, final_obs: bool = False):
+    def step_host(self, action: np.ndarray, act_dim: int, compact: bool = False, final_obs: bool = False,
+                  final_state: bool = False):
         """``upkie_b200_step_host``: host arrays, ``truncated`` written by the kernel on every path. ``act_dim`` 36
         (servos, ``compact`` = rows ``[N, 6, 3]``), 2 (gyropod) or 1 (pendulum). ``final_obs=True`` (same-step
         auto-reset): the envs that reset in this step also store the observation they reached into a pinned buffer
-        of the observation's layout; its other rows keep their values. Returns ``(obs, terminated, truncated,
-        final_obs or None)``: pinned arrays that the next ``*_host`` call overwrites."""
+        of the observation's layout; its other rows keep their values. ``final_state=True``: they stash their
+        pre-reset state in device memory (``final_spine_obs()``). Returns ``(obs, terminated, truncated, final_obs or
+        None)``: pinned arrays that the next ``*_host`` call overwrites."""
         hb = self._host_buffers()
         a = action
         if a.dtype != np.float32 or not a.flags["C_CONTIGUOUS"]:
@@ -406,7 +413,8 @@ class UpkieSim:
         dim = {36: 18 if compact else 30, 2: 6, 1: 4}[act_dim]
         obs, term, trunc = hb[f"obs{dim}"], hb["term"], hb["trunc_dev"]
         fin = self._host_final_obs(dim) if final_obs else None
-        out = _abi.UpkieStepOutputs(_addr(obs), None, _addr(term), _addr(trunc), _addr(fin), 1 if compact else 0, 0)
+        out = _abi.UpkieStepOutputs(_addr(obs), None, _addr(term), _addr(trunc), _addr(fin), 1 if compact else 0,
+                                    1 if final_state else 0)
         check(lib().upkie_b200_step_host(self._h, int(act_dim), a.ctypes.data, C.byref(out)))
         return obs, term, trunc, fin
 
@@ -422,6 +430,19 @@ class UpkieSim:
         """``get_spine_observation`` for all envs, flattened ``[N, 62]``."""
         out = torch.empty((self.n, _abi.SPINE_DIM), dtype=torch.float32, device=self.device)
         check(lib().upkie_b200_spine_obs(self._h, _ptr(out), self._stream()))
+        return out
+
+    def final_spine_obs(self, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Spine observations ``[N, 62]`` of the terminal step of the same-step auto-resets of the last step, which
+        must have been taken with ``final_state=True`` (Gymnasium's ``info["final_info"]``): row ``i`` of an env that
+        reset is what ``spine_obs()`` would have returned after that step without the reset. The other rows of
+        ``out`` (zeros when ``out`` is None) are left untouched. Raises once the simulator has been stepped or reset
+        again."""
+        if out is None:
+            out = torch.zeros((self.n, _abi.SPINE_DIM), dtype=torch.float32, device=self.device)
+        else:
+            self._check_tensor(out, (self.n, _abi.SPINE_DIM), name="out")
+        check(lib().upkie_b200_final_spine_obs(self._h, _ptr(out), self._stream()))
         return out
 
     def reset_obs(self, obs_dim: int) -> torch.Tensor:
