@@ -428,6 +428,44 @@ int upkie_b200_get_env_params(void* handle, float* rows, void* stream);
  * one per non-base body; mass and inertia scale by (1 + eps). */
 int upkie_b200_set_randomization(void* handle, const float* friction,
                                  const float* inertia_eps, void* stream);
+/* The randomisation in force: friction[N] and inertia_eps[N][6] (device pointers, either may be NULL). Without a
+ * buffer set, the nominal values: the config's friction, epsilon 0. An addition to ABI 8. */
+int upkie_b200_get_randomization(void* handle, float* friction, float* inertia_eps, void* stream);
+
+/* Reset randomisation (an addition to ABI 8: no existing layout, constant or signature changed). While a spec is set,
+ * every reset of an env - both fused auto-resets, and upkie_b200_reset with device-sampled or host init rows, masked or
+ * not - redraws the selected columns of that env on the device, each uniformly from [low, high]:
+ *   columns 0 .. UPKIE_EP_DIM - 1    the env's row of the per-env parameter table (UPKIE_EP_*),
+ *   UPKIE_RR_INERTIA + b (b < 6)     inertia_eps of body b + 1 (upkie_b200_set_randomization; randomize_inertias),
+ *   UPKIE_RR_FRICTION                the floor friction.
+ * Bit k of `columns` selects column k; the other columns keep their values bit for bit.
+ * Draw law: env i's draws are numbered 1, 2, ... by a per-env counter (upkie_b200_get_draws / set_draws); draw d of
+ * the env of global index g = env_offset + i is keyed on (seed, g, d), with the seed and env_offset of
+ * upkie_b200_set_autoreset: block b = 0 .. 8 of Philox4x32-10 with counter (g, 2^63 | d << 4 | b) and key seed gives
+ * the uniform words of columns 4b .. 4b + 3, u = (word >> 8) * 2^-24, value = min(low + (high - low) * u, high) in
+ * fp32, the product rounded on its own (no FMA). All 35 columns are always drawn. The values are in force from the
+ * env's reset substep on, as if set with upkie_b200_set_env_params / set_randomization just before the reset; the
+ * terminal observations of same-step auto-resets (final_obs, upkie_b200_final_spine_obs) still use the values of the
+ * episode that ended.
+ * Setting a spec gives the handle a parameter table (the config's values) and randomisation buffers (friction of the
+ * config, epsilon 0) if it has none; noise models that some range can turn on are switched on. Needs
+ * joint_limits != 0. Rejected with UPKIE_B200_EINVAL, the previous spec kept: a bound that is not finite, low > high,
+ * low < 0 on a gain, joint friction or noise standard deviation column, an inertia bound <= -1, a floor friction low < 0.
+ * While a spec is set, upkie_b200_set_env_params(NULL) and upkie_b200_set_randomization with a NULL pointer return
+ * UPKIE_B200_EINVAL (the draws write into those buffers). NULL turns reset randomisation off; the values then in force
+ * stay. The in-kernel rollout transports reject a handle with a parameter table, hence with this. */
+#define UPKIE_RR_INERTIA 28 /* [6] inertia_eps of the non-base bodies */
+#define UPKIE_RR_FRICTION 34 /* floor friction */
+#define UPKIE_RR_DIM 35
+typedef struct UpkieResetRandomization {
+  uint64_t columns;          /* bit k: column k is redrawn at every reset */
+  float low[UPKIE_RR_DIM];
+  float high[UPKIE_RR_DIM];
+} UpkieResetRandomization;
+int upkie_b200_set_reset_randomization(void* handle, const UpkieResetRandomization* spec);
+/* Per-env draw counters draws[N] (device pointers), for checkpoints: 0 = never drawn. */
+int upkie_b200_get_draws(void* handle, uint32_t* draws, void* stream);
+int upkie_b200_set_draws(void* handle, const uint32_t* draws, void* stream);
 
 /* Replaces UpkieEnv.reset -> PyBulletBackend.reset (upkie_env.py:162-194,
  * pybullet_backend.py:220-267): set state, ONE physics substep, observe.

@@ -13,4 +13,5 @@ g++ -O1 -g -std=c++17 -fPIC -shared -fsanitize=address,undefined -fno-omit-frame
 touch "$LIB"
 trap 'cp /tmp/libhostsim_plain.so "$LIB"; touch "$LIB"' EXIT
 ASAN_OPTIONS=detect_leaks=0 LD_PRELOAD="$(g++ -print-file-name=libasan.so):$(g++ -print-file-name=libubsan.so)" \
-  python -m pytest tests/test_kernel_arithmetic_cpu.py tests/test_controllers.py tests/test_observers.py tests/test_body_contacts.py tests/test_spine_mode.py -q -m "not gpu"
+  UPKIE_HOSTSIM_CXXFLAGS="-O1 -g -fsanitize=address,undefined -fno-omit-frame-pointer" \
+  python -m pytest tests/test_kernel_arithmetic_cpu.py tests/test_controllers.py tests/test_observers.py tests/test_body_contacts.py tests/test_spine_mode.py tests/test_reset_randomization_cpu.py -q -m "not gpu"

@@ -59,6 +59,8 @@ ST_FRICTION_IMPULSE = 46  # rolling / lateral friction impulses of the last subs
 EP_KP, EP_KD, EP_FRICTION, EP_CTRL_NOISE, EP_MEAS_NOISE = 0, 1, 2, 8, 14
 EP_IMU_ACC_BIAS, EP_IMU_ACC_NOISE, EP_IMU_GYRO_BIAS, EP_IMU_GYRO_NOISE = 20, 23, 24, 27
 EP_DIM = 28
+# reset randomisation (upkie_b200_set_reset_randomization): columns 0 .. EP_DIM - 1 are the table's, then UPKIE_RR_*
+RR_INERTIA, RR_FRICTION, RR_DIM = 28, 34, 35
 # spine observation offsets
 SP_BASE_ANGVEL, SP_BASE_LINVEL, SP_PITCH, SP_ROT = 0, 3, 6, 7
 SP_IMU_QUAT, SP_IMU_ANGVEL, SP_IMU_LINACC, SP_IMU_RAWACC = 16, 20, 23, 26
@@ -347,6 +349,16 @@ class UpkieBaseVelocityPost(C.Structure):
         ("final_obs", C.c_void_p),
         ("dt", C.c_float),
         ("autoreset_mode", C.c_int32),
+    ]
+
+
+class UpkieResetRandomization(C.Structure):
+    """``UpkieResetRandomization`` of include/upkie_b200.h: which columns every reset redraws, and their ranges."""
+
+    _fields_ = [
+        ("columns", C.c_uint64),  # bit k: column k is redrawn
+        ("low", C.c_float * RR_DIM),
+        ("high", C.c_float * RR_DIM),
     ]
 
 

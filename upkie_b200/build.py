@@ -10,7 +10,8 @@ LIB_PATH = os.path.join(_HERE, "libupkie_b200.so")
 # compiled in parallel, then linked
 SOURCES = ["upkie_b200.cu", "step_device.cu", "step_host.cu", "step_multicast.cu", "step_device_limits.cu",
            "step_host_limits.cu", "step_multicast_limits.cu", "step_device_spine.cu", "step_host_spine.cu",
-           "step_device_body.cu", "step_host_body.cu", "step_device_table.cu", "step_host_table.cu", "base_velocity.cu"]
+           "step_device_body.cu", "step_host_body.cu", "step_device_table.cu", "step_host_table.cu", "base_velocity.cu",
+           "reset_randomization.cu"]
 DEPS = SOURCES + ["base_velocity.cuh", "base_velocity_core.cuh",
     "sim_core.cuh", "sim_pair.cuh", "kernel_common.cuh", "step_kernel.cuh", "params.h", "mpc.cuh", "mpc_core.cuh",
     "observers.cuh", "observers_core.cuh", "controllers.cuh", "controllers_core.cuh", "../../include/upkie_b200.h",
@@ -60,7 +61,8 @@ def is_stale() -> bool:
 # tests/test_gpu_exact_mode.py and bench.py's `exact_mode` line: what the one shortcut of the timed kernel (fast-math)
 # costs in accuracy and buys in time.
 EXACT_LIB_PATH = os.path.join(_HERE, "libupkie_b200_exact.so")
-EXACT_SOURCES = ["upkie_b200.cu", "step_device.cu", "step_device_limits.cu", "exact_stubs.cu", "base_velocity.cu"]
+EXACT_SOURCES = ["upkie_b200.cu", "step_device.cu", "step_device_limits.cu", "exact_stubs.cu", "base_velocity.cu",
+                 "reset_randomization.cu"]
 EXACT_FLAGS = [f for f in NVCC_FLAGS if f != "--use_fast_math"] + ["-DUPKIE_EXACT_BUILD=1"]
 
 

@@ -67,6 +67,9 @@ __device__ __forceinline__ void store_state(float* __restrict__ st, int n_pad, i
 // spine mode the lag record (lag_to_row layout)
 constexpr int kFinalMarkRow = 0, kFinalStateRow = 1, kFinalLagRow = 1 + UPKIE_STATE_DIM;
 constexpr int kFinalRows = kFinalLagRow, kFinalRowsSpine = kFinalLagRow + UPKIE_LAG_DIM;
+// with reset randomisation, kFinalParamCols more rows after those: the pre-reset values of the parameter-table columns
+// UPKIE_EP_MEAS_NOISE .. UPKIE_EP_DIM - 1 (torque measurement noise, IMU uncertainty)
+constexpr int kFinalParamCols = UPKIE_EP_DIM - UPKIE_EP_MEAS_NOISE;
 
 // TILE=2 (rollout rows leave the GPU from inside the step kernel): n = 0 -> `obs` / `terminated` are NVSwitch multicast
 // addresses (multimem.st, the switch replicates the store into every GPU's buffer); n > 0 -> plain stores into the n
@@ -127,5 +130,12 @@ cudaError_t launch_step_device_spine(const StepArgs& a);  // step_device_spine.c
 cudaError_t launch_step_host_spine(const StepArgs& a);    // step_host_spine.cu: NOISE=3, TILE=1
 cudaError_t launch_step_device_table(const StepArgs& a);  // step_device_table.cu: NOISE=5 (limits + per-env table), TILE=0
 cudaError_t launch_step_host_table(const StepArgs& a);    // step_host_table.cu: NOISE=5, TILE=1
+// reset_randomization.cu: the handle-side kernels of reset randomisation (upkie_b200_set_reset_randomization)
+cudaError_t launch_reset_rand(const ResetRand* R, int n, const uint8_t* mask, uint64_t seed, uint64_t env_offset,
+                              cudaStream_t stream);  // draw of the envs an upkie_b200_reset takes, before k_reset
+cudaError_t launch_get_randomization(const SimParams& P, int n, const float* mu, const float* eps, float* friction,
+                                     float* inertia_eps, cudaStream_t stream);
+cudaError_t launch_fill(int n, float* out, float v, cudaStream_t stream);
+cudaError_t launch_env_params_from_config(const SimParams& P, int n, int n_pad, float* table, cudaStream_t stream);
 
 }  // namespace upkie_b200

@@ -256,6 +256,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.env_params_stride = 0;
   P.final_gen = 0;
   P.final_state = nullptr;
+  P.reset_rand = nullptr;
   return 0;
 }
 
@@ -299,6 +300,29 @@ inline uint32_t noise_flags(const SimParams& P) {
   return (P.any_ctrl_noise ? kEpCtrlNoise : 0u) | (P.any_meas_noise ? kEpMeasNoise : 0u) |
          (P.any_imu_uncertainty ? kEpImuUncertainty : 0u);
 }
+// The noise models a reset randomisation spec can switch on in some env: a selected noise column whose range reaches
+// above 0, a selected IMU bias column with a nonzero bound. kEpInvalid: a range the spec must not hold (a bound not
+// finite, low > high, low < 0 where the table needs >= 0, an inertia bound <= -1, a floor friction low < 0).
+inline uint32_t reset_rand_flags(const UpkieResetRandomization& R) {
+  uint32_t f = 0;
+  for (int k = 0; k < UPKIE_RR_DIM; ++k) {
+    const float lo = R.low[k], hi = R.high[k];
+    const bool bias = (k >= UPKIE_EP_IMU_ACC_BIAS && k < UPKIE_EP_IMU_ACC_BIAS + 3) ||
+                      (k >= UPKIE_EP_IMU_GYRO_BIAS && k < UPKIE_EP_IMU_GYRO_BIAS + 3);
+    if (!(std::fabs(lo) <= 3.402823466e38f) || !(std::fabs(hi) <= 3.402823466e38f) || lo > hi) f |= kEpInvalid;
+    if (k < UPKIE_EP_DIM && !bias && lo < 0.f) f |= kEpInvalid;
+    if (k >= UPKIE_RR_INERTIA && k < UPKIE_RR_FRICTION && lo <= -1.f) f |= kEpInvalid;
+    if (k == UPKIE_RR_FRICTION && lo < 0.f) f |= kEpInvalid;
+    if (!((R.columns >> k) & 1u)) continue;
+    if (k >= UPKIE_EP_CTRL_NOISE && k < UPKIE_EP_MEAS_NOISE && hi > 0.f) f |= kEpCtrlNoise;
+    if (k >= UPKIE_EP_MEAS_NOISE && k < UPKIE_EP_IMU_ACC_BIAS && hi > 0.f) f |= kEpMeasNoise;
+    if ((k == UPKIE_EP_IMU_ACC_NOISE || k == UPKIE_EP_IMU_GYRO_NOISE) && hi > 0.f) f |= kEpImuUncertainty;
+    if (bias && (lo != 0.f || hi != 0.f)) f |= kEpImuUncertainty;
+  }
+  if (R.columns >> UPKIE_RR_DIM) f |= kEpInvalid;  // no such column
+  return f;
+}
+
 inline void set_noise_flags(SimParams& P, uint32_t f) {
   P.any_ctrl_noise = (f & kEpCtrlNoise) ? 1 : 0;
   P.any_meas_noise = (f & kEpMeasNoise) ? 1 : 0;

@@ -132,6 +132,9 @@ struct SimParams {
   // Appended after every other field, so that their offsets stay where the kernels read them.
   uint32_t final_gen;
   float* final_state;
+  // reset randomisation (upkie_b200_set_reset_randomization): the handle's device block, null = off. Read by the
+  // NOISE >= 3 step kernels and k_reset only. Appended last, as final_state above.
+  const struct ResetRand* reset_rand;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -1555,15 +1558,18 @@ UPKIE_HD void apply_imu_uncertainty(const SimParams& P, const NoiseCtx& nz, floa
 }
 
 // observed torques: commanded torque + measurement noise (pybullet_backend.py:457-466); the standard deviations of
-// the config or of the env's row (`env`, < 0: never a table, see servo_substep) of the parameter table
+// the config or of the env's row (`env`, < 0: never a table, see servo_substep) of the parameter table, or `meas_sd`
+// when `own` (a lane that redrew its row in this launch: the values in force, in registers)
 UPKIE_HD void measured_torques(const SimParams& P, const RobotState& S, const NoiseCtx* nz, float out[6],
-                               int env = -1) {
+                               int env = -1, const float* meas_sd = nullptr, bool own = false) {
   float noise[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   const bool draw = P.any_meas_noise && nz;
   if (draw) gaussian8(P.noise_seed, *nz, 255u, noise);
 #pragma unroll
   for (int j = 0; j < 6; ++j) {
-    const float sd = (draw && env >= 0 && P.env_params) ? env_param(P, env, UPKIE_EP_MEAS_NOISE + j) : P.meas_noise[j];
+    const float sd = (draw && own) ? meas_sd[j]
+                     : (draw && env >= 0 && P.env_params) ? env_param(P, env, UPKIE_EP_MEAS_NOISE + j)
+                                                          : P.meas_noise[j];
     out[j] = S.torque[j] + (sd > 1e-10f ? noise[j] * sd : 0.f);
   }
 }
@@ -1612,6 +1618,63 @@ UPKIE_HD void sample_init_state(const SimParams& P, uint64_t seed, uint64_t env_
     init[UPKIE_INIT_Q + j] = P.init_q[j];  // joint configuration is not randomised (robot_state.py:183)
     init[UPKIE_INIT_QD + j] = 0.f;         // resetJointState zeroes the rates (pybullet_backend.py:262-267)
   }
+}
+
+// ---- reset randomisation (upkie_b200_set_reset_randomization) ----
+// The handle's device block: the spec and the buffers a reset writes its draw to. Its pointers stay valid while the
+// spec is set (the handle refuses to drop those buffers then).
+struct ResetRand {
+  UpkieResetRandomization spec;
+  uint32_t* draws;  // [n] draws so far per env
+  float* table;     // [UPKIE_EP_DIM][stride] the per-env parameter table
+  int stride;
+  float* eps;       // [n][6] inertia epsilons
+  float* mu;        // [n] floor friction
+};
+
+// bit 63 of the high counter word: never set by sample_init_state ((episode << 2) | b, episode < 2^32) or the noise
+// ((tick << 10) | (slot << 1) | b, tick < 2^32)
+constexpr uint64_t kResetRandTag = uint64_t(1) << 63;
+
+// Draw `draw` (1, 2, ...) of the env of global index `env_index`: all UPKIE_RR_DIM columns, whatever is selected, so
+// that selecting a column never changes another one's value. The product is rounded on its own (no FMA), so that a
+// NumPy statement in fp32 reproduces it bit for bit.
+UPKIE_HD void reset_rand_draw(const UpkieResetRandomization& R, uint64_t seed, uint64_t env_index, uint32_t draw,
+                              float v[UPKIE_RR_DIM]) {
+#pragma unroll 1
+  for (int b = 0; b < (UPKIE_RR_DIM + 3) / 4; ++b) {
+    const Philox4 r = philox4x32_10(env_index, kResetRandTag | (uint64_t(draw) << 4) | uint64_t(b), seed);
+    for (int k = 0; k < 4 && 4 * b + k < UPKIE_RR_DIM; ++k) {
+      const int c = 4 * b + k;
+      const float lo = R.low[c], hi = R.high[c];
+#if defined(__CUDA_ARCH__)
+      const float span = __fmul_rn(hi - lo, u01(r.v[k]));
+#else
+      const float span = (hi - lo) * u01(r.v[k]);  // ISO C++ mode: g++ does not contract this into an FMA
+#endif
+      v[c] = fminf(lo + span, hi);
+    }
+  }
+}
+
+// Env i's draw `v`, stored into the selected columns of the table / eps / mu, and its number into the counter
+UPKIE_HD void reset_rand_store(const ResetRand& R, int i, const float v[UPKIE_RR_DIM]) {
+  R.draws[i] += 1u;
+  const uint64_t cols = R.spec.columns;
+  for (int k = 0; k < UPKIE_EP_DIM; ++k)
+    if ((cols >> k) & 1u) R.table[size_t(k) * size_t(R.stride) + size_t(i)] = v[k];
+  for (int b = 0; b < 6; ++b)
+    if ((cols >> (UPKIE_RR_INERTIA + b)) & 1u) R.eps[size_t(i) * 6 + b] = v[UPKIE_RR_INERTIA + b];
+  if ((cols >> UPKIE_RR_FRICTION) & 1u) R.mu[i] = v[UPKIE_RR_FRICTION];
+}
+
+// Env i's next draw (number draws[i] + 1) into v, then stored (`store` false: a tail lane shadowing another env,
+// which stores nothing). A caller that reads the buffers again in the same launch keeps the values it uses from v
+// instead (the step kernels: reset_rand_draw, then reset_rand_store at the end of the tick).
+UPKIE_HD void reset_randomize(const ResetRand& R, uint64_t seed, uint64_t env_index, int i, bool store,
+                              float v[UPKIE_RR_DIM]) {
+  reset_rand_draw(R.spec, seed, env_index, R.draws[i] + 1u, v);
+  if (store) reset_rand_store(R, i, v);
 }
 
 }  // namespace upkie_b200

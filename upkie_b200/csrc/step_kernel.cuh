@@ -93,6 +93,38 @@ __device__ __forceinline__ void store_final_state(const SimParams& P, const Robo
   }
 }
 
+// Reset randomisation, same-step auto-reset with the stash requested: the pre-reset values of the parameter-table
+// columns k_final_spine_obs reads (torque measurement noise and IMU uncertainty), read before the reset's draw
+// overwrites them, in the stash rows after the state (and lag) rows
+template <bool SPINE>
+__device__ __forceinline__ void store_final_params(const SimParams& P, int n_pad, int i) {
+  constexpr int row0 = SPINE ? kFinalRowsSpine : kFinalRows;
+#pragma unroll
+  for (int k = 0; k < kFinalParamCols; ++k)
+    P.final_state[size_t(row0 + k) * n_pad + i] = env_param(P, i, UPKIE_EP_MEAS_NOISE + k);
+}
+
+// Reset randomisation of a resetting lane (P.reset_rand set): env i's next draw into v, and in registers the values
+// the rest of this launch uses from it: the inertia epsilons, the floor friction and the torque measurement-noise
+// levels of the observation (an unselected column keeps the table's value). The draw is stored at the end of the
+// tick (reset_rand_store), after every read of the lane's row: the read-only path the table is read through need not
+// see a lane's own stores of the same launch.
+__device__ __forceinline__ void reset_rand_lane(const SimParams& P, uint64_t seed, uint64_t env_index, int i,
+                                                float v[UPKIE_RR_DIM], float eps[6], float& mu, float meas_sd[6]) {
+  const ResetRand& R = *P.reset_rand;
+#pragma unroll
+  for (int j = 0; j < 6; ++j) meas_sd[j] = env_param(P, i, UPKIE_EP_MEAS_NOISE + j);
+  reset_rand_draw(R.spec, seed, env_index, R.draws[i] + 1u, v);
+  const uint64_t cols = R.spec.columns;
+#pragma unroll
+  for (int b = 0; b < 6; ++b)
+    if ((cols >> (UPKIE_RR_INERTIA + b)) & 1u) eps[b] = v[UPKIE_RR_INERTIA + b];
+  if ((cols >> UPKIE_RR_FRICTION) & 1u) mu = v[UPKIE_RR_FRICTION];
+#pragma unroll
+  for (int j = 0; j < 6; ++j)
+    if ((cols >> (UPKIE_EP_MEAS_NOISE + j)) & 1u) meas_sd[j] = v[UPKIE_EP_MEAS_NOISE + j];
+}
+
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE=1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), and it is reused to transpose the observation rows on the way out.
@@ -119,7 +151,12 @@ __device__ __forceinline__ void step_env(
     for (int k = 0; k < 6; ++k) epsv[k] = eps_all[size_t(i) * 6 + k];
     eps = epsv;
   }
-  const float mu = mu_all ? mu_all[i] : P.friction;
+  float mu = mu_all ? mu_all[i] : P.friction;
+  // reset randomisation (NOISE >= 3 kernels, P.reset_rand set; the handle gives it eps_all and mu_all, so that `eps`
+  // is epsv): whether this lane drew in this launch, its draw, and the measurement-noise levels of its observation
+  bool drawn = false;
+  float rr_v[UPKIE_RR_DIM];
+  float meas_sd[6];
 
   bool resetting = false;
   if (AUTORESET == AUTORESET_NEXT_STEP) resetting = done_prev[i] != 0;
@@ -183,6 +220,10 @@ __device__ __forceinline__ void step_env(
     if (live) episode[i] = ep;
     float init[UPKIE_INIT_DIM];
     sample_init_state(P, seed, env_offset + uint64_t(i), uint64_t(ep), init);
+    if (NOISE >= 3 && P.reset_rand) {
+      reset_rand_lane(P, seed, env_offset + uint64_t(i), i, rr_v, epsv, mu, meas_sd);
+      drawn = true;
+    }
     if (spine) {
       reset_pose_spine(P, S, init, L);
       nsub = 3;  // three cycles with the servos stopped (Spine.cpp:119-125)
@@ -279,13 +320,20 @@ __device__ __forceinline__ void step_env(
     if (term || trunc) {
       if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, NOISE ? &nz : nullptr, TILE && compact, i, env_col);
       // neither the reset below nor the rest of the tick writes tick[i] (written above, before the physics) or the
-      // parameter table, so the stash and those give the rows k_spine_obs would have returned without the reset
+      // parameter table, so the stash and those give the rows k_spine_obs would have returned without the reset (a
+      // reset randomisation draw overwrites the table at the end of the tick, and the stash then also holds the
+      // pre-reset columns k_final_spine_obs reads, store_final_params)
       if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
+      if (NOISE >= 3 && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
       elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
       float init[UPKIE_INIT_DIM];
       sample_init_state(P, seed, env_offset + uint64_t(i), uint64_t(ep), init);
+      if (NOISE >= 3 && P.reset_rand) {
+        reset_rand_lane(P, seed, env_offset + uint64_t(i), i, rr_v, epsv, mu, meas_sd);
+        drawn = true;
+      }
       const BodyRecOut br{((NOISE == 3 || NOISE == 4) && P.body_rec && live) ? P.body_rec + i : nullptr,
                           size_t(P.body_rec_stride)};
       if (spine) reset_robot_spine(P, S, L, init, eps, mu, WarpAny(), P.joint_limits, br);
@@ -304,7 +352,7 @@ __device__ __forceinline__ void step_env(
   if (MODE == MODE_SERVOS) {
     float o[UPKIE_OBS_DIM];
     float tq[6];
-    measured_torques(P, S, NOISE ? &nz : nullptr, tq, env_col);
+    measured_torques(P, S, NOISE ? &nz : nullptr, tq, env_col, meas_sd, NOISE >= 3 && drawn);
 #pragma unroll
     for (int j = 0; j < 6; ++j) {
       o[j * 5 + 0] = S.q[j]; o[j * 5 + 1] = S.qd[j]; o[j * 5 + 2] = tq[j];
@@ -405,6 +453,7 @@ __device__ __forceinline__ void step_env(
     }
   }
   if (!live) return;
+  if (NOISE >= 3 && drawn) reset_rand_store(*P.reset_rand, i, rr_v);  // after the last read of the lane's row
   if (reward) reward[i] = 0.0f;  // upkie_env.py:230
   if (TILE != 2) terminated[i] = term ? 1 : 0;
   if (truncated) truncated[i] = trunc ? 1 : 0;

@@ -89,8 +89,15 @@ struct Handle {
   // [kFinalRows or kFinalRowsSpine][n_pad] (allocated on the first request), the number of the last step that asked for
   // it, and whether that step is the last call that advanced or reset the simulator
   float* final_state = nullptr;
+  int final_rows = 0;            // rows of the stash allocated (kFinalParamCols more with reset randomisation)
   uint32_t final_gen = 0;
   bool final_valid = false;
+  bool final_params = false;     // the stashing step ran with reset randomisation: the stash holds the table columns
+  // reset randomisation (upkie_b200_set_reset_randomization): the device block P.reset_rand points to while a spec is
+  // set, the per-env draw counters (allocated on the first spec or set_draws), and the noise flags the spec implies
+  ResetRand* rr_dev = nullptr;
+  uint32_t* draws = nullptr;
+  uint32_t rr_flags = 0;
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -386,8 +393,19 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
 int prepare_final_state(Handle* h, int32_t flag, bool& stash) {
   stash = flag != 0 && h->autoreset == AUTORESET_SAME_STEP;
   if (!stash) return UPKIE_B200_OK;
+  // reset randomisation: the pre-reset parameter-table columns go to kFinalParamCols more rows
+  const bool params = h->P.reset_rand != nullptr;
+  const int rows = (h->lag ? kFinalRowsSpine : kFinalRows) + (params ? kFinalParamCols : 0);
+  if (h->final_state && h->final_rows < rows) {
+    CUDA_TRY(cudaSetDevice(h->device));
+    CUDA_TRY(cudaDeviceSynchronize());  // steps in flight may still write the smaller stash
+    cudaFree(h->final_state);
+    h->final_state = nullptr;
+  }
+  h->final_params = params;
   if (!h->final_state) {
-    const size_t bytes = size_t(h->lag ? kFinalRowsSpine : kFinalRows) * h->n_pad * sizeof(float);
+    const size_t bytes = size_t(rows) * h->n_pad * sizeof(float);
+    h->final_rows = rows;
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->final_state, bytes));
     CUDA_TRY(cudaMemset(h->final_state, 0, bytes));
@@ -676,7 +694,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->state); cudaFree(h->eps); cudaFree(h->mu); cudaFree(h->err); cudaFree(h->done_prev); cudaFree(h->episode);
   cudaFree(h->bv_episode);
   cudaFree(h->tick); cudaFree(h->elapsed); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
-  cudaFree(h->env_params); cudaFree(h->ep_check); cudaFree(h->final_state);
+  cudaFree(h->env_params); cudaFree(h->ep_check); cudaFree(h->final_state); cudaFree(h->rr_dev); cudaFree(h->draws);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -702,6 +720,8 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   int rc = make_sim_params(h->model, *config, P, err);
   if (rc) return fail(rc, err);
   if (P.spine_mode != h->P.spine_mode) return fail(UPKIE_B200_EINVAL, "set_config: spine_mode is fixed at creation");
+  if (h->P.reset_rand && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: reset randomisation needs joint_limits != 0");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -715,8 +735,9 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   if (h->env_params) {
     P.env_params = h->env_params;
     P.env_params_stride = h->n_pad;
-    set_noise_flags(P, h->env_param_flags);
+    set_noise_flags(P, h->env_param_flags | h->rr_flags);
   }
+  P.reset_rand = h->P.reset_rand;  // so does the reset randomisation
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -738,6 +759,9 @@ int upkie_b200_set_env_params(void* handle, const float* rows, void* stream) {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaSetDevice(h->device));
   if (!rows) {
+    if (h->P.reset_rand)
+      return fail(UPKIE_B200_EINVAL, "set_env_params: reset randomisation writes into the table; turn it off first "
+                                     "(upkie_b200_set_reset_randomization(NULL))");
     if (h->env_params) {
       CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may still read the table
       cudaFree(h->env_params);
@@ -771,7 +795,95 @@ int upkie_b200_set_env_params(void* handle, const float* rows, void* stream) {
   h->env_param_flags = flags;
   h->P.env_params = h->env_params;
   h->P.env_params_stride = h->n_pad;
-  set_noise_flags(h->P, flags);
+  set_noise_flags(h->P, flags | h->rr_flags);
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_reset_randomization(void* handle, const UpkieResetRandomization* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  h->final_valid = false;  // the stash's layout follows the spec
+  if (!spec) {
+    // off: the kernels enqueued before keep the block they were launched with, which stays allocated; the values
+    // in force and the noise flags they needed stay
+    h->P.reset_rand = nullptr;
+    return UPKIE_B200_OK;
+  }
+  if (h->P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_reset_randomization: needs joint_limits != 0 (the table kernels carry it)");
+  const uint32_t flags = reset_rand_flags(*spec);
+  if (flags & kEpInvalid)
+    return fail(UPKIE_B200_EINVAL, "set_reset_randomization: every bound must be finite with low <= high, low >= 0 on "
+                                   "gains, joint friction, noise standard deviations and the floor friction, and "
+                                   "inertia bounds > -1; columns < UPKIE_RR_DIM");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
+  if (!h->env_params) {
+    CUDA_TRY(cudaMalloc(&h->env_params, size_t(UPKIE_EP_DIM) * h->n_pad * sizeof(float)));
+    CUDA_TRY(cudaMemset(h->env_params, 0, size_t(UPKIE_EP_DIM) * h->n_pad * sizeof(float)));
+    CUDA_TRY(launch_env_params_from_config(h->P, h->n, h->n_pad, h->env_params, nullptr));
+    h->env_param_flags = h->config_flags;
+    h->P.env_params = h->env_params;
+    h->P.env_params_stride = h->n_pad;
+  }
+  if (!h->eps) {
+    CUDA_TRY(cudaMalloc(&h->eps, size_t(h->n) * 6 * sizeof(float)));
+    CUDA_TRY(cudaMemset(h->eps, 0, size_t(h->n) * 6 * sizeof(float)));
+  }
+  if (!h->mu) {
+    CUDA_TRY(cudaMalloc(&h->mu, size_t(h->n) * sizeof(float)));
+    CUDA_TRY(launch_fill(h->n, h->mu, h->P.friction, nullptr));
+  }
+  if (!h->draws) {
+    CUDA_TRY(cudaMalloc(&h->draws, size_t(h->n) * sizeof(uint32_t)));
+    CUDA_TRY(cudaMemset(h->draws, 0, size_t(h->n) * sizeof(uint32_t)));
+  }
+  if (!h->rr_dev) CUDA_TRY(cudaMalloc(&h->rr_dev, sizeof(ResetRand)));
+  ResetRand R;
+  std::memset(&R, 0, sizeof(R));
+  R.spec = *spec;
+  R.draws = h->draws;
+  R.table = h->env_params;
+  R.stride = h->n_pad;
+  R.eps = h->eps;
+  R.mu = h->mu;
+  CUDA_TRY(cudaMemcpy(h->rr_dev, &R, sizeof(R), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  // the noise models some drawn level may need; a spec that is replaced or turned off leaves its flags on (the levels
+  // it drew stay in force)
+  h->rr_flags |= flags;
+  set_noise_flags(h->P, h->env_param_flags | h->rr_flags);
+  h->P.reset_rand = h->rr_dev;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_draws(void* handle, uint32_t* draws, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !draws) return fail(UPKIE_B200_EINVAL, "get_draws: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  if (h->draws) CUDA_TRY(cudaMemcpyAsync(draws, h->draws, bytes, cudaMemcpyDeviceToDevice, s));
+  else CUDA_TRY(cudaMemsetAsync(draws, 0, bytes, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_draws(void* handle, const uint32_t* draws, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !draws) return fail(UPKIE_B200_EINVAL, "set_draws: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (!h->draws) CUDA_TRY(cudaMalloc(&h->draws, size_t(h->n) * sizeof(uint32_t)));
+  CUDA_TRY(cudaMemcpyAsync(h->draws, draws, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice,
+                           static_cast<cudaStream_t>(stream)));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_randomization(void* handle, float* friction, float* inertia_eps, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!friction && !inertia_eps) return UPKIE_B200_OK;
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(launch_get_randomization(h->P, h->n, h->mu, h->eps, friction, inertia_eps, static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 
@@ -799,6 +911,9 @@ int upkie_b200_set_autoreset(void* handle, int mode, uint64_t seed, uint64_t env
 int upkie_b200_set_randomization(void* handle, const float* friction, const float* inertia_eps, void* stream) {
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (h->P.reset_rand && (!friction || !inertia_eps))
+    return fail(UPKIE_B200_EINVAL, "set_randomization: reset randomisation writes into both buffers; turn it off "
+                                   "first (upkie_b200_set_reset_randomization(NULL)) to drop one");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaSetDevice(h->device));
   if (friction) {
@@ -829,6 +944,9 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int rblock = 128;
   const int grid = (h->n + rblock - 1) / rblock;
+  // reset randomisation: the envs this reset takes draw first, keyed on the auto-reset's seed and env offset whatever
+  // init rows the reset takes; k_reset then runs the reset substep with the drawn epsilons and friction
+  if (h->P.reset_rand) CUDA_TRY(launch_reset_rand(h->rr_dev, h->n, mask, h->seed, h->env_offset, s));
   k_reset<<<grid, rblock, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
                                     h->done_prev, h->episode, seed, env_offset, h->lag);
   CUDA_TRY(cudaGetLastError());
@@ -1033,8 +1151,17 @@ int upkie_b200_final_spine_obs(void* handle, float* out, void* stream) {
     return fail(UPKIE_B200_EINVAL, "final_spine_obs: the last call that advanced or reset the simulator was not a "
                                    "same-step auto-reset step with final_state = 1");
   CUDA_TRY(cudaSetDevice(h->device));
+  SimParams P = h->P;
+  if (h->final_params) {
+    // reset randomisation: the resets of that step redrew the table, the stash holds its pre-reset columns
+    // UPKIE_EP_MEAS_NOISE .. UPKIE_EP_DIM - 1 (the only ones k_final_spine_obs reads): the launch's table is the stash,
+    // shifted so that column k of env i is stash row (first parameter row + k - UPKIE_EP_MEAS_NOISE)
+    const int row0 = h->lag ? kFinalRowsSpine : kFinalRows;
+    P.env_params = h->final_state + size_t(row0 - UPKIE_EP_MEAS_NOISE) * h->n_pad;
+    P.env_params_stride = h->n_pad;
+  }
   k_final_spine_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-      h->P, h->n, h->n_pad, h->final_state, h->final_gen, h->tick, h->env_offset, out, h->lag ? 1 : 0);
+      P, h->n, h->n_pad, h->final_state, h->final_gen, h->tick, h->env_offset, out, h->lag ? 1 : 0);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }

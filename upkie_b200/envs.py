@@ -377,6 +377,81 @@ def env_params_table(num_envs: int, base: np.ndarray, torque_control_kp=None, to
     return table
 
 
+_IMU_RANGE_COLUMNS = {
+    "accelerometer_bias": (_abi.EP_IMU_ACC_BIAS, 3),
+    "accelerometer_noise": (_abi.EP_IMU_ACC_NOISE, 1),
+    "gyroscope_bias": (_abi.EP_IMU_GYRO_BIAS, 3),
+    "gyroscope_noise": (_abi.EP_IMU_GYRO_NOISE, 1),
+}
+
+
+def reset_randomization_spec(spec: Optional[dict]) -> Optional[_abi.UpkieResetRandomization]:
+    """``UpkieResetRandomization`` (``UpkieSim.set_reset_randomization``) from a dict in the argument forms of the
+    constructor: ``inertia_variation=v`` (``[-v, v]`` on the six bodies, as ``randomize_inertias``),
+    ``floor_friction=(lo, hi)``, ``torque_control_kp`` / ``torque_control_kd=(lo, hi)``,
+    ``joint_properties={joint: {"friction" | "torque_control_noise" | "torque_measurement_noise": (lo, hi)}}`` and
+    ``imu_uncertainty={"accelerometer_bias" | "accelerometer_noise" | "gyroscope_bias" | "gyroscope_noise": (lo, hi)}``
+    whose bias bounds are floats or per-axis triples. Every reset of an env draws the given columns uniformly from their
+    ranges; the others keep their values. Raises ``UpkieException`` on an unknown key or joint, a bound that is not
+    finite, ``lo > hi``, a negative low bound on a gain, friction or noise level, or an inertia bound <= -1."""
+    if spec is None:
+        return None
+    out = _abi.UpkieResetRandomization()
+    out.columns = 0
+
+    def put(col, lo, hi, name, min_low=None):
+        lo, hi = float(lo), float(hi)
+        if not (np.isfinite(lo) and np.isfinite(hi)) or lo > hi:
+            raise UpkieException(f"{name}: expected finite bounds with low <= high, got ({lo}, {hi})")
+        if min_low is not None and not lo >= min_low:
+            raise UpkieException(f"{name}: low bound must be >= {min_low}, got {lo}")
+        out.columns |= 1 << col
+        out.low[col], out.high[col] = lo, hi
+
+    def pair(value, name):
+        try:
+            lo, hi = value
+        except (TypeError, ValueError):
+            raise UpkieException(f"{name}: expected a (low, high) pair, got {value!r}") from None
+        return lo, hi
+
+    known = {"inertia_variation", "floor_friction", "torque_control_kp", "torque_control_kd", "joint_properties",
+             "imu_uncertainty"}
+    unknown = set(spec) - known
+    if unknown:
+        raise UpkieException(f"reset_randomization: unknown keys {sorted(unknown)} (known: {sorted(known)})")
+    if spec.get("inertia_variation") is not None:
+        v = float(spec["inertia_variation"])
+        if not (np.isfinite(v) and 0.0 <= v < 1.0):
+            raise UpkieException(f"inertia_variation: expected 0 <= v < 1, got {v}")
+        for b in range(6):
+            put(_abi.RR_INERTIA + b, -v, v, "inertia_variation")
+    if spec.get("floor_friction") is not None:
+        put(_abi.RR_FRICTION, *pair(spec["floor_friction"], "floor_friction"), "floor_friction", 0.0)
+    for name, col in (("torque_control_kp", _abi.EP_KP), ("torque_control_kd", _abi.EP_KD)):
+        if spec.get(name) is not None:
+            put(col, *pair(spec[name], name), name, 0.0)
+    fields = dict(_JOINT_PROPERTY_COLUMNS)
+    for joint, props in (spec.get("joint_properties") or {}).items():
+        if joint not in _abi.JOINT_NAMES:
+            raise UpkieException(f"joint_properties: unknown joint {joint!r} (joints: {_abi.JOINT_NAMES})")
+        for field, value in props.items():
+            if field not in fields:
+                raise UpkieException(f"joint_properties[{joint!r}]: unknown field {field!r} (fields: {tuple(fields)})")
+            name = f"joint_properties[{joint!r}].{field}"
+            put(fields[field] + _abi.JOINT_NAMES.index(joint), *pair(value, name), name, 0.0)
+    for key, value in (spec.get("imu_uncertainty") or {}).items():
+        if key not in _IMU_RANGE_COLUMNS:
+            raise UpkieException(f"imu_uncertainty: unknown key {key!r} (keys: {tuple(_IMU_RANGE_COLUMNS)})")
+        col, dim = _IMU_RANGE_COLUMNS[key]
+        lo, hi = pair(value, f"imu_uncertainty[{key!r}]")
+        lo = np.broadcast_to(np.asarray(lo, dtype=np.float64), (dim,))
+        hi = np.broadcast_to(np.asarray(hi, dtype=np.float64), (dim,))
+        for k in range(dim):
+            put(col + k, lo[k], hi[k], f"imu_uncertainty[{key!r}]", None if dim == 3 else 0.0)
+    return out
+
+
 class B200VectorEnv(VectorEnv):
     """N Upkie environments stepped by one kernel launch per ``step()``.
 
@@ -402,6 +477,12 @@ class B200VectorEnv(VectorEnv):
     sequence of N such dicts (one per env, as N reference envs would be built). Per-env values go to the handle's
     parameter table (``UpkieSim.set_env_params``, which also takes per-env IMU uncertainty); all-scalar arguments
     build none. ``set_joint_properties`` changes them between episodes.
+
+    ``reset_randomization`` (a dict, see ``reset_randomization_spec``) redraws the given actuator, IMU, inertia and
+    floor-friction parameters of an env on the device at every reset of that env, fused auto-resets included: the
+    per-episode randomisation a reset wrapper around each env of a ``SyncVectorEnv`` would do. The draws are keyed on
+    the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets, so a seeded run repeats.
+    ``set_reset_randomization`` changes or (``None``) stops it.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -435,8 +516,10 @@ class B200VectorEnv(VectorEnv):
         spine_mode: bool = False,
         body_contacts: bool = False,
         max_episode_steps: int = 0,
+        reset_randomization: Optional[dict] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
+        rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
         if env_type not in ENV_TYPES:
             raise UpkieException(f"env_type must be one of {ENV_TYPES}")
         if autoreset_mode not in _AUTORESET:
@@ -517,6 +600,13 @@ class B200VectorEnv(VectorEnv):
         self.inertia_variation = inertia_variation
         if abs(inertia_variation) > 1e-10:
             self.randomize_inertias(inertia_variation)
+        if rr_spec is not None:
+            self.sim.set_reset_randomization(rr_spec)
+
+    def set_reset_randomization(self, spec: Optional[dict]) -> None:
+        """Redraw the parameters ``spec`` names at every later reset of an env (``reset_randomization_spec``);
+        ``None`` stops redrawing, the values then in force stay."""
+        self.sim.set_reset_randomization(reset_randomization_spec(spec))
 
     # ------------------------------------------------------------------
     def get_neutral_action(self) -> dict:
@@ -630,6 +720,14 @@ class B200VectorEnv(VectorEnv):
             seeds = [int(seed) + self.env_offset + i for i in range(n)]
             self._seed = int(seed)
             self.sim.set_autoreset(_AUTORESET[self.autoreset_mode], self._seed, self.env_offset)
+            if getattr(self.sim, "_reset_randomization", None) is not None:
+                # the reset randomisation is keyed on this seed: the envs reset here draw again from draw 1
+                draws = self.sim.get_draws()
+                if mask is None:
+                    draws.zero_()
+                else:
+                    draws.masked_fill_(torch.from_numpy(mask).to(draws.device).bool(), 0)
+                self.sim.set_draws(draws)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

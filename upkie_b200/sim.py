@@ -135,6 +135,32 @@ class UpkieSim:
         check(lib().upkie_b200_get_env_params(self._h, _ptr(out), self._stream()))
         return out
 
+    def get_randomization(self):
+        """The randomisation in force: ``(friction[N], inertia_eps[N, 6])``, the nominal values where none is set."""
+        friction = torch.empty(self.n, dtype=torch.float32, device=self.device)
+        eps = torch.empty((self.n, 6), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_randomization(self._h, _ptr(friction), _ptr(eps), self._stream()))
+        return friction, eps
+
+    def set_reset_randomization(self, spec: Optional[_abi.UpkieResetRandomization]) -> None:
+        """While ``spec`` is set, every reset of an env (fused auto-resets and ``reset``) redraws its selected columns
+        uniformly from their ranges, keyed on the auto-reset seed, the global env index and the env's draw counter
+        (``include/upkie_b200.h``). ``None`` turns it off; the values in force stay."""
+        check(lib().upkie_b200_set_reset_randomization(self._h, C.byref(spec) if spec is not None else None))
+        self._reset_randomization = None if spec is None else _abi.UpkieResetRandomization.from_buffer_copy(spec)
+        if spec is not None:
+            self._randomized_at_reset = True  # the values in force are no longer the ones last set from the host
+
+    def get_draws(self) -> torch.Tensor:
+        """Per-env draw counters of the reset randomisation ``[N]`` (int32 bits of uint32)."""
+        out = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        check(lib().upkie_b200_get_draws(self._h, _ptr(out), self._stream()))
+        return out
+
+    def set_draws(self, draws: torch.Tensor) -> None:
+        self._check_tensor(draws, (self.n,), torch.int32, "draws")
+        check(lib().upkie_b200_set_draws(self._h, _ptr(draws), self._stream()))
+
     def set_external_forces(self, force: Optional[torch.Tensor] = None, local_mask: int = 0) -> None:
         """``force[N, 7, 3]`` newtons at the centres of mass of the 7 bodies, applied on every substep of
         the following steps until overwritten; ``None`` clears. Bit ``b`` of ``local_mask``: the force on
@@ -494,13 +520,21 @@ class UpkieSim:
         elapsed = torch.empty(self.n, dtype=i32, device=self.device)
         check(lib().upkie_b200_get_elapsed(self._h, _ptr(elapsed), self._stream()))
         friction, eps = getattr(self, "_randomization", (None, None))
+        env_params = getattr(self, "_env_params", None)
+        if getattr(self, "_randomized_at_reset", False):
+            # resets drew on the device: the values in force are the device's
+            friction, eps = self.get_randomization()
+            env_params = self.get_env_params()
+        spec = getattr(self, "_reset_randomization", None)
         force, local_mask = getattr(self, "_external", (None, 0))
         return {
+            "reset_randomization": None if spec is None else bytes(spec),  # the UpkieResetRandomization in force
+            "draws": self.get_draws(),  # per-env draw counters of the reset randomisation
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
             "elapsed": elapsed,  # steps since each env's last reset (the time limit's counts)
             "friction": friction, "inertia_eps": eps, "external_force": force, "external_local_mask": local_mask,
-            "env_params": getattr(self, "_env_params", None),  # per-env parameter table, None = the config's values
+            "env_params": env_params,  # per-env parameter table, None = the config's values
             "autoreset": getattr(self, "_autoreset", (AUTORESET_DISABLED, 0, 0)),
         }
 
@@ -517,6 +551,10 @@ class UpkieSim:
         elapsed = torch.zeros(self.n, dtype=torch.int32, device=dev) if elapsed is None else elapsed.to(dev).contiguous()
         check(lib().upkie_b200_set_elapsed(self._h, _ptr(elapsed), self._stream()))
         torch.cuda.current_stream(dev).synchronize()
+        # the buffers a reset randomisation spec writes into are restored with the spec off; a checkpoint written
+        # before reset randomisation existed loads as "off, counters 0"
+        if getattr(self, "_reset_randomization", None) is not None:
+            self.set_reset_randomization(None)
         self.set_randomization(None if sd["friction"] is None else sd["friction"].to(dev),
                                None if sd["inertia_eps"] is None else sd["inertia_eps"].to(dev))
         self.set_external_forces(None if sd["external_force"] is None else sd["external_force"].to(dev),
@@ -524,6 +562,13 @@ class UpkieSim:
         # a checkpoint written before the per-env parameter table existed loads as "no table"
         env_params = sd.get("env_params")
         self.set_env_params(None if env_params is None else env_params.to(dev).contiguous())
+        spec = sd.get("reset_randomization")
+        if spec is not None:
+            self.set_reset_randomization(_abi.UpkieResetRandomization.from_buffer_copy(spec))
+        draws = sd.get("draws")
+        if spec is not None or getattr(self, "_randomized_at_reset", False) or (draws is not None and bool(draws.any())):
+            draws = torch.zeros(self.n, dtype=torch.int32, device=dev) if draws is None else draws.to(dev).contiguous()
+            self.set_draws(draws)
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
