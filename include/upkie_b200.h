@@ -646,6 +646,53 @@ int upkie_b200_set_elapsed(void* handle, const uint32_t* elapsed, void* stream);
  * centre of mass of its lump). */
 int upkie_b200_set_external_forces(void* handle, const float* force, uint32_t local_mask, void* stream);
 
+/* Push randomisation (an addition to ABI 8: no existing layout, constant or signature changed). While a spec is set,
+ * every env runs a schedule of random pushes, drawn and applied inside the step kernels. After every reset of the env
+ * (both fused auto-resets, and upkie_b200_reset with device-sampled or host init rows, masked or not) it
+ *   1. waits `gap` steps without a push,
+ *   2. is pushed for `duration` steps by a constant world-frame force F on body `body`, acting at the body's centre
+ *      of mass exactly as a force of upkie_b200_set_external_forces, and added to any force that call put there,
+ *   3. draws the next (gap, duration, F) and repeats.
+ * Steps are counted on the clock of max_episode_steps: the step of a next-step auto-reset is not counted. The reset
+ * substep runs without external forces; the terminal step of a same-step auto-reset runs under the push then in
+ * force, and the reset starts a new schedule.
+ * Draw law: a per-env counter k numbers the draws, +1 at every reset and +1 at the end of every push. Draw k of the env
+ * of global index g = env_offset + i (the seed and env_offset of upkie_b200_set_autoreset) is Philox4x32-10 with key
+ * seed and counter (g, 2^62 | k << 4 | b) for blocks b = 0, 1, whose words w0 .. w3 of block 0 and w0 of block 1 are
+ * numbered words 0 .. 4:
+ *   gap      = gap_low + (((word0 >> 8) * (gap_high - gap_low + 1)) >> 24)                (integer arithmetic, exact)
+ *   duration = duration_low + (((word1 >> 8) * (duration_high - duration_low + 1)) >> 24)
+ *   F[a]     = min(force_low[a] + (force_high[a] - force_low[a]) * u, force_high[a]), u = (word(2 + a) >> 8) * 2^-24,
+ *              in fp32 with the product rounded on its own (no FMA), a = x, y, z.
+ * The tag bit 62 keeps these counters apart from those of the initial states ((episode << 2) | b) and of the reset
+ * randomisation (bit 63). The schedule depends neither on the physics nor on the number of GPUs.
+ * Per-env state (upkie_b200_get_push_state / set_push_state, for checkpoints): count[i] = k, the draw in force, and
+ * timer[i] = steps taken since draw k was made, 0 .. gap + duration. The steps gap + 1 .. gap + duration of a draw are
+ * pushed; a timer at gap + duration means the push has run out, and the next step starts draw k + 1 (a reset then
+ * starts draw k + 2). A reset sets the timer to 0. A new spec restarts no counter; while no spec is set, neither steps
+ * nor resets change the state.
+ * Needs joint_limits != 0 (the pushes run in copies of the table and body-contact kernels). Rejected with UPKIE_B200_EINVAL, the
+ * previous spec kept: body outside 0 .. UPKIE_NB - 1, a low above its high, duration_low == 0, gap_high or
+ * duration_high above UPKIE_PUSH_MAX_STEPS, a force bound that is not finite, spine_mode (whose cycles take no external
+ * forces), a body whose bit is set in the local_mask of upkie_b200_set_external_forces (which rejects that bit while a
+ * spec pushes the body). The in-kernel rollout transports (step_servos_multicast / _peers / push rows) reject a
+ * handle with a spec. NULL turns pushes off; the state stays. The call waits for the device. */
+#define UPKIE_PUSH_MAX_STEPS (1u << 30)
+typedef struct UpkiePushRandomization {
+  int32_t body;            /* the pushed body: 0 .. UPKIE_NB - 1, the lumps of UpkieModel */
+  uint32_t gap_low, gap_high;            /* steps without a push after a reset or a push, >= 0 */
+  uint32_t duration_low, duration_high;  /* steps of a push, >= 1 */
+  float force_low[3];      /* newtons, world frame */
+  float force_high[3];
+} UpkiePushRandomization;
+int upkie_b200_set_push_randomization(void* handle, const UpkiePushRandomization* spec);
+/* The push force applied in each env's last step, force[N][3] (device pointer, world frame); zero where that step was
+ * not pushed, after a reset (whose substep runs without it), and while no spec is set. */
+int upkie_b200_get_push_forces(void* handle, float* force, void* stream);
+/* The per-env push state count[N], timer[N] (device pointers), see above; 0, 0 on a handle that never had one. */
+int upkie_b200_get_push_state(void* handle, uint32_t* count, uint32_t* timer, void* stream);
+int upkie_b200_set_push_state(void* handle, const uint32_t* count, const uint32_t* timer, void* stream);
+
 /* Number of step-kernel launches issued through this handle since create
  * (bench.py's `gpu_launches`). */
 int upkie_b200_launch_count(void* handle, uint64_t* count);

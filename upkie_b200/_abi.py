@@ -362,6 +362,24 @@ class UpkieResetRandomization(C.Structure):
     ]
 
 
+PUSH_MAX_STEPS = 1 << 30  # UPKIE_PUSH_MAX_STEPS
+
+
+class UpkiePushRandomization(C.Structure):
+    """``UpkiePushRandomization`` of include/upkie_b200.h: the pushed body, and the ranges of the gaps, durations (steps)
+    and world-frame forces (N) of the pushes."""
+
+    _fields_ = [
+        ("body", C.c_int32),
+        ("gap_low", C.c_uint32),
+        ("gap_high", C.c_uint32),
+        ("duration_low", C.c_uint32),
+        ("duration_high", C.c_uint32),
+        ("force_low", C.c_float * 3),
+        ("force_high", C.c_float * 3),
+    ]
+
+
 def default_mpc_config() -> UpkieMpcConfig:
     """``MPCBalancer.__init__`` defaults (``mpc_balancer.py:168-181``)."""
     c = UpkieMpcConfig()

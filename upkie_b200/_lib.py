@@ -43,6 +43,10 @@ SYMBOLS = {
     "upkie_b200_set_reset_randomization": (C.c_int, [_vp, C.POINTER(_abi.UpkieResetRandomization)]),
     "upkie_b200_get_draws": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_set_draws": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_push_randomization": (C.c_int, [_vp, C.POINTER(_abi.UpkiePushRandomization)]),
+    "upkie_b200_get_push_forces": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_get_push_state": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_set_push_state": (C.c_int, [_vp, _vp, _vp, _vp]),
     "upkie_b200_reset": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, _vp]),
     "upkie_b200_step_servos": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_step_gyropod": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]),

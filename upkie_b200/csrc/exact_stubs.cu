@@ -10,4 +10,6 @@ cudaError_t launch_push_rows(const PeerPtrs&, int, cudaStream_t) { return cudaEr
 cudaError_t launch_step_device_spine(const StepArgs&) { return cudaErrorNotSupported; }
 cudaError_t launch_step_device_body(const StepArgs&) { return cudaErrorNotSupported; }
 cudaError_t launch_step_device_table(const StepArgs&) { return cudaErrorNotSupported; }
+cudaError_t launch_step_device_push(const StepArgs&) { return cudaErrorNotSupported; }
+cudaError_t launch_step_device_body_push(const StepArgs&) { return cudaErrorNotSupported; }
 }  // namespace upkie_b200

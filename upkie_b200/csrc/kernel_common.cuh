@@ -93,7 +93,7 @@ struct PeerPtrs {
 // One launch of the env-step kernel over the envs [i0, i0 + cnt) of a handle.
 struct StepArgs {
   const SimParams* P;
-  int mode, autoreset, noise;  // noise: 1 = the "extras" instantiation (torque noise models, external forces), 2 = extras + joint-limit rows, 3 = 2 + spine timing, 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table
+  int mode, autoreset, noise;  // noise: 1 = the "extras" instantiation (torque noise models, external forces), 2 = extras + joint-limit rows, 3 = 2 + spine timing, 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table, 6 = 5 + pushes, 7 = 4 + pushes
   int i0, cnt, n_pad, block;
   int compact_obs;      // TILE=1, servos: observation rows [6][3] (position, velocity, torque) instead of [6][5]
   int grid;             // TILE=1: number of persistent blocks (0 = one block per tile)
@@ -130,6 +130,10 @@ cudaError_t launch_step_device_spine(const StepArgs& a);  // step_device_spine.c
 cudaError_t launch_step_host_spine(const StepArgs& a);    // step_host_spine.cu: NOISE=3, TILE=1
 cudaError_t launch_step_device_table(const StepArgs& a);  // step_device_table.cu: NOISE=5 (limits + per-env table), TILE=0
 cudaError_t launch_step_host_table(const StepArgs& a);    // step_host_table.cu: NOISE=5, TILE=1
+cudaError_t launch_step_device_push(const StepArgs& a);   // step_device_push.cu: NOISE=6 (table family + pushes), TILE=0
+cudaError_t launch_step_host_push(const StepArgs& a);     // step_host_push.cu: NOISE=6, TILE=1
+cudaError_t launch_step_device_body_push(const StepArgs& a);  // step_device_body_push.cu: NOISE=7 (body family + pushes), TILE=0
+cudaError_t launch_step_host_body_push(const StepArgs& a);    // step_host_body_push.cu: NOISE=7, TILE=1
 // reset_randomization.cu: the handle-side kernels of reset randomisation (upkie_b200_set_reset_randomization)
 cudaError_t launch_reset_rand(const ResetRand* R, int n, const uint8_t* mask, uint64_t seed, uint64_t env_offset,
                               cudaStream_t stream);  // draw of the envs an upkie_b200_reset takes, before k_reset
@@ -137,5 +141,10 @@ cudaError_t launch_get_randomization(const SimParams& P, int n, const float* mu,
                                      float* inertia_eps, cudaStream_t stream);
 cudaError_t launch_fill(int n, float* out, float v, cudaStream_t stream);
 cudaError_t launch_env_params_from_config(const SimParams& P, int n, int n_pad, float* table, cudaStream_t stream);
+// pushes.cu: the handle-side kernels of push randomisation (upkie_b200_set_push_randomization)
+cudaError_t launch_push_reset(const PushRand* R, int n, const uint8_t* mask, uint64_t seed, uint64_t env_offset,
+                              cudaStream_t stream);  // the envs an upkie_b200_reset takes restart, before k_reset
+cudaError_t launch_push_forces(const PushRand* R, int n, uint64_t seed, uint64_t env_offset, float* force,
+                               cudaStream_t stream);  // R null: zeros
 
 }  // namespace upkie_b200

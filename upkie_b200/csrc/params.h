@@ -257,6 +257,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.final_gen = 0;
   P.final_state = nullptr;
   P.reset_rand = nullptr;
+  P.push = nullptr;
   return 0;
 }
 
@@ -321,6 +322,20 @@ inline uint32_t reset_rand_flags(const UpkieResetRandomization& R) {
   }
   if (R.columns >> UPKIE_RR_DIM) f |= kEpInvalid;  // no such column
   return f;
+}
+
+// Whether a push randomisation spec holds valid ranges: a body of the model, low <= high everywhere, step bounds up to
+// UPKIE_PUSH_MAX_STEPS with at least one step of push, finite forces. (The handle's own conditions, joint_limits,
+// spine_mode and local_mask, are checked by upkie_b200_set_push_randomization.)
+inline bool push_spec_valid(const UpkiePushRandomization& s) {
+  if (s.body < 0 || s.body >= UPKIE_NB) return false;
+  if (s.gap_low > s.gap_high || s.duration_low > s.duration_high || s.duration_low == 0) return false;
+  if (s.gap_high > UPKIE_PUSH_MAX_STEPS || s.duration_high > UPKIE_PUSH_MAX_STEPS) return false;
+  for (int a = 0; a < 3; ++a) {
+    const float lo = s.force_low[a], hi = s.force_high[a];
+    if (!(std::fabs(lo) <= 3.402823466e38f) || !(std::fabs(hi) <= 3.402823466e38f) || lo > hi) return false;
+  }
+  return true;
 }
 
 inline void set_noise_flags(SimParams& P, uint32_t f) {

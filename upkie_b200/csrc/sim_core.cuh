@@ -135,6 +135,9 @@ struct SimParams {
   // reset randomisation (upkie_b200_set_reset_randomization): the handle's device block, null = off. Read by the
   // NOISE >= 3 step kernels and k_reset only. Appended last, as final_state above.
   const struct ResetRand* reset_rand;
+  // push randomisation (upkie_b200_set_push_randomization): the handle's device block, null = off. Read by the
+  // NOISE = 6, 7 step kernels only. Appended last, as reset_rand above.
+  const struct PushRand* push;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -903,16 +906,35 @@ struct ExtForces {
   uint32_t local;
 };
 
+// The push of push randomisation (PushRand below) in force in this tick: a world-frame force on one body, zero when
+// the env is not being pushed
+struct ExtPush {
+  int body;
+  float f[3];
+};
+
+// PUSH (the NOISE = 6, 7 kernels while a push spec is set): `push` is added to the force of X on its body, and X.f may
+// be null (no forces of upkie_b200_set_external_forces). A push body is never in X.local (the handle rejects it).
+template <bool PUSH = false>
 UPKIE_HD void external_generalized_forces(const SimParams& P, const RobotState& S, const ExtForces& X,
-                                          float tau_add[6], float wbase[6]) {
+                                          float tau_add[6], float wbase[6], const ExtPush* push = nullptr) {
   float R[9];
   quat_to_rot(S.quat, R);
 #pragma unroll
   for (int k = 0; k < 6; ++k) { tau_add[k] = 0.f; wbase[k] = 0.f; }
   auto body_force = [&](int b, float out[3]) {
-    out[0] = X.f[(3 * b + 0) * X.stride];
-    out[1] = X.f[(3 * b + 1) * X.stride];
-    out[2] = X.f[(3 * b + 2) * X.stride];
+    if (!PUSH || X.f) {
+      out[0] = X.f[(3 * b + 0) * X.stride];
+      out[1] = X.f[(3 * b + 1) * X.stride];
+      out[2] = X.f[(3 * b + 2) * X.stride];
+    } else {
+      out[0] = 0.f; out[1] = 0.f; out[2] = 0.f;
+    }
+    if (PUSH && b == push->body) {
+      // the sum a host-written force of (user force + push) would hold; the push alone without user forces
+#pragma unroll
+      for (int k = 0; k < 3; ++k) out[k] = X.f ? out[k] + push->f[k] : push->f[k];
+    }
   };
   auto add_base = [&](const float c[3], const float f[3]) {
     wbase[0] += c[1] * f[2] - c[2] * f[1];
@@ -1118,7 +1140,8 @@ template <typename AnyFn, typename SyncFn = NoSync>
 UPKIE_HD void servo_substep(const SimParams& P, RobotState& S, const float a[UPKIE_ACT_DIM], bool zero_torque,
                             const float* eps, float mu, AnyFn warp_any, SyncFn phase_sync = SyncFn(),
                             const NoiseCtx* nz = nullptr, int sub = 0, const ExtForces* ext = nullptr,
-                            int limits = 0, BodyRecOut rec = BodyRecOut{nullptr, 0}, int env = -1) {
+                            int limits = 0, BodyRecOut rec = BodyRecOut{nullptr, 0}, int env = -1,
+                            const ExtPush* push = nullptr) {
   // `env`: this robot's column of the per-env parameter table; env < 0 (the default, and a constant in the
   // instantiations that never run with a table) compiles the table reads out. Its values are read where they are used, under a uniform branch
   // on the table pointer; the arithmetic is the same for the config's values and the table's.
@@ -1147,11 +1170,13 @@ UPKIE_HD void servo_substep(const SimParams& P, RobotState& S, const float a[UPK
   }
   if (limits != 0) {
     // joint-limit instantiations: ONE inlined copy of the substep (its code is twice as long there), the external
-    // wrench passed through a nullable pointer
+    // wrench passed through a nullable pointer. `push` (non-null in every lane of a launch with a push spec, the
+    // NOISE = 6, 7 kernels) adds the lane's push to `ext`, which may then be null.
     float tau_add[6], wbase[6];
-    const bool forced = ext && !zero_torque;
+    const bool forced = (ext || push) && !zero_torque;
     if (forced) {
-      external_generalized_forces(P, S, *ext, tau_add, wbase);
+      if (push) external_generalized_forces<true>(P, S, ext ? *ext : ExtForces{nullptr, 0, 0u}, tau_add, wbase, push);
+      else external_generalized_forces(P, S, *ext, tau_add, wbase);
 #pragma unroll
       for (int j = 0; j < 6; ++j) tau[j] += tau_add[j];
     }
@@ -1675,6 +1700,96 @@ UPKIE_HD void reset_randomize(const ResetRand& R, uint64_t seed, uint64_t env_in
                               float v[UPKIE_RR_DIM]) {
   reset_rand_draw(R.spec, seed, env_index, R.draws[i] + 1u, v);
   if (store) reset_rand_store(R, i, v);
+}
+
+// ---- push randomisation (upkie_b200_set_push_randomization) ----
+// The handle's device block: the spec and the per-env schedule state (include/upkie_b200.h): count[i] = k, the draw in
+// force, and timer[i] = steps taken since it was made, 0 .. gap + duration.
+struct PushRand {
+  UpkiePushRandomization spec;
+  uint32_t* count;
+  uint32_t* timer;
+};
+
+// bit 62 of the high counter word: never set by sample_init_state ((episode << 2) | b, episode < 2^32), the noise
+// ((tick << 10) | (slot << 1) | b) or the reset randomisation (bit 63 set)
+constexpr uint64_t kPushTag = uint64_t(1) << 62;
+
+// an integer of [lo, hi] from the top 24 bits of a word, exact (hi - lo <= UPKIE_PUSH_MAX_STEPS, so no overflow)
+UPKIE_HD uint32_t push_steps(uint32_t w, uint32_t lo, uint32_t hi) {
+  return lo + uint32_t((uint64_t(w >> 8) * uint64_t(hi - lo + 1u)) >> 24);
+}
+
+// a value of [lo, hi] as reset_rand_draw draws one: the product rounded on its own (no FMA)
+UPKIE_HD float push_value(uint32_t w, float lo, float hi) {
+#if defined(__CUDA_ARCH__)
+  const float span = __fmul_rn(hi - lo, u01(w));
+#else
+  const float span = (hi - lo) * u01(w);  // ISO C++ mode: g++ does not contract this into an FMA
+#endif
+  return fminf(lo + span, hi);
+}
+
+// Draw k of the env of global index g: its gap and duration, and block 0, which also holds words 2 and 3 of the force
+struct PushDraw {
+  uint32_t gap, duration;
+  Philox4 r0;
+};
+UPKIE_HD PushDraw push_draw(const UpkiePushRandomization& s, uint64_t seed, uint64_t g, uint32_t k) {
+  PushDraw d;
+  d.r0 = philox4x32_10(g, kPushTag | (uint64_t(k) << 4), seed);
+  d.gap = push_steps(d.r0.v[0], s.gap_low, s.gap_high);
+  d.duration = push_steps(d.r0.v[1], s.duration_low, s.duration_high);
+  return d;
+}
+
+// the force of draw k (words 2, 3 of block 0 and word 0 of block 1)
+UPKIE_HD void push_force(const UpkiePushRandomization& s, uint64_t seed, uint64_t g, uint32_t k, const PushDraw& d,
+                         float f[3]) {
+  const Philox4 r1 = philox4x32_10(g, kPushTag | (uint64_t(k) << 4) | 1u, seed);
+  f[0] = push_value(d.r0.v[2], s.force_low[0], s.force_high[0]);
+  f[1] = push_value(d.r0.v[3], s.force_low[1], s.force_high[1]);
+  f[2] = push_value(r1.v[0], s.force_low[2], s.force_high[2]);
+}
+
+// One counted step of an env's schedule: (k, t) before the step -> after it, the push of the step in f (zero when not
+// pushed), and `end` = gap + duration of the draw in force after the step. A push that ran out at the last step
+// (t = gap + duration) starts draw k + 1 here.
+UPKIE_HD void push_step(const UpkiePushRandomization& s, uint64_t seed, uint64_t g, uint32_t& k, uint32_t& t,
+                        uint32_t& end, float f[3]) {
+  PushDraw d = push_draw(s, seed, g, k);
+  if (t >= d.gap + d.duration) {
+    k += 1u;
+    t = 0u;
+    d = push_draw(s, seed, g, k);
+  }
+  t += 1u;
+  end = d.gap + d.duration;
+  f[0] = 0.f; f[1] = 0.f; f[2] = 0.f;
+  if (t > d.gap) push_force(s, seed, g, k, d, f);
+}
+
+// A reset of an env whose draw in force has gap + duration = end: the next draw, after the +1 of a push that ran out
+UPKIE_HD void push_restart(uint32_t& k, uint32_t& t, uint32_t end) {
+  k += t >= end ? 2u : 1u;
+  t = 0u;
+}
+
+// The push force env state (k, t) says was applied in the last step (upkie_b200_get_push_forces)
+UPKIE_HD void push_last_force(const UpkiePushRandomization& s, uint64_t seed, uint64_t g, uint32_t k, uint32_t t,
+                              float f[3]) {
+  const PushDraw d = push_draw(s, seed, g, k);
+  f[0] = 0.f; f[1] = 0.f; f[2] = 0.f;
+  if (t > d.gap && t <= d.gap + d.duration) push_force(s, seed, g, k, d, f);
+}
+
+// An explicit reset of env i (k_push_reset, upkie_b200_reset)
+UPKIE_HD void push_reset(const PushRand& R, uint64_t seed, uint64_t g, int i) {
+  const PushDraw d = push_draw(R.spec, seed, g, R.count[i]);
+  uint32_t k = R.count[i], t = R.timer[i];
+  push_restart(k, t, d.gap + d.duration);
+  R.count[i] = k;
+  R.timer[i] = t;
 }
 
 }  // namespace upkie_b200

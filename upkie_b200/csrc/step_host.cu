@@ -6,6 +6,8 @@
 namespace upkie_b200 {
 cudaError_t launch_step_host(const StepArgs& a) {
   if (a.noise == 4) return launch_step_host_body(a);  // step_host_body.cu
+  if (a.noise == 6) return launch_step_host_push(a);  // step_host_push.cu
+  if (a.noise == 7) return launch_step_host_body_push(a);  // step_host_body_push.cu
   if (a.noise == 3) return launch_step_host_spine(a);  // step_host_spine.cu
   if (a.noise == 5) return launch_step_host_table(a);  // step_host_table.cu
   if (a.noise == 2) return launch_step_host_limits(a);  // step_host_limits.cu

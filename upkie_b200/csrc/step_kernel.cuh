@@ -5,7 +5,8 @@
 //       articulated-body dynamics, wheel-ground contact solve, semi-implicit integration), observation,
 //       termination; optional fused auto-reset; optional torque noise models.
 //       NOISE: 0 plain, 1 "extras" (noise models, external forces), 2 extras + joint-limit rows, 3 = 2 + spine timing
-//       (+ body-ground contact rows), 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table.
+//       (+ body-ground contact rows), 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table, 6 = 5 + push
+//       randomisation (P.push; runs correctly without a table), 7 = 4 + push randomisation.
 // Included by step_device.cu (TILE=0), step_host.cu (TILE=1), step_multicast.cu (TILE=2) and the two *_limits.cu
 // units (NOISE=2), see kernel_common.cuh.
 #pragma once
@@ -25,6 +26,9 @@
 #endif
 #ifndef UPKIE_STEP_TABLE_TU
 #define UPKIE_STEP_TABLE_TU 0  // 1 in step_*_table.cu: the NOISE=5 instantiations (extras + limits + per-env parameter table)
+#endif
+#ifndef UPKIE_STEP_PUSH_TU
+#define UPKIE_STEP_PUSH_TU 0  // 6 / 7 in step_*_push.cu / step_*_body_push.cu: the NOISE=6 / 7 instantiations (pushes)
 #endif
 #ifndef UPKIE_ACTION_IN_TILE
 #define UPKIE_ACTION_IN_TILE 0  // build-time experiment (tools/variants.py)
@@ -161,6 +165,24 @@ __device__ __forceinline__ void step_env(
   bool resetting = false;
   if (AUTORESET == AUTORESET_NEXT_STEP) resetting = done_prev[i] != 0;
 
+  // push randomisation (NOISE = 6, 7 kernels, P.push set: a uniform branch): this tick's push, in registers, and the
+  // env's schedule state after the tick (stored at its end). The step of a next-step reset is not counted.
+  const bool pushing = NOISE >= 6 && P.push;
+  ExtPush pu{0, {0.f, 0.f, 0.f}};
+  uint32_t push_k = 0, push_t = 0, push_end = 0;
+  if (pushing) {
+    const PushRand& R = *P.push;
+    pu.body = R.spec.body;
+    push_k = R.count[i];
+    push_t = R.timer[i];
+    if (resetting) {
+      const PushDraw d = push_draw(R.spec, seed, env_offset + uint64_t(i), push_k);
+      push_restart(push_k, push_t, d.gap + d.duration);
+    } else {
+      push_step(R.spec, seed, env_offset + uint64_t(i), push_k, push_t, push_end, pu.f);
+    }
+  }
+
   uint32_t e = 0;
   float a[UPKIE_ACT_DIM];
   float a0 = 0.f, a1 = 0.f;
@@ -263,7 +285,7 @@ __device__ __forceinline__ void step_env(
 #endif
     if (sub < nsub) {
       // the body-ground contacts of the tick's last substep go to the handle's record (NOISE = 3, 4 kernels)
-      const BodyRecOut br{((NOISE == 3 || NOISE == 4) && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
+      const BodyRecOut br{((NOISE == 3 || NOISE == 4 || NOISE == 7) && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
                           size_t(P.body_rec_stride)};
       if (spine) {
         if (resetting && sub == 2) spine_assemble_observation(S, L);
@@ -274,7 +296,8 @@ __device__ __forceinline__ void step_env(
         // a choice between two nonzero constants so that the compiler drops servo_substep's limits == 0 branches, a
         // second and third inlined copy of the substep that these kernels never run
         servo_substep(P, S, a, resetting, eps, mu, WarpAny(), PhaseSync(), NOISE ? &nz : nullptr, sub,
-                      (NOISE && ext) ? &xf : nullptr, NOISE >= 2 ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col);
+                      (NOISE && ext) ? &xf : nullptr, NOISE >= 2 ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
+                      pushing ? &pu : nullptr);
       }
     } else {
 #pragma unroll
@@ -325,6 +348,7 @@ __device__ __forceinline__ void step_env(
       // pre-reset columns k_final_spine_obs reads, store_final_params)
       if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
       if (NOISE >= 3 && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
+      if (pushing) push_restart(push_k, push_t, push_end);  // the terminal step ran under its push; a new schedule
       elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
@@ -334,7 +358,7 @@ __device__ __forceinline__ void step_env(
         reset_rand_lane(P, seed, env_offset + uint64_t(i), i, rr_v, epsv, mu, meas_sd);
         drawn = true;
       }
-      const BodyRecOut br{((NOISE == 3 || NOISE == 4) && P.body_rec && live) ? P.body_rec + i : nullptr,
+      const BodyRecOut br{((NOISE == 3 || NOISE == 4 || NOISE == 7) && P.body_rec && live) ? P.body_rec + i : nullptr,
                           size_t(P.body_rec_stride)};
       if (spine) reset_robot_spine(P, S, L, init, eps, mu, WarpAny(), P.joint_limits, br);
       else reset_robot(P, S, init, eps, mu, WarpAny(), NOISE >= 2 ? P.joint_limits : 0, br);
@@ -454,6 +478,10 @@ __device__ __forceinline__ void step_env(
   }
   if (!live) return;
   if (NOISE >= 3 && drawn) reset_rand_store(*P.reset_rand, i, rr_v);  // after the last read of the lane's row
+  if (pushing) {
+    P.push->count[i] = push_k;
+    P.push->timer[i] = push_t;
+  }
   if (reward) reward[i] = 0.0f;  // upkie_env.py:230
   if (TILE != 2) terminated[i] = term ? 1 : 0;
   if (truncated) truncated[i] = trunc ? 1 : 0;
@@ -605,6 +633,8 @@ cudaError_t launch_step_mode(const StepArgs& a) {
 #define LAUNCH(AR) LAUNCH_N(AR, 2)
 #elif UPKIE_STEP_TABLE_TU
 #define LAUNCH(AR) LAUNCH_N(AR, 5)
+#elif UPKIE_STEP_PUSH_TU
+#define LAUNCH(AR) LAUNCH_N(AR, UPKIE_STEP_PUSH_TU)
 #else
 #define LAUNCH(AR)                \
   do {                            \

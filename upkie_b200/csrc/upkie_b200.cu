@@ -98,6 +98,12 @@ struct Handle {
   ResetRand* rr_dev = nullptr;
   uint32_t* draws = nullptr;
   uint32_t rr_flags = 0;
+  // push randomisation (upkie_b200_set_push_randomization): the device block P.push points to while a spec is set, and
+  // the per-env schedule state (allocated on the first spec or set_push_state)
+  PushRand* push_dev = nullptr;
+  uint32_t* push_count = nullptr;
+  uint32_t* push_timer = nullptr;
+  int push_body = 0;             // the body of the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -320,6 +326,9 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   if (multicast && h->P.env_params)
     return fail(UPKIE_B200_EINVAL, "the per-env parameter table has no in-kernel rollout transport (use upkie_b200_step "
                                    "with compact rows)");
+  if (multicast && h->P.push)
+    return fail(UPKIE_B200_EINVAL, "push randomisation has no in-kernel rollout transport (use upkie_b200_step with "
+                                   "compact rows)");
   if (multicast && h->P.max_episode_steps > 0)
     return fail(UPKIE_B200_EINVAL, "max_episode_steps has no in-kernel rollout transport: it does not carry truncated "
                                    "(use upkie_b200_step with compact rows)");
@@ -347,6 +356,9 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
     if (multicast) return fail(UPKIE_B200_EINVAL, "body_contacts has no in-kernel rollout transport (use upkie_b200_step_servos_compact)");
     a.noise = 4;
   }
+  // push randomisation: the table or body-contact family compiled with the pushes (step_*_push.cu), so that the
+  // NOISE=4 / 5 kernels keep their code (the set call rejects spine mode and joint_limits = 0)
+  if (h->P.push) a.noise = a.noise == 4 ? 7 : 6;
   a.lag = nullptr;
   if (h->P.spine_mode) {
     if (mode != MODE_SERVOS) return fail(UPKIE_B200_EINVAL, "spine_mode supports UpkieServos steps only");
@@ -695,6 +707,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->bv_episode);
   cudaFree(h->tick); cudaFree(h->elapsed); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
   cudaFree(h->env_params); cudaFree(h->ep_check); cudaFree(h->final_state); cudaFree(h->rr_dev); cudaFree(h->draws);
+  cudaFree(h->push_dev); cudaFree(h->push_count); cudaFree(h->push_timer);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -722,6 +735,8 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   if (P.spine_mode != h->P.spine_mode) return fail(UPKIE_B200_EINVAL, "set_config: spine_mode is fixed at creation");
   if (h->P.reset_rand && P.joint_limits == 0)
     return fail(UPKIE_B200_EINVAL, "set_config: reset randomisation needs joint_limits != 0");
+  if (h->P.push && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: push randomisation needs joint_limits != 0");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -738,6 +753,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     set_noise_flags(P, h->env_param_flags | h->rr_flags);
   }
   P.reset_rand = h->P.reset_rand;  // so does the reset randomisation
+  P.push = h->P.push;              // and the push randomisation
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -947,6 +963,8 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
   // reset randomisation: the envs this reset takes draw first, keyed on the auto-reset's seed and env offset whatever
   // init rows the reset takes; k_reset then runs the reset substep with the drawn epsilons and friction
   if (h->P.reset_rand) CUDA_TRY(launch_reset_rand(h->rr_dev, h->n, mask, h->seed, h->env_offset, s));
+  // push randomisation: the envs this reset takes start a new schedule
+  if (h->P.push) CUDA_TRY(launch_push_reset(h->push_dev, h->n, mask, h->seed, h->env_offset, s));
   k_reset<<<grid, rblock, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
                                     h->done_prev, h->episode, seed, env_offset, h->lag);
   CUDA_TRY(cudaGetLastError());
@@ -1243,6 +1261,9 @@ int upkie_b200_set_lag(void* handle, const float* lag_rows, void* stream) {
 int upkie_b200_set_external_forces(void* handle, const float* force, uint32_t local_mask, void* stream) {
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "set_external_forces: invalid handle");
+  if (h->P.push && ((local_mask >> h->push_body) & 1u))
+    return fail(UPKIE_B200_EINVAL, "set_external_forces: the push randomisation pushes this body in the world frame; "
+                                   "its bit of local_mask must be 0");
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   h->ext_local = local_mask;
@@ -1260,6 +1281,91 @@ int upkie_b200_set_external_forces(void* handle, const float* force, uint32_t lo
   }
   k_set_ext<<<(h->n + 127) / 128, 128, 0, s>>>(h->n, h->n_pad, h->ext, force);
   CUDA_TRY(cudaGetLastError());
+  return UPKIE_B200_OK;
+}
+
+namespace {
+// the per-env push state, zeros on a handle that has none yet
+int alloc_push_state(Handle* h) {
+  if (h->push_count) return UPKIE_B200_OK;
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  CUDA_TRY(cudaMalloc(&h->push_count, bytes));
+  CUDA_TRY(cudaMalloc(&h->push_timer, bytes));
+  CUDA_TRY(cudaMemset(h->push_count, 0, bytes));
+  CUDA_TRY(cudaMemset(h->push_timer, 0, bytes));
+  return UPKIE_B200_OK;
+}
+}  // namespace
+
+int upkie_b200_set_push_randomization(void* handle, const UpkiePushRandomization* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    // off: the kernels enqueued before keep the block they were launched with, which stays allocated
+    h->P.push = nullptr;
+    return UPKIE_B200_OK;
+  }
+  const UpkiePushRandomization& s = *spec;
+  if (!push_spec_valid(s))
+    return fail(UPKIE_B200_EINVAL, "set_push_randomization: body must be 0 .. UPKIE_NB - 1, step bounds low <= high <= "
+                                   "UPKIE_PUSH_MAX_STEPS with duration_low >= 1, force bounds finite with low <= high");
+  if (h->P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_push_randomization: needs joint_limits != 0 (the pushes run in the table and "
+                                   "body-contact kernels)");
+  if (h->P.spine_mode)
+    return fail(UPKIE_B200_EINVAL, "set_push_randomization: spine_mode cycles take no external forces");
+  if ((h->ext_local >> s.body) & 1u)
+    return fail(UPKIE_B200_EINVAL, "set_push_randomization: the forces of set_external_forces on this body are in its "
+                                   "body frame (local_mask); pushes are world-frame");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
+  if (alloc_push_state(h)) return UPKIE_B200_ECUDA;
+  if (!h->push_dev) CUDA_TRY(cudaMalloc(&h->push_dev, sizeof(PushRand)));
+  PushRand R;
+  std::memset(&R, 0, sizeof(R));
+  R.spec = s;
+  R.count = h->push_count;
+  R.timer = h->push_timer;
+  CUDA_TRY(cudaMemcpy(h->push_dev, &R, sizeof(R), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->push_body = s.body;
+  h->P.push = h->push_dev;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_push_forces(void* handle, float* force, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !force) return fail(UPKIE_B200_EINVAL, "get_push_forces: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(launch_push_forces(h->P.push, h->n, h->seed, h->env_offset, force, static_cast<cudaStream_t>(stream)));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_push_state(void* handle, uint32_t* count, uint32_t* timer, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !timer) return fail(UPKIE_B200_EINVAL, "get_push_state: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  if (h->push_count) {
+    CUDA_TRY(cudaMemcpyAsync(count, h->push_count, bytes, cudaMemcpyDeviceToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(timer, h->push_timer, bytes, cudaMemcpyDeviceToDevice, s));
+  } else {
+    CUDA_TRY(cudaMemsetAsync(count, 0, bytes, s));
+    CUDA_TRY(cudaMemsetAsync(timer, 0, bytes, s));
+  }
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_push_state(void* handle, const uint32_t* count, const uint32_t* timer, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !timer) return fail(UPKIE_B200_EINVAL, "set_push_state: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (alloc_push_state(h)) return UPKIE_B200_ECUDA;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  CUDA_TRY(cudaMemcpyAsync(h->push_count, count, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(h->push_timer, timer, bytes, cudaMemcpyDeviceToDevice, s));
   return UPKIE_B200_OK;
 }
 

@@ -452,6 +452,65 @@ def reset_randomization_spec(spec: Optional[dict]) -> Optional[_abi.UpkieResetRa
     return out
 
 
+def push_randomization_spec(spec: Optional[dict], model: Model, dt: float) -> Optional[_abi.UpkiePushRandomization]:
+    """``UpkiePushRandomization`` (``UpkieSim.set_push_randomization``) from a dict ``{"link": name, "interval": (lo,
+    hi), "duration": (lo, hi), "force": ((fx, fy, fz) low, (fx, fy, fz) high)}``: after every reset, an env waits a gap
+    drawn from ``interval`` seconds, is pushed for a time drawn from ``duration`` seconds by a world-frame force drawn
+    from ``force`` newtons (bounds: floats or per-axis triples) on ``link``, then draws the next push. Times are rounded
+    to the nearest step of ``dt`` (halves up). A link maps to the body it is lumped into, as in
+    ``Model.external_force_rows``. Raises ``UpkieException`` on an unknown key or link, a bound that is not finite,
+    ``lo > hi``, a negative time, a duration that rounds to 0 steps, or more than ``_abi.PUSH_MAX_STEPS`` steps."""
+    if spec is None:
+        return None
+    known = {"link", "interval", "duration", "force"}
+    unknown = set(spec) - known
+    if unknown:
+        raise UpkieException(f"push_randomization: unknown keys {sorted(unknown)} (known: {sorted(known)})")
+    missing = known - set(spec)
+    if missing:
+        raise UpkieException(f"push_randomization: missing keys {sorted(missing)}")
+    link = spec["link"]
+    if not isinstance(link, str) or link not in model.link_body:
+        raise UpkieException(f"push_randomization: unknown link {link!r} (links: {sorted(model.link_body)})")
+
+    def pair(value, name):
+        try:
+            lo, hi = value
+        except (TypeError, ValueError):
+            raise UpkieException(f"push_randomization[{name!r}]: expected a (low, high) pair, got {value!r}") from None
+        return lo, hi
+
+    def steps(name):
+        lo, hi = (float(x) for x in pair(spec[name], name))
+        if not (np.isfinite(lo) and np.isfinite(hi)) or not 0.0 <= lo <= hi:
+            raise UpkieException(f"push_randomization[{name!r}]: expected finite seconds 0 <= low <= high, got "
+                                 f"({lo}, {hi})")
+        lo_s, hi_s = (int(np.floor(x / dt + 0.5)) for x in (lo, hi))
+        if hi_s > _abi.PUSH_MAX_STEPS:
+            raise UpkieException(f"push_randomization[{name!r}]: more than {_abi.PUSH_MAX_STEPS} steps")
+        return lo_s, hi_s
+
+    out = _abi.UpkiePushRandomization()
+    out.body = int(model.link_body[link])
+    out.gap_low, out.gap_high = steps("interval")
+    out.duration_low, out.duration_high = steps("duration")
+    if out.duration_low == 0:
+        raise UpkieException(f"push_randomization['duration']: the low bound rounds to 0 steps of {dt} s")
+    lo, hi = pair(spec["force"], "force")
+    try:
+        lo = np.broadcast_to(np.asarray(lo, dtype=np.float64), (3,))
+        hi = np.broadcast_to(np.asarray(hi, dtype=np.float64), (3,))
+    except ValueError:
+        raise UpkieException(f"push_randomization['force']: expected floats or (fx, fy, fz) bounds") from None
+    with np.errstate(over="ignore"):
+        finite = np.all(np.isfinite(lo.astype(np.float32))) and np.all(np.isfinite(hi.astype(np.float32)))
+    if not (finite and np.all(lo <= hi)):
+        raise UpkieException(f"push_randomization['force']: expected finite bounds with low <= high, got ({lo}, {hi})")
+    for a in range(3):
+        out.force_low[a], out.force_high[a] = lo[a], hi[a]
+    return out
+
+
 class B200VectorEnv(VectorEnv):
     """N Upkie environments stepped by one kernel launch per ``step()``.
 
@@ -483,6 +542,12 @@ class B200VectorEnv(VectorEnv):
     per-episode randomisation a reset wrapper around each env of a ``SyncVectorEnv`` would do. The draws are keyed on
     the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets, so a seeded run repeats.
     ``set_reset_randomization`` changes or (``None``) stops it.
+
+    ``push_randomization`` (a dict, see ``push_randomization_spec``) pushes every env on one link at random times by
+    random world-frame forces, scheduled and applied inside the step kernel from each env's own resets: the loop around
+    ``set_external_forces`` of the reference's ``apply_external_forces.py``, without a host round trip per step. The
+    pushes add to the forces of ``set_external_forces``. They are keyed on the seed of ``reset(seed=s)``, which also
+    restarts the schedules of the envs it resets. ``set_push_randomization`` changes or (``None``) stops them.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -517,9 +582,12 @@ class B200VectorEnv(VectorEnv):
         body_contacts: bool = False,
         max_episode_steps: int = 0,
         reset_randomization: Optional[dict] = None,
+        push_randomization: Optional[dict] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
+        push_spec = push_randomization_spec(push_randomization, model if model is not None else default_model(),
+                                            1.0 / frequency)
         if env_type not in ENV_TYPES:
             raise UpkieException(f"env_type must be one of {ENV_TYPES}")
         if autoreset_mode not in _AUTORESET:
@@ -602,11 +670,18 @@ class B200VectorEnv(VectorEnv):
             self.randomize_inertias(inertia_variation)
         if rr_spec is not None:
             self.sim.set_reset_randomization(rr_spec)
+        if push_spec is not None:
+            self.sim.set_push_randomization(push_spec)
 
     def set_reset_randomization(self, spec: Optional[dict]) -> None:
         """Redraw the parameters ``spec`` names at every later reset of an env (``reset_randomization_spec``);
         ``None`` stops redrawing, the values then in force stay."""
         self.sim.set_reset_randomization(reset_randomization_spec(spec))
+
+    def set_push_randomization(self, spec: Optional[dict]) -> None:
+        """Push every env at random times by random forces (``push_randomization_spec``, times in seconds of this
+        env's ``dt``); ``None`` stops pushing. Takes effect from the next step; no schedule restarts."""
+        self.sim.set_push_randomization(push_randomization_spec(spec, self.model, self.dt))
 
     # ------------------------------------------------------------------
     def get_neutral_action(self) -> dict:
@@ -728,6 +803,18 @@ class B200VectorEnv(VectorEnv):
                 else:
                     draws.masked_fill_(torch.from_numpy(mask).to(draws.device).bool(), 0)
                 self.sim.set_draws(draws)
+            if getattr(self.sim, "_push_randomization", None) is not None:
+                # so is the push schedule: the envs reset here restart from count 0, timer 0 (their reset then
+                # makes draw 1)
+                count, timer = self.sim.get_push_state()
+                if mask is None:
+                    count.zero_()
+                    timer.zero_()
+                else:
+                    m = torch.from_numpy(mask).to(count.device).bool()
+                    count.masked_fill_(m, 0)
+                    timer.masked_fill_(m, 0)
+                self.sim.set_push_state(count, timer)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

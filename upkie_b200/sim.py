@@ -161,6 +161,31 @@ class UpkieSim:
         self._check_tensor(draws, (self.n,), torch.int32, "draws")
         check(lib().upkie_b200_set_draws(self._h, _ptr(draws), self._stream()))
 
+    def set_push_randomization(self, spec: Optional[_abi.UpkiePushRandomization]) -> None:
+        """While ``spec`` is set, every env is pushed on one body by random world-frame forces at random times, drawn
+        and applied by the step kernel: after each reset, ``gap`` steps without a push, ``duration`` steps of a
+        constant force, then the next draw (``include/upkie_b200.h``). ``None`` turns it off; no counter restarts."""
+        check(lib().upkie_b200_set_push_randomization(self._h, C.byref(spec) if spec is not None else None))
+        self._push_randomization = None if spec is None else _abi.UpkiePushRandomization.from_buffer_copy(spec)
+
+    def get_push_forces(self) -> torch.Tensor:
+        """The push force ``[N, 3]`` (world frame, N) applied in each env's last step; zero where none was."""
+        out = torch.empty((self.n, 3), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_push_forces(self._h, _ptr(out), self._stream()))
+        return out
+
+    def get_push_state(self):
+        """Per-env push schedule state ``(count[N], timer[N])`` (int32 bits of uint32)."""
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        timer = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        check(lib().upkie_b200_get_push_state(self._h, _ptr(count), _ptr(timer), self._stream()))
+        return count, timer
+
+    def set_push_state(self, count: torch.Tensor, timer: torch.Tensor) -> None:
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(timer, (self.n,), torch.int32, "timer")
+        check(lib().upkie_b200_set_push_state(self._h, _ptr(count), _ptr(timer), self._stream()))
+
     def set_external_forces(self, force: Optional[torch.Tensor] = None, local_mask: int = 0) -> None:
         """``force[N, 7, 3]`` newtons at the centres of mass of the 7 bodies, applied on every substep of
         the following steps until overwritten; ``None`` clears. Bit ``b`` of ``local_mask``: the force on
@@ -526,10 +551,14 @@ class UpkieSim:
             friction, eps = self.get_randomization()
             env_params = self.get_env_params()
         spec = getattr(self, "_reset_randomization", None)
+        push = getattr(self, "_push_randomization", None)
+        push_count, push_timer = self.get_push_state()
         force, local_mask = getattr(self, "_external", (None, 0))
         return {
             "reset_randomization": None if spec is None else bytes(spec),  # the UpkieResetRandomization in force
             "draws": self.get_draws(),  # per-env draw counters of the reset randomisation
+            "push_randomization": None if push is None else bytes(push),  # the UpkiePushRandomization in force
+            "push_count": push_count, "push_timer": push_timer,  # per-env push schedule state
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
             "elapsed": elapsed,  # steps since each env's last reset (the time limit's counts)
@@ -555,6 +584,9 @@ class UpkieSim:
         # before reset randomisation existed loads as "off, counters 0"
         if getattr(self, "_reset_randomization", None) is not None:
             self.set_reset_randomization(None)
+        # so is the push spec (it would refuse a checkpoint's body-frame force on its body); a checkpoint written before
+        # push randomisation existed loads as "off, counters 0"
+        self.set_push_randomization(None)
         self.set_randomization(None if sd["friction"] is None else sd["friction"].to(dev),
                                None if sd["inertia_eps"] is None else sd["inertia_eps"].to(dev))
         self.set_external_forces(None if sd["external_force"] is None else sd["external_force"].to(dev),
@@ -569,6 +601,13 @@ class UpkieSim:
         if spec is not None or getattr(self, "_randomized_at_reset", False) or (draws is not None and bool(draws.any())):
             draws = torch.zeros(self.n, dtype=torch.int32, device=dev) if draws is None else draws.to(dev).contiguous()
             self.set_draws(draws)
+        push = sd.get("push_randomization")
+        if push is not None:
+            self.set_push_randomization(_abi.UpkiePushRandomization.from_buffer_copy(push))
+        zeros = torch.zeros(self.n, dtype=torch.int32, device=dev)
+        count, timer = sd.get("push_count"), sd.get("push_timer")
+        self.set_push_state(zeros if count is None else count.to(dev).contiguous(),
+                            zeros if timer is None else timer.to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
