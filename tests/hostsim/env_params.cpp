@@ -24,7 +24,7 @@ uint32_t hostsim_ep_set_env_params(void* hv, int n, const float* rows, float* so
   return f;
 }
 
-// one env tick with the torque noise models, env i reading column i (k_step<.., NOISE=1/5>'s sequence)
+// one env tick with the torque noise models, env i reading column i (the sequence of k_step<.., FAM_EXTRAS / FAM_TABLE, ..>)
 void hostsim_ep_step_servos_noise(void* hv, int n, float* state, const float* action, uint32_t tick,
                                   uint64_t env_offset, float* obs) {
   HostSim* h = static_cast<HostSim*>(hv);

@@ -197,7 +197,7 @@ void hostsim_gaussian8(uint64_t seed, uint64_t env, uint32_t tick, uint32_t slot
   gaussian8(seed, nz, slot, out);
 }
 
-// one env tick with the torque noise models on (same sequence as k_step<.., NOISE=1>)
+// one env tick with the torque noise models on (same sequence as k_step<.., FAM_EXTRAS, ..>)
 void hostsim_step_servos_noise(void* hv, int n, float* state, const float* action, uint32_t tick, uint64_t env_offset,
                                float* obs) {
   HostSim* h = static_cast<HostSim*>(hv);

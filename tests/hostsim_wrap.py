@@ -132,7 +132,7 @@ class HostSim:
         return obs
 
     def step_servos_noise(self, action, tick, env_offset=0):
-        """One tick with the torque noise models, keyed like k_step<.., NOISE=1> at per-env tick ``tick``."""
+        """One tick with the torque noise models, keyed like k_step<.., FAM_EXTRAS, ..> at per-env tick ``tick``."""
         a = np.ascontiguousarray(action, dtype=np.float32).reshape(self.n, 36)
         obs = np.empty((self.n, 6, 5), dtype=np.float32)
         lib().hostsim_step_servos_noise(self._h, self.n, _f(self.state), _f(a), tick, env_offset, _f(obs))

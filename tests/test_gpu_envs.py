@@ -487,7 +487,7 @@ def test_full_size_invariants(model, torch):
 
 
 def test_torque_noise_models(model, torch):
-    """The NOISE=1 instantiation of the step kernel: same draws as the CPU build of the same code (keyed on
+    """The FAM_EXTRAS instantiation of the step kernel: same draws as the CPU build of the same code (keyed on
     seed, global env index, per-env tick), reproducible, invariant to sharding, inert at sigma = 0."""
     from hostsim_wrap import HostSim
     from upkie_b200.envs import B200VectorEnv

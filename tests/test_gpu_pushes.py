@@ -41,7 +41,7 @@ def _sim(model, cfg, n, mode, spec=None, env_offset=0, table=False):
 
     s = UpkieSim(n, model=model, config=cfg)
     s.set_autoreset(mode, SEED, env_offset)
-    if table:  # the config's values in a table: the NOISE=5 kernels
+    if table:  # the config's values in a table: the FAM_TABLE kernels
         s.set_env_params(s.get_env_params())
     if spec is not None:
         s.set_push_randomization(spec)

@@ -4,7 +4,7 @@ section 8 - upkie/cpp/spine/Spine.cpp:116-140,185-265 (which observation a step 
 upkie/cpp/interfaces/BulletInterface.cpp:129-163,228-352 (reset, cycle, torque law), bullet/read_imu_data.h:25-89.
 
 CPU: the oracle's restatement is checked against the semantics read off the reference (black-box, through its public
-state accessors), then the kernels' fp32 arithmetic (host build) against the oracle. GPU: the NOISE=3 kernels through
+state accessors), then the kernels' fp32 arithmetic (host build) against the oracle. GPU: the FAM_SPINE kernels through
 the C ABI against the oracle."""
 import numpy as np
 import pytest
@@ -195,7 +195,7 @@ def test_spine_mode_on_device_matches_the_oracle(model, oracle_lib):
 
 @pytest.mark.gpu
 def test_spine_mode_vector_env_and_fused_autoreset(model):
-    """B200VectorEnv(spine_mode=True): host path (TILE=1, NOISE=3 kernel) and device path agree; a fused auto-reset
+    """B200VectorEnv(spine_mode=True): host path (TILE=1, FAM_SPINE kernel) and device path agree; a fused auto-reset
     runs the three stopped cycles and reports the reset configuration."""
     import torch
 

@@ -1,5 +1,5 @@
 # SPDX-License-Identifier: Apache-2.0
-"""GPU tests of the joint-limit rows on the device (k_step<.., NOISE=2, ..>: config.joint_limits = 1 -> 3 on the
+"""GPU tests of the joint-limit rows on the device (k_step<.., FAM_LIMITS, ..>: config.joint_limits = 1 -> 3 on the
 device, 2, 3) against the oracle, the Backend contact query, and the parity-audit recorder.
 
 Written at the end of round 1 (hence the file name: it sorted last so that its first run on a GPU could not mask the

@@ -14,4 +14,4 @@ touch "$LIB"
 trap 'cp /tmp/libhostsim_plain.so "$LIB"; touch "$LIB"' EXIT
 ASAN_OPTIONS=detect_leaks=0 LD_PRELOAD="$(g++ -print-file-name=libasan.so):$(g++ -print-file-name=libubsan.so)" \
   UPKIE_HOSTSIM_CXXFLAGS="-O1 -g -fsanitize=address,undefined -fno-omit-frame-pointer" \
-  python -m pytest tests/test_kernel_arithmetic_cpu.py tests/test_controllers.py tests/test_observers.py tests/test_body_contacts.py tests/test_spine_mode.py tests/test_reset_randomization_cpu.py tests/test_push_randomization_cpu.py -q -m "not gpu"
+  python -m pytest tests/test_kernel_arithmetic_cpu.py tests/test_controllers.py tests/test_observers.py tests/test_body_contacts.py tests/test_spine_mode.py tests/test_reset_randomization_cpu.py tests/test_push_randomization_cpu.py tests/test_step_family_cpu.py -q -m "not gpu"

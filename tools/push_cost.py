@@ -6,8 +6,8 @@
 Two workloads: 65 536 UpkieServos envs (the headline's physics: fall termination, joint limits, compact rows on
 device buffers) and 4 096 UpkiePendulum envs, both with next-step auto-reset and max_episode_steps = 100. Each times
 three handles, alternating them ROUNDS times, with CUDA events around STEPS steps after WARMUP:
-  default  the default kernels (no table, no spec: the NOISE=2 family),
-  table    a parameter table equal to the config's values, no spec (the NOISE=5 family the pushes run in),
+  default  the default kernels (no table, no spec: the FAM_LIMITS family),
+  table    a parameter table equal to the config's values, no spec (the FAM_TABLE family; pushes run in its FAM_PUSH copy),
   push     that table plus a push spec on the torso, gap 0-20 steps, duration 1-9 steps, +-20 N horizontal, which
            keeps about a third of the envs pushed.
 Prints one JSON line with ms per tick per round, the medians, the share of env-ticks pushed, and the card's name and

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 # SPDX-License-Identifier: Apache-2.0
-"""What the body-contact kernel family (NOISE = 4) costs when no torso touches the floor: 4 096 pendulum envs with
+"""What the body-contact kernel family (FAM_BODY) costs when no torso touches the floor: 4 096 pendulum envs with
 body_contacts off / on, device time per tick from a CUDA-graph replay (run on a GPU; prints two lines)."""
 import os
 import sys

@@ -5,7 +5,7 @@
     python tools/variants.py run [names]  # on the GPU box: times each variant with bench.py (UPKIE_B200_LIB)
 
 Round 2: the variants differ in the translation unit of the benchmarked kernel only (step_host_limits.cu: TILE=1,
-extras + joint-limit rows); every other object is taken from the in-tree build (upkie_b200/build/*.o).
+FAM_LIMITS); every other object is taken from the in-tree build (upkie_b200/build/*.o).
 """
 import json
 import os
@@ -19,8 +19,6 @@ OBJ = os.path.join(ROOT, "upkie_b200", "build")
 OUT = os.path.join(ROOT, "variants")
 VARIANTS = {
     "new_paired": [],
-    "new_scalarW": ["-DUPKIE_TENROW_PAIRED_COLS=0"],
-    "v1": ["-DUPKIE_TENROW_V1=1"],
 }
 UNIT = "step_host_limits"
 KERNEL = "k_stepILi0ELi1ELi2ELi1E"

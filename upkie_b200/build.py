@@ -7,14 +7,16 @@ import subprocess
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libupkie_b200.so")
-# compiled in parallel, then linked
+# compiled in parallel, then linked; the step_*.cu units hold the step kernels of one TILE of one or two families each
+# (csrc/step_family.h)
 SOURCES = ["upkie_b200.cu", "step_device.cu", "step_host.cu", "step_multicast.cu", "step_device_limits.cu",
            "step_host_limits.cu", "step_multicast_limits.cu", "step_device_spine.cu", "step_host_spine.cu",
            "step_device_body.cu", "step_host_body.cu", "step_device_table.cu", "step_host_table.cu", "base_velocity.cu",
            "reset_randomization.cu", "pushes.cu", "step_device_push.cu", "step_host_push.cu",
            "step_device_body_push.cu", "step_host_body_push.cu"]
 DEPS = SOURCES + ["base_velocity.cuh", "base_velocity_core.cuh",
-    "sim_core.cuh", "sim_pair.cuh", "kernel_common.cuh", "step_kernel.cuh", "params.h", "mpc.cuh", "mpc_core.cuh",
+    "sim_core.cuh", "sim_pair.cuh", "kernel_common.cuh", "step_kernel.cuh", "step_family.h", "params.h", "mpc.cuh",
+    "mpc_core.cuh",
     "observers.cuh", "observers_core.cuh", "controllers.cuh", "controllers_core.cuh", "../../include/upkie_b200.h",
 ]
 
@@ -58,9 +60,9 @@ def is_stale() -> bool:
 
 # ---- exact-arithmetic build (test / measurement companion of the product library) ------------------------------------
 # Same sources WITHOUT --use_fast_math (IEEE division / sqrt / sincos, no flush-to-zero), device-buffer kernels only
-# (TILE=0: plain, extras, extras + limits); the other launchers are stubs that return cudaErrorNotSupported. Used by
-# tests/test_gpu_exact_mode.py and bench.py's `exact_mode` line: what the one shortcut of the timed kernel (fast-math)
-# costs in accuracy and buys in time.
+# (TILE=0: plain, extras, extras + limits); the step dispatch reports the other families as cudaErrorNotSupported.
+# Used by tests/test_gpu_exact_mode.py and bench.py's `exact_mode` line: what the one shortcut of the timed kernel
+# (fast-math) costs in accuracy and buys in time.
 EXACT_LIB_PATH = os.path.join(_HERE, "libupkie_b200_exact.so")
 EXACT_SOURCES = ["upkie_b200.cu", "step_device.cu", "step_device_limits.cu", "exact_stubs.cu", "base_velocity.cu",
                  "reset_randomization.cu", "pushes.cu"]

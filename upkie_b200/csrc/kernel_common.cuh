@@ -2,16 +2,18 @@
 //
 // kernel_common.cuh -- what the translation units of libupkie_b200.so share: build-time knobs, the
 // state load/store helpers, and the launch descriptor of the env-step kernel. The step kernel itself
-// (step_kernel.cuh) is instantiated in two translation units that nvcc compiles in parallel:
-//   step_device.cu  TILE=0  per-thread action loads / observation stores (device buffers)
-//   step_host.cu    TILE=1  per-warp shared-memory tile with coalesced 16 B accesses, the variant whose
-//                           warps read actions from and write observations to mapped pinned HOST memory
-// Keeping them apart leaves the register allocation of the device-buffer kernel untouched by the tile path.
+// (step_kernel.cuh) is instantiated in the step_*.cu units, each one TILE of one or two families, that nvcc
+// compiles in parallel (step_family.h, DESIGN.md section 4). TILE is how the rows travel:
+//   0  per-thread action loads / observation stores (device buffers)
+//   1  per-warp shared-memory tile with coalesced 16 B accesses, the variant whose warps read actions from and
+//      write observations to mapped pinned HOST memory
+//   2  the TILE=1 tile path whose compact rows leave through the in-kernel rollout transport (UpkieServos only)
 #pragma once
 
 #include <cuda_runtime.h>
 
 #include "params.h"
+#include "step_family.h"
 
 namespace upkie_b200 {
 
@@ -29,7 +31,6 @@ namespace upkie_b200 {
 #define UPKIE_PHASE_SYNC_LEVEL 1
 #endif
 
-enum { MODE_SERVOS = 0, MODE_GYROPOD = 1, MODE_PENDULUM = 2 };
 enum { AUTORESET_DISABLED = 0, AUTORESET_NEXT_STEP = 1, AUTORESET_SAME_STEP = 2 };
 
 // CTA-wide barrier that tolerates intra-warp divergence (non-.aligned form): every
@@ -93,7 +94,7 @@ struct PeerPtrs {
 // One launch of the env-step kernel over the envs [i0, i0 + cnt) of a handle.
 struct StepArgs {
   const SimParams* P;
-  int mode, autoreset, noise;  // noise: 1 = the "extras" instantiation (torque noise models, external forces), 2 = extras + joint-limit rows, 3 = 2 + spine timing, 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table, 6 = 5 + pushes, 7 = 4 + pushes
+  int mode, autoreset, family;  // family: FAM_* of step_family.h
   int i0, cnt, n_pad, block;
   int compact_obs;      // TILE=1, servos: observation rows [6][3] (position, velocity, torque) instead of [6][5]
   int grid;             // TILE=1: number of persistent blocks (0 = one block per tile)
@@ -110,30 +111,17 @@ struct StepArgs {
   uint32_t* episode;
   uint32_t* tick;
   uint64_t seed, env_offset;
-  const float* ext;     // external forces [21][n_pad] or null (noise != 0 when set)
+  const float* ext;     // external forces [21][n_pad] or null (the family has `extras` when set)
   uint32_t ext_local;
   cudaStream_t stream;
   PeerPtrs peers;       // TILE=2 only
   float* lag;           // spine mode: [UPKIE_LAG_DIM][n_pad] lag records, else null
 };
 
-cudaError_t launch_step_device(const StepArgs& a);  // step_device.cu
-cudaError_t launch_step_host(const StepArgs& a);    // step_host.cu
-cudaError_t launch_step_multicast(const StepArgs& a);  // step_multicast.cu: TILE=2, UpkieServos, compact rows
-cudaError_t launch_step_device_limits(const StepArgs& a);  // step_device_limits.cu: NOISE=2 (joint-limit rows), TILE=0
-cudaError_t launch_step_host_limits(const StepArgs& a);    // step_host_limits.cu: NOISE=2, TILE=1
-cudaError_t launch_step_multicast_limits(const StepArgs& a);  // step_multicast_limits.cu: NOISE=2, TILE=2
+// The step kernels of one (TILE, FAMILY) pair (step_kernel.cuh), explicitly instantiated in its step_*.cu unit
+template <int TILE, int FAMILY>
+cudaError_t launch_step(const StepArgs& a);
 cudaError_t launch_push_rows(const PeerPtrs& pp, int n, cudaStream_t stream);  // step_multicast.cu: flush of a rollout's last rows
-cudaError_t launch_step_device_body(const StepArgs& a);  // step_device_body.cu: NOISE=4 (limits + body-ground contact rows), TILE=0
-cudaError_t launch_step_host_body(const StepArgs& a);    // step_host_body.cu: NOISE=4, TILE=1
-cudaError_t launch_step_device_spine(const StepArgs& a);  // step_device_spine.cu: NOISE=3 (spine timing), TILE=0
-cudaError_t launch_step_host_spine(const StepArgs& a);    // step_host_spine.cu: NOISE=3, TILE=1
-cudaError_t launch_step_device_table(const StepArgs& a);  // step_device_table.cu: NOISE=5 (limits + per-env table), TILE=0
-cudaError_t launch_step_host_table(const StepArgs& a);    // step_host_table.cu: NOISE=5, TILE=1
-cudaError_t launch_step_device_push(const StepArgs& a);   // step_device_push.cu: NOISE=6 (table family + pushes), TILE=0
-cudaError_t launch_step_host_push(const StepArgs& a);     // step_host_push.cu: NOISE=6, TILE=1
-cudaError_t launch_step_device_body_push(const StepArgs& a);  // step_device_body_push.cu: NOISE=7 (body family + pushes), TILE=0
-cudaError_t launch_step_host_body_push(const StepArgs& a);    // step_host_body_push.cu: NOISE=7, TILE=1
 // reset_randomization.cu: the handle-side kernels of reset randomisation (upkie_b200_set_reset_randomization)
 cudaError_t launch_reset_rand(const ResetRand* R, int n, const uint8_t* mask, uint64_t seed, uint64_t env_offset,
                               cudaStream_t stream);  // draw of the envs an upkie_b200_reset takes, before k_reset

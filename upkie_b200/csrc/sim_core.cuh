@@ -99,7 +99,7 @@ struct SimParams {
   // nominal joint configuration / base velocities of the initial state (RobotState.sample_state keeps / adds them)
   float init_q[6], init_angvel[3], init_linvel[3];
   int spine_mode;  // 1: timing of the C++ Bullet spine in simulate() mode (include/upkie_b200.h: spine_mode)
-  // body-ground contacts (config.body_contacts; the NOISE >= 2 instantiations). Collision points of the model:
+  // body-ground contacts (config.body_contacts; the families with the body trait). Collision points of the model:
   int body_contacts;       // 1: on AND the model has collision points
   int n_bp;
   int bp_body[UPKIE_MAX_COLLISION_POINTS];
@@ -133,10 +133,10 @@ struct SimParams {
   uint32_t final_gen;
   float* final_state;
   // reset randomisation (upkie_b200_set_reset_randomization): the handle's device block, null = off. Read by the
-  // NOISE >= 3 step kernels and k_reset only. Appended last, as final_state above.
+  // step kernels of the reset_rand families (step_family.h) and k_reset only. Appended last, as final_state above.
   const struct ResetRand* reset_rand;
   // push randomisation (upkie_b200_set_push_randomization): the handle's device block, null = off. Read by the
-  // NOISE = 6, 7 step kernels only. Appended last, as reset_rand above.
+  // step kernels of the push families (step_family.h) only. Appended last, as reset_rand above.
   const struct PushRand* push;
 };
 
@@ -913,7 +913,7 @@ struct ExtPush {
   float f[3];
 };
 
-// PUSH (the NOISE = 6, 7 kernels while a push spec is set): `push` is added to the force of X on its body, and X.f may
+// PUSH (the push families' kernels with a push spec set): `push` is added to the force of X on its body, and X.f may
 // be null (no forces of upkie_b200_set_external_forces). A push body is never in X.local (the handle rejects it).
 template <bool PUSH = false>
 UPKIE_HD void external_generalized_forces(const SimParams& P, const RobotState& S, const ExtForces& X,
@@ -1171,7 +1171,7 @@ UPKIE_HD void servo_substep(const SimParams& P, RobotState& S, const float a[UPK
   if (limits != 0) {
     // joint-limit instantiations: ONE inlined copy of the substep (its code is twice as long there), the external
     // wrench passed through a nullable pointer. `push` (non-null in every lane of a launch with a push spec, the
-    // NOISE = 6, 7 kernels) adds the lane's push to `ext`, which may then be null.
+    // push families' kernels) adds the lane's push to `ext`, which may then be null.
     float tau_add[6], wbase[6];
     const bool forced = (ext || push) && !zero_torque;
     if (forced) {

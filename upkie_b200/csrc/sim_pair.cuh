@@ -849,9 +849,9 @@ UPKIE_HD void contact_solve_ten_rows(const SimParams& P, RobotState& S, const Le
 // Restated from Bullet 3.24 (third-party, absent from the reference tree: parity unpinned): rigid contact for links
 // without <contact> stiffness (cfm 0, erp = m_erp2), friction directions btPlaneSpace1(normal), at most four manifold
 // points per pair, rows ordered limits / normals / frictions as in btMultiBodyConstraintSolver::solveSingleIteration.
-// 0 in the translation units whose kernels never take the body-contact path (step_device.cu, step_host.cu,
-// step_multicast.cu and the three *_limits.cu units: their SASS is what it was before the rows existed); 1 in the
-// *_body.cu / *_spine.cu units, in upkie_b200.cu (reset kernels) and in the host build
+// 0 in the step units whose kernel families have no body-contact rows (their SASS is what it was before the rows
+// existed), 1 in those of the families with the `body` trait (step_family.h; launch_step checks it at compile time),
+// in upkie_b200.cu (reset kernels) and in the host build
 #ifndef UPKIE_BODY_CONTACTS_BUILD
 #define UPKIE_BODY_CONTACTS_BUILD 1
 #endif
@@ -1262,7 +1262,7 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
   // limits: 0 no joint-limit rows, 1 scalar slow path for the robots that have one, 2 packed ten-row solver for all
   // The scalar slow path exists in the HOST build only (the CPU test-suite's independent second implementation of the
   // limit rows): on the device the whole warp would wait for the lanes that take it, and its
-  // dynamically indexed local arrays cost every NOISE=2 kernel a 2 KB stack frame. On the device 1 aliases to 3.
+  // dynamically indexed local arrays cost every FAM_LIMITS kernel a 2 KB stack frame. On the device 1 aliases to 3.
   // body-ground contacts: a warp that holds a robot with a collision point near the ground solves all rows of its
   // robots in general_contact_solve() instead of the packed solvers (warp-uniform choice)
   bool body_slow = false;

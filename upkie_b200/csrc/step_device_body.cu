@@ -1,11 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=0 instantiations with joint-limit rows AND body-ground contact rows (NOISE=4; config.body_contacts): the
-// kernels of handles whose model carries collision points. Their own translation unit, so that the NOISE=2 kernels
-// (the benchmarked ones) keep the code and register allocation they had before the rows existed. See kernel_common.cuh.
-#define UPKIE_STEP_BODY_TU 1
+// Device-buffer step kernels (TILE=0) of the body-contact family. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 1
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_device_body(const StepArgs& a) { return launch_step_kernels<0>(a); }
+template cudaError_t launch_step<0, FAM_BODY>(const StepArgs&);
 }  // namespace upkie_b200

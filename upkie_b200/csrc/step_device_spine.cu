@@ -1,12 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=0 instantiations with the spine timing (NOISE=3: extras + joint-limit rows + one Bullet-spine cycle per
-// substep, lagged observations; config.spine_mode), UpkieServos only. See kernel_common.cuh.
-#define UPKIE_STEP_SPINE_TU 1
+// Device-buffer step kernels (TILE=0) of the spine-timing family. See step_family.h.
+#define UPKIE_BODY_CONTACTS_BUILD 1
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_device_spine(const StepArgs& a) {
-  if (a.mode != MODE_SERVOS) return cudaErrorNotSupported;
-  return launch_step_mode<0, MODE_SERVOS>(a);
-}
+template cudaError_t launch_step<0, FAM_SPINE>(const StepArgs&);
 }  // namespace upkie_b200

@@ -1,10 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=0 instantiations with joint-limit rows and the reads of the per-env parameter table (NOISE=5): the NOISE=2
-// kernels with a table set (upkie_b200_set_env_params), see kernel_common.cuh.
-#define UPKIE_STEP_TABLE_TU 1
+// Device-buffer step kernels (TILE=0) of the parameter-table family. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 0
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_device_table(const StepArgs& a) { return launch_step_kernels<0>(a); }
+template cudaError_t launch_step<0, FAM_TABLE>(const StepArgs&);
 }  // namespace upkie_b200

@@ -1,9 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=1 instantiations with joint-limit rows and body-ground contact rows (NOISE=4), see step_device_body.cu.
-#define UPKIE_STEP_BODY_TU 1
+// Host-buffer tile step kernels (TILE=1) of the body-contact family. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 1
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_host_body(const StepArgs& a) { return launch_step_kernels<1>(a); }
+template cudaError_t launch_step<1, FAM_BODY>(const StepArgs&);
 }  // namespace upkie_b200

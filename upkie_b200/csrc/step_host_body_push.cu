@@ -1,10 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=1 instantiations of the body-contact family with the push randomisation (NOISE=7), see
-// step_device_body_push.cu.
-#define UPKIE_STEP_PUSH_TU 7
+// Host-buffer tile step kernels (TILE=1) of the body-contact family with pushes. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 1
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_host_body_push(const StepArgs& a) { return launch_step_kernels<1>(a); }
+template cudaError_t launch_step<1, FAM_BODY_PUSH>(const StepArgs&);
 }  // namespace upkie_b200

@@ -1,9 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=1 instantiations with joint-limit rows (NOISE=2: extras + limits), see kernel_common.cuh.
-#define UPKIE_STEP_LIMITS_TU 1
+// Host-buffer tile step kernels (TILE=1) of the joint-limit family: the headline kernel. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 0
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_host_limits(const StepArgs& a) { return launch_step_kernels<1>(a); }
+template cudaError_t launch_step<1, FAM_LIMITS>(const StepArgs&);
 }  // namespace upkie_b200

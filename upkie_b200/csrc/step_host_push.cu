@@ -1,9 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=1 instantiations of the table family with the push randomisation (NOISE=6), see step_device_push.cu.
-#define UPKIE_STEP_PUSH_TU 6
+// Host-buffer tile step kernels (TILE=1) of the table family with pushes. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 0
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_host_push(const StepArgs& a) { return launch_step_kernels<1>(a); }
+template cudaError_t launch_step<1, FAM_PUSH>(const StepArgs&);
 }  // namespace upkie_b200

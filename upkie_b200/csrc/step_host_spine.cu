@@ -1,11 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=1 instantiations with the spine timing (NOISE=3), UpkieServos only. See kernel_common.cuh.
-#define UPKIE_STEP_SPINE_TU 1
+// Host-buffer tile step kernels (TILE=1) of the spine-timing family. See step_family.h.
+#define UPKIE_BODY_CONTACTS_BUILD 1
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_host_spine(const StepArgs& a) {
-  if (a.mode != MODE_SERVOS) return cudaErrorNotSupported;
-  return launch_step_mode<1, MODE_SERVOS>(a);
-}
+template cudaError_t launch_step<1, FAM_SPINE>(const StepArgs&);
 }  // namespace upkie_b200

@@ -1,10 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=1 instantiations with joint-limit rows and the reads of the per-env parameter table (NOISE=5), see
-// step_device_table.cu.
-#define UPKIE_STEP_TABLE_TU 1
+// Host-buffer tile step kernels (TILE=1) of the parameter-table family. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 0
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_host_table(const StepArgs& a) { return launch_step_kernels<1>(a); }
+template cudaError_t launch_step<1, FAM_TABLE>(const StepArgs&);
 }  // namespace upkie_b200

@@ -1,38 +1,14 @@
 // SPDX-License-Identifier: Apache-2.0
 //
 // step_kernel.cuh -- the env-step kernel (one thread = one robot) and its launcher template.
-//   k_step<MODE, AUTORESET, NOISE, TILE>   one 5 ms env tick: action front-end, 5 x (moteus torque law,
+//   k_step<MODE, AUTORESET, FAMILY, TILE>   one 5 ms env tick: action front-end, 5 x (moteus torque law,
 //       articulated-body dynamics, wheel-ground contact solve, semi-implicit integration), observation,
-//       termination; optional fused auto-reset; optional torque noise models.
-//       NOISE: 0 plain, 1 "extras" (noise models, external forces), 2 extras + joint-limit rows, 3 = 2 + spine timing
-//       (+ body-ground contact rows), 4 = 2 + body-ground contact rows, 5 = 2 + per-env parameter table, 6 = 5 + push
-//       randomisation (P.push; runs correctly without a table), 7 = 4 + push randomisation.
-// Included by step_device.cu (TILE=0), step_host.cu (TILE=1), step_multicast.cu (TILE=2) and the two *_limits.cu
-// units (NOISE=2), see kernel_common.cuh.
+//       termination; optional fused auto-reset; the optional features of FAMILY (step_family.h).
+//   launch_step<TILE, FAMILY>   the launcher of a (TILE, FAMILY) pair, explicitly instantiated in its step_*.cu unit
+//       (kernel_common.cuh, DESIGN.md section 4).
 #pragma once
 
 #include "kernel_common.cuh"
-
-// 1 in step_device_limits.cu / step_host_limits.cu: that translation unit holds the NOISE=2 instantiations only
-// (separate units so that the build stays parallel and the other units' kernels are untouched)
-#ifndef UPKIE_STEP_LIMITS_TU
-#define UPKIE_STEP_LIMITS_TU 0
-#endif
-#ifndef UPKIE_STEP_SPINE_TU
-#define UPKIE_STEP_SPINE_TU 0  // 1 in step_*_spine.cu: the NOISE=3 instantiations (extras + limits + spine timing), UpkieServos
-#endif
-#ifndef UPKIE_STEP_BODY_TU
-#define UPKIE_STEP_BODY_TU 0  // 1 in step_*_body.cu: the NOISE=4 instantiations (extras + limits + body-ground contact rows)
-#endif
-#ifndef UPKIE_STEP_TABLE_TU
-#define UPKIE_STEP_TABLE_TU 0  // 1 in step_*_table.cu: the NOISE=5 instantiations (extras + limits + per-env parameter table)
-#endif
-#ifndef UPKIE_STEP_PUSH_TU
-#define UPKIE_STEP_PUSH_TU 0  // 6 / 7 in step_*_push.cu / step_*_body_push.cu: the NOISE=6 / 7 instantiations (pushes)
-#endif
-#ifndef UPKIE_ACTION_IN_TILE
-#define UPKIE_ACTION_IN_TILE 0  // build-time experiment (tools/variants.py)
-#endif
 
 namespace upkie_b200 {
 namespace {
@@ -132,7 +108,7 @@ __device__ __forceinline__ void reset_rand_lane(const SimParams& P, uint64_t see
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE=1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), and it is reused to transpose the observation rows on the way out.
-template <int MODE, int AUTORESET, int NOISE, int TILE>
+template <int MODE, int AUTORESET, int FAMILY, int TILE>
 __device__ __forceinline__ void step_env(
     const SimParams& P, int tid, int n, int n_pad, float* __restrict__ state, const float* __restrict__ action,
     float* __restrict__ obs, float* __restrict__ reward, uint8_t* __restrict__ terminated,
@@ -145,6 +121,7 @@ __device__ __forceinline__ void step_env(
   const int i = live ? tid : n - 1;  // tail lanes shadow the last robot, stores masked
   const int lane = threadIdx.x & 31;
   const int wb = tid - lane;  // first env of this warp
+  constexpr StepFamily F = step_family_traits(FAMILY);
 
   RobotState S;
   load_state(state, n_pad, i, S);
@@ -156,7 +133,7 @@ __device__ __forceinline__ void step_env(
     eps = epsv;
   }
   float mu = mu_all ? mu_all[i] : P.friction;
-  // reset randomisation (NOISE >= 3 kernels, P.reset_rand set; the handle gives it eps_all and mu_all, so that `eps`
+  // reset randomisation (F.reset_rand kernels, P.reset_rand set; the handle gives it eps_all and mu_all, so that `eps`
   // is epsv): whether this lane drew in this launch, its draw, and the measurement-noise levels of its observation
   bool drawn = false;
   float rr_v[UPKIE_RR_DIM];
@@ -165,9 +142,9 @@ __device__ __forceinline__ void step_env(
   bool resetting = false;
   if (AUTORESET == AUTORESET_NEXT_STEP) resetting = done_prev[i] != 0;
 
-  // push randomisation (NOISE = 6, 7 kernels, P.push set: a uniform branch): this tick's push, in registers, and the
+  // push randomisation (F.push kernels, P.push set: a uniform branch): this tick's push, in registers, and the
   // env's schedule state after the tick (stored at its end). The step of a next-step reset is not counted.
-  const bool pushing = NOISE >= 6 && P.push;
+  const bool pushing = F.push && P.push;
   ExtPush pu{0, {0.f, 0.f, 0.f}};
   uint32_t push_k = 0, push_t = 0, push_end = 0;
   if (pushing) {
@@ -216,20 +193,20 @@ __device__ __forceinline__ void step_env(
   // single iteration of the same loop, which keeps the kernel's code small
   // (instruction-cache footprint) and the warp converged.
   NoiseCtx nz{env_offset + uint64_t(i), 0u};
-  if (NOISE) {
+  if (F.extras) {
     nz.tick = tick[i] + 1u;
     if (live) tick[i] = nz.tick;
   }
-  // external forces ride on the NOISE ("extras") instantiations so the plain kernels stay untouched
+  // external forces ride on the F.extras instantiations so the plain kernels stay untouched
   const ExtForces xf{ext ? ext + i : nullptr, size_t(n_pad), ext_local};
-  // this robot's column of the per-env parameter table. The NOISE=2 kernels (the headline's family) never run with a
-  // table, the host picks the NOISE=5 copy of them then: -1 compiles the table reads out of them, so that their
-  // register allocation is the one they have without the feature
-  const int env_col = NOISE == 2 ? -1 : i;
+  // this robot's column of the per-env parameter table. The FAM_LIMITS kernels (the headline's family) never run with
+  // a table, the host picks their FAM_TABLE copy then: -1 compiles the table reads out of them, so that their register
+  // allocation is the one they have without the feature
+  const int env_col = F.table ? i : -1;
   int nsub = P.nb_substeps;
-  // spine mode (config.spine_mode, UpkieServos, the NOISE=2 kernels): every substep is one cycle of the Bullet spine
-  // (NOISE = 3: its own instantiations, step_*_spine.cu, so that the other kernels do not carry the lag record)
-  constexpr bool spine = NOISE == 3 && MODE == MODE_SERVOS;
+  // spine mode (config.spine_mode, UpkieServos): every substep is one cycle of the Bullet spine (FAM_SPINE: its own
+  // instantiations, step_*_spine.cu, so that the other kernels do not carry the lag record)
+  constexpr bool spine = F.spine && MODE == MODE_SERVOS;
   SpineLag L;
   if (spine) {
     float lr[UPKIE_LAG_DIM];
@@ -242,7 +219,7 @@ __device__ __forceinline__ void step_env(
     if (live) episode[i] = ep;
     float init[UPKIE_INIT_DIM];
     sample_init_state(P, seed, env_offset + uint64_t(i), uint64_t(ep), init);
-    if (NOISE >= 3 && P.reset_rand) {
+    if (F.reset_rand && P.reset_rand) {
       reset_rand_lane(P, seed, env_offset + uint64_t(i), i, rr_v, epsv, mu, meas_sd);
       drawn = true;
     }
@@ -257,46 +234,26 @@ __device__ __forceinline__ void step_env(
     if (MODE != MODE_SERVOS) e |= gyropod_action(P, S, a0, a1, a);
     e |= clamp_servo_action(P, a);
   }
-#if UPKIE_ACTION_IN_TILE
-  // TILE kernels: the clamped action row goes back to the warp's staging tile and is re-read at the top of every
-  // substep (9 conflict-free LDS.128), instead of living in 36 registers / local-memory slots across the substep body
-  const bool a_in_tile = TILE && full && MODE == MODE_SERVOS;
-  if (a_in_tile) {
-#pragma unroll
-    for (int k = 0; k < UPKIE_ACT_DIM / 4; ++k)
-      tile4[lane * (UPKIE_ACT_DIM / 4) + k] = make_float4(a[4 * k], a[4 * k + 1], a[4 * k + 2], a[4 * k + 3]);
-    __syncwarp();
-  }
-#endif
   if (spine && !resetting) spine_assemble_observation(S, L);  // the first cycle's observation (Spine.cpp:126-131)
   const int nloop = (AUTORESET == AUTORESET_NEXT_STEP && spine && P.nb_substeps < 3) ? 3 : P.nb_substeps;
   for (int sub = 0; sub < nloop; ++sub) {
 #if UPKIE_PHASE_SYNC_LEVEL >= 1
     __syncthreads();  // once per substep: all threads are converged here
 #endif
-#if UPKIE_ACTION_IN_TILE
-    if (a_in_tile) {
-#pragma unroll
-      for (int k = 0; k < UPKIE_ACT_DIM / 4; ++k) {
-        const float4 v = tile4[lane * (UPKIE_ACT_DIM / 4) + k];
-        a[4 * k + 0] = v.x; a[4 * k + 1] = v.y; a[4 * k + 2] = v.z; a[4 * k + 3] = v.w;
-      }
-    }
-#endif
     if (sub < nsub) {
-      // the body-ground contacts of the tick's last substep go to the handle's record (NOISE = 3, 4 kernels)
-      const BodyRecOut br{((NOISE == 3 || NOISE == 4 || NOISE == 7) && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
+      // the body-ground contacts of the tick's last substep go to the handle's record (F.body kernels)
+      const BodyRecOut br{(F.body && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
                           size_t(P.body_rec_stride)};
       if (spine) {
         if (resetting && sub == 2) spine_assemble_observation(S, L);
         spine_cycle(P, S, L, a, resetting, eps, mu, WarpAny(), PhaseSync(), P.joint_limits >= 1 ? P.joint_limits : 1, br,
                     i);
       } else {
-        // NOISE >= 2: the device's two limit modes (1 and 0 alias to 3 there, see physics_substep_paired), spelled as
+        // F.limits: the device's two limit modes (1 and 0 alias to 3 there, see physics_substep_paired), spelled as
         // a choice between two nonzero constants so that the compiler drops servo_substep's limits == 0 branches, a
         // second and third inlined copy of the substep that these kernels never run
-        servo_substep(P, S, a, resetting, eps, mu, WarpAny(), PhaseSync(), NOISE ? &nz : nullptr, sub,
-                      (NOISE && ext) ? &xf : nullptr, NOISE >= 2 ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
+        servo_substep(P, S, a, resetting, eps, mu, WarpAny(), PhaseSync(), F.extras ? &nz : nullptr, sub,
+                      (F.extras && ext) ? &xf : nullptr, F.limits ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
                       pushing ? &pu : nullptr);
       }
     } else {
@@ -341,27 +298,27 @@ __device__ __forceinline__ void step_env(
 
   if (AUTORESET == AUTORESET_SAME_STEP) {
     if (term || trunc) {
-      if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, NOISE ? &nz : nullptr, TILE && compact, i, env_col);
+      if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
       // neither the reset below nor the rest of the tick writes tick[i] (written above, before the physics) or the
       // parameter table, so the stash and those give the rows k_spine_obs would have returned without the reset (a
       // reset randomisation draw overwrites the table at the end of the tick, and the stash then also holds the
       // pre-reset columns k_final_spine_obs reads, store_final_params)
       if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
-      if (NOISE >= 3 && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
+      if (F.reset_rand && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
       if (pushing) push_restart(push_k, push_t, push_end);  // the terminal step ran under its push; a new schedule
       elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
       float init[UPKIE_INIT_DIM];
       sample_init_state(P, seed, env_offset + uint64_t(i), uint64_t(ep), init);
-      if (NOISE >= 3 && P.reset_rand) {
+      if (F.reset_rand && P.reset_rand) {
         reset_rand_lane(P, seed, env_offset + uint64_t(i), i, rr_v, epsv, mu, meas_sd);
         drawn = true;
       }
-      const BodyRecOut br{((NOISE == 3 || NOISE == 4 || NOISE == 7) && P.body_rec && live) ? P.body_rec + i : nullptr,
+      const BodyRecOut br{(F.body && P.body_rec && live) ? P.body_rec + i : nullptr,
                           size_t(P.body_rec_stride)};
       if (spine) reset_robot_spine(P, S, L, init, eps, mu, WarpAny(), P.joint_limits, br);
-      else reset_robot(P, S, init, eps, mu, WarpAny(), NOISE >= 2 ? P.joint_limits : 0, br);
+      else reset_robot(P, S, init, eps, mu, WarpAny(), F.limits ? P.joint_limits : 0, br);
       if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
     }
   }
@@ -376,7 +333,7 @@ __device__ __forceinline__ void step_env(
   if (MODE == MODE_SERVOS) {
     float o[UPKIE_OBS_DIM];
     float tq[6];
-    measured_torques(P, S, NOISE ? &nz : nullptr, tq, env_col, meas_sd, NOISE >= 3 && drawn);
+    measured_torques(P, S, F.extras ? &nz : nullptr, tq, env_col, meas_sd, F.reset_rand && drawn);
 #pragma unroll
     for (int j = 0; j < 6; ++j) {
       o[j * 5 + 0] = S.q[j]; o[j * 5 + 1] = S.qd[j]; o[j * 5 + 2] = tq[j];
@@ -477,7 +434,7 @@ __device__ __forceinline__ void step_env(
     }
   }
   if (!live) return;
-  if (NOISE >= 3 && drawn) reset_rand_store(*P.reset_rand, i, rr_v);  // after the last read of the lane's row
+  if (F.reset_rand && drawn) reset_rand_store(*P.reset_rand, i, rr_v);  // after the last read of the lane's row
   if (pushing) {
     P.push->count[i] = push_k;
     P.push->timer[i] = push_t;
@@ -543,7 +500,7 @@ __device__ __forceinline__ void cp_async_wait() {
 // shared-memory buffer while the current tile computes, and observation rows leave through coalesced
 // 16 B stores, so the link streams in both directions for the whole launch instead of in bursts
 // between compute phases.
-template <int MODE, int AUTORESET, int NOISE, int TILE>
+template <int MODE, int AUTORESET, int FAMILY, int TILE>
 #ifdef UPKIE_MAXNREG
 __global__ void __maxnreg__(UPKIE_MAXNREG)
 #else
@@ -558,9 +515,9 @@ k_step(const __grid_constant__ SimParams P, int i0, int n, int n_pad, float* __r
        float* __restrict__ lag) {
   // this launch covers the envs [i0, n)
   if (!TILE) {
-    step_env<MODE, AUTORESET, NOISE, 0>(P, i0 + blockIdx.x * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
-                                        reward, terminated, truncated, eps_all, mu_all, err, done_prev, episode, tick,
-                                        seed, env_offset, ext, ext_local, nullptr, false, false, nullptr, lag);
+    step_env<MODE, AUTORESET, FAMILY, 0>(P, i0 + blockIdx.x * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
+                                         reward, terminated, truncated, eps_all, mu_all, err, done_prev, episode, tick,
+                                         seed, env_offset, ext, ext_local, nullptr, false, false, nullptr, lag);
     return;
   }
   extern __shared__ float4 s_tile[];
@@ -593,17 +550,16 @@ k_step(const __grid_constant__ SimParams P, int i0, int n, int n_pad, float* __r
     if (TILE == 2) {
       if (peers.deferred && peers.src_obs) push_rows(peers, i0 + t * int(blockDim.x) + warp * 32, lane);
     }
-    step_env<MODE, AUTORESET, NOISE, TILE>(P, i0 + t * blockDim.x + threadIdx.x, n, n_pad, state, action, obs, reward,
-                                        terminated, truncated, eps_all, mu_all, err, done_prev, episode, tick, seed,
-                                        env_offset, ext, ext_local, buf[it & 1], warp_full(t), (coalesce & 2) != 0,
-                                        TILE == 2 ? &peers : nullptr, lag);
+    step_env<MODE, AUTORESET, FAMILY, TILE>(P, i0 + t * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
+                                         reward, terminated, truncated, eps_all, mu_all, err, done_prev, episode, tick,
+                                         seed, env_offset, ext, ext_local, buf[it & 1], warp_full(t),
+                                         (coalesce & 2) != 0, TILE == 2 ? &peers : nullptr, lag);
     __syncwarp();  // the tile is free again before the next prefetch lands in it
   }
 }
 
-
-template <int TILE, int MODE>
-cudaError_t launch_step_mode(const StepArgs& a) {
+template <int TILE, int MODE, int AUTORESET, int FAMILY>
+cudaError_t launch_k_step(const StepArgs& a) {
   const int tiles = (a.cnt + a.block - 1) / a.block;
   const int grid = (TILE && a.grid > 0 && a.grid < tiles) ? a.grid : tiles;
   const size_t smem = TILE ? size_t(2) * (a.block / 32) * 32 * UPKIE_ACT_DIM * sizeof(float) : 0;
@@ -613,49 +569,38 @@ cudaError_t launch_step_mode(const StepArgs& a) {
   const int coalesce = (aligned ? 1 : 0) | ((TILE && a.compact_obs) ? 2 : 0);  // bit 0 tile path, bit 1 compact rows
   // a 256-thread block's two tile buffers take 72 KB: above 48 KB of dynamic shared memory a kernel must opt in (per
   // device, so on every launch)
-#define LAUNCH_N(AR, NZ)                                                                                          \
-  do {                                                                                                            \
-    if (smem > 48 * 1024) {                                                                                       \
-      const cudaError_t e = cudaFuncSetAttribute(k_step<MODE, AR, NZ, TILE>,                                      \
-                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));         \
-      if (e != cudaSuccess) return e;                                                                             \
-    }                                                                                                             \
-    k_step<MODE, AR, NZ, TILE><<<grid, a.block, smem, a.stream>>>(                                                \
-        *a.P, a.i0, a.i0 + a.cnt, a.n_pad, a.state, a.action, a.obs, a.reward, a.terminated, a.truncated, a.eps,  \
-        a.mu, a.err, a.done_prev, a.episode, a.tick, a.seed, a.env_offset, a.ext, a.ext_local, coalesce, a.peers, \
-        a.lag);                                                                                                   \
-  } while (0)
-#if UPKIE_STEP_SPINE_TU
-#define LAUNCH(AR) LAUNCH_N(AR, 3)
-#elif UPKIE_STEP_BODY_TU
-#define LAUNCH(AR) LAUNCH_N(AR, 4)
-#elif UPKIE_STEP_LIMITS_TU
-#define LAUNCH(AR) LAUNCH_N(AR, 2)
-#elif UPKIE_STEP_TABLE_TU
-#define LAUNCH(AR) LAUNCH_N(AR, 5)
-#elif UPKIE_STEP_PUSH_TU
-#define LAUNCH(AR) LAUNCH_N(AR, UPKIE_STEP_PUSH_TU)
-#else
-#define LAUNCH(AR)                \
-  do {                            \
-    if (a.noise) LAUNCH_N(AR, 1); \
-    else LAUNCH_N(AR, 0);         \
-  } while (0)
-#endif
-  if (a.autoreset == AUTORESET_NEXT_STEP) LAUNCH(AUTORESET_NEXT_STEP);
-  else if (a.autoreset == AUTORESET_SAME_STEP) LAUNCH(AUTORESET_SAME_STEP);
-  else LAUNCH(AUTORESET_DISABLED);
-#undef LAUNCH
-#undef LAUNCH_N
+  if (smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(k_step<MODE, AUTORESET, FAMILY, TILE>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return e;
+  }
+  k_step<MODE, AUTORESET, FAMILY, TILE><<<grid, a.block, smem, a.stream>>>(
+      *a.P, a.i0, a.i0 + a.cnt, a.n_pad, a.state, a.action, a.obs, a.reward, a.terminated, a.truncated, a.eps, a.mu,
+      a.err, a.done_prev, a.episode, a.tick, a.seed, a.env_offset, a.ext, a.ext_local, coalesce, a.peers, a.lag);
   return cudaGetLastError();
 }
 
-template <int TILE>
-cudaError_t launch_step_kernels(const StepArgs& a) {
-  if (a.mode == MODE_SERVOS) return launch_step_mode<TILE, MODE_SERVOS>(a);
-  if (a.mode == MODE_GYROPOD) return launch_step_mode<TILE, MODE_GYROPOD>(a);
-  return launch_step_mode<TILE, MODE_PENDULUM>(a);
+template <int TILE, int MODE, int FAMILY>
+cudaError_t launch_step_mode(const StepArgs& a) {
+  if (a.autoreset == AUTORESET_NEXT_STEP) return launch_k_step<TILE, MODE, AUTORESET_NEXT_STEP, FAMILY>(a);
+  if (a.autoreset == AUTORESET_SAME_STEP) return launch_k_step<TILE, MODE, AUTORESET_SAME_STEP, FAMILY>(a);
+  return launch_k_step<TILE, MODE, AUTORESET_DISABLED, FAMILY>(a);
 }
 
 }  // namespace
+
+template <int TILE, int FAMILY>
+cudaError_t launch_step(const StepArgs& a) {
+  static_assert(bool(UPKIE_BODY_CONTACTS_BUILD) == step_family_traits(FAMILY).body,
+                "a unit's UPKIE_BODY_CONTACTS_BUILD is 1 exactly when its families carry body-contact rows");
+  // the spine family and the in-kernel transport (TILE=2) are instantiated for UpkieServos only
+  if (a.mode == MODE_SERVOS) return launch_step_mode<TILE, MODE_SERVOS, FAMILY>(a);
+  if constexpr (TILE == 2 || step_family_traits(FAMILY).spine) {
+    return cudaErrorNotSupported;
+  } else {
+    if (a.mode == MODE_GYROPOD) return launch_step_mode<TILE, MODE_GYROPOD, FAMILY>(a);
+    return launch_step_mode<TILE, MODE_PENDULUM, FAMILY>(a);
+  }
+}
+
 }  // namespace upkie_b200

@@ -1,7 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
 // NVSwitch-multicast instantiations of the env-step kernel (TILE=2): the TILE=1 tile path whose compact observation
 // rows and `terminated` words leave through multimem.st to the multicast address of a symmetric rollout buffer, so
-// that every GPU's buffer receives them without a collective. UpkieServos only. See kernel_common.cuh.
+// that every GPU's buffer receives them without a collective: the plain and extras families, UpkieServos only.
+// See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 0
 #include "step_kernel.cuh"
 
@@ -19,9 +20,6 @@ cudaError_t launch_push_rows(const PeerPtrs& pp, int n, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
-cudaError_t launch_step_multicast(const StepArgs& a) {
-  if (a.noise == 3 || a.noise == 4) return cudaErrorNotSupported;  // no spine-timing / body-contact instantiation of the in-kernel transports
-  if (a.noise == 2) return launch_step_multicast_limits(a);  // step_multicast_limits.cu
-  return launch_step_mode<2, MODE_SERVOS>(a);
-}
+template cudaError_t launch_step<2, FAM_PLAIN>(const StepArgs&);
+template cudaError_t launch_step<2, FAM_EXTRAS>(const StepArgs&);
 }  // namespace upkie_b200

@@ -1,10 +1,8 @@
 // SPDX-License-Identifier: Apache-2.0
-// TILE=2 (rollout rows stored to the NVSwitch multicast address or into the peers' buffers) with joint-limit rows
-// (NOISE=2: extras + limits), UpkieServos only. See kernel_common.cuh.
-#define UPKIE_STEP_LIMITS_TU 1
+// In-kernel rollout transport step kernels (TILE=2) of the joint-limit family. See step_family.h.
 #define UPKIE_BODY_CONTACTS_BUILD 0
 #include "step_kernel.cuh"
 
 namespace upkie_b200 {
-cudaError_t launch_step_multicast_limits(const StepArgs& a) { return launch_step_mode<2, MODE_SERVOS>(a); }
+template cudaError_t launch_step<2, FAM_LIMITS>(const StepArgs&);
 }  // namespace upkie_b200

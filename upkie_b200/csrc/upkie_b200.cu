@@ -311,6 +311,36 @@ int pick_block(const Handle* h, int cnt) {
   return block;
 }
 
+// The step kernels of (TILE, family), instantiated in the step_*.cu units; cudaErrorNotSupported for a pair without an
+// instantiation. The exact-arithmetic library (build.py: build_exact) has the device-buffer kernels of families 0-2 only.
+constexpr int tile_family(int tile, int family) { return tile * kNumFamilies + family; }
+cudaError_t dispatch_step(int tile, const StepArgs& a) {
+  switch (tile_family(tile, a.family)) {
+    case tile_family(0, FAM_PLAIN): return launch_step<0, FAM_PLAIN>(a);
+    case tile_family(0, FAM_EXTRAS): return launch_step<0, FAM_EXTRAS>(a);
+    case tile_family(0, FAM_LIMITS): return launch_step<0, FAM_LIMITS>(a);
+#if !UPKIE_EXACT_BUILD
+    case tile_family(0, FAM_SPINE): return launch_step<0, FAM_SPINE>(a);
+    case tile_family(0, FAM_BODY): return launch_step<0, FAM_BODY>(a);
+    case tile_family(0, FAM_TABLE): return launch_step<0, FAM_TABLE>(a);
+    case tile_family(0, FAM_PUSH): return launch_step<0, FAM_PUSH>(a);
+    case tile_family(0, FAM_BODY_PUSH): return launch_step<0, FAM_BODY_PUSH>(a);
+    case tile_family(1, FAM_PLAIN): return launch_step<1, FAM_PLAIN>(a);
+    case tile_family(1, FAM_EXTRAS): return launch_step<1, FAM_EXTRAS>(a);
+    case tile_family(1, FAM_LIMITS): return launch_step<1, FAM_LIMITS>(a);
+    case tile_family(1, FAM_SPINE): return launch_step<1, FAM_SPINE>(a);
+    case tile_family(1, FAM_BODY): return launch_step<1, FAM_BODY>(a);
+    case tile_family(1, FAM_TABLE): return launch_step<1, FAM_TABLE>(a);
+    case tile_family(1, FAM_PUSH): return launch_step<1, FAM_PUSH>(a);
+    case tile_family(1, FAM_BODY_PUSH): return launch_step<1, FAM_BODY_PUSH>(a);
+    case tile_family(2, FAM_PLAIN): return launch_step<2, FAM_PLAIN>(a);
+    case tile_family(2, FAM_EXTRAS): return launch_step<2, FAM_EXTRAS>(a);
+    case tile_family(2, FAM_LIMITS): return launch_step<2, FAM_LIMITS>(a);
+#endif
+    default: return cudaErrorNotSupported;
+  }
+}
+
 // envs [i0, i0 + cnt): all buffers are indexed by the env index of the handle. `tile` selects the
 // shared-memory-tile instantiation (host buffers), see kernel_common.cuh.
 // `final_obs`: rows of the same-step auto-resets' terminal observations (null = not requested): it travels in a copy of
@@ -323,15 +353,10 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   h->final_valid = false;  // the simulator moves on: the caller marks the stash valid once the whole step is enqueued
   if (multicast && final_state)
     return fail(UPKIE_B200_EINVAL, "final_state has no in-kernel rollout transport (use upkie_b200_step)");
-  if (multicast && h->P.env_params)
-    return fail(UPKIE_B200_EINVAL, "the per-env parameter table has no in-kernel rollout transport (use upkie_b200_step "
-                                   "with compact rows)");
-  if (multicast && h->P.push)
-    return fail(UPKIE_B200_EINVAL, "push randomisation has no in-kernel rollout transport (use upkie_b200_step with "
-                                   "compact rows)");
-  if (multicast && h->P.max_episode_steps > 0)
-    return fail(UPKIE_B200_EINVAL, "max_episode_steps has no in-kernel rollout transport: it does not carry truncated "
-                                   "(use upkie_b200_step with compact rows)");
+  const int transport = multicast ? 2 : (tile ? 1 : 0);  // the TILE of the step kernels
+  const char* why = nullptr;
+  const int family = step_family(h->P, h->ext != nullptr, mode, transport, &why);
+  if (family < 0) return fail(UPKIE_B200_EINVAL, why);
   StepArgs a;
   std::memset(&a.peers, 0, sizeof(a.peers));
   if (peers) a.peers = *peers;
@@ -350,22 +375,8 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   }
   a.mode = mode;
   a.autoreset = h->autoreset;
-  a.noise = h->P.joint_limits ? 2 : ((h->P.any_ctrl_noise || h->P.any_meas_noise || h->ext) ? 1 : 0);  // "extras" kernels
-  if (a.noise == 2 && h->P.env_params) a.noise = 5;  // the NOISE=2 kernels carry no table reads (step_*_table.cu)
-  if (h->P.body_contacts) {  // the model's collision points hold contact rows: the NOISE=4 kernels (step_*_body.cu)
-    if (multicast) return fail(UPKIE_B200_EINVAL, "body_contacts has no in-kernel rollout transport (use upkie_b200_step_servos_compact)");
-    a.noise = 4;
-  }
-  // push randomisation: the table or body-contact family compiled with the pushes (step_*_push.cu), so that the
-  // NOISE=4 / 5 kernels keep their code (the set call rejects spine mode and joint_limits = 0)
-  if (h->P.push) a.noise = a.noise == 4 ? 7 : 6;
-  a.lag = nullptr;
-  if (h->P.spine_mode) {
-    if (mode != MODE_SERVOS) return fail(UPKIE_B200_EINVAL, "spine_mode supports UpkieServos steps only");
-    if (multicast) return fail(UPKIE_B200_EINVAL, "spine_mode has no in-kernel rollout transport");
-    a.noise = 3;
-    a.lag = h->lag;
-  }
+  a.family = family;
+  a.lag = h->P.spine_mode ? h->lag : nullptr;
   a.ext = h->ext;
   a.ext_local = h->ext_local;
   a.i0 = i0;
@@ -394,7 +405,7 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   a.seed = h->seed;
   a.env_offset = h->env_offset;
   a.stream = s;
-  CUDA_TRY(multicast ? launch_step_multicast(a) : (tile ? launch_step_host(a) : launch_step_device(a)));
+  CUDA_TRY(dispatch_step(transport, a));
   h->step_launches += 1;
   return UPKIE_B200_OK;
 }
