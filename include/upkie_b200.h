@@ -693,6 +693,43 @@ int upkie_b200_get_push_forces(void* handle, float* force, void* stream);
 int upkie_b200_get_push_state(void* handle, uint32_t* count, uint32_t* timer, void* stream);
 int upkie_b200_set_push_state(void* handle, const uint32_t* count, const uint32_t* timer, void* stream);
 
+/* Action-delay randomisation (an addition to ABI 8: no existing layout, constant or signature changed). While a spec is
+ * set, every env applies its servo command d_i substeps into the tick, 0 <= d_i <= nb_substeps. The servo command is
+ * the clamped [UPKIE_ACT_DIM] row the torque law reads: the clamped action of step_servos, and of step_gyropod /
+ * step_pendulum the row their action front end builds from the action. A tick then runs substeps 0 .. d_i - 1 under the
+ * command of the env's previous tick and substeps d_i .. nb_substeps - 1 under its own; d_i = nb_substeps runs the
+ * whole tick on the previous command (one tick of latency, the most there is). The gyropod leg filter, the yaw
+ * integration and the clamp flags of the error flags stay at the start of the tick; torque-control noise keeps its
+ * per-substep keys.
+ * At every reset of the env (both fused auto-resets, and upkie_b200_reset with device-sampled or host init rows, masked
+ * or not) the previous command becomes the stop row, per joint {position NaN, velocity 0, feedforward 0, kp_scale 0,
+ * kd_scale 0, maximum_torque 0}, whose torque is exactly 0 (the torque limit is applied last), and a new d_i is drawn:
+ * the first d_i substeps of an episode run with the servos stopped. The reset substep runs as without a spec; the
+ * terminal step of a same-step auto-reset runs under the delay in force, and its reset then applies.
+ * Draw law: a per-env counter k, +1 at every reset; the reset uses draw k (after the +1). Draw k of the env of global
+ * index g = env_offset + i (the seed and env_offset of upkie_b200_set_autoreset) is Philox4x32-10 with key seed and
+ * counter (g, 2^61 | k << 4), whose word w0 gives
+ *   d = substeps_low + (((w0 >> 8) * (substeps_high - substeps_low + 1)) >> 24)          (integer arithmetic, exact)
+ * The tag bit 61 keeps these counters apart from those of the initial states ((episode << 2) | b, below 2^34), the
+ * reset randomisation (bit 63) and the push randomisation (bit 62). The draws depend neither on the physics nor on the
+ * number of GPUs.
+ * Setting a spec draws nothing: each env keeps its delay (0 on a handle that never had a spec) until its next reset,
+ * where a changed spec takes effect. NULL turns the delay off; the state stays. Per-env state
+ * (upkie_b200_get_action_delay_state / set_action_delay_state, for checkpoints): count[N], delay[N] and the previous
+ * command[N][UPKIE_ACT_DIM] (device pointers); 0, 0 and stop rows on a handle that never had a spec. A delay above
+ * nb_substeps acts as nb_substeps.
+ * Needs joint_limits != 0 (the delay runs in copies of the table and body-contact kernels). Rejected with
+ * UPKIE_B200_EINVAL, the previous spec kept: substeps_low > substeps_high, substeps_high > nb_substeps, joint_limits
+ * == 0, spine_mode (which models the spine's own lag). upkie_b200_set_config rejects an nb_substeps below a set spec's
+ * substeps_high; the in-kernel rollout transports reject a handle with a spec. The set call waits for the device. */
+typedef struct UpkieActionDelay {
+  uint32_t substeps_low, substeps_high; /* range of the delay, in substeps of dt / nb_substeps */
+} UpkieActionDelay;
+int upkie_b200_set_action_delay(void* handle, const UpkieActionDelay* spec);
+int upkie_b200_get_action_delay_state(void* handle, uint32_t* count, uint32_t* delay, float* command, void* stream);
+int upkie_b200_set_action_delay_state(void* handle, const uint32_t* count, const uint32_t* delay, const float* command,
+                                      void* stream);
+
 /* Number of step-kernel launches issued through this handle since create
  * (bench.py's `gpu_launches`). */
 int upkie_b200_launch_count(void* handle, uint64_t* count);

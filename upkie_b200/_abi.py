@@ -380,6 +380,15 @@ class UpkiePushRandomization(C.Structure):
     ]
 
 
+class UpkieActionDelay(C.Structure):
+    """``UpkieActionDelay`` of include/upkie_b200.h: the range of each env's action delay, in substeps."""
+
+    _fields_ = [
+        ("substeps_low", C.c_uint32),
+        ("substeps_high", C.c_uint32),
+    ]
+
+
 def default_mpc_config() -> UpkieMpcConfig:
     """``MPCBalancer.__init__`` defaults (``mpc_balancer.py:168-181``)."""
     c = UpkieMpcConfig()

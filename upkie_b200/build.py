@@ -13,7 +13,8 @@ SOURCES = ["upkie_b200.cu", "step_device.cu", "step_host.cu", "step_multicast.cu
            "step_host_limits.cu", "step_multicast_limits.cu", "step_device_spine.cu", "step_host_spine.cu",
            "step_device_body.cu", "step_host_body.cu", "step_device_table.cu", "step_host_table.cu", "base_velocity.cu",
            "reset_randomization.cu", "pushes.cu", "step_device_push.cu", "step_host_push.cu",
-           "step_device_body_push.cu", "step_host_body_push.cu"]
+           "step_device_body_push.cu", "step_host_body_push.cu", "action_delay.cu", "step_device_delay.cu",
+           "step_host_delay.cu", "step_device_body_delay.cu", "step_host_body_delay.cu"]
 DEPS = SOURCES + ["base_velocity.cuh", "base_velocity_core.cuh",
     "sim_core.cuh", "sim_pair.cuh", "kernel_common.cuh", "step_kernel.cuh", "step_family.h", "params.h", "mpc.cuh",
     "mpc_core.cuh",
@@ -65,7 +66,8 @@ def is_stale() -> bool:
 # (fast-math) costs in accuracy and buys in time.
 EXACT_LIB_PATH = os.path.join(_HERE, "libupkie_b200_exact.so")
 EXACT_SOURCES = ["upkie_b200.cu", "step_device.cu", "step_device_limits.cu", "exact_stubs.cu", "base_velocity.cu",
-                 "reset_randomization.cu", "pushes.cu"]
+                 "reset_randomization.cu", "pushes.cu",
+                 "action_delay.cu"]
 EXACT_FLAGS = [f for f in NVCC_FLAGS if f != "--use_fast_math"] + ["-DUPKIE_EXACT_BUILD=1"]
 
 

@@ -134,5 +134,11 @@ cudaError_t launch_push_reset(const PushRand* R, int n, const uint8_t* mask, uin
                               cudaStream_t stream);  // the envs an upkie_b200_reset takes restart, before k_reset
 cudaError_t launch_push_forces(const PushRand* R, int n, uint64_t seed, uint64_t env_offset, float* force,
                                cudaStream_t stream);  // R null: zeros
+// action_delay.cu: the handle-side kernels of action-delay randomisation (upkie_b200_set_action_delay)
+cudaError_t launch_action_delay_reset(const ActionDelay* A, int n, const uint8_t* mask, uint64_t seed,
+                                      uint64_t env_offset, cudaStream_t stream);  // before k_reset
+// command rows [n][UPKIE_ACT_DIM] <-> the buffer's columns [UPKIE_ACT_DIM][stride]; a null source gives stop rows
+cudaError_t launch_command_rows(const float* cols, int n, int stride, float* rows, cudaStream_t stream);
+cudaError_t launch_command_cols(const float* rows, int n, int stride, float* cols, cudaStream_t stream);
 
 }  // namespace upkie_b200

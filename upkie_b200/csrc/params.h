@@ -258,6 +258,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.final_state = nullptr;
   P.reset_rand = nullptr;
   P.push = nullptr;
+  P.action_delay = nullptr;
   return 0;
 }
 
@@ -336,6 +337,17 @@ inline bool push_spec_valid(const UpkiePushRandomization& s) {
     if (!(std::fabs(lo) <= 3.402823466e38f) || !(std::fabs(hi) <= 3.402823466e38f) || lo > hi) return false;
   }
   return true;
+}
+
+// Why a handle with parameters P refuses an action-delay spec (upkie_b200_set_action_delay), null when it takes it
+inline const char* action_delay_spec_error(const UpkieActionDelay& s, const SimParams& P) {
+  if (s.substeps_low > s.substeps_high) return "set_action_delay: substeps_low > substeps_high";
+  if (s.substeps_high > uint32_t(P.nb_substeps))
+    return "set_action_delay: substeps_high above nb_substeps (the delay is at most one tick)";
+  if (P.joint_limits == 0)
+    return "set_action_delay: needs joint_limits != 0 (the delay runs in the table and body-contact kernels)";
+  if (P.spine_mode) return "set_action_delay: spine_mode models the spine's own lag";
+  return nullptr;
 }
 
 inline void set_noise_flags(SimParams& P, uint32_t f) {

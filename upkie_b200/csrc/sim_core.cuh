@@ -138,6 +138,9 @@ struct SimParams {
   // push randomisation (upkie_b200_set_push_randomization): the handle's device block, null = off. Read by the
   // step kernels of the push families (step_family.h) only. Appended last, as reset_rand above.
   const struct PushRand* push;
+  // action-delay randomisation (upkie_b200_set_action_delay): the handle's device block, null = off. Read by the step
+  // kernels of the delay families (step_family.h) only. Appended last, as push above.
+  const struct ActionDelay* action_delay;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -1790,6 +1793,59 @@ UPKIE_HD void push_reset(const PushRand& R, uint64_t seed, uint64_t g, int i) {
   push_restart(k, t, d.gap + d.duration);
   R.count[i] = k;
   R.timer[i] = t;
+}
+
+// ---- action-delay randomisation (upkie_b200_set_action_delay) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw, delay[i] = d_i in substeps, and command = the servo command of each env's previous tick,
+// [UPKIE_ACT_DIM][stride] structure-of-arrays like the state, env i in column i.
+struct ActionDelay {
+  UpkieActionDelay spec;
+  uint32_t* count;
+  uint32_t* delay;
+  float* command;
+  int stride;
+};
+
+// bit 61 of the high counter word: never set by sample_init_state ((episode << 2) | b, episode < 2^32), the noise
+// ((tick << 10) | (slot << 1) | b, tick < 2^32), the reset randomisation (bit 63 set) or the pushes (bit 62 set)
+constexpr uint64_t kActionDelayTag = uint64_t(1) << 61;
+
+// Draw k of the env of global index g: its delay in substeps, push_steps' exact integer form
+UPKIE_HD uint32_t action_delay_draw(const UpkieActionDelay& s, uint64_t seed, uint64_t g, uint32_t k) {
+  const Philox4 r = philox4x32_10(g, kActionDelayTag | (uint64_t(k) << 4), seed);
+  return push_steps(r.v[0], s.substeps_low, s.substeps_high);
+}
+
+// The previous command an env holds after a reset: servos stopped, {position NaN, velocity 0, feedforward 0, kp_scale 0,
+// kd_scale 0, maximum_torque 0} per joint. joint_torque clips last, to [-0, 0]: the torque is exactly zero whatever
+// the state, friction and torque-control noise.
+UPKIE_HD float action_delay_stop_value(int k) { return (k % UPKIE_ACT_KEYS) == UPKIE_ACT_POSITION ? nanf("") : 0.f; }
+
+// The command of substep `sub` of a tick with delay d, in `a`: the tick enters its substeps with the previous command in
+// `a`, and substep d (never reached for d >= nb_substeps) first replaces it with this tick's, load(c) for c = 0 ..
+// UPKIE_ACT_DIM - 1. The step kernels load it back from the command buffer, so that only one row is held in registers.
+template <typename Load>
+UPKIE_HD void action_delay_substep(int sub, uint32_t d, float a[UPKIE_ACT_DIM], Load load) {
+  if (uint32_t(sub) == d) {
+#pragma unroll
+    for (int c = 0; c < UPKIE_ACT_DIM; ++c) a[c] = load(c);
+  }
+}
+
+// A reset of env i (the step kernels' fused resets, k_action_delay_reset): the next draw, and the stop row as the
+// previous command. The block's fields are copied before the first store, which the compiler cannot tell apart from
+// the block itself.
+UPKIE_HD void action_delay_reset(const ActionDelay& A, uint64_t seed, uint64_t g, int i) {
+  const UpkieActionDelay spec = A.spec;
+  uint32_t* const count = A.count;
+  uint32_t* const delay = A.delay;
+  float* const col = A.command + size_t(i);
+  const size_t stride = size_t(A.stride);
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  delay[i] = action_delay_draw(spec, seed, g, k);
+  for (int c = 0; c < UPKIE_ACT_DIM; ++c) col[size_t(c) * stride] = action_delay_stop_value(c);
 }
 
 }  // namespace upkie_b200

@@ -22,7 +22,9 @@ enum {
   FAM_TABLE = 5,      // extras + limits + the per-env parameter table + reset randomisation
   FAM_PUSH = 6,       // FAM_TABLE + push randomisation
   FAM_BODY_PUSH = 7,  // FAM_BODY + push randomisation
-  kNumFamilies = 8
+  FAM_DELAY = 8,      // FAM_PUSH + action delay
+  FAM_BODY_DELAY = 9, // FAM_BODY_PUSH + action delay
+  kNumFamilies = 10
 };
 
 // What a family's kernels compile in
@@ -34,19 +36,22 @@ struct StepFamily {
   bool spine;       // spine timing, UpkieServos: the lag record, spine_cycle
   bool body;        // body-contact record (BodyRecOut); units built with UPKIE_BODY_CONTACTS_BUILD 1
   bool push;        // the push schedule
+  bool delay;       // the action delay: previous command rows, per-env delays
 };
 
 UPKIE_HD constexpr StepFamily step_family_traits(int family) {
   constexpr StepFamily t[kNumFamilies] = {
-      // extras limits table  reset_rand spine  body   push
-      {false, false, true, false, false, false, false},  // FAM_PLAIN
-      {true, false, true, false, false, false, false},   // FAM_EXTRAS
-      {true, true, false, false, false, false, false},   // FAM_LIMITS
-      {true, true, true, true, true, true, false},       // FAM_SPINE
-      {true, true, true, true, false, true, false},      // FAM_BODY
-      {true, true, true, true, false, false, false},     // FAM_TABLE
-      {true, true, true, true, false, false, true},      // FAM_PUSH
-      {true, true, true, true, false, true, true},       // FAM_BODY_PUSH
+      // extras limits table  reset_rand spine  body   push   delay
+      {false, false, true, false, false, false, false, false},  // FAM_PLAIN
+      {true, false, true, false, false, false, false, false},   // FAM_EXTRAS
+      {true, true, false, false, false, false, false, false},   // FAM_LIMITS
+      {true, true, true, true, true, true, false, false},       // FAM_SPINE
+      {true, true, true, true, false, true, false, false},      // FAM_BODY
+      {true, true, true, true, false, false, false, false},     // FAM_TABLE
+      {true, true, true, true, false, false, true, false},      // FAM_PUSH
+      {true, true, true, true, false, true, true, false},       // FAM_BODY_PUSH
+      {true, true, true, true, false, false, true, true},       // FAM_DELAY
+      {true, true, true, true, false, true, true, true},        // FAM_BODY_DELAY
   };
   return t[family];
 }
@@ -61,6 +66,8 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "the per-env parameter table has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.push)
     no = "push randomisation has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
+  else if (in_kernel && P.action_delay)
+    no = "action delay has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.max_episode_steps > 0)
     no = "max_episode_steps has no in-kernel rollout transport: it does not carry truncated (use upkie_b200_step with "
          "compact rows)";
@@ -75,6 +82,9 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     return -1;
   }
   if (P.spine_mode) return FAM_SPINE;
+  // the delay families carry the pushes too (a runtime-uniform branch on P.push); the set calls reject spine mode and
+  // no limits
+  if (P.action_delay) return P.body_contacts ? FAM_BODY_DELAY : FAM_DELAY;
   if (P.push) return P.body_contacts ? FAM_BODY_PUSH : FAM_PUSH;  // the set call rejects spine mode and no limits
   if (P.body_contacts) return FAM_BODY;  // the model's collision points hold contact rows
   if (P.joint_limits) return P.env_params ? FAM_TABLE : FAM_LIMITS;

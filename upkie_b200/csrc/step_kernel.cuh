@@ -234,6 +234,36 @@ __device__ __forceinline__ void step_env(
     if (MODE != MODE_SERVOS) e |= gyropod_action(P, S, a0, a1, a);
     e |= clamp_servo_action(P, a);
   }
+  // action delay (F.delay kernels, P.action_delay set: a uniform branch). A tick swaps this tick's command into the
+  // env's column of the command buffer and enters its substeps with the previous one in `a`; substep `dly` loads the
+  // new one back (action_delay_substep), so that one row is held in registers. A next-step reset draws and holds the
+  // stop row instead; its reset substep never switches.
+  // The buffer's address and stride are read into registers once and the row goes through global-space accesses:
+  // reached through the generic pointers of the device block, every store of the row could alias the block, and each
+  // of the 36 elements then re-read the pointer and waited for it (a chain of dependent loads per env that made the
+  // tick 2.2 times as long). The previous row is read whole before the new one is written. The loads are coherent
+  // (ld.global.cg), not the read-only path, which need not return a thread's own stores of the same launch.
+  const bool delaying = F.delay && P.action_delay;
+  uint32_t dly = 0xffffffffu;
+  if (delaying) {
+    const ActionDelay& A = *P.action_delay;
+    if (resetting) {
+      if (live) action_delay_reset(A, seed, env_offset + uint64_t(i), i);
+    } else {
+      float* const col = A.command + size_t(i);
+      const size_t stride = size_t(A.stride);
+      dly = __ldcg(A.delay + i);
+      float prev[UPKIE_ACT_DIM];
+#pragma unroll
+      for (int c = 0; c < UPKIE_ACT_DIM; ++c) prev[c] = __ldcg(col + size_t(c) * stride);
+      if (live) {
+#pragma unroll
+        for (int c = 0; c < UPKIE_ACT_DIM; ++c) __stcg(col + size_t(c) * stride, a[c]);
+      }
+#pragma unroll
+      for (int c = 0; c < UPKIE_ACT_DIM; ++c) a[c] = prev[c];
+    }
+  }
   if (spine && !resetting) spine_assemble_observation(S, L);  // the first cycle's observation (Spine.cpp:126-131)
   const int nloop = (AUTORESET == AUTORESET_NEXT_STEP && spine && P.nb_substeps < 3) ? 3 : P.nb_substeps;
   for (int sub = 0; sub < nloop; ++sub) {
@@ -241,6 +271,12 @@ __device__ __forceinline__ void step_env(
     __syncthreads();  // once per substep: all threads are converged here
 #endif
     if (sub < nsub) {
+      if (delaying) {
+        action_delay_substep(sub, dly, a, [&](int c) {
+          const ActionDelay& A = *P.action_delay;
+          return __ldcg(A.command + size_t(c) * size_t(A.stride) + size_t(i));
+        });
+      }
       // the body-ground contacts of the tick's last substep go to the handle's record (F.body kernels)
       const BodyRecOut br{(F.body && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
                           size_t(P.body_rec_stride)};
@@ -306,6 +342,8 @@ __device__ __forceinline__ void step_env(
       if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
       if (F.reset_rand && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
       if (pushing) push_restart(push_k, push_t, push_end);  // the terminal step ran under its push; a new schedule
+      // the terminal step ran under its delay; the next tick starts from the stop row with a new one
+      if (delaying && live) action_delay_reset(*P.action_delay, seed, env_offset + uint64_t(i), i);
       elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;

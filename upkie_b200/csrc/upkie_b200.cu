@@ -104,6 +104,13 @@ struct Handle {
   uint32_t* push_count = nullptr;
   uint32_t* push_timer = nullptr;
   int push_body = 0;             // the body of the spec in force
+  // action-delay randomisation (upkie_b200_set_action_delay): the device block P.action_delay points to while a spec
+  // is set, and the per-env state (allocated on the first spec or set_action_delay_state)
+  ActionDelay* delay_dev = nullptr;
+  uint32_t* delay_count = nullptr;
+  uint32_t* delay_delay = nullptr;
+  float* delay_command = nullptr;  // [UPKIE_ACT_DIM][n_pad]
+  uint32_t delay_high = 0;         // substeps_high of the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -325,6 +332,8 @@ cudaError_t dispatch_step(int tile, const StepArgs& a) {
     case tile_family(0, FAM_TABLE): return launch_step<0, FAM_TABLE>(a);
     case tile_family(0, FAM_PUSH): return launch_step<0, FAM_PUSH>(a);
     case tile_family(0, FAM_BODY_PUSH): return launch_step<0, FAM_BODY_PUSH>(a);
+    case tile_family(0, FAM_DELAY): return launch_step<0, FAM_DELAY>(a);
+    case tile_family(0, FAM_BODY_DELAY): return launch_step<0, FAM_BODY_DELAY>(a);
     case tile_family(1, FAM_PLAIN): return launch_step<1, FAM_PLAIN>(a);
     case tile_family(1, FAM_EXTRAS): return launch_step<1, FAM_EXTRAS>(a);
     case tile_family(1, FAM_LIMITS): return launch_step<1, FAM_LIMITS>(a);
@@ -333,6 +342,8 @@ cudaError_t dispatch_step(int tile, const StepArgs& a) {
     case tile_family(1, FAM_TABLE): return launch_step<1, FAM_TABLE>(a);
     case tile_family(1, FAM_PUSH): return launch_step<1, FAM_PUSH>(a);
     case tile_family(1, FAM_BODY_PUSH): return launch_step<1, FAM_BODY_PUSH>(a);
+    case tile_family(1, FAM_DELAY): return launch_step<1, FAM_DELAY>(a);
+    case tile_family(1, FAM_BODY_DELAY): return launch_step<1, FAM_BODY_DELAY>(a);
     case tile_family(2, FAM_PLAIN): return launch_step<2, FAM_PLAIN>(a);
     case tile_family(2, FAM_EXTRAS): return launch_step<2, FAM_EXTRAS>(a);
     case tile_family(2, FAM_LIMITS): return launch_step<2, FAM_LIMITS>(a);
@@ -719,6 +730,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->tick); cudaFree(h->elapsed); cudaFree(h->ext); cudaFree(h->lag); cudaFree(h->body_rec);
   cudaFree(h->env_params); cudaFree(h->ep_check); cudaFree(h->final_state); cudaFree(h->rr_dev); cudaFree(h->draws);
   cudaFree(h->push_dev); cudaFree(h->push_count); cudaFree(h->push_timer);
+  cudaFree(h->delay_dev); cudaFree(h->delay_count); cudaFree(h->delay_delay); cudaFree(h->delay_command);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -748,6 +760,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: reset randomisation needs joint_limits != 0");
   if (h->P.push && P.joint_limits == 0)
     return fail(UPKIE_B200_EINVAL, "set_config: push randomisation needs joint_limits != 0");
+  if (h->P.action_delay && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: action delay needs joint_limits != 0");
+  if (h->P.action_delay && uint32_t(P.nb_substeps) < h->delay_high)
+    return fail(UPKIE_B200_EINVAL, "set_config: nb_substeps below the action delay's substeps_high");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -765,6 +781,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   }
   P.reset_rand = h->P.reset_rand;  // so does the reset randomisation
   P.push = h->P.push;              // and the push randomisation
+  P.action_delay = h->P.action_delay;  // and the action delay
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -976,6 +993,9 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
   if (h->P.reset_rand) CUDA_TRY(launch_reset_rand(h->rr_dev, h->n, mask, h->seed, h->env_offset, s));
   // push randomisation: the envs this reset takes start a new schedule
   if (h->P.push) CUDA_TRY(launch_push_reset(h->push_dev, h->n, mask, h->seed, h->env_offset, s));
+  // action delay: the envs this reset takes draw their next delay and hold the stop row
+  if (h->P.action_delay)
+    CUDA_TRY(launch_action_delay_reset(h->delay_dev, h->n, mask, h->seed, h->env_offset, s));
   k_reset<<<grid, rblock, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
                                     h->done_prev, h->episode, seed, env_offset, h->lag);
   CUDA_TRY(cudaGetLastError());
@@ -1377,6 +1397,91 @@ int upkie_b200_set_push_state(void* handle, const uint32_t* count, const uint32_
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
   CUDA_TRY(cudaMemcpyAsync(h->push_count, count, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(h->push_timer, timer, bytes, cudaMemcpyDeviceToDevice, s));
+  return UPKIE_B200_OK;
+}
+
+namespace {
+// the per-env action-delay state: counters 0, delays 0 and stop rows on a handle that has none yet
+// (the three buffers are set together: a failure frees what was allocated, so that a handle holds all or none)
+int alloc_delay_state(Handle* h) {
+  if (h->delay_count) return UPKIE_B200_OK;
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  uint32_t *count = nullptr, *delay = nullptr;
+  float* command = nullptr;
+  cudaError_t e = cudaMalloc(&count, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&delay, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&command, size_t(UPKIE_ACT_DIM) * h->n_pad * sizeof(float));
+  if (e == cudaSuccess) e = cudaMemset(count, 0, bytes);
+  if (e == cudaSuccess) e = cudaMemset(delay, 0, bytes);
+  if (e == cudaSuccess) e = launch_command_cols(nullptr, h->n, h->n_pad, command, nullptr);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    cudaFree(count); cudaFree(delay); cudaFree(command);
+    return fail(UPKIE_B200_ECUDA, std::string("action delay state: ") + cudaGetErrorString(e));
+  }
+  h->delay_count = count;
+  h->delay_delay = delay;
+  h->delay_command = command;
+  return UPKIE_B200_OK;
+}
+}  // namespace
+
+int upkie_b200_set_action_delay(void* handle, const UpkieActionDelay* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    // off: the kernels enqueued before keep the block they were launched with, which stays allocated
+    h->P.action_delay = nullptr;
+    h->delay_high = 0;
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = action_delay_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
+  if (alloc_delay_state(h)) return UPKIE_B200_ECUDA;
+  if (!h->delay_dev) CUDA_TRY(cudaMalloc(&h->delay_dev, sizeof(ActionDelay)));
+  ActionDelay A;
+  std::memset(&A, 0, sizeof(A));
+  A.spec = *spec;
+  A.count = h->delay_count;
+  A.delay = h->delay_delay;
+  A.command = h->delay_command;
+  A.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->delay_dev, &A, sizeof(A), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->delay_high = spec->substeps_high;
+  h->P.action_delay = h->delay_dev;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_action_delay_state(void* handle, uint32_t* count, uint32_t* delay, float* command, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !delay || !command) return fail(UPKIE_B200_EINVAL, "get_action_delay_state: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  if (h->delay_count) {
+    CUDA_TRY(cudaMemcpyAsync(count, h->delay_count, bytes, cudaMemcpyDeviceToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(delay, h->delay_delay, bytes, cudaMemcpyDeviceToDevice, s));
+  } else {
+    CUDA_TRY(cudaMemsetAsync(count, 0, bytes, s));
+    CUDA_TRY(cudaMemsetAsync(delay, 0, bytes, s));
+  }
+  CUDA_TRY(launch_command_rows(h->delay_command, h->n, h->n_pad, command, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_action_delay_state(void* handle, const uint32_t* count, const uint32_t* delay, const float* command,
+                                      void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !delay || !command) return fail(UPKIE_B200_EINVAL, "set_action_delay_state: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (alloc_delay_state(h)) return UPKIE_B200_ECUDA;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  CUDA_TRY(cudaMemcpyAsync(h->delay_count, count, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(h->delay_delay, delay, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(launch_command_cols(command, h->n, h->n_pad, h->delay_command, s));
   return UPKIE_B200_OK;
 }
 

@@ -511,6 +511,39 @@ def push_randomization_spec(spec: Optional[dict], model: Model, dt: float) -> Op
     return out
 
 
+def action_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool = False,
+                      joint_limits: Union[bool, int] = True) -> Optional[Tuple[int, int]]:
+    """``(substeps_low, substeps_high)`` (``UpkieSim.set_action_delay``) from an action delay in seconds: a float, or a
+    ``(low, high)`` pair from which every reset draws an env's delay. Rounded to the nearest substep of ``dt /
+    nb_substeps`` (halves up). Raises ``UpkieException`` on a negative or non-finite bound, ``low > high``, a delay
+    of more than one tick (``nb_substeps`` substeps), ``spine_mode`` (which models the spine's own lag) and no joint
+    limits (the delay runs in the kernels with joint-limit rows)."""
+    if delay is None:
+        return None
+    if isinstance(delay, (int, float, np.integer, np.floating)):
+        lo, hi = delay, delay
+    else:
+        try:
+            lo, hi = delay
+        except (TypeError, ValueError):
+            raise UpkieException(f"action_delay: expected seconds or a (low, high) pair, got {delay!r}") from None
+    try:
+        lo, hi = float(lo), float(hi)
+    except (TypeError, ValueError):
+        raise UpkieException(f"action_delay: expected seconds, got ({lo!r}, {hi!r})") from None
+    if not (np.isfinite(lo) and np.isfinite(hi)) or not 0.0 <= lo <= hi:
+        raise UpkieException(f"action_delay: expected finite seconds 0 <= low <= high, got ({lo}, {hi})")
+    if spine_mode:
+        raise UpkieException("action_delay: spine_mode models the spine's own lag; the delay is not available there")
+    if not joint_limits:
+        raise UpkieException("action_delay: needs joint_limits (the delay runs in the kernels with joint-limit rows)")
+    substep = dt / int(nb_substeps)
+    lo_s, hi_s = (int(np.floor(x / substep + 0.5)) for x in (lo, hi))
+    if hi_s > int(nb_substeps):
+        raise UpkieException(f"action_delay: {hi} s is more than one tick ({nb_substeps} substeps of {substep} s)")
+    return lo_s, hi_s
+
+
 class B200VectorEnv(VectorEnv):
     """N Upkie environments stepped by one kernel launch per ``step()``.
 
@@ -548,6 +581,12 @@ class B200VectorEnv(VectorEnv):
     ``set_external_forces`` of the reference's ``apply_external_forces.py``, without a host round trip per step. The
     pushes add to the forces of ``set_external_forces``. They are keyed on the seed of ``reset(seed=s)``, which also
     restarts the schedules of the envs it resets. ``set_push_randomization`` changes or (``None``) stops them.
+
+    ``action_delay`` (seconds, a float or a ``(low, high)`` range, see ``action_delay_spec``) delays each env's servo
+    command by a number of substeps drawn at every reset of that env, up to one tick: the substeps before it run the
+    command of the previous tick, and the first ones of an episode run with the servos stopped. The draws are keyed on
+    the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets.
+    ``set_action_delay`` changes or (``None``) stops it from each env's next reset.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -583,6 +622,7 @@ class B200VectorEnv(VectorEnv):
         max_episode_steps: int = 0,
         reset_randomization: Optional[dict] = None,
         push_randomization: Optional[dict] = None,
+        action_delay: Optional[Union[float, Tuple[float, float]]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -624,6 +664,8 @@ class B200VectorEnv(VectorEnv):
             config = _abi.UpkieSimConfig.from_buffer_copy(config)
             config.max_episode_steps = max_episode_steps
         self.config = config
+        delay_spec = action_delay_spec(action_delay, 1.0 / frequency, config.nb_substeps, bool(config.spine_mode),
+                                       config.joint_limits)  # validated before any device is touched
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -672,6 +714,8 @@ class B200VectorEnv(VectorEnv):
             self.sim.set_reset_randomization(rr_spec)
         if push_spec is not None:
             self.sim.set_push_randomization(push_spec)
+        if delay_spec is not None:
+            self.sim.set_action_delay(*delay_spec)  # before the first reset, which draws every env's delay
 
     def set_reset_randomization(self, spec: Optional[dict]) -> None:
         """Redraw the parameters ``spec`` names at every later reset of an env (``reset_randomization_spec``);
@@ -682,6 +726,13 @@ class B200VectorEnv(VectorEnv):
         """Push every env at random times by random forces (``push_randomization_spec``, times in seconds of this
         env's ``dt``); ``None`` stops pushing. Takes effect from the next step; no schedule restarts."""
         self.sim.set_push_randomization(push_randomization_spec(spec, self.model, self.dt))
+
+    def set_action_delay(self, delay) -> None:
+        """Delay the servo commands by ``delay`` seconds, a float or a ``(low, high)`` range (``action_delay_spec``);
+        ``None`` turns the delay off. A new range takes effect at each env's next reset."""
+        spec = action_delay_spec(delay, self.dt, self.config.nb_substeps, bool(self.config.spine_mode),
+                                 self.config.joint_limits)
+        self.sim.set_action_delay(*(spec if spec is not None else (None,)))
 
     # ------------------------------------------------------------------
     def get_neutral_action(self) -> dict:
@@ -815,6 +866,14 @@ class B200VectorEnv(VectorEnv):
                     count.masked_fill_(m, 0)
                     timer.masked_fill_(m, 0)
                 self.sim.set_push_state(count, timer)
+            if getattr(self.sim, "_action_delay", None) is not None:
+                # so is the action delay: the envs reset here restart from count 0 (their reset then makes draw 1)
+                count, delay, command = self.sim.get_action_delay_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_action_delay_state(count, delay, command)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

@@ -186,6 +186,39 @@ class UpkieSim:
         self._check_tensor(timer, (self.n,), torch.int32, "timer")
         check(lib().upkie_b200_set_push_state(self._h, _ptr(count), _ptr(timer), self._stream()))
 
+    def set_action_delay(self, low: Optional[int], high: Optional[int] = None) -> None:
+        """While a range is set, every env applies its servo command ``d`` substeps into each tick, ``low <= d <= high
+        <= nb_substeps``: the substeps before ``d`` run the command of its previous tick. Each reset of the env draws a
+        new ``d`` (keyed on the auto-reset seed and the env's counter, ``include/upkie_b200.h``) and stops the servos
+        until the first command takes over. ``high`` defaults to ``low``; ``None`` turns the delay off. Setting a range
+        draws nothing: it takes effect at each env's next reset."""
+        if low is None:
+            check(lib().upkie_b200_set_action_delay(self._h, None))
+            self._action_delay = None
+            return
+        spec = _abi.UpkieActionDelay(int(low), int(low if high is None else high))
+        check(lib().upkie_b200_set_action_delay(self._h, C.byref(spec)))
+        self._action_delay = (spec.substeps_low, spec.substeps_high)
+        self._delay_state_set = True  # the handle holds a state from now on
+
+    def get_action_delay_state(self):
+        """Per-env action-delay state ``(count[N], delay[N], command[N, 6, 6])``: the draw counters (int32 bits of
+        uint32), the delays in substeps and the servo command of each env's previous tick."""
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        delay = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        command = torch.empty((self.n, _abi.NJ, len(_abi.ACT_KEYS)), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_action_delay_state(self._h, _ptr(count), _ptr(delay), _ptr(command),
+                                                      self._stream()))
+        return count, delay, command
+
+    def set_action_delay_state(self, count: torch.Tensor, delay: torch.Tensor, command: torch.Tensor) -> None:
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(delay, (self.n,), torch.int32, "delay")
+        self._check_tensor(command, (self.n, _abi.NJ, len(_abi.ACT_KEYS)), name="command")
+        check(lib().upkie_b200_set_action_delay_state(self._h, _ptr(count), _ptr(delay), _ptr(command),
+                                                      self._stream()))
+        self._delay_state_set = True
+
     def set_external_forces(self, force: Optional[torch.Tensor] = None, local_mask: int = 0) -> None:
         """``force[N, 7, 3]`` newtons at the centres of mass of the 7 bodies, applied on every substep of
         the following steps until overwritten; ``None`` clears. Bit ``b`` of ``local_mask``: the force on
@@ -553,12 +586,17 @@ class UpkieSim:
         spec = getattr(self, "_reset_randomization", None)
         push = getattr(self, "_push_randomization", None)
         push_count, push_timer = self.get_push_state()
+        delay_count, delay_delay, delay_command = self.get_action_delay_state()
         force, local_mask = getattr(self, "_external", (None, 0))
         return {
             "reset_randomization": None if spec is None else bytes(spec),  # the UpkieResetRandomization in force
             "draws": self.get_draws(),  # per-env draw counters of the reset randomisation
             "push_randomization": None if push is None else bytes(push),  # the UpkiePushRandomization in force
             "push_count": push_count, "push_timer": push_timer,  # per-env push schedule state
+            "action_delay": getattr(self, "_action_delay", None),  # (substeps_low, substeps_high) in force, or None
+            # per-env action-delay state: draw counters, delays, previous servo commands
+            "action_delay_count": delay_count, "action_delay_delay": delay_delay,
+            "action_delay_command": delay_command,
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
             "elapsed": elapsed,  # steps since each env's last reset (the time limit's counts)
@@ -608,12 +646,34 @@ class UpkieSim:
         count, timer = sd.get("push_count"), sd.get("push_timer")
         self.set_push_state(zeros if count is None else count.to(dev).contiguous(),
                             zeros if timer is None else timer.to(dev).contiguous())
+        # a checkpoint written before the action delay existed loads as "off, counters 0, delays 0" (and stop rows)
+        delay = sd.get("action_delay")
+        self.set_action_delay(*(delay if delay is not None else (None,)))
+        count, delay_d, command = (sd.get(k) for k in ("action_delay_count", "action_delay_delay",
+                                                       "action_delay_command"))
+        stop = stop_commands(self.n, dev)
+        default = count is None or (not count.any() and not delay_d.any()
+                                    and torch.equal(command.to(dev).nan_to_num(7.0), stop.nan_to_num(7.0)))
+        if delay is not None or not default or getattr(self, "_delay_state_set", False):
+            # the handle's state is replaced; a handle that never had one and a checkpoint without one (no spec and
+            # the state of a fresh handle) leave the buffers unallocated
+            self.set_action_delay_state(zeros if count is None else count.to(dev).contiguous(),
+                                        zeros if delay_d is None else delay_d.to(dev).contiguous(),
+                                        stop if command is None else command.to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
         out = torch.empty(self.n, dtype=torch.int32, device=self.device)
         check(lib().upkie_b200_error_flags(self._h, _ptr(out), self._stream()))
         return out
+
+
+def stop_commands(n: int, device=None) -> torch.Tensor:
+    """``[n, 6, 6]`` stop rows, the servo command an env holds after a reset under an action delay: per joint position
+    NaN, every other key 0 (``include/upkie_b200.h``)."""
+    out = torch.zeros((n, _abi.NJ, len(_abi.ACT_KEYS)), dtype=torch.float32, device=device)
+    out[:, :, 0] = float("nan")
+    return out
 
 
 def neutral_action(model: Model, n: int, device=None) -> torch.Tensor:
