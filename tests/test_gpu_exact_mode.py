@@ -82,5 +82,6 @@ def test_exact_mode_one_tick_against_the_oracle(model, oracle_lib):
     assert e["qd_median"] < 5e-5 and e["qd_p99"] < 1e-3 and e["qd_worst"] < 2e-2 and e["twist"] < 1e-3
     # the shortcut of the product library (fast-math) stays in the same error class as plain fp32 (no order-of-magnitude loss)
     f = err["fast"]
+    assert f["pose"] < 2e-5 and f["twist"] < 1e-3, (f["pose"], f["twist"])  # the caps of the exact library
     assert f["qd_median"] < 5 * max(e["qd_median"], 2e-6) and f["qd_p99"] < 5 * max(e["qd_p99"], 5e-5)
     assert np.array_equal(eterm, oterm) and np.array_equal(fterm, oterm)

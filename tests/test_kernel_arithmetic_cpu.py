@@ -844,3 +844,21 @@ def test_frozen_lanes_keep_bullets_result(model, oracle_lib):
     assert np.abs(hs0.state[:, 19:25] - results[(3, 0)][:, 19:25]).max() > 0  # not the same iteration count
     d = np.abs(hs0.state[:, :25].astype(np.float64) - osim0.get_state()[:, :25])
     assert np.median(d[:, 19:25].max(axis=1)) < 5e-4
+
+
+def test_config_keeps_the_substep_rotation_in_the_integrators_range(model):
+    """The base-orientation integrator evaluates polynomials of sin(x) / x and cos(x), fp32-exact for x = |w| h / 2 up
+    to 0.52: a config whose substep h and velocity clamp allow more is refused when the parameters are built."""
+    import ctypes as C
+
+    import hostsim_wrap
+
+    L, m = hostsim_wrap.lib(), model.to_struct()
+    for dt, nb, vmax, ok in ((0.005, 5, 100.0, True), (0.005, 1, 100.0, True), (0.02, 1, 100.0, False),
+                             (0.005, 1, 150.0, False), (0.02, 1, 25.0, True)):
+        cfg = _abi.default_sim_config()
+        cfg.dt, cfg.nb_substeps, cfg.max_coordinate_velocity = dt, nb, vmax
+        h = L.hostsim_create(C.byref(m), C.byref(cfg))
+        assert bool(h) == ok, (dt, nb, vmax)
+        if h:
+            L.hostsim_destroy(h)

@@ -157,6 +157,12 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
     return UPKIE_B200_EINVAL;
   }
   const double h = c.dt / c.nb_substeps;
+  // the base-orientation integrator's polynomials of sin(x) / x and cos(x) (sim_pair.cuh) are fp32-exact for
+  // x = |w| h / 2 <= 0.6 sqrt(3) / 2: truncation below 1.4e-7 with every angular velocity component at the clamp
+  if (!(h * c.max_coordinate_velocity <= 0.6)) {
+    err = "config: dt / nb_substeps * max_coordinate_velocity <= 0.6 required (substep rotation of the base)";
+    return UPKIE_B200_EINVAL;
+  }
   P.dt = float(c.dt);
   P.inv_dt = float(1.0 / c.dt);
   P.h = float(h);

@@ -858,14 +858,16 @@ UPKIE_HD void physics_substep(const SimParams& P, RobotState& S, const float tau
 #pragma unroll
   for (int i = 0; i < 3; ++i) S.pos[i] += P.h * S.linvel[i];
   {
+    // rotation increment exp(w h / 2): the even Taylor polynomials of sin(x) / x and cos(x) to degree 6, x = |w| h / 2.
+    // make_sim_params bounds h * max_coordinate_velocity by 0.6, so x <= 0.52 and the truncation stays below 1.4e-7
+    // (defaults, h = 1 ms and the clamp at 100: x <= 0.087, ~1e-14). Not sinf / cosf: under --use_fast_math they
+    // carry an absolute error of up to 3.6e-7, as large as the increment itself at slow rates
     const float* om = S.angvel;
-    const float ang2 = om[0] * om[0] + om[1] * om[1] + om[2] * om[2];
-    const float ang = sqrtf(ang2);
-    float sc;
-    if (ang < 0.001f) sc = 0.5f * P.h - P.h * P.h * P.h * 0.020833333333f * ang2;
-    else sc = sinf(0.5f * ang * P.h) / ang;
+    const float hh = 0.5f * P.h;
+    const float x2 = (om[0] * om[0] + om[1] * om[1] + om[2] * om[2]) * hh * hh;
+    const float sc = hh * (1.f + x2 * (-1.f / 6.f + x2 * (1.f / 120.f - x2 * (1.f / 5040.f))));
     const float ax = om[0] * sc, ay = om[1] * sc, az = om[2] * sc;
-    const float dqw = cosf(ang * P.h * 0.5f);
+    const float dqw = 1.f + x2 * (-0.5f + x2 * (1.f / 24.f - x2 * (1.f / 720.f)));
     const float qw = S.quat[0], qx = S.quat[1], qy = S.quat[2], qz = S.quat[3];
     const float nw = dqw * qw - ax * qx - ay * qy - az * qz;
     const float nx = dqw * qx + ax * qw + ay * qz - az * qy;
