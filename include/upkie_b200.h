@@ -269,7 +269,7 @@ typedef struct UpkieSimConfig {
    * cfm 0, Baumgarte factor body_contact_erp, friction coefficient = the env's floor friction x body_friction, friction
    * directions world -y and +x (btPlaneSpace1 of the plane normal); rows are solved after the wheel rows of their kind
    * (normals, then frictions). At most UPKIE_MAX_BODY_CONTACTS points (the deepest) are active per robot. Needs
-   * joint_limits != 0. Handles with body_contacts = 1 run their own kernel instantiations (step_*_body.cu); there a
+   * joint_limits != 0. Handles with body_contacts = 1 run their own kernel instantiations (csrc/step_family.h); there a
    * warp that holds no such point runs the packed solvers, one that does solves ALL rows of its 32 robots in a general
    * scalar solver - many times the packed cost for that warp and substep (DESIGN.md section 3), which is
    * why the default is 0 = off (a fallen robot's torso passes through the floor, as in round 1) for batched handles:

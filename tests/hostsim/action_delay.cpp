@@ -2,10 +2,8 @@
 //
 // action_delay.cpp -- TEST INFRASTRUCTURE. The CPU build of the action delay's draw, reset and delayed tick
 // (sim_core.cuh action_delay_draw / action_delay_reset / action_delay_substep, the code the step kernels and
-// action_delay.cu inline), and of the step kernels' family choice with a delay (step_family.h). Built by
-// tests/test_action_delay_cpu.py; never loaded by the product.
+// action_delay.cu inline). Built by tests/test_action_delay_cpu.py; never loaded by the product.
 #include "hostsim.cpp"
-#include "../../upkie_b200/csrc/step_family.h"
 
 extern "C" {
 
@@ -122,37 +120,6 @@ int hostsim_action_delay_spec_error(const UpkieActionDelay* spec, int nb_substep
     why[why_len - 1] = '\0';
   }
   return msg ? 1 : 0;
-}
-
-// what `family` compiles in: extras, limits, table, reset_rand, spine, body, push, delay
-void hostsim_family_traits_delay(int family, uint8_t* out) {
-  const StepFamily f = step_family_traits(family);
-  const bool v[8] = {f.extras, f.limits, f.table, f.reset_rand, f.spine, f.body, f.push, f.delay};
-  for (int k = 0; k < 8; ++k) out[k] = v[k] ? 1 : 0;
-}
-
-// step_family of a handle with the given features, an action delay among them
-int hostsim_step_family_delay(int joint_limits, int table, int body_contacts, int push, int delay, int spine_mode,
-                              int max_episode_steps, int mode, int transport, char* why, int why_len) {
-  static float table_storage[1];
-  static char push_storage[1], delay_storage[1];
-  SimParams P;
-  std::memset(&P, 0, sizeof(P));
-  P.joint_limits = joint_limits;
-  P.env_params = table ? table_storage : nullptr;
-  P.body_contacts = body_contacts;
-  P.push = push ? reinterpret_cast<const PushRand*>(push_storage) : nullptr;
-  P.action_delay = delay ? reinterpret_cast<const ActionDelay*>(delay_storage) : nullptr;
-  P.spine_mode = spine_mode;
-  P.max_episode_steps = max_episode_steps;
-  const char* msg = nullptr;
-  const int family = step_family(P, false, mode, transport, &msg);
-  why[0] = '\0';
-  if (msg) {
-    std::strncpy(why, msg, why_len - 1);
-    why[why_len - 1] = '\0';
-  }
-  return family;
 }
 
 }  // extern "C"

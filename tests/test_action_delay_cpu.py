@@ -1,8 +1,8 @@
 # SPDX-License-Identifier: Apache-2.0
 """Action-delay randomisation (upkie_b200_set_action_delay): the C struct against its mirror, the draw and the delayed
 tick the kernels run, compiled for the CPU (tests/hostsim/action_delay.cpp), against a NumPy statement of the draw and
-against the same substeps composed from the single substep of every tick; the families the host picks with a delay;
-the spec's validation on both sides. No GPU needed."""
+against the same substeps composed from the single substep of every tick; the spec's validation on both sides. The
+families the host picks with a delay are tested with the others' (test_step_family_cpu.py). No GPU needed."""
 import ctypes as C
 import os
 import re
@@ -21,9 +21,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(HERE, "..", "include", "upkie_b200.h")
 
 MODE_SERVOS, MODE_GYROPOD, MODE_PENDULUM = 0, 1, 2
-DEVICE, HOST_TILE, IN_KERNEL = 0, 1, 2
-FAM_TABLE, FAM_PUSH, FAM_BODY_PUSH, FAM_DELAY, FAM_BODY_DELAY, FAM_SPINE, FAM_BODY = 5, 6, 7, 8, 9, 3, 4
-TRAITS = ("extras", "limits", "table", "reset_rand", "spine", "body", "push", "delay")
 
 
 def test_struct_matches_the_header():
@@ -80,9 +77,6 @@ def _lib():
         L.hostsim_step_servos_noise.argtypes = [vp, C.c_int, fp, fp, C.c_uint32, C.c_uint64, fp]
         L.hostsim_step_gyropod.argtypes = [vp, C.c_int, fp, fp, C.c_int, fp, u8p]
         L.hostsim_action_delay_spec_error.argtypes = [sp, C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_int]
-        L.hostsim_family_traits_delay.argtypes = [C.c_int, u8p]
-        L.hostsim_step_family_delay.argtypes = [C.c_int] * 9 + [C.c_char_p, C.c_int]
-        L.hostsim_step_family_delay.restype = C.c_int
         _LIB = L
     return _LIB
 
@@ -274,63 +268,6 @@ def test_stop_row_gives_zero_torque(noise):
     # the torque the substep applied is the state's torque record
     assert np.all(state[:, _abi.ST_TORQUE:_abi.ST_TORQUE + 6] == 0.0)
     assert state.tobytes() != ref.tobytes()
-
-
-# ---- the families --------------------------------------------------------------------------------------------------------
-
-
-def traits(family):
-    out = (C.c_uint8 * len(TRAITS))()
-    _lib().hostsim_family_traits_delay(family, out)
-    return {name for name, v in zip(TRAITS, out) if v}
-
-
-def step_family(mode=MODE_SERVOS, transport=DEVICE, joint_limits=2, table=0, body_contacts=0, push=0, delay=0,
-                spine_mode=0, max_episode_steps=0):
-    why = C.create_string_buffer(256)
-    f = _lib().hostsim_step_family_delay(joint_limits, table, body_contacts, push, delay, spine_mode,
-                                         max_episode_steps, mode, transport, why, len(why))
-    return f, (why.value.decode() or None)
-
-
-def test_delay_traits():
-    base = {"extras", "limits", "table", "reset_rand", "push"}
-    assert traits(FAM_DELAY) == base | {"delay"}
-    assert traits(FAM_BODY_DELAY) == base | {"body", "delay"}
-    assert traits(FAM_DELAY) - {"delay"} == traits(FAM_PUSH)
-    assert traits(FAM_BODY_DELAY) - {"delay"} == traits(FAM_BODY_PUSH)
-    for fam in range(8):
-        assert "delay" not in traits(fam)
-
-
-@pytest.mark.parametrize("transport", [DEVICE, HOST_TILE])
-@pytest.mark.parametrize("mode", [MODE_SERVOS, MODE_GYROPOD, MODE_PENDULUM])
-def test_delay_families(mode, transport):
-    assert step_family(mode, transport, delay=1) == (FAM_DELAY, None)
-    assert step_family(mode, transport, delay=1, table=1) == (FAM_DELAY, None)
-    assert step_family(mode, transport, delay=1, push=1) == (FAM_DELAY, None)
-    assert step_family(mode, transport, delay=1, table=1, push=1, max_episode_steps=9) == (FAM_DELAY, None)
-    assert step_family(mode, transport, delay=1, body_contacts=1) == (FAM_BODY_DELAY, None)
-    assert step_family(mode, transport, delay=1, body_contacts=1, push=1) == (FAM_BODY_DELAY, None)
-    # without a delay the choice is the one before the feature
-    assert step_family(mode, transport, push=1) == (FAM_PUSH, None)
-    assert step_family(mode, transport, table=1) == (FAM_TABLE, None)
-    assert step_family(mode, transport, body_contacts=1) == (FAM_BODY, None)
-
-
-NO_PUSH = "push randomisation has no in-kernel rollout transport (use upkie_b200_step with compact rows)"
-NO_DELAY = "action delay has no in-kernel rollout transport (use upkie_b200_step with compact rows)"
-NO_TABLE = "the per-env parameter table has no in-kernel rollout transport (use upkie_b200_step with compact rows)"
-NO_LIMIT = ("max_episode_steps has no in-kernel rollout transport: it does not carry truncated (use upkie_b200_step "
-            "with compact rows)")
-
-
-def test_in_kernel_transport_rejects_a_delay_after_the_push_message():
-    assert step_family(MODE_SERVOS, IN_KERNEL, delay=1) == (-1, NO_DELAY)
-    assert step_family(MODE_SERVOS, IN_KERNEL, delay=1, push=1)[1] == NO_PUSH
-    assert step_family(MODE_SERVOS, IN_KERNEL, delay=1, table=1)[1] == NO_TABLE
-    assert step_family(MODE_SERVOS, IN_KERNEL, delay=1, max_episode_steps=1, body_contacts=1)[1] == NO_DELAY
-    assert step_family(MODE_SERVOS, IN_KERNEL, max_episode_steps=1)[1] == NO_LIMIT
 
 
 # ---- the spec ------------------------------------------------------------------------------------------------------------

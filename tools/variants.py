@@ -4,8 +4,9 @@
     python tools/variants.py build      # here (no GPU): compiles variants/lib_<name>.so
     python tools/variants.py run [names]  # on the GPU box: times each variant with bench.py (UPKIE_B200_LIB)
 
-Round 2: the variants differ in the translation unit of the benchmarked kernel only (step_host_limits.cu: TILE=1,
-FAM_LIMITS); every other object is taken from the in-tree build (upkie_b200/build/*.o).
+Round 2: the variants differ in the translation unit of the benchmarked kernel only (the step_host_limits unit of
+build.py: csrc/step_unit.cu for TILE=1, FAM_LIMITS); every other object is taken from the in-tree build
+(upkie_b200/build/*.o).
 """
 import json
 import os
@@ -28,11 +29,13 @@ def build():
     from upkie_b200 import build as b
 
     b.build()
+    unit = next(u for u in b.UNITS if isinstance(u, b.StepUnit) and u.name == UNIT)
     os.makedirs(OUT, exist_ok=True)
     procs = []
     for name, flags in VARIANTS.items():
         obj = os.path.join(OUT, f"{UNIT}_{name}.o")
-        cmd = ["nvcc"] + b.NVCC_FLAGS + flags + ["-Xptxas", "-v", "-c", "-o", obj, os.path.join(CSRC, UNIT + ".cu")]
+        cmd = (["nvcc"] + b.NVCC_FLAGS + unit.flags() + flags +
+               ["-Xptxas", "-v", "-c", "-o", obj, os.path.join(CSRC, "step_unit.cu")])
         procs.append((name, obj, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
     for name, obj, p in procs:
         out, _ = p.communicate()
@@ -41,7 +44,7 @@ def build():
         for i, l in enumerate(lines):
             if KERNEL in l and "Function properties" in l:
                 info = " | ".join(x.strip() for x in lines[i + 1:i + 3])
-        objs = [os.path.join(OBJ, os.path.splitext(s)[0] + ".o") for s in b.SOURCES if not s.startswith(UNIT)] + [obj]
+        objs = [os.path.join(OBJ, n + ".o") if n != UNIT else obj for n, _, _ in b.compile_jobs(b.UNITS)]
         rc = subprocess.call(["nvcc"] + b.GENCODE + ["-shared", "-o", os.path.join(OUT, f"lib_{name}.so")] + objs)
         print(f"{name:16s} rc={p.returncode}/{rc} {info}")
 

@@ -2,8 +2,8 @@
 //
 // kernel_common.cuh -- what the translation units of libupkie_b200.so share: build-time knobs, the
 // state load/store helpers, and the launch descriptor of the env-step kernel. The step kernel itself
-// (step_kernel.cuh) is instantiated in the step_*.cu units, each one TILE of one or two families, that nvcc
-// compiles in parallel (step_family.h, DESIGN.md section 4). TILE is how the rows travel:
+// (step_kernel.cuh) is instantiated in the step units, step_unit.cu compiled once per TILE and one or two families,
+// that nvcc compiles in parallel (build.py, step_family.h, DESIGN.md section 4). TILE is how the rows travel:
 //   0  per-thread action loads / observation stores (device buffers)
 //   1  per-warp shared-memory tile with coalesced 16 B accesses, the variant whose warps read actions from and
 //      write observations to mapped pinned HOST memory
@@ -118,10 +118,10 @@ struct StepArgs {
   float* lag;           // spine mode: [UPKIE_LAG_DIM][n_pad] lag records, else null
 };
 
-// The step kernels of one (TILE, FAMILY) pair (step_kernel.cuh), explicitly instantiated in its step_*.cu unit
+// The step kernels of one (TILE, FAMILY) pair (step_kernel.cuh), explicitly instantiated in its step unit (step_unit.cu)
 template <int TILE, int FAMILY>
 cudaError_t launch_step(const StepArgs& a);
-cudaError_t launch_push_rows(const PeerPtrs& pp, int n, cudaStream_t stream);  // step_multicast.cu: flush of a rollout's last rows
+cudaError_t launch_push_rows(const PeerPtrs& pp, int n, cudaStream_t stream);  // step_unit.cu, TILE=2: flush of a rollout's last rows
 // reset_randomization.cu: the handle-side kernels of reset randomisation (upkie_b200_set_reset_randomization)
 cudaError_t launch_reset_rand(const ResetRand* R, int n, const uint8_t* mask, uint64_t seed, uint64_t env_offset,
                               cudaStream_t stream);  // draw of the envs an upkie_b200_reset takes, before k_reset

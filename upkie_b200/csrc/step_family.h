@@ -3,7 +3,8 @@
 // step_family.h -- the kernel families of the env-step kernel k_step<MODE, AUTORESET, FAMILY, TILE> (step_kernel.cuh):
 // what each family compiles in, and which family a step launch runs. Every feature that costs the kernels code,
 // registers or stack is compiled into the families that need it only, so that the others keep their code; each family
-// has translation units of its own (DESIGN.md section 4). Compiles with nvcc and with g++ (the CPU test of the choice).
+// has translation units of its own (step_unit.cu, DESIGN.md section 4). Compiles with nvcc and with g++ (the CPU test of
+// the choice).
 #pragma once
 
 #include "sim_core.cuh"
@@ -54,6 +55,21 @@ UPKIE_HD constexpr StepFamily step_family_traits(int family) {
       {true, true, true, true, false, true, true, true},        // FAM_BODY_DELAY
   };
   return t[family];
+}
+
+// The TILEs of k_step: 0 device buffers, 1 host-buffer tiles, 2 in-kernel rollout transport
+constexpr int kNumTiles = 3;
+
+// Whether the library holds the step kernels of (tile, family): every family on TILE 0 and 1, families 0-2 on TILE 2,
+// and in the exact-arithmetic library (build.py: build_exact) TILE 0, families 0-2 only. Each pair is instantiated by one
+// row of build.py's unit table; the step dispatch (upkie_b200.cu) launches exactly these pairs.
+UPKIE_HD constexpr bool step_instantiated(int tile, int family) {
+  if (tile < 0 || tile >= kNumTiles || family < 0 || family >= kNumFamilies) return false;
+#if UPKIE_EXACT_BUILD
+  return tile == 0 && family <= FAM_LIMITS;
+#else
+  return tile < 2 || family <= FAM_LIMITS;
+#endif
 }
 
 // The family of a step launch of `mode` on `transport` (the TILE of k_step: 0 device buffers, 1 host-buffer tiles,

@@ -4,8 +4,8 @@
 //   k_step<MODE, AUTORESET, FAMILY, TILE>   one 5 ms env tick: action front-end, 5 x (moteus torque law,
 //       articulated-body dynamics, wheel-ground contact solve, semi-implicit integration), observation,
 //       termination; optional fused auto-reset; the optional features of FAMILY (step_family.h).
-//   launch_step<TILE, FAMILY>   the launcher of a (TILE, FAMILY) pair, explicitly instantiated in its step_*.cu unit
-//       (kernel_common.cuh, DESIGN.md section 4).
+//   launch_step<TILE, FAMILY>   the launcher of a (TILE, FAMILY) pair, explicitly instantiated in its step unit
+//       (step_unit.cu, build.py, DESIGN.md section 4).
 #pragma once
 
 #include "kernel_common.cuh"
@@ -205,7 +205,7 @@ __device__ __forceinline__ void step_env(
   const int env_col = F.table ? i : -1;
   int nsub = P.nb_substeps;
   // spine mode (config.spine_mode, UpkieServos): every substep is one cycle of the Bullet spine (FAM_SPINE: its own
-  // instantiations, step_*_spine.cu, so that the other kernels do not carry the lag record)
+  // step units, step_*_spine, so that the other kernels do not carry the lag record)
   constexpr bool spine = F.spine && MODE == MODE_SERVOS;
   SpineLag L;
   if (spine) {

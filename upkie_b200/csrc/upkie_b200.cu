@@ -318,37 +318,19 @@ int pick_block(const Handle* h, int cnt) {
   return block;
 }
 
-// The step kernels of (TILE, family), instantiated in the step_*.cu units; cudaErrorNotSupported for a pair without an
-// instantiation. The exact-arithmetic library (build.py: build_exact) has the device-buffer kernels of families 0-2 only.
-constexpr int tile_family(int tile, int family) { return tile * kNumFamilies + family; }
+// The step kernels of (TILE, family): a compile-time walk over the pairs that step_instantiated names, the others
+// cudaErrorNotSupported.
+template <int TILE = 0, int FAMILY = 0>
 cudaError_t dispatch_step(int tile, const StepArgs& a) {
-  switch (tile_family(tile, a.family)) {
-    case tile_family(0, FAM_PLAIN): return launch_step<0, FAM_PLAIN>(a);
-    case tile_family(0, FAM_EXTRAS): return launch_step<0, FAM_EXTRAS>(a);
-    case tile_family(0, FAM_LIMITS): return launch_step<0, FAM_LIMITS>(a);
-#if !UPKIE_EXACT_BUILD
-    case tile_family(0, FAM_SPINE): return launch_step<0, FAM_SPINE>(a);
-    case tile_family(0, FAM_BODY): return launch_step<0, FAM_BODY>(a);
-    case tile_family(0, FAM_TABLE): return launch_step<0, FAM_TABLE>(a);
-    case tile_family(0, FAM_PUSH): return launch_step<0, FAM_PUSH>(a);
-    case tile_family(0, FAM_BODY_PUSH): return launch_step<0, FAM_BODY_PUSH>(a);
-    case tile_family(0, FAM_DELAY): return launch_step<0, FAM_DELAY>(a);
-    case tile_family(0, FAM_BODY_DELAY): return launch_step<0, FAM_BODY_DELAY>(a);
-    case tile_family(1, FAM_PLAIN): return launch_step<1, FAM_PLAIN>(a);
-    case tile_family(1, FAM_EXTRAS): return launch_step<1, FAM_EXTRAS>(a);
-    case tile_family(1, FAM_LIMITS): return launch_step<1, FAM_LIMITS>(a);
-    case tile_family(1, FAM_SPINE): return launch_step<1, FAM_SPINE>(a);
-    case tile_family(1, FAM_BODY): return launch_step<1, FAM_BODY>(a);
-    case tile_family(1, FAM_TABLE): return launch_step<1, FAM_TABLE>(a);
-    case tile_family(1, FAM_PUSH): return launch_step<1, FAM_PUSH>(a);
-    case tile_family(1, FAM_BODY_PUSH): return launch_step<1, FAM_BODY_PUSH>(a);
-    case tile_family(1, FAM_DELAY): return launch_step<1, FAM_DELAY>(a);
-    case tile_family(1, FAM_BODY_DELAY): return launch_step<1, FAM_BODY_DELAY>(a);
-    case tile_family(2, FAM_PLAIN): return launch_step<2, FAM_PLAIN>(a);
-    case tile_family(2, FAM_EXTRAS): return launch_step<2, FAM_EXTRAS>(a);
-    case tile_family(2, FAM_LIMITS): return launch_step<2, FAM_LIMITS>(a);
-#endif
-    default: return cudaErrorNotSupported;
+  if constexpr (TILE == kNumTiles) {
+    return cudaErrorNotSupported;
+  } else if constexpr (FAMILY == kNumFamilies) {
+    return dispatch_step<TILE + 1, 0>(tile, a);
+  } else {
+    if constexpr (step_instantiated(TILE, FAMILY)) {
+      if (tile == TILE && a.family == FAMILY) return launch_step<TILE, FAMILY>(a);
+    }
+    return dispatch_step<TILE, FAMILY + 1>(tile, a);
   }
 }
 
@@ -1109,7 +1091,11 @@ int upkie_b200_push_rows(void* handle, const UpkiePush* push, void* stream) {
   int rc = fill_push(h, push, pp, "push_rows");
   if (rc) return rc;
   CUDA_TRY(cudaSetDevice(h->device));
+#if UPKIE_EXACT_BUILD
+  CUDA_TRY(cudaErrorNotSupported);  // the exact-arithmetic library has no in-kernel rollout transport (build.py)
+#else
   CUDA_TRY(launch_push_rows(pp, h->n, static_cast<cudaStream_t>(stream)));
+#endif
   return UPKIE_B200_OK;
 }
 
