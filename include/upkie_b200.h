@@ -730,6 +730,54 @@ int upkie_b200_get_action_delay_state(void* handle, uint32_t* count, uint32_t* d
 int upkie_b200_set_action_delay_state(void* handle, const uint32_t* count, const uint32_t* delay, const float* command,
                                       void* stream);
 
+/* Observation-delay randomisation (an addition to ABI 8: no existing layout, constant or signature changed). While a
+ * spec is set, env i holds a delay d_i, 0 <= d_i <= nb_substeps, and everything a step reports about the robot's
+ * sensors describes the robot at the end of substep nb_substeps - d_i of the tick, d_i substeps old: the observation of
+ * all four env types (servo rows full and compact, gyropod, pendulum rows, and so UpkieBaseVelocity's), the spine
+ * observation (upkie_b200_spine_obs), the same-step final_obs and upkie_b200_final_spine_obs, and
+ * upkie_b200_reset_obs (whose envs a reset took report their post-reset state, the others their last snapshot). d_i = 0 is the
+ * observation without a spec; d_i = nb_substeps is the state at the start of the tick (one tick of latency, the most
+ * there is). The sensed fields of a state row are the base pose and twist, the joint positions and velocities, the
+ * commanded torques (the measured torques are those of the last substep that ran before the snapshot, with this tick's
+ * noise keys), the floor contact and the IMU pair: the IMU acceleration is the finite difference over dt of the IMU
+ * velocities of two consecutive snapshots, as the undelayed observation differentiates two consecutive ticks, so the
+ * sensed rows carry their own UPKIE_ST_PREV_IMU_VEL.
+ * Not delayed: terminated, truncated and the auto-resets (a fall is the simulator's judgement, not a sensor's: under
+ * the same actions the physics and the reset schedule do not depend on the draws), upkie_b200_get_state, the
+ * contact impulses of the state rows (get_contact_points), body contacts, push forces, error flags, and the gyropod
+ * wrapper's own state (yaw, yaw_vel, leg targets), which is software.
+ * Every reset has no earlier state to lag behind: the env's sensed row becomes a copy of the post-reset state, so a
+ * reset's observation is undelayed (both fused auto-resets, and upkie_b200_reset with device-sampled or host init rows,
+ * masked or not), and a new d_i is drawn. upkie_b200_set_state copies the state into the sensed rows while a spec is
+ * set. The terminal step of a same-step auto-reset is observed under the delay in force (final_obs, final spine obs).
+ * Draw law: a per-env counter k, +1 at every reset; the reset uses draw k (after the +1). Draw k of the env of global
+ * index g = env_offset + i (the seed and env_offset of upkie_b200_set_autoreset) is Philox4x32-10 with key seed and
+ * counter (g, 2^60 | k << 4), whose word w0 gives
+ *   d = substeps_low + (((w0 >> 8) * (substeps_high - substeps_low + 1)) >> 24)          (integer arithmetic, exact)
+ * The tag bit 60 keeps these counters apart from those of the initial states ((episode << 2) | b, below 2^34), the
+ * reset randomisation (bit 63), the pushes (bit 62) and the action delay (bit 61). The draws depend neither on the
+ * physics nor on the number of GPUs.
+ * Setting a spec draws nothing: each env keeps its delay (0 on a handle that never had a spec) until its next reset.
+ * The first spec (or set_observation_delay_state) allocates the sensed rows and fills them from the current state; a
+ * spec set while the delay is off fills them again from the current state (the sensors did not follow the robot while
+ * it was off), while replacing a spec in force keeps them. NULL turns the delay off: upkie_b200_spine_obs and
+ * upkie_b200_reset_obs read the true state again; the counters and delays stay for a later spec.
+ * Per-env state (upkie_b200_get_observation_delay_state / set_observation_delay_state, for checkpoints): count[N],
+ * delay[N] and the sensed rows[N][UPKIE_STATE_DIM] (device pointers); 0, 0 and the current state on a handle that never
+ * had one. A delay above nb_substeps acts as nb_substeps.
+ * Needs joint_limits != 0 (the delay runs in a copy of the table kernels). Rejected with UPKIE_B200_EINVAL, the
+ * previous spec kept: substeps_low > substeps_high, substeps_high > nb_substeps, joint_limits == 0, spine_mode (which
+ * models the spine's own lag), body_contacts (no body-contact copy of the kernels). upkie_b200_set_config rejects an
+ * nb_substeps below a set spec's substeps_high, and turning body_contacts on while a spec is set; the in-kernel rollout
+ * transports reject a handle with a spec. The set call waits for the device. */
+typedef struct UpkieObservationDelay {
+  uint32_t substeps_low, substeps_high; /* range of the delay, in substeps of dt / nb_substeps */
+} UpkieObservationDelay;
+int upkie_b200_set_observation_delay(void* handle, const UpkieObservationDelay* spec);
+int upkie_b200_get_observation_delay_state(void* handle, uint32_t* count, uint32_t* delay, float* rows, void* stream);
+int upkie_b200_set_observation_delay_state(void* handle, const uint32_t* count, const uint32_t* delay,
+                                           const float* rows, void* stream);
+
 /* Number of step-kernel launches issued through this handle since create
  * (bench.py's `gpu_launches`). */
 int upkie_b200_launch_count(void* handle, uint64_t* count);

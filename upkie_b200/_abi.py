@@ -389,6 +389,15 @@ class UpkieActionDelay(C.Structure):
     ]
 
 
+class UpkieObservationDelay(C.Structure):
+    """``UpkieObservationDelay`` of include/upkie_b200.h: the range of each env's observation delay, in substeps."""
+
+    _fields_ = [
+        ("substeps_low", C.c_uint32),
+        ("substeps_high", C.c_uint32),
+    ]
+
+
 def default_mpc_config() -> UpkieMpcConfig:
     """``MPCBalancer.__init__`` defaults (``mpc_balancer.py:168-181``)."""
     c = UpkieMpcConfig()

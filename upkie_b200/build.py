@@ -11,7 +11,7 @@ LIB_PATH = os.path.join(_HERE, "libupkie_b200.so")
 
 # the step-kernel families, numbered as in csrc/step_family.h
 (FAM_PLAIN, FAM_EXTRAS, FAM_LIMITS, FAM_SPINE, FAM_BODY, FAM_TABLE, FAM_PUSH, FAM_BODY_PUSH, FAM_DELAY,
- FAM_BODY_DELAY) = range(10)
+ FAM_BODY_DELAY, FAM_SENSE) = range(11)
 
 
 class StepUnit(NamedTuple):
@@ -55,6 +55,9 @@ UNITS = [
     StepUnit("step_host_delay", 1, (FAM_DELAY,), 0),
     StepUnit("step_device_body_delay", 0, (FAM_BODY_DELAY,), 1),
     StepUnit("step_host_body_delay", 1, (FAM_BODY_DELAY,), 1),
+    "observation_delay.cu",
+    StepUnit("step_device_sense", 0, (FAM_SENSE,), 0),
+    StepUnit("step_host_sense", 1, (FAM_SENSE,), 0),
 ]
 # every source and header of the library: the staleness check and the key of source_hash
 DEPS = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh", ".h"))) + [

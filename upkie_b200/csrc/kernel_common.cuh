@@ -140,5 +140,11 @@ cudaError_t launch_action_delay_reset(const ActionDelay* A, int n, const uint8_t
 // command rows [n][UPKIE_ACT_DIM] <-> the buffer's columns [UPKIE_ACT_DIM][stride]; a null source gives stop rows
 cudaError_t launch_command_rows(const float* cols, int n, int stride, float* rows, cudaStream_t stream);
 cudaError_t launch_command_cols(const float* rows, int n, int stride, float* cols, cudaStream_t stream);
+// observation_delay.cu: the handle-side kernels of observation-delay randomisation (upkie_b200_set_observation_delay)
+cudaError_t launch_obs_delay_reset(const ObsDelay* O, int n, int n_pad, const float* state, const uint8_t* mask,
+                                   uint64_t seed, uint64_t env_offset, cudaStream_t stream);  // after k_reset
+// sensed rows [n][UPKIE_STATE_DIM] <-> the buffer's columns [UPKIE_STATE_DIM][stride]
+cudaError_t launch_sensed_rows(const float* cols, int n, int stride, float* rows, cudaStream_t stream);
+cudaError_t launch_sensed_cols(const float* rows, int n, int stride, float* cols, cudaStream_t stream);
 
 }  // namespace upkie_b200

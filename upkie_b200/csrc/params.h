@@ -265,6 +265,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.reset_rand = nullptr;
   P.push = nullptr;
   P.action_delay = nullptr;
+  P.obs_delay = nullptr;
   return 0;
 }
 
@@ -356,6 +357,19 @@ inline const char* action_delay_spec_error(const UpkieActionDelay& s, const SimP
   return nullptr;
 }
 
+// Why a handle with parameters P refuses an observation-delay spec (upkie_b200_set_observation_delay), null when it
+// takes it
+inline const char* obs_delay_spec_error(const UpkieObservationDelay& s, const SimParams& P) {
+  if (s.substeps_low > s.substeps_high) return "set_observation_delay: substeps_low > substeps_high";
+  if (s.substeps_high > uint32_t(P.nb_substeps))
+    return "set_observation_delay: substeps_high above nb_substeps (the delay is at most one tick)";
+  if (P.joint_limits == 0)
+    return "set_observation_delay: needs joint_limits != 0 (the delay runs in a copy of the table kernels)";
+  if (P.spine_mode) return "set_observation_delay: spine_mode models the spine's own lag";
+  if (P.body_contacts) return "set_observation_delay: body_contacts has no observation-delay kernels";
+  return nullptr;
+}
+
 inline void set_noise_flags(SimParams& P, uint32_t f) {
   P.any_ctrl_noise = (f & kEpCtrlNoise) ? 1 : 0;
   P.any_meas_noise = (f & kEpMeasNoise) ? 1 : 0;
@@ -411,6 +425,39 @@ UPKIE_HD void state_to_row(const RobotState& S, float* r) {
   r[UPKIE_ST_CONTACT_IMPULSE] = S.lam_n[0];
   r[UPKIE_ST_CONTACT_IMPULSE + 1] = S.lam_n[1];
   for (int k = 0; k < 4; ++k) r[UPKIE_ST_FRICTION_IMPULSE + k] = S.lam_t[k];
+}
+
+// ---- observation delay: the sensed rows (sim_core.cuh ObsDelay) ----
+// A snapshot of S into an env's sensed row: store(k, value) for every sensed column k. The IMU pair is differentiated
+// against the row's previous snapshot, load(k) of its UPKIE_ST_PREV_IMU_VEL columns (read before any store), over dt as
+// observe_update does: acceleration (v - previous) / dt, then v becomes the previous velocity. `v` is the IMU velocity
+// of S (imu_velocity, or observe_update's S.prev_imu_vel right after it ran).
+template <typename Load, typename Store>
+UPKIE_HD void obs_delay_snapshot(const SimParams& P, const RobotState& S, const float v[3], Load load, Store store) {
+  float r[UPKIE_STATE_DIM];
+  state_to_row(S, r);
+  float prev[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) prev[k] = load(UPKIE_ST_PREV_IMU_VEL + k);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    r[UPKIE_ST_IMU_ACC + k] = (v[k] - prev[k]) * P.inv_dt;  // dt, not the substep (pybullet_backend.py:405-408)
+    r[UPKIE_ST_PREV_IMU_VEL + k] = v[k];
+  }
+#pragma unroll
+  for (int k = 0; k < UPKIE_STATE_DIM; ++k)
+    if (obs_delay_sensed(k)) store(k, r[k]);
+}
+
+// S with its sensed fields replaced by load(k) of the env's sensed row: the state the observation is built from
+template <typename Load>
+UPKIE_HD void obs_delay_sensed_state(RobotState& S, Load load) {
+  float r[UPKIE_STATE_DIM];
+  state_to_row(S, r);
+#pragma unroll
+  for (int k = 0; k < UPKIE_STATE_DIM; ++k)
+    if (obs_delay_sensed(k)) r[k] = load(k);
+  state_from_row(r, S);
 }
 
 }  // namespace upkie_b200

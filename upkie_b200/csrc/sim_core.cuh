@@ -141,6 +141,9 @@ struct SimParams {
   // action-delay randomisation (upkie_b200_set_action_delay): the handle's device block, null = off. Read by the step
   // kernels of the delay families (step_family.h) only. Appended last, as push above.
   const struct ActionDelay* action_delay;
+  // observation-delay randomisation (upkie_b200_set_observation_delay): the handle's device block, null = off. Read by
+  // the step kernels of FAM_SENSE (step_family.h) only. Appended last, as action_delay above.
+  const struct ObsDelay* obs_delay;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -1848,6 +1851,59 @@ UPKIE_HD void action_delay_reset(const ActionDelay& A, uint64_t seed, uint64_t g
   count[i] = k;
   delay[i] = action_delay_draw(spec, seed, g, k);
   for (int c = 0; c < UPKIE_ACT_DIM; ++c) col[size_t(c) * stride] = action_delay_stop_value(c);
+}
+
+// ---- observation-delay randomisation (upkie_b200_set_observation_delay) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw, delay[i] = d_i in substeps, and rows = the sensed state of each env, [UPKIE_STATE_DIM][stride]
+// structure-of-arrays like the state, env i in column i: what the env's sensors report, the state whose observation
+// the step returns and upkie_b200_spine_obs reads.
+struct ObsDelay {
+  UpkieObservationDelay spec;
+  uint32_t* count;
+  uint32_t* delay;
+  float* rows;
+  int stride;
+};
+
+// bit 60 of the high counter word: never set by sample_init_state ((episode << 2) | b, episode < 2^32), the noise
+// ((tick << 10) | (slot << 1) | b, tick < 2^32), the reset randomisation (bit 63), the pushes (bit 62) or the action
+// delay (bit 61)
+constexpr uint64_t kObsDelayTag = uint64_t(1) << 60;
+
+// Draw k of the env of global index g: its delay in substeps, push_steps' exact integer form
+UPKIE_HD uint32_t obs_delay_draw(const UpkieObservationDelay& s, uint64_t seed, uint64_t g, uint32_t k) {
+  const Philox4 r = philox4x32_10(g, kObsDelayTag | (uint64_t(k) << 4), seed);
+  return push_steps(r.v[0], s.substeps_low, s.substeps_high);
+}
+
+// Whether column k of a state row is sensed (delayed): base pose and twist, joint positions and velocities, the IMU
+// velocity of the last snapshot, the commanded torques, the floor contact and the IMU acceleration. The others (leg
+// targets, yaw, yaw velocity: the gyropod wrapper's software state; the contact impulses) are the true state's.
+UPKIE_HD constexpr bool obs_delay_sensed(int k) {
+  return k < UPKIE_ST_LEG_TARGET || k == UPKIE_ST_CONTACT || (k >= UPKIE_ST_IMU_ACC && k < UPKIE_ST_IMU_ACC + 3);
+}
+
+// The world-frame velocity of the IMU of state S (what observe_update differentiates)
+UPKIE_HD void imu_velocity(const SimParams& P, const RobotState& S, float v[3]) {
+  float R[9];
+  quat_to_rot(S.quat, R);
+  float rp[3], w[3];
+  rot_mul(R, P.imu_pos, rp);
+  cross3(S.angvel, rp, w);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) v[i] = S.linvel[i] + w[i];
+}
+
+// A reset of env i (the step kernels' fused resets, k_obs_delay_reset): the next draw. The caller then copies the
+// post-reset state into the sensed row. The block's fields are copied before the first store, as action_delay_reset.
+UPKIE_HD void obs_delay_reset(const ObsDelay& O, uint64_t seed, uint64_t g, int i) {
+  const UpkieObservationDelay spec = O.spec;
+  uint32_t* const count = O.count;
+  uint32_t* const delay = O.delay;
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  delay[i] = obs_delay_draw(spec, seed, g, k);
 }
 
 }  // namespace upkie_b200

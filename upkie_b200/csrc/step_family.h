@@ -25,7 +25,8 @@ enum {
   FAM_BODY_PUSH = 7,  // FAM_BODY + push randomisation
   FAM_DELAY = 8,      // FAM_PUSH + action delay
   FAM_BODY_DELAY = 9, // FAM_BODY_PUSH + action delay
-  kNumFamilies = 10
+  FAM_SENSE = 10,     // FAM_DELAY + observation delay
+  kNumFamilies = 11
 };
 
 // What a family's kernels compile in
@@ -38,21 +39,23 @@ struct StepFamily {
   bool body;        // body-contact record (BodyRecOut); units built with UPKIE_BODY_CONTACTS_BUILD 1
   bool push;        // the push schedule
   bool delay;       // the action delay: previous command rows, per-env delays
+  bool sense;       // the observation delay: sensed state rows, per-env delays
 };
 
 UPKIE_HD constexpr StepFamily step_family_traits(int family) {
   constexpr StepFamily t[kNumFamilies] = {
-      // extras limits table  reset_rand spine  body   push   delay
-      {false, false, true, false, false, false, false, false},  // FAM_PLAIN
-      {true, false, true, false, false, false, false, false},   // FAM_EXTRAS
-      {true, true, false, false, false, false, false, false},   // FAM_LIMITS
-      {true, true, true, true, true, true, false, false},       // FAM_SPINE
-      {true, true, true, true, false, true, false, false},      // FAM_BODY
-      {true, true, true, true, false, false, false, false},     // FAM_TABLE
-      {true, true, true, true, false, false, true, false},      // FAM_PUSH
-      {true, true, true, true, false, true, true, false},       // FAM_BODY_PUSH
-      {true, true, true, true, false, false, true, true},       // FAM_DELAY
-      {true, true, true, true, false, true, true, true},        // FAM_BODY_DELAY
+      // extras limits table  reset_rand spine  body   push   delay  sense
+      {false, false, true, false, false, false, false, false, false},  // FAM_PLAIN
+      {true, false, true, false, false, false, false, false, false},   // FAM_EXTRAS
+      {true, true, false, false, false, false, false, false, false},   // FAM_LIMITS
+      {true, true, true, true, true, true, false, false, false},       // FAM_SPINE
+      {true, true, true, true, false, true, false, false, false},      // FAM_BODY
+      {true, true, true, true, false, false, false, false, false},     // FAM_TABLE
+      {true, true, true, true, false, false, true, false, false},      // FAM_PUSH
+      {true, true, true, true, false, true, true, false, false},       // FAM_BODY_PUSH
+      {true, true, true, true, false, false, true, true, false},       // FAM_DELAY
+      {true, true, true, true, false, true, true, true, false},        // FAM_BODY_DELAY
+      {true, true, true, true, false, false, true, true, true},        // FAM_SENSE
   };
   return t[family];
 }
@@ -84,6 +87,8 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "push randomisation has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.action_delay)
     no = "action delay has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
+  else if (in_kernel && P.obs_delay)
+    no = "observation delay has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.max_episode_steps > 0)
     no = "max_episode_steps has no in-kernel rollout transport: it does not carry truncated (use upkie_b200_step with "
          "compact rows)";
@@ -93,11 +98,20 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "spine_mode supports UpkieServos steps only";
   else if (P.spine_mode && in_kernel)
     no = "spine_mode has no in-kernel rollout transport";
+  else if (P.obs_delay && P.spine_mode)
+    no = "observation delay: spine_mode models the spine's own lag";
+  else if (P.obs_delay && P.joint_limits == 0)
+    no = "observation delay needs joint_limits != 0";
+  else if (P.obs_delay && P.body_contacts)
+    no = "observation delay has no body-contact kernels";
   if (no) {
     *why = no;
     return -1;
   }
   if (P.spine_mode) return FAM_SPINE;
+  // the observation-delay family carries the action delay and the pushes too (runtime-uniform branches on
+  // P.action_delay and P.push); the set calls reject spine mode, no limits and body contacts
+  if (P.obs_delay) return FAM_SENSE;
   // the delay families carry the pushes too (a runtime-uniform branch on P.push); the set calls reject spine mode and
   // no limits
   if (P.action_delay) return P.body_contacts ? FAM_BODY_DELAY : FAM_DELAY;

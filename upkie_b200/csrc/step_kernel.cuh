@@ -264,6 +264,34 @@ __device__ __forceinline__ void step_env(
       for (int c = 0; c < UPKIE_ACT_DIM; ++c) a[c] = prev[c];
     }
   }
+  // observation delay (F.sense kernels, P.obs_delay set: a uniform branch). A lane with delay `sdl` stores the sensed
+  // fields of its state at the end of substep nb_substeps - sdl - 1 (before the loop for sdl = nb_substeps, after the
+  // observation update for sdl = 0) into the env's column of the sensed rows, and builds its observation from them
+  // after the tick (obs_delay_snapshot, obs_delay_sensed_state). A resetting lane draws its next delay, and its row
+  // becomes a copy of the post-reset state at the end of the tick. As for the action delay, the column's address and
+  // stride are read into registers once and the row goes through global-space coherent accesses (ld/st.global.cg):
+  // the loads read back this thread's own stores of the same launch.
+  const bool sensing = F.sense && P.obs_delay;
+  float* scol = nullptr;
+  size_t sstride = 0;
+  uint32_t sdl = 0xffffffffu;  // resetting lanes: no snapshot
+  if (sensing) {
+    const ObsDelay& O = *P.obs_delay;
+    scol = O.rows + size_t(i);
+    sstride = size_t(O.stride);
+    if (resetting) {
+      if (live) obs_delay_reset(O, seed, env_offset + uint64_t(i), i);
+    } else {
+      sdl = min(__ldcg(O.delay + i), uint32_t(P.nb_substeps));
+    }
+  }
+  auto sense_load = [&](int k) { return __ldcg(scol + size_t(k) * sstride); };
+  auto sense_store = [&](int k, float v) { __stcg(scol + size_t(k) * sstride, v); };
+  if (sensing && live && sdl == uint32_t(P.nb_substeps)) {  // the state at the start of the tick
+    float v[3];
+    imu_velocity(P, S, v);
+    obs_delay_snapshot(P, S, v, sense_load, sense_store);
+  }
   if (spine && !resetting) spine_assemble_observation(S, L);  // the first cycle's observation (Spine.cpp:126-131)
   const int nloop = (AUTORESET == AUTORESET_NEXT_STEP && spine && P.nb_substeps < 3) ? 3 : P.nb_substeps;
   for (int sub = 0; sub < nloop; ++sub) {
@@ -292,12 +320,20 @@ __device__ __forceinline__ void step_env(
                       (F.extras && ext) ? &xf : nullptr, F.limits ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
                       pushing ? &pu : nullptr);
       }
+      // the end of substep nb_substeps - sdl - 1 (0 < sdl < nb_substeps)
+      if (sensing && live && sdl != 0 && uint32_t(sub) + sdl + 1u == uint32_t(P.nb_substeps)) {
+        float v[3];
+        imu_velocity(P, S, v);
+        obs_delay_snapshot(P, S, v, sense_load, sense_store);
+      }
     } else {
 #pragma unroll
       for (int k = 0; k < kPhaseSyncs; ++k) PhaseSync()();
     }
   }
   if (!spine) observe_update(P, S);  // spine mode: the cycles read the IMU
+  // sdl = 0: the end of the tick, with the IMU velocity observe_update just computed
+  if (sensing && live && sdl == 0) obs_delay_snapshot(P, S, S.prev_imu_vel, sense_load, sense_store);
   if (resetting) {
     reset_wrapper_state(S);
   } else {
@@ -332,18 +368,36 @@ __device__ __forceinline__ void step_env(
     trunc = elapsed >= uint32_t(P.max_episode_steps);
   }
 
+  bool fin_pending = false;  // F.sense, same-step reset: the terminal observation is stashed after the tick
+  float fin_o6[6], fin_yaw = 0.f, fin_yaw_vel = 0.f;
   if (AUTORESET == AUTORESET_SAME_STEP) {
     if (term || trunc) {
-      if (P.final_obs && live) store_final_obs<MODE, spine>(P, S, L, o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
-      // neither the reset below nor the rest of the tick writes tick[i] (written above, before the physics) or the
-      // parameter table, so the stash and those give the rows k_spine_obs would have returned without the reset (a
-      // reset randomisation draw overwrites the table at the end of the tick, and the stash then also holds the
-      // pre-reset columns k_final_spine_obs reads, store_final_params)
-      if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
+      if constexpr (F.sense) {
+        // the terminal step's observation is delayed: it is stashed from the env's sensed row after the tick (below);
+        // what the reset overwrites and the stash needs is kept here, the gyropod observation and the wrapper's yaw
+        fin_pending = sensing;
+        if (MODE != MODE_SERVOS) {  // (UpkieServos rows hold no gyropod observation)
+#pragma unroll
+          for (int k = 0; k < 6; ++k) fin_o6[k] = o6[k];
+        }
+        fin_yaw = S.yaw;
+        fin_yaw_vel = S.yaw_vel;
+      }
+      if (!(F.sense && sensing)) {
+        if (P.final_obs && live)
+          store_final_obs<MODE, spine>(P, S, L, o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
+        // neither the reset below nor the rest of the tick writes tick[i] (written above, before the physics) or the
+        // parameter table, so the stash and those give the rows k_spine_obs would have returned without the reset (a
+        // reset randomisation draw overwrites the table at the end of the tick, and the stash then also holds the
+        // pre-reset columns k_final_spine_obs reads, store_final_params)
+        if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
+      }
       if (F.reset_rand && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
       if (pushing) push_restart(push_k, push_t, push_end);  // the terminal step ran under its push; a new schedule
       // the terminal step ran under its delay; the next tick starts from the stop row with a new one
       if (delaying && live) action_delay_reset(*P.action_delay, seed, env_offset + uint64_t(i), i);
+      // the terminal step was observed under its delay; the reset is observed undelayed, with a new draw
+      if (sensing && live) obs_delay_reset(*P.obs_delay, seed, env_offset + uint64_t(i), i);
       elapsed = 0;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
@@ -362,6 +416,43 @@ __device__ __forceinline__ void step_env(
   }
 
   if (live) store_state(state, n_pad, i, S);
+  if (sensing) {
+    if (fin_pending) {
+      // the terminal step's sensed state: its snapshot, with the terminal step's wrapper yaw, built in S (the post-reset
+      // state is stored, and read back below). sdl = 0: the snapshot is the true state, whose gyropod observation fin_o6
+      // already holds (computed again, the pitch could round differently: fast-math contracts the products of another
+      // inlined copy differently). Neither the reset nor the rest of the tick writes tick[i] or the parameter table
+      // (see the stash above).
+      S.yaw = fin_yaw;
+      S.yaw_vel = fin_yaw_vel;
+      obs_delay_sensed_state(S, sense_load);
+      if (MODE != MODE_SERVOS && sdl != 0) gyropod_obs(P, S, fin_o6);
+      if (P.final_obs && live)
+        store_final_obs<MODE, spine>(P, S, L, fin_o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
+      if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
+      load_state(state, n_pad, i, S);  // the post-reset state, which this thread stored (plain coherent loads)
+    } else if (!resetting) {
+      // the row's wrapper fields and contact impulses are the true state's; the observation is built from the snapshot,
+      // reloaded into S in place (the true state is stored). sdl = 0: the snapshot is the true state, whose gyropod
+      // observation o6 already holds (as above)
+      if (live) {
+        float r[UPKIE_STATE_DIM];
+        state_to_row(S, r);
+#pragma unroll
+        for (int k = 0; k < UPKIE_STATE_DIM; ++k)
+          if (!obs_delay_sensed(k)) sense_store(k, r[k]);
+      }
+      obs_delay_sensed_state(S, sense_load);
+      if (MODE != MODE_SERVOS && sdl != 0) gyropod_obs(P, S, o6);
+    }
+    if ((resetting || fin_pending) && live) {
+      // a reset in this tick: the sensed row becomes a copy of the post-reset state, the observation is undelayed
+      float r[UPKIE_STATE_DIM];
+      state_to_row(S, r);
+#pragma unroll
+      for (int k = 0; k < UPKIE_STATE_DIM; ++k) sense_store(k, r[k]);
+    }
+  }
   if (spine && live) {
     float lr[UPKIE_LAG_DIM];
     lag_to_row(L, lr);

@@ -111,6 +111,13 @@ struct Handle {
   uint32_t* delay_delay = nullptr;
   float* delay_command = nullptr;  // [UPKIE_ACT_DIM][n_pad]
   uint32_t delay_high = 0;         // substeps_high of the spec in force
+  // observation-delay randomisation (upkie_b200_set_observation_delay): the device block P.obs_delay points to while a
+  // spec is set, and the per-env state (allocated on the first spec or set_observation_delay_state)
+  ObsDelay* sense_dev = nullptr;
+  uint32_t* sense_count = nullptr;
+  uint32_t* sense_delay = nullptr;
+  float* sense_rows = nullptr;     // [UPKIE_STATE_DIM][n_pad] sensed states
+  uint32_t sense_high = 0;         // substeps_high of the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -713,6 +720,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->env_params); cudaFree(h->ep_check); cudaFree(h->final_state); cudaFree(h->rr_dev); cudaFree(h->draws);
   cudaFree(h->push_dev); cudaFree(h->push_count); cudaFree(h->push_timer);
   cudaFree(h->delay_dev); cudaFree(h->delay_count); cudaFree(h->delay_delay); cudaFree(h->delay_command);
+  cudaFree(h->sense_dev); cudaFree(h->sense_count); cudaFree(h->sense_delay); cudaFree(h->sense_rows);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -746,6 +754,12 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: action delay needs joint_limits != 0");
   if (h->P.action_delay && uint32_t(P.nb_substeps) < h->delay_high)
     return fail(UPKIE_B200_EINVAL, "set_config: nb_substeps below the action delay's substeps_high");
+  if (h->P.obs_delay && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: observation delay needs joint_limits != 0");
+  if (h->P.obs_delay && uint32_t(P.nb_substeps) < h->sense_high)
+    return fail(UPKIE_B200_EINVAL, "set_config: nb_substeps below the observation delay's substeps_high");
+  if (h->P.obs_delay && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no observation-delay kernels");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -764,6 +778,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.reset_rand = h->P.reset_rand;  // so does the reset randomisation
   P.push = h->P.push;              // and the push randomisation
   P.action_delay = h->P.action_delay;  // and the action delay
+  P.obs_delay = h->P.obs_delay;        // and the observation delay
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -981,6 +996,10 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
   k_reset<<<grid, rblock, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
                                     h->done_prev, h->episode, seed, env_offset, h->lag);
   CUDA_TRY(cudaGetLastError());
+  // observation delay: the envs this reset takes draw their next delay, and their sensed rows become the post-reset
+  // state (the reset's observation is undelayed)
+  if (h->P.obs_delay)
+    CUDA_TRY(launch_obs_delay_reset(h->sense_dev, h->n, h->n_pad, h->state, mask, h->seed, h->env_offset, s));
   // a reset sampled on the device counts an episode: it is not one the base-velocity post step has to carry out
   if (!init_state)
     CUDA_TRY(cudaMemcpyAsync(h->bv_episode, h->episode, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
@@ -1174,7 +1193,9 @@ int upkie_b200_spine_obs(void* handle, float* out, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !out) return fail(UPKIE_B200_EINVAL, "spine_obs: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  k_spine_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, h->state, h->tick, h->env_offset, out, h->lag);
+  // observation delay: the spine observation of the sensed states
+  const float* state = h->P.obs_delay ? h->sense_rows : h->state;
+  k_spine_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, state, h->tick, h->env_offset, out, h->lag);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1206,7 +1227,10 @@ int upkie_b200_reset_obs(void* handle, int obs_dim, float* obs, void* stream) {
   if (!h || !obs) return fail(UPKIE_B200_EINVAL, "reset_obs: invalid argument");
   if (obs_dim != 4 && obs_dim != 6 && obs_dim != UPKIE_OBS_DIM) return fail(UPKIE_B200_EINVAL, "reset_obs: obs_dim must be 4, 6 or 30");
   CUDA_TRY(cudaSetDevice(h->device));
-  k_reset_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, h->state, h->tick, h->env_offset, obs_dim, obs, h->lag);
+  // observation delay: the observation of the sensed states (those of the envs a reset took are the post-reset state;
+  // the others report their robot as the last step observed it)
+  const float* state = h->P.obs_delay ? h->sense_rows : h->state;
+  k_reset_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, state, h->tick, h->env_offset, obs_dim, obs, h->lag);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1227,6 +1251,10 @@ int upkie_b200_set_state(void* handle, const float* state, void* stream) {
   CUDA_TRY(cudaSetDevice(h->device));
   k_set_state<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->state, state);
   CUDA_TRY(cudaGetLastError());
+  // observation delay: the sensors see the state set, without a lag behind it
+  if (h->P.obs_delay)
+    CUDA_TRY(cudaMemcpyAsync(h->sense_rows, h->state, size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float),
+                             cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 
@@ -1468,6 +1496,103 @@ int upkie_b200_set_action_delay_state(void* handle, const uint32_t* count, const
   CUDA_TRY(cudaMemcpyAsync(h->delay_count, count, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(h->delay_delay, delay, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(launch_command_cols(command, h->n, h->n_pad, h->delay_command, s));
+  return UPKIE_B200_OK;
+}
+
+namespace {
+// the per-env observation-delay state: counters 0, delays 0 and the sensed rows filled from the current state on a
+// handle that has none yet (the three buffers are set together: a failure frees what was allocated)
+int alloc_sense_state(Handle* h) {
+  if (h->sense_count) return UPKIE_B200_OK;
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  const size_t row_bytes = size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float);
+  uint32_t *count = nullptr, *delay = nullptr;
+  float* rows = nullptr;
+  cudaError_t e = cudaDeviceSynchronize();  // the state of the steps in flight
+  if (e == cudaSuccess) e = cudaMalloc(&count, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&delay, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&rows, row_bytes);
+  if (e == cudaSuccess) e = cudaMemset(count, 0, bytes);
+  if (e == cudaSuccess) e = cudaMemset(delay, 0, bytes);
+  if (e == cudaSuccess) e = cudaMemcpy(rows, h->state, row_bytes, cudaMemcpyDeviceToDevice);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    cudaFree(count); cudaFree(delay); cudaFree(rows);
+    return fail(UPKIE_B200_ECUDA, std::string("observation delay state: ") + cudaGetErrorString(e));
+  }
+  h->sense_count = count;
+  h->sense_delay = delay;
+  h->sense_rows = rows;
+  return UPKIE_B200_OK;
+}
+}  // namespace
+
+int upkie_b200_set_observation_delay(void* handle, const UpkieObservationDelay* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    // off: the kernels enqueued before keep the block they were launched with, which stays allocated
+    h->P.obs_delay = nullptr;
+    h->sense_high = 0;
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = obs_delay_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
+  const bool allocated = h->sense_rows != nullptr;
+  if (alloc_sense_state(h)) return UPKIE_B200_ECUDA;  // a first allocation fills the rows from the state
+  if (allocated && !h->P.obs_delay) {
+    // turned on again: the sensors did not follow the robot while the delay was off, so the rows start from the
+    // current state (its IMU velocity is what the next snapshot differentiates against); counters and delays stay
+    CUDA_TRY(cudaMemcpy(h->sense_rows, h->state, size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float),
+                        cudaMemcpyDeviceToDevice));
+  }
+  if (!h->sense_dev) CUDA_TRY(cudaMalloc(&h->sense_dev, sizeof(ObsDelay)));
+  ObsDelay O;
+  std::memset(&O, 0, sizeof(O));
+  O.spec = *spec;
+  O.count = h->sense_count;
+  O.delay = h->sense_delay;
+  O.rows = h->sense_rows;
+  O.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->sense_dev, &O, sizeof(O), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->sense_high = spec->substeps_high;
+  h->P.obs_delay = h->sense_dev;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_observation_delay_state(void* handle, uint32_t* count, uint32_t* delay, float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !delay || !rows)
+    return fail(UPKIE_B200_EINVAL, "get_observation_delay_state: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  if (h->sense_count) {
+    CUDA_TRY(cudaMemcpyAsync(count, h->sense_count, bytes, cudaMemcpyDeviceToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(delay, h->sense_delay, bytes, cudaMemcpyDeviceToDevice, s));
+  } else {
+    CUDA_TRY(cudaMemsetAsync(count, 0, bytes, s));
+    CUDA_TRY(cudaMemsetAsync(delay, 0, bytes, s));
+  }
+  // a handle without a state: the current state, what its first spec would fill the rows with
+  CUDA_TRY(launch_sensed_rows(h->sense_rows ? h->sense_rows : h->state, h->n, h->n_pad, rows, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_observation_delay_state(void* handle, const uint32_t* count, const uint32_t* delay,
+                                           const float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !delay || !rows)
+    return fail(UPKIE_B200_EINVAL, "set_observation_delay_state: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (alloc_sense_state(h)) return UPKIE_B200_ECUDA;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  CUDA_TRY(cudaMemcpyAsync(h->sense_count, count, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(h->sense_delay, delay, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(launch_sensed_cols(rows, h->n, h->n_pad, h->sense_rows, s));
   return UPKIE_B200_OK;
 }
 

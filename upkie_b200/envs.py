@@ -544,6 +544,44 @@ def action_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool = Fal
     return lo_s, hi_s
 
 
+def observation_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool = False,
+                           joint_limits: Union[bool, int] = True,
+                           body_contacts: Union[bool, int] = False) -> Optional[Tuple[int, int]]:
+    """``(substeps_low, substeps_high)`` (``UpkieSim.set_observation_delay``) from an observation delay in seconds: a
+    float, or a ``(low, high)`` pair from which every reset draws an env's delay. Rounded to the nearest substep of
+    ``dt / nb_substeps`` (halves up). Raises ``UpkieException`` on a negative or non-finite bound, ``low > high``, a
+    delay of more than one tick (``nb_substeps`` substeps), ``spine_mode`` (which models the spine's own lag), no joint
+    limits (the delay runs in the kernels with joint-limit rows) and ``body_contacts`` (no such kernels)."""
+    if delay is None:
+        return None
+    if isinstance(delay, (int, float, np.integer, np.floating)):
+        lo, hi = delay, delay
+    else:
+        try:
+            lo, hi = delay
+        except (TypeError, ValueError):
+            raise UpkieException(f"observation_delay: expected seconds or a (low, high) pair, got {delay!r}") from None
+    try:
+        lo, hi = float(lo), float(hi)
+    except (TypeError, ValueError):
+        raise UpkieException(f"observation_delay: expected seconds, got ({lo!r}, {hi!r})") from None
+    if not (np.isfinite(lo) and np.isfinite(hi)) or not 0.0 <= lo <= hi:
+        raise UpkieException(f"observation_delay: expected finite seconds 0 <= low <= high, got ({lo}, {hi})")
+    if spine_mode:
+        raise UpkieException("observation_delay: spine_mode models the spine's own lag; the delay is not available "
+                             "there")
+    if not joint_limits:
+        raise UpkieException("observation_delay: needs joint_limits (the delay runs in the kernels with joint-limit "
+                             "rows)")
+    if body_contacts:
+        raise UpkieException("observation_delay: body_contacts has no observation-delay kernels")
+    substep = dt / int(nb_substeps)
+    lo_s, hi_s = (int(np.floor(x / substep + 0.5)) for x in (lo, hi))
+    if hi_s > int(nb_substeps):
+        raise UpkieException(f"observation_delay: {hi} s is more than one tick ({nb_substeps} substeps of {substep} s)")
+    return lo_s, hi_s
+
+
 class B200VectorEnv(VectorEnv):
     """N Upkie environments stepped by one kernel launch per ``step()``.
 
@@ -587,6 +625,13 @@ class B200VectorEnv(VectorEnv):
     command of the previous tick, and the first ones of an episode run with the servos stopped. The draws are keyed on
     the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets.
     ``set_action_delay`` changes or (``None``) stops it from each env's next reset.
+
+    ``observation_delay`` (seconds, a float or a ``(low, high)`` range, see ``observation_delay_spec``) makes each env
+    observe its robot a number of substeps before the end of the tick, drawn at every reset of that env, up to one
+    tick: the observation (and ``base_velocity``'s, through its gyropod rows) describes the robot at that instant,
+    while terminations and resets judge the true state; the observation of a reset is undelayed. The draws are keyed on
+    the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets.
+    ``set_observation_delay`` changes or (``None``) stops it from each env's next reset.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -623,6 +668,7 @@ class B200VectorEnv(VectorEnv):
         reset_randomization: Optional[dict] = None,
         push_randomization: Optional[dict] = None,
         action_delay: Optional[Union[float, Tuple[float, float]]] = None,
+        observation_delay: Optional[Union[float, Tuple[float, float]]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -666,6 +712,9 @@ class B200VectorEnv(VectorEnv):
         self.config = config
         delay_spec = action_delay_spec(action_delay, 1.0 / frequency, config.nb_substeps, bool(config.spine_mode),
                                        config.joint_limits)  # validated before any device is touched
+        sense_spec = observation_delay_spec(observation_delay, 1.0 / frequency, config.nb_substeps,
+                                            bool(config.spine_mode), config.joint_limits,
+                                            config.body_contacts)  # validated before any device is touched
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -716,6 +765,8 @@ class B200VectorEnv(VectorEnv):
             self.sim.set_push_randomization(push_spec)
         if delay_spec is not None:
             self.sim.set_action_delay(*delay_spec)  # before the first reset, which draws every env's delay
+        if sense_spec is not None:
+            self.sim.set_observation_delay(*sense_spec)  # before the first reset, which draws every env's delay
 
     def set_reset_randomization(self, spec: Optional[dict]) -> None:
         """Redraw the parameters ``spec`` names at every later reset of an env (``reset_randomization_spec``);
@@ -733,6 +784,14 @@ class B200VectorEnv(VectorEnv):
         spec = action_delay_spec(delay, self.dt, self.config.nb_substeps, bool(self.config.spine_mode),
                                  self.config.joint_limits)
         self.sim.set_action_delay(*(spec if spec is not None else (None,)))
+
+    def set_observation_delay(self, delay) -> None:
+        """Observe each robot ``delay`` seconds before the end of the tick, a float or a ``(low, high)`` range
+        (``observation_delay_spec``); ``None`` turns the delay off. A new range takes effect at each env's next
+        reset."""
+        spec = observation_delay_spec(delay, self.dt, self.config.nb_substeps, bool(self.config.spine_mode),
+                                      self.config.joint_limits, self.config.body_contacts)
+        self.sim.set_observation_delay(*(spec if spec is not None else (None,)))
 
     # ------------------------------------------------------------------
     def get_neutral_action(self) -> dict:
@@ -874,6 +933,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_action_delay_state(count, delay, command)
+            if getattr(self.sim, "_observation_delay", None) is not None:
+                # so is the observation delay
+                count, delay, rows = self.sim.get_observation_delay_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_observation_delay_state(count, delay, rows)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

@@ -219,6 +219,41 @@ class UpkieSim:
                                                       self._stream()))
         self._delay_state_set = True
 
+    def set_observation_delay(self, low: Optional[int], high: Optional[int] = None) -> None:
+        """While a range is set, everything a step reports about each env's sensors (its observation, ``spine_obs``,
+        ``final_obs`` and the final spine observation) describes the robot ``d`` substeps before the end of the tick,
+        ``low <= d <= high <= nb_substeps``; the IMU acceleration differentiates consecutive snapshots. Terminations,
+        resets and ``get_state`` read the true state. Each reset of the env draws a new ``d`` (keyed on the auto-reset
+        seed and the env's counter, ``include/upkie_b200.h``) and is observed undelayed. ``high`` defaults to ``low``;
+        ``None`` turns the delay off. Setting a range draws nothing: it takes effect at each env's next reset."""
+        if low is None:
+            check(lib().upkie_b200_set_observation_delay(self._h, None))
+            self._observation_delay = None
+            return
+        spec = _abi.UpkieObservationDelay(int(low), int(low if high is None else high))
+        check(lib().upkie_b200_set_observation_delay(self._h, C.byref(spec)))
+        self._observation_delay = (spec.substeps_low, spec.substeps_high)
+        self._sense_state_set = True  # the handle holds a state from now on
+
+    def get_observation_delay_state(self):
+        """Per-env observation-delay state ``(count[N], delay[N], rows[N, STATE_DIM])``: the draw counters (int32 bits
+        of uint32), the delays in substeps and the sensed state rows (``get_state`` layout), what the observations are
+        built from; the current state on a handle that never had a delay."""
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        delay = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        rows = torch.empty((self.n, _abi.STATE_DIM), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_observation_delay_state(self._h, _ptr(count), _ptr(delay), _ptr(rows),
+                                                           self._stream()))
+        return count, delay, rows
+
+    def set_observation_delay_state(self, count: torch.Tensor, delay: torch.Tensor, rows: torch.Tensor) -> None:
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(delay, (self.n,), torch.int32, "delay")
+        self._check_tensor(rows, (self.n, _abi.STATE_DIM), name="rows")
+        check(lib().upkie_b200_set_observation_delay_state(self._h, _ptr(count), _ptr(delay), _ptr(rows),
+                                                           self._stream()))
+        self._sense_state_set = True
+
     def set_external_forces(self, force: Optional[torch.Tensor] = None, local_mask: int = 0) -> None:
         """``force[N, 7, 3]`` newtons at the centres of mass of the 7 bodies, applied on every substep of
         the following steps until overwritten; ``None`` clears. Bit ``b`` of ``local_mask``: the force on
@@ -587,6 +622,7 @@ class UpkieSim:
         push = getattr(self, "_push_randomization", None)
         push_count, push_timer = self.get_push_state()
         delay_count, delay_delay, delay_command = self.get_action_delay_state()
+        sense_count, sense_delay, sense_rows = self.get_observation_delay_state()
         force, local_mask = getattr(self, "_external", (None, 0))
         return {
             "reset_randomization": None if spec is None else bytes(spec),  # the UpkieResetRandomization in force
@@ -597,6 +633,11 @@ class UpkieSim:
             # per-env action-delay state: draw counters, delays, previous servo commands
             "action_delay_count": delay_count, "action_delay_delay": delay_delay,
             "action_delay_command": delay_command,
+            # (substeps_low, substeps_high) of the observation delay in force, or None
+            "observation_delay": getattr(self, "_observation_delay", None),
+            # per-env observation-delay state: draw counters, delays, sensed state rows
+            "observation_delay_count": sense_count, "observation_delay_delay": sense_delay,
+            "observation_delay_rows": sense_rows,
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
             "elapsed": elapsed,  # steps since each env's last reset (the time limit's counts)
@@ -660,6 +701,20 @@ class UpkieSim:
             self.set_action_delay_state(zeros if count is None else count.to(dev).contiguous(),
                                         zeros if delay_d is None else delay_d.to(dev).contiguous(),
                                         stop if command is None else command.to(dev).contiguous())
+        # a checkpoint written before the observation delay existed loads as "off, counters 0, delays 0" (and the
+        # state as the sensed rows)
+        sense = sd.get("observation_delay")
+        self.set_observation_delay(*(sense if sense is not None else (None,)))
+        count, delay_d, rows = (sd.get(k) for k in ("observation_delay_count", "observation_delay_delay",
+                                                    "observation_delay_rows"))
+        state = sd["state"].to(dev)
+        default = count is None or (not count.any() and not delay_d.any()
+                                    and torch.equal(rows.to(dev).nan_to_num(7.0), state.nan_to_num(7.0)))
+        if sense is not None or not default or getattr(self, "_sense_state_set", False):
+            # as the action delay's: a handle that never had a state and a checkpoint without one allocate nothing
+            self.set_observation_delay_state(zeros if count is None else count.to(dev).contiguous(),
+                                             zeros if delay_d is None else delay_d.to(dev).contiguous(),
+                                             state.contiguous() if rows is None else rows.to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
