@@ -284,11 +284,18 @@ class _Exact:
 
 
 # -- closed-loop runner ---------------------------------------------------------------------------------------------
-def _config(kind, joint_limits=3, body=0):
+CONFIG_KEYS = ("joint_limits", "body", "overrides")
+
+
+def _config(kind, joint_limits=3, body=0, overrides=()):
+    """``overrides``: ``(field, value)`` pairs of UpkieSimConfig set last, e.g. ``(("dt", 0.01), ("nb_substeps", 10))``
+    (a tuple, so that it keys the reference cache)."""
     cfg = _abi.default_sim_config()
     if kind == "servos":  # the headline workload's termination (bench.py: servos_config)
         cfg.servos_fall_termination, cfg.min_base_height = 1, 0.15
         cfg.joint_limits, cfg.body_contacts = joint_limits, body
+    for k, v in overrides:
+        setattr(cfg, k, v)
     return cfg
 
 
@@ -345,7 +352,7 @@ def _references(model, oracle_lib, torch, kind, n=N, ticks=TICKS, exact=True, **
     physics, so that runs which differ only in the device path share them."""
     key = (kind, n, ticks, exact, tuple(sorted(kw.items(), key=lambda x: x[0])))
     if key not in _REFERENCES:
-        cfg = _config(kind, **{k: v for k, v in kw.items() if k in ("joint_limits", "body")})
+        cfg = _config(kind, **{k: v for k, v in kw.items() if k in CONFIG_KEYS})
         sides = {"oracle": _Oracle(oracle_lib, model, cfg, n, False), "oracle32": _Oracle(oracle_lib, model, cfg, n, True),
                  "host": _Host(model, cfg, n)}
         if exact:
@@ -392,7 +399,8 @@ def _check_run(model, name, dev, refs, caps=(CAP_PITCH, CAP_POS)):
 # Caps: the CPU test's 1e-4 rad / 5e-4 m where the host build stays well inside them. UpkieServos runs carry the
 # headline's randomisation, and there fp32 alone drifts further. Measured with the host build over these 1 027 robots:
 # 9.6e-5 rad / 1.3e-4 m with straight legs, 1.8e-4 rad / 1.8e-3 m with the squat (the fp32 oracle: 7.6e-5 / 1.1e-4 and
-# 2.0e-4 / 1.9e-3). Those caps are ten times the host build's drift.
+# 2.0e-4 / 1.9e-3). Those caps are ten times the host build's drift. The gyropod at 1 000 Hz, one substep, drifts
+# further in its 0.4 s than at 200 Hz in 2 s (host build 7.3e-5 rad / 1.4e-5 m, fp32 oracle 6.5e-5 / 1.3e-5): CAPS_SERVOS.
 CAPS_SERVOS = (1e-3, 2e-3)
 CAPS_SQUAT = (2e-3, 2e-2)
 RUNS = {
@@ -406,6 +414,14 @@ RUNS = {
     "servos_headline_squat": ("servos", "compact", {"joint_limits": 3, "squat": SQUAT}, CAPS_SQUAT),
     "servos_table_squat": ("servos", "table", {"joint_limits": 3, "squat": SQUAT}, CAPS_SQUAT),
     "servos_body": ("servos", "servos", {"joint_limits": 3, "body": 1, "exact": False}, CAPS_SERVOS),
+    # away from the default config (test_gpu_config_parity.py holds the same knobs to the oracle over one tick)
+    "gyropod_100hz_10_substeps": ("gyropod", "gyropod", {"overrides": (("dt", 0.01), ("nb_substeps", 10))},
+                                  (CAP_PITCH, CAP_POS)),
+    "gyropod_1000hz_1_substep": ("gyropod", "gyropod", {"overrides": (("dt", 0.001), ("nb_substeps", 1))},
+                                 CAPS_SERVOS),
+    "gyropod_friction_0.3": ("gyropod", "gyropod", {"overrides": (("friction", 0.3),)}, (CAP_PITCH, CAP_POS)),
+    "servos_warm_start_3_sweeps_squat": ("servos", "servos", {"joint_limits": 3, "squat": SQUAT, "overrides": (
+        ("warmstarting_factor", 0.85), ("pgs_iterations", 3), ("solver_residual_threshold", 0.0))}, CAPS_SQUAT),
 }
 
 
@@ -416,7 +432,7 @@ def test_two_second_closed_loop_on_the_device(model, oracle_lib, torch, name):
     the worst fp32 side's."""
     kind, path, kw, caps = RUNS[name]
     refs = _references(model, oracle_lib, torch, kind, **kw)
-    cfg = _config(kind, **{k: v for k, v in kw.items() if k in ("joint_limits", "body")})
+    cfg = _config(kind, **{k: v for k, v in kw.items() if k in CONFIG_KEYS})
     dev = _rollout(model, {"device": _Device(torch, model, cfg, N, path)}, kind, N, TICKS,
                    squat=kw.get("squat"))["device"]
     _check_run(model, name, dev, refs, caps)

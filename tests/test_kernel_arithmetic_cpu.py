@@ -862,3 +862,54 @@ def test_config_keeps_the_substep_rotation_in_the_integrators_range(model):
         assert bool(h) == ok, (dt, nb, vmax)
         if h:
             L.hostsim_destroy(h)
+
+
+def _config_cases():
+    """One (row, path) of test_gpu_config_parity.VARIANTS per distinct physics: on the host the headline and table
+    paths compute what limits3 does."""
+    from test_gpu_config_parity import CASES, PATHS
+
+    seen, out = set(), []
+    for row, path in CASES:
+        if (row,) + PATHS[path][:3] not in seen:
+            seen.add((row,) + PATHS[path][:3])
+            out.append((row, path))
+    return out
+
+
+HOST_RATIO = 10.0  # measured: the host build's error is 0.5x to 8x the fp32 oracle's on these rows (8x: spine, 100 Hz)
+
+
+@pytest.mark.parametrize("row,path", _config_cases())
+def test_host_build_away_from_the_default_config(model, oracle_lib, row, path):
+    """The CPU twin of test_gpu_config_parity.py: one tick of the same robots under each row's configuration, the host
+    build against the fp64 oracle. The row bites (it moves the fp64 one-tick state by BITE x the fp32 sides' 99th
+    percentile error) and its inputs reach the code under test (body contact rows, spine-mode contact), the host
+    build's base twist, joint rates and impulses stay within HOST_RATIO x the fp32 oracle's
+    error plus the GPU test's floors, worst robot and 99th percentile, and it flips at most one contact flag more."""
+    import test_gpu_config_parity as G
+
+    refs = G.references(model, oracle_lib, row, path)
+    ref = refs["oracle"]
+    flips = {k: G.contact_mismatch(refs[k], ref) for k in ("oracle32", "host")}
+    assert flips["host"].sum() <= flips["oracle32"].sum() + 1
+    mask = ~(flips["oracle32"] | flips["host"])
+    err = {k: G.errors(refs[k], ref, mask) for k in ("oracle32", "host")}
+    move, fp32 = G.bite(refs)
+    assert move >= G.BITE * fp32, (row, path, move, fp32)
+    G.check_inputs_exercise_the_path(refs, path)
+    for g in G.GROUPS:
+        for i, q in enumerate(("worst", "p99")):
+            assert err["host"][g][i] <= HOST_RATIO * err["oracle32"][g][i] + G.FLOOR[g], (row, path, g, q, err)
+
+
+def test_friction_rows_sit_on_their_bounds_at_friction_0_1(model, oracle_lib):
+    """The friction_0.1 row of test_gpu_config_parity.py binds: on the fp64 oracle, a friction impulse of more than a
+    hundred wheels is at +-mu times the wheel's normal impulse."""
+    import test_gpu_config_parity as G
+
+    st = G.references(model, oracle_lib, "friction_0.1", "limits3")["oracle"][0]
+    lam_n = np.repeat(st[:, _abi.ST_CONTACT_IMPULSE:_abi.ST_CONTACT_IMPULSE + 2], 2, axis=1)
+    lam_t = np.abs(st[:, _abi.ST_FRICTION_IMPULSE:_abi.ST_FRICTION_IMPULSE + 4])
+    on_bound = (lam_n > 1e-4) & (np.abs(lam_t - 0.1 * lam_n) <= 1e-6 * lam_n)
+    assert on_bound.sum() > 100, on_bound.sum()
