@@ -778,6 +778,40 @@ int upkie_b200_get_observation_delay_state(void* handle, uint32_t* count, uint32
 int upkie_b200_set_observation_delay_state(void* handle, const uint32_t* count, const uint32_t* delay,
                                            const float* rows, void* stream);
 
+/* Delays of more than one tick (an addition to ABI 8: no existing layout, constant or signature changed). Each delay
+ * may keep a history of max_ticks whole ticks, 1 <= max_ticks <= UPKIE_MAX_DELAY_TICKS, and then takes any delay
+ * d <= max_ticks * nb_substeps (a delay stored above acts as max_ticks * nb_substeps). upkie_b200_set_action_delay and
+ * upkie_b200_set_observation_delay are the max_ticks = 1 calls. Write d = q * nb + r with 0 <= q < max_ticks and
+ * 1 <= r <= nb (nb = nb_substeps; q = r = 0 for d = 0): a delay of at most one tick is q = 0, the rule above.
+ * - Action delay: in tick t, substeps s < r run the servo command of tick t - q - 1 and substeps s >= r that of tick
+ *   t - q. A command from before the env's last reset is the stop row, so the first d substeps of an episode run with
+ *   the servos stopped. Everything else is as for one tick (leg filter, yaw, clamps and noise keys at the start of the
+ *   tick, an undelayed reset substep, a same-step terminal tick under the delay in force).
+ * - Observation delay: after tick t everything the step reports about the sensors (the observations, spine_obs,
+ *   final_obs, the final spine observation, reset_obs of the envs a reset does not take) is the snapshot that a delay
+ *   of r substeps takes in tick t - q: what a handle with delay r reported q ticks earlier under the same actions, IMU
+ *   acceleration included. If tick t - q comes before the env's last reset, the report is the post-reset state.
+ *   Terminations, truncations, auto-resets, get_state and the gyropod wrapper's yaw and leg targets are not delayed.
+ * The draws keep their laws, counters and tags; only the range widens. A reset (fused or upkie_b200_reset) fills the
+ * whole history with stop rows / the post-reset state, and upkie_b200_set_state fills the snapshots with the state.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: max_ticks of 0 or above UPKIE_MAX_DELAY_TICKS,
+ * substeps_high > max_ticks * nb_substeps, and everything the one-tick calls reject; upkie_b200_set_config rejects an
+ * nb_substeps below ceil(substeps_high / max_ticks).
+ * The depth may change between calls: the history is kept in age order and truncated or extended, the added commands
+ * stop rows and the added snapshots copies of the oldest.
+ * History (for checkpoints), in age order, index 0 the newest (device pointers): the commands [max_ticks][N]
+ * [UPKIE_ACT_DIM] of the env's last ticks, and the snapshots [max_ticks][N][UPKIE_STATE_DIM] of its last ticks (at
+ * depth 1 the sensed rows of get_observation_delay_state; their unsensed columns carry no meaning at depth > 1). The
+ * *_delay_state calls keep their meaning: count, delay, the previous tick's command (age 0 of the history) and the
+ * sensed rows the last step reported. */
+#define UPKIE_MAX_DELAY_TICKS 8
+int upkie_b200_set_action_delay_ticks(void* handle, const UpkieActionDelay* spec, uint32_t max_ticks);
+int upkie_b200_get_action_delay_history(void* handle, float* commands, void* stream);
+int upkie_b200_set_action_delay_history(void* handle, const float* commands, void* stream);
+int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationDelay* spec, uint32_t max_ticks);
+int upkie_b200_get_observation_delay_history(void* handle, float* rows, void* stream);
+int upkie_b200_set_observation_delay_history(void* handle, const float* rows, void* stream);
+
 /* Number of step-kernel launches issued through this handle since create
  * (bench.py's `gpu_launches`). */
 int upkie_b200_launch_count(void* handle, uint64_t* count);

@@ -389,6 +389,9 @@ class UpkieActionDelay(C.Structure):
     ]
 
 
+MAX_DELAY_TICKS = 8  # UPKIE_MAX_DELAY_TICKS: the deepest history of an action or observation delay, in ticks
+
+
 class UpkieObservationDelay(C.Structure):
     """``UpkieObservationDelay`` of include/upkie_b200.h: the range of each env's observation delay, in substeps."""
 

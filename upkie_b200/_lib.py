@@ -53,6 +53,12 @@ SYMBOLS = {
     "upkie_b200_set_observation_delay": (C.c_int, [_vp, C.POINTER(_abi.UpkieObservationDelay)]),
     "upkie_b200_get_observation_delay_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_set_observation_delay_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
+    "upkie_b200_set_action_delay_ticks": (C.c_int, [_vp, C.POINTER(_abi.UpkieActionDelay), C.c_uint32]),
+    "upkie_b200_get_action_delay_history": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_action_delay_history": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_observation_delay_ticks": (C.c_int, [_vp, C.POINTER(_abi.UpkieObservationDelay), C.c_uint32]),
+    "upkie_b200_get_observation_delay_history": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_observation_delay_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_reset": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, _vp]),
     "upkie_b200_step_servos": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_step_gyropod": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]),

@@ -115,6 +115,7 @@ struct StepArgs {
   uint32_t ext_local;
   cudaStream_t stream;
   PeerPtrs peers;       // TILE=2 only
+  int history;          // the delay families: a delay keeps more than one tick (the k_step_hist kernels)
   float* lag;           // spine mode: [UPKIE_LAG_DIM][n_pad] lag records, else null
 };
 
@@ -146,5 +147,14 @@ cudaError_t launch_obs_delay_reset(const ObsDelay* O, int n, int n_pad, const fl
 // sensed rows [n][UPKIE_STATE_DIM] <-> the buffer's columns [UPKIE_STATE_DIM][stride]
 cudaError_t launch_sensed_rows(const float* cols, int n, int stride, float* rows, cudaStream_t stream);
 cudaError_t launch_sensed_cols(const float* rows, int n, int stride, float* cols, cudaStream_t stream);
+// (action_delay.cu) the delay histories, rings [K][dim][stride] whose next write is row head[i] (null: 0), in age order:
+// rows [ages][n][dim] <-> ages 0 .. ages - 1 (0 the newest); and a ring copied into one of another depth, row 0 its next
+// write, the ages it adds stop rows (stop) or copies of the oldest, `columns` the mask of the columns copied
+cudaError_t launch_ring_rows(const float* ring, const uint32_t* head, int ticks, int dim, int n, int stride, int ages,
+                             float* rows, cudaStream_t stream);
+cudaError_t launch_ring_cols(const float* rows, const uint32_t* head, int ticks, int dim, int n, int stride, int ages,
+                             float* ring, cudaStream_t stream);
+cudaError_t launch_ring_resize(const float* src, const uint32_t* head, int src_ticks, float* dst, int dst_ticks,
+                               int dim, int n, int stride, int stop, uint64_t columns, cudaStream_t stream);
 
 }  // namespace upkie_b200

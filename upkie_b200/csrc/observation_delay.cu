@@ -19,7 +19,10 @@ __global__ void k_obs_delay_reset(const ObsDelay* __restrict__ O, int n, int n_p
   obs_delay_reset(*O, seed, env_offset + uint64_t(i), i);
   float* const col = O->rows + size_t(i);
   const size_t stride = size_t(O->stride);
-  for (int k = 0; k < UPKIE_STATE_DIM; ++k) col[size_t(k) * stride] = state[size_t(k) * n_pad + i];
+  float r[UPKIE_STATE_DIM];
+  for (int k = 0; k < UPKIE_STATE_DIM; ++k) r[k] = state[size_t(k) * n_pad + i];
+  for (int k = 0; k < UPKIE_STATE_DIM; ++k) col[size_t(k) * stride] = r[k];
+  if (O->ticks > 1) obs_delay_fill_history(*O, i, r);  // and so does every snapshot of the history
 }
 
 // rows [n][UPKIE_STATE_DIM] <-> columns [UPKIE_STATE_DIM][stride]

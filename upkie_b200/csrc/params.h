@@ -347,10 +347,13 @@ inline bool push_spec_valid(const UpkiePushRandomization& s) {
 }
 
 // Why a handle with parameters P refuses an action-delay spec (upkie_b200_set_action_delay), null when it takes it
-inline const char* action_delay_spec_error(const UpkieActionDelay& s, const SimParams& P) {
+// (with a history of `ticks` whole ticks, upkie_b200_set_action_delay_ticks: one tick is the call without it)
+inline const char* action_delay_spec_error(const UpkieActionDelay& s, const SimParams& P, uint32_t ticks = 1) {
   if (s.substeps_low > s.substeps_high) return "set_action_delay: substeps_low > substeps_high";
-  if (s.substeps_high > uint32_t(P.nb_substeps))
+  if (ticks == 1 && s.substeps_high > uint32_t(P.nb_substeps))
     return "set_action_delay: substeps_high above nb_substeps (the delay is at most one tick)";
+  if (s.substeps_high > uint64_t(ticks) * uint32_t(P.nb_substeps))
+    return "set_action_delay: substeps_high above max_ticks * nb_substeps (the delay is at most max_ticks ticks)";
   if (P.joint_limits == 0)
     return "set_action_delay: needs joint_limits != 0 (the delay runs in the table and body-contact kernels)";
   if (P.spine_mode) return "set_action_delay: spine_mode models the spine's own lag";
@@ -359,10 +362,13 @@ inline const char* action_delay_spec_error(const UpkieActionDelay& s, const SimP
 
 // Why a handle with parameters P refuses an observation-delay spec (upkie_b200_set_observation_delay), null when it
 // takes it
-inline const char* obs_delay_spec_error(const UpkieObservationDelay& s, const SimParams& P) {
+// (with a history of `ticks` whole ticks, upkie_b200_set_observation_delay_ticks: one tick is the call without it)
+inline const char* obs_delay_spec_error(const UpkieObservationDelay& s, const SimParams& P, uint32_t ticks = 1) {
   if (s.substeps_low > s.substeps_high) return "set_observation_delay: substeps_low > substeps_high";
-  if (s.substeps_high > uint32_t(P.nb_substeps))
+  if (ticks == 1 && s.substeps_high > uint32_t(P.nb_substeps))
     return "set_observation_delay: substeps_high above nb_substeps (the delay is at most one tick)";
+  if (s.substeps_high > uint64_t(ticks) * uint32_t(P.nb_substeps))
+    return "set_observation_delay: substeps_high above max_ticks * nb_substeps (the delay is at most max_ticks ticks)";
   if (P.joint_limits == 0)
     return "set_observation_delay: needs joint_limits != 0 (the delay runs in a copy of the table kernels)";
   if (P.spine_mode) return "set_observation_delay: spine_mode models the spine's own lag";

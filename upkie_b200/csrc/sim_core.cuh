@@ -1810,6 +1810,10 @@ struct ActionDelay {
   uint32_t* delay;
   float* command;
   int stride;
+  // the history depth K (upkie_b200_set_action_delay_ticks; 0 acts as 1): command holds K rows [K][UPKIE_ACT_DIM][stride]
+  // of the env's last K ticks, a ring whose next write is row head[i] (read by the K > 1 branch only)
+  int ticks;
+  uint32_t* head;
 };
 
 // bit 61 of the high counter word: never set by sample_init_state ((episode << 2) | b, episode < 2^32), the noise
@@ -1838,6 +1842,47 @@ UPKIE_HD void action_delay_substep(int sub, uint32_t d, float a[UPKIE_ACT_DIM], 
   }
 }
 
+// ---- delays of more than one tick (a history of K ticks, upkie_b200_set_*_delay_ticks) ----
+// A delay of d substeps, clamped to K * nb, as whole ticks q and a part r of a tick: d = q * nb + r with 0 <= q < K and
+// 1 <= r <= nb (q = r = 0 for d = 0). r = nb is the whole tick, which the one-tick kernels already run (the action
+// delay switches at no substep, the observation delay snapshots the start of the tick), so a delay of at most nb
+// substeps is q = 0 and the one-tick rule itself.
+struct DelaySplit {
+  uint32_t q, r;
+};
+UPKIE_HD DelaySplit delay_split(uint32_t d, uint32_t nb, uint32_t ticks) {
+  const uint32_t cap = ticks * nb;
+  const uint32_t dd = d < cap ? d : cap;
+  const uint32_t q = dd ? (dd - 1u) / nb : 0u;
+  return {q, dd - q * nb};
+}
+
+// The ring row of age `age` (0 the newest) of a history of K rows whose next write is row `head`
+UPKIE_HD uint32_t delay_ring_row(uint32_t head, uint32_t ticks, uint32_t age) { return (head + ticks - 1u - age) % ticks; }
+
+// The ring rows of one tick of an action delay d with a history of K ticks whose next write is row `head`: the tick
+// enters its substeps with the command of row `first` (age q: tick t - q - 1), then stores this tick's command into row
+// `head` (age K - 1, the oldest, read first when q = K - 1), and substep r loads the command of tick t - q from row
+// `second` (the row just stored for q = 0). The next tick writes row (head + 1) % K.
+struct ActionDelayRows {
+  uint32_t first, second, r;
+};
+UPKIE_HD ActionDelayRows action_delay_rows(uint32_t d, uint32_t nb, uint32_t ticks, uint32_t head) {
+  const DelaySplit s = delay_split(d, nb, ticks);
+  return {delay_ring_row(head, ticks, s.q), (head + ticks - s.q) % ticks, s.r};
+}
+
+// The ring rows of one tick of an observation delay d with a history of K ticks whose next write is row `head`: the
+// snapshot of substep nb - r goes into row `head` and differentiates its IMU velocity against row `newest` (age 0, the
+// last tick's), and after the tick the step reports row `report` (age q of the ring with this tick's snapshot in it).
+struct ObsDelayRows {
+  uint32_t newest, report, r;
+};
+UPKIE_HD ObsDelayRows obs_delay_rows(uint32_t d, uint32_t nb, uint32_t ticks, uint32_t head) {
+  const DelaySplit s = delay_split(d, nb, ticks);
+  return {delay_ring_row(head, ticks, 0u), (head + ticks - s.q) % ticks, s.r};
+}
+
 // A reset of env i (the step kernels' fused resets, k_action_delay_reset): the next draw, and the stop row as the
 // previous command. The block's fields are copied before the first store, which the compiler cannot tell apart from
 // the block itself.
@@ -1853,6 +1898,13 @@ UPKIE_HD void action_delay_reset(const ActionDelay& A, uint64_t seed, uint64_t g
   for (int c = 0; c < UPKIE_ACT_DIM; ++c) col[size_t(c) * stride] = action_delay_stop_value(c);
 }
 
+// With a history of K > 1 ticks, after action_delay_reset: the stop row as the other K - 1 commands too
+UPKIE_HD void action_delay_fill_history(const ActionDelay& A, int i) {
+  float* const col = A.command + size_t(i);
+  const size_t stride = size_t(A.stride);
+  for (int c = UPKIE_ACT_DIM; c < A.ticks * UPKIE_ACT_DIM; ++c) col[size_t(c) * stride] = action_delay_stop_value(c);
+}
+
 // ---- observation-delay randomisation (upkie_b200_set_observation_delay) ----
 // The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
 // env's last draw, delay[i] = d_i in substeps, and rows = the sensed state of each env, [UPKIE_STATE_DIM][stride]
@@ -1864,6 +1916,12 @@ struct ObsDelay {
   uint32_t* delay;
   float* rows;
   int stride;
+  // the history depth K (upkie_b200_set_observation_delay_ticks; 0 acts as 1). K > 1: hist holds the snapshots of the
+  // env's last K ticks [K][UPKIE_STATE_DIM][stride], a ring whose next write is row head[i]; `rows` is then a copy of
+  // the sensed columns of the snapshot the last step reported
+  int ticks;
+  float* hist;
+  uint32_t* head;
 };
 
 // bit 60 of the high counter word: never set by sample_init_state ((episode << 2) | b, episode < 2^32), the noise
@@ -1904,6 +1962,14 @@ UPKIE_HD void obs_delay_reset(const ObsDelay& O, uint64_t seed, uint64_t g, int 
   const uint32_t k = count[i] + 1u;
   count[i] = k;
   delay[i] = obs_delay_draw(spec, seed, g, k);
+}
+
+// A reset of env i with a history of K > 1 ticks: every snapshot of the ring becomes the post-reset state row r
+UPKIE_HD void obs_delay_fill_history(const ObsDelay& O, int i, const float r[UPKIE_STATE_DIM]) {
+  float* const col = O.hist + size_t(i);
+  const size_t stride = size_t(O.stride);
+  for (int s = 0; s < O.ticks; ++s)
+    for (int k = 0; k < UPKIE_STATE_DIM; ++k) col[(size_t(s) * UPKIE_STATE_DIM + k) * stride] = r[k];
 }
 
 }  // namespace upkie_b200

@@ -105,10 +105,32 @@ __device__ __forceinline__ void reset_rand_lane(const SimParams& P, uint64_t see
     if ((cols >> (UPKIE_EP_MEAS_NOISE + j)) & 1u) meas_sd[j] = v[UPKIE_EP_MEAS_NOISE + j];
 }
 
+// A history of K > 1 ticks: the env's ring moves on by one row. Every step advances every env's ring, a resetting lane
+// included (its reset refills the whole ring, so the row it lands on does not matter to it), and nothing else moves
+// them: the rings of all envs stay on the same row, and a warp's history loads and stores stay coalesced rows.
+__device__ __forceinline__ void delay_ring_advance(uint32_t* head, int ticks, int i) {
+  if (ticks > 1) __stcg(head + i, (__ldcg(head + i) + 1u) % uint32_t(ticks));
+}
+
+// Observation delay with a history of K > 1 ticks: the sensed columns of ring row `srep` (the snapshot the step
+// reports) into env i's sensed row, stored by live lanes; the sensed row's address
+__device__ __forceinline__ float* obs_delay_report(const ObsDelay& O, uint32_t srep, int i, bool live) {
+  const size_t stride = size_t(O.stride);
+  float* const row = O.rows + size_t(i);
+  const float* const src = O.hist + size_t(i) + size_t(srep) * UPKIE_STATE_DIM * stride;
+  if (live) {
+#pragma unroll
+    for (int k = 0; k < UPKIE_STATE_DIM; ++k)
+      if (obs_delay_sensed(k)) __stcg(row + size_t(k) * stride, __ldcg(src + size_t(k) * stride));
+  }
+  return row;
+}
+
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE=1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), and it is reused to transpose the observation rows on the way out.
-template <int MODE, int AUTORESET, int FAMILY, int TILE>
+// HIST (the delay families' k_step_hist kernels): a delay keeps a history of more than one tick; compiled out of k_step
+template <int MODE, int AUTORESET, int FAMILY, int TILE, bool HIST = false>
 __device__ __forceinline__ void step_env(
     const SimParams& P, int tid, int n, int n_pad, float* __restrict__ state, const float* __restrict__ action,
     float* __restrict__ obs, float* __restrict__ reward, uint8_t* __restrict__ terminated,
@@ -243,19 +265,41 @@ __device__ __forceinline__ void step_env(
   // of the 36 elements then re-read the pointer and waited for it (a chain of dependent loads per env that made the
   // tick 2.2 times as long). The previous row is read whole before the new one is written. The loads are coherent
   // (ld.global.cg), not the read-only path, which need not return a thread's own stores of the same launch.
+  // A history of K > 1 ticks (A.ticks, a uniform branch; delay_split): the buffer is a ring of K rows, and a delay of
+  // q whole ticks and r substeps enters the tick with the command of age q (tick t - q - 1), stores this tick's into the
+  // oldest row (age K - 1, read before it is overwritten when q = K - 1), and substep r loads the command of tick t - q
+  // from row `dsec` (this tick's own for q = 0).
   const bool delaying = F.delay && P.action_delay;
   uint32_t dly = 0xffffffffu;
+  size_t dsec = 0;  // the ring row substep dly loads, in floats (0 for K = 1)
   if (delaying) {
     const ActionDelay& A = *P.action_delay;
     if (resetting) {
-      if (live) action_delay_reset(A, seed, env_offset + uint64_t(i), i);
+      if (live) {
+        action_delay_reset(A, seed, env_offset + uint64_t(i), i);
+        if (HIST) {
+          action_delay_fill_history(A, i);
+          delay_ring_advance(A.head, A.ticks, i);
+        }
+      }
     } else {
-      float* const col = A.command + size_t(i);
+      float* col = A.command + size_t(i);
       const size_t stride = size_t(A.stride);
       dly = __ldcg(A.delay + i);
+      const float* first = col;
+      if (HIST && A.ticks > 1) {
+        const uint32_t K = uint32_t(A.ticks), h = __ldcg(A.head + i);
+        const ActionDelayRows dr = action_delay_rows(dly, uint32_t(P.nb_substeps), K, h);
+        const size_t row = size_t(UPKIE_ACT_DIM) * stride;
+        dly = dr.r;
+        first = col + dr.first * row;
+        dsec = dr.second * row;
+        col += h * row;
+        if (live) __stcg(A.head + i, (h + 1u) % K);
+      }
       float prev[UPKIE_ACT_DIM];
 #pragma unroll
-      for (int c = 0; c < UPKIE_ACT_DIM; ++c) prev[c] = __ldcg(col + size_t(c) * stride);
+      for (int c = 0; c < UPKIE_ACT_DIM; ++c) prev[c] = __ldcg(first + size_t(c) * stride);
       if (live) {
 #pragma unroll
         for (int c = 0; c < UPKIE_ACT_DIM; ++c) __stcg(col + size_t(c) * stride, a[c]);
@@ -275,12 +319,36 @@ __device__ __forceinline__ void step_env(
   float* scol = nullptr;
   size_t sstride = 0;
   uint32_t sdl = 0xffffffffu;  // resetting lanes: no snapshot
+  uint32_t srep = 0;           // K > 1: the ring row of the snapshot the step reports
+  // A history of K > 1 ticks (O.ticks, a uniform branch; delay_split): a delay of q whole ticks and r substeps takes
+  // this tick's snapshot at substep nb - r into the oldest row of the ring (`scol` points there for the substeps; it
+  // first takes the newest snapshot's IMU velocity, which the snapshot differentiates against), and the step reports
+  // the snapshot of age q, copied into the sensed row after the substeps (obs_delay_report).
   if (sensing) {
     const ObsDelay& O = *P.obs_delay;
     scol = O.rows + size_t(i);
     sstride = size_t(O.stride);
     if (resetting) {
-      if (live) obs_delay_reset(O, seed, env_offset + uint64_t(i), i);
+      if (live) {
+        obs_delay_reset(O, seed, env_offset + uint64_t(i), i);
+        if (HIST) delay_ring_advance(O.head, O.ticks, i);
+      }
+    } else if (HIST && O.ticks > 1) {
+      const uint32_t K = uint32_t(O.ticks), h = __ldcg(O.head + i);
+      const ObsDelayRows dr = obs_delay_rows(__ldcg(O.delay + i), uint32_t(P.nb_substeps), K, h);
+      sdl = dr.r;
+      srep = dr.report;
+      const size_t row = size_t(UPKIE_STATE_DIM) * sstride;
+      float* const hcol = O.hist + size_t(i);
+      scol = hcol + h * row;
+      const float* const newest = hcol + dr.newest * row;
+      if (live) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+          __stcg(scol + size_t(UPKIE_ST_PREV_IMU_VEL + k) * sstride,
+                 __ldcg(newest + size_t(UPKIE_ST_PREV_IMU_VEL + k) * sstride));
+        __stcg(O.head + i, (h + 1u) % K);
+      }
     } else {
       sdl = min(__ldcg(O.delay + i), uint32_t(P.nb_substeps));
     }
@@ -302,7 +370,7 @@ __device__ __forceinline__ void step_env(
       if (delaying) {
         action_delay_substep(sub, dly, a, [&](int c) {
           const ActionDelay& A = *P.action_delay;
-          return __ldcg(A.command + size_t(c) * size_t(A.stride) + size_t(i));
+          return __ldcg(A.command + dsec + size_t(c) * size_t(A.stride) + size_t(i));
         });
       }
       // the body-ground contacts of the tick's last substep go to the handle's record (F.body kernels)
@@ -395,7 +463,10 @@ __device__ __forceinline__ void step_env(
       if (F.reset_rand && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
       if (pushing) push_restart(push_k, push_t, push_end);  // the terminal step ran under its push; a new schedule
       // the terminal step ran under its delay; the next tick starts from the stop row with a new one
-      if (delaying && live) action_delay_reset(*P.action_delay, seed, env_offset + uint64_t(i), i);
+      if (delaying && live) {
+        action_delay_reset(*P.action_delay, seed, env_offset + uint64_t(i), i);
+        if (HIST) action_delay_fill_history(*P.action_delay, i);
+      }
       // the terminal step was observed under its delay; the reset is observed undelayed, with a new draw
       if (sensing && live) obs_delay_reset(*P.obs_delay, seed, env_offset + uint64_t(i), i);
       elapsed = 0;
@@ -417,6 +488,8 @@ __device__ __forceinline__ void step_env(
 
   if (live) store_state(state, n_pad, i, S);
   if (sensing) {
+    // K > 1: the sensed row becomes the report, and the end of the tick works on it as for one tick
+    if (HIST && !resetting && P.obs_delay->ticks > 1) scol = obs_delay_report(*P.obs_delay, srep, i, live);
     if (fin_pending) {
       // the terminal step's sensed state: its snapshot, with the terminal step's wrapper yaw, built in S (the post-reset
       // state is stored, and read back below). sdl = 0: the snapshot is the true state, whose gyropod observation fin_o6
@@ -451,6 +524,7 @@ __device__ __forceinline__ void step_env(
       state_to_row(S, r);
 #pragma unroll
       for (int k = 0; k < UPKIE_STATE_DIM; ++k) sense_store(k, r[k]);
+      if (HIST && P.obs_delay->ticks > 1) obs_delay_fill_history(*P.obs_delay, i, r);  // and so does every snapshot
     }
   }
   if (spine && live) {
@@ -629,22 +703,17 @@ __device__ __forceinline__ void cp_async_wait() {
 // shared-memory buffer while the current tile computes, and observation rows leave through coalesced
 // 16 B stores, so the link streams in both directions for the whole launch instead of in bursts
 // between compute phases.
-template <int MODE, int AUTORESET, int FAMILY, int TILE>
-#ifdef UPKIE_MAXNREG
-__global__ void __maxnreg__(UPKIE_MAXNREG)
-#else
-__global__ void __launch_bounds__(UPKIE_MAX_THREADS, UPKIE_MIN_BLOCKS)
-#endif
-k_step(const __grid_constant__ SimParams P, int i0, int n, int n_pad, float* __restrict__ state,
+template <int MODE, int AUTORESET, int FAMILY, int TILE, bool HIST>
+__device__ __forceinline__ void step_tiles(const SimParams& P, int i0, int n, int n_pad, float* __restrict__ state,
        const float* __restrict__ action, float* __restrict__ obs, float* __restrict__ reward,
        uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated, const float* __restrict__ eps_all,
        const float* __restrict__ mu_all, uint32_t* __restrict__ err, uint8_t* __restrict__ done_prev,
        uint32_t* __restrict__ episode, uint32_t* __restrict__ tick, uint64_t seed, uint64_t env_offset,
-       const float* __restrict__ ext, uint32_t ext_local, int coalesce, const __grid_constant__ PeerPtrs peers,
+       const float* __restrict__ ext, uint32_t ext_local, int coalesce, const PeerPtrs& peers,
        float* __restrict__ lag) {
   // this launch covers the envs [i0, n)
   if (!TILE) {
-    step_env<MODE, AUTORESET, FAMILY, 0>(P, i0 + blockIdx.x * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
+    step_env<MODE, AUTORESET, FAMILY, 0, HIST>(P, i0 + blockIdx.x * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
                                          reward, terminated, truncated, eps_all, mu_all, err, done_prev, episode, tick,
                                          seed, env_offset, ext, ext_local, nullptr, false, false, nullptr, lag);
     return;
@@ -679,12 +748,51 @@ k_step(const __grid_constant__ SimParams P, int i0, int n, int n_pad, float* __r
     if (TILE == 2) {
       if (peers.deferred && peers.src_obs) push_rows(peers, i0 + t * int(blockDim.x) + warp * 32, lane);
     }
-    step_env<MODE, AUTORESET, FAMILY, TILE>(P, i0 + t * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
+    step_env<MODE, AUTORESET, FAMILY, TILE, HIST>(P, i0 + t * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
                                          reward, terminated, truncated, eps_all, mu_all, err, done_prev, episode, tick,
                                          seed, env_offset, ext, ext_local, buf[it & 1], warp_full(t),
                                          (coalesce & 2) != 0, TILE == 2 ? &peers : nullptr, lag);
     __syncwarp();  // the tile is free again before the next prefetch lands in it
   }
+}
+
+
+template <int MODE, int AUTORESET, int FAMILY, int TILE>
+#ifdef UPKIE_MAXNREG
+__global__ void __maxnreg__(UPKIE_MAXNREG)
+#else
+__global__ void __launch_bounds__(UPKIE_MAX_THREADS, UPKIE_MIN_BLOCKS)
+#endif
+k_step(const __grid_constant__ SimParams P, int i0, int n, int n_pad, float* __restrict__ state,
+       const float* __restrict__ action, float* __restrict__ obs, float* __restrict__ reward,
+       uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated, const float* __restrict__ eps_all,
+       const float* __restrict__ mu_all, uint32_t* __restrict__ err, uint8_t* __restrict__ done_prev,
+       uint32_t* __restrict__ episode, uint32_t* __restrict__ tick, uint64_t seed, uint64_t env_offset,
+       const float* __restrict__ ext, uint32_t ext_local, int coalesce, const __grid_constant__ PeerPtrs peers,
+       float* __restrict__ lag) {
+  step_tiles<MODE, AUTORESET, FAMILY, TILE, false>(P, i0, n, n_pad, state, action, obs, reward, terminated, truncated,
+                                                 eps_all, mu_all, err, done_prev, episode, tick, seed, env_offset, ext,
+                                                 ext_local, coalesce, peers, lag);
+}
+
+// the delay families with a history of more than one tick (StepArgs::history): their own kernels, so that k_step keeps
+// the one-tick code
+template <int MODE, int AUTORESET, int FAMILY, int TILE>
+#ifdef UPKIE_MAXNREG
+__global__ void __maxnreg__(UPKIE_MAXNREG)
+#else
+__global__ void __launch_bounds__(UPKIE_MAX_THREADS, UPKIE_MIN_BLOCKS)
+#endif
+k_step_hist(const __grid_constant__ SimParams P, int i0, int n, int n_pad, float* __restrict__ state,
+       const float* __restrict__ action, float* __restrict__ obs, float* __restrict__ reward,
+       uint8_t* __restrict__ terminated, uint8_t* __restrict__ truncated, const float* __restrict__ eps_all,
+       const float* __restrict__ mu_all, uint32_t* __restrict__ err, uint8_t* __restrict__ done_prev,
+       uint32_t* __restrict__ episode, uint32_t* __restrict__ tick, uint64_t seed, uint64_t env_offset,
+       const float* __restrict__ ext, uint32_t ext_local, int coalesce, const __grid_constant__ PeerPtrs peers,
+       float* __restrict__ lag) {
+  step_tiles<MODE, AUTORESET, FAMILY, TILE, true>(P, i0, n, n_pad, state, action, obs, reward, terminated, truncated,
+                                                 eps_all, mu_all, err, done_prev, episode, tick, seed, env_offset, ext,
+                                                 ext_local, coalesce, peers, lag);
 }
 
 template <int TILE, int MODE, int AUTORESET, int FAMILY>
@@ -698,12 +806,15 @@ cudaError_t launch_k_step(const StepArgs& a) {
   const int coalesce = (aligned ? 1 : 0) | ((TILE && a.compact_obs) ? 2 : 0);  // bit 0 tile path, bit 1 compact rows
   // a 256-thread block's two tile buffers take 72 KB: above 48 KB of dynamic shared memory a kernel must opt in (per
   // device, so on every launch)
+  auto kernel = k_step<MODE, AUTORESET, FAMILY, TILE>;
+  if constexpr (step_family_traits(FAMILY).delay && TILE != 2) {
+    if (a.history) kernel = k_step_hist<MODE, AUTORESET, FAMILY, TILE>;
+  }
   if (smem > 48 * 1024) {
-    const cudaError_t e = cudaFuncSetAttribute(k_step<MODE, AUTORESET, FAMILY, TILE>,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
     if (e != cudaSuccess) return e;
   }
-  k_step<MODE, AUTORESET, FAMILY, TILE><<<grid, a.block, smem, a.stream>>>(
+  kernel<<<grid, a.block, smem, a.stream>>>(
       *a.P, a.i0, a.i0 + a.cnt, a.n_pad, a.state, a.action, a.obs, a.reward, a.terminated, a.truncated, a.eps, a.mu,
       a.err, a.done_prev, a.episode, a.tick, a.seed, a.env_offset, a.ext, a.ext_local, coalesce, a.peers, a.lag);
   return cudaGetLastError();

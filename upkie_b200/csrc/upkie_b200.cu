@@ -109,8 +109,10 @@ struct Handle {
   ActionDelay* delay_dev = nullptr;
   uint32_t* delay_count = nullptr;
   uint32_t* delay_delay = nullptr;
-  float* delay_command = nullptr;  // [UPKIE_ACT_DIM][n_pad]
+  float* delay_command = nullptr;  // [delay_ticks][UPKIE_ACT_DIM][n_pad], a ring of the last delay_ticks commands
+  uint32_t* delay_head = nullptr;  // the ring row each env's next tick writes
   uint32_t delay_high = 0;         // substeps_high of the spec in force
+  int delay_ticks = 1;             // the history depth (upkie_b200_set_action_delay_ticks)
   // observation-delay randomisation (upkie_b200_set_observation_delay): the device block P.obs_delay points to while a
   // spec is set, and the per-env state (allocated on the first spec or set_observation_delay_state)
   ObsDelay* sense_dev = nullptr;
@@ -118,6 +120,9 @@ struct Handle {
   uint32_t* sense_delay = nullptr;
   float* sense_rows = nullptr;     // [UPKIE_STATE_DIM][n_pad] sensed states
   uint32_t sense_high = 0;         // substeps_high of the spec in force
+  int sense_ticks = 1;             // the history depth (upkie_b200_set_observation_delay_ticks)
+  float* sense_hist = nullptr;     // sense_ticks > 1: [sense_ticks][UPKIE_STATE_DIM][n_pad], a ring of snapshots
+  uint32_t* sense_head = nullptr;  // the ring row each env's next tick writes
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -360,6 +365,7 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   StepArgs a;
   std::memset(&a.peers, 0, sizeof(a.peers));
   if (peers) a.peers = *peers;
+  a.history = (h->P.action_delay && h->delay_ticks > 1) || (h->P.obs_delay && h->sense_ticks > 1);
   SimParams P_launch;
   const bool stash = final_state && h->final_state && h->autoreset == AUTORESET_SAME_STEP;
   if ((final_obs || stash) && h->autoreset == AUTORESET_SAME_STEP) {
@@ -720,7 +726,9 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->env_params); cudaFree(h->ep_check); cudaFree(h->final_state); cudaFree(h->rr_dev); cudaFree(h->draws);
   cudaFree(h->push_dev); cudaFree(h->push_count); cudaFree(h->push_timer);
   cudaFree(h->delay_dev); cudaFree(h->delay_count); cudaFree(h->delay_delay); cudaFree(h->delay_command);
+  cudaFree(h->delay_head);
   cudaFree(h->sense_dev); cudaFree(h->sense_count); cudaFree(h->sense_delay); cudaFree(h->sense_rows);
+  cudaFree(h->sense_hist); cudaFree(h->sense_head);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -752,11 +760,11 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: push randomisation needs joint_limits != 0");
   if (h->P.action_delay && P.joint_limits == 0)
     return fail(UPKIE_B200_EINVAL, "set_config: action delay needs joint_limits != 0");
-  if (h->P.action_delay && uint32_t(P.nb_substeps) < h->delay_high)
+  if (h->P.action_delay && uint64_t(P.nb_substeps) * uint32_t(h->delay_ticks) < h->delay_high)
     return fail(UPKIE_B200_EINVAL, "set_config: nb_substeps below the action delay's substeps_high");
   if (h->P.obs_delay && P.joint_limits == 0)
     return fail(UPKIE_B200_EINVAL, "set_config: observation delay needs joint_limits != 0");
-  if (h->P.obs_delay && uint32_t(P.nb_substeps) < h->sense_high)
+  if (h->P.obs_delay && uint64_t(P.nb_substeps) * uint32_t(h->sense_ticks) < h->sense_high)
     return fail(UPKIE_B200_EINVAL, "set_config: nb_substeps below the observation delay's substeps_high");
   if (h->P.obs_delay && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no observation-delay kernels");
@@ -1251,10 +1259,14 @@ int upkie_b200_set_state(void* handle, const float* state, void* stream) {
   CUDA_TRY(cudaSetDevice(h->device));
   k_set_state<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->state, state);
   CUDA_TRY(cudaGetLastError());
-  // observation delay: the sensors see the state set, without a lag behind it
-  if (h->P.obs_delay)
+  // observation delay: the sensors see the state set, without a lag behind it (every snapshot of a history too)
+  if (h->P.obs_delay) {
     CUDA_TRY(cudaMemcpyAsync(h->sense_rows, h->state, size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float),
                              cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+    if (h->sense_hist)
+      CUDA_TRY(launch_ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad,
+                                  0, ~uint64_t(0), static_cast<cudaStream_t>(stream)));
+  }
   return UPKIE_B200_OK;
 }
 
@@ -1420,27 +1432,57 @@ namespace {
 int alloc_delay_state(Handle* h) {
   if (h->delay_count) return UPKIE_B200_OK;
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
-  uint32_t *count = nullptr, *delay = nullptr;
+  uint32_t *count = nullptr, *delay = nullptr, *head = nullptr;
   float* command = nullptr;
   cudaError_t e = cudaMalloc(&count, bytes);
   if (e == cudaSuccess) e = cudaMalloc(&delay, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&head, bytes);
   if (e == cudaSuccess) e = cudaMalloc(&command, size_t(UPKIE_ACT_DIM) * h->n_pad * sizeof(float));
   if (e == cudaSuccess) e = cudaMemset(count, 0, bytes);
   if (e == cudaSuccess) e = cudaMemset(delay, 0, bytes);
+  if (e == cudaSuccess) e = cudaMemset(head, 0, bytes);
   if (e == cudaSuccess) e = launch_command_cols(nullptr, h->n, h->n_pad, command, nullptr);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
-    cudaFree(count); cudaFree(delay); cudaFree(command);
+    cudaFree(count); cudaFree(delay); cudaFree(head); cudaFree(command);
     return fail(UPKIE_B200_ECUDA, std::string("action delay state: ") + cudaGetErrorString(e));
   }
   h->delay_count = count;
   h->delay_delay = delay;
+  h->delay_head = head;
   h->delay_command = command;
+  h->delay_ticks = 1;
+  return UPKIE_B200_OK;
+}
+}  // namespace
+
+namespace {
+// a history of `ticks` rows [ticks][dim][n_pad] in place of `*ring` ([*cur][dim][n_pad], next writes *head): the newest
+// min(ticks, *cur) rows in age order, the ages added stop rows (stop) or copies of the oldest, every next write row 0
+int resize_ring(Handle* h, float** ring, uint32_t* head, int* cur, int ticks, int dim, int stop, const char* what) {
+  if (ticks == *cur) return UPKIE_B200_OK;
+  float* next = nullptr;
+  cudaError_t e = cudaMalloc(&next, size_t(ticks) * dim * h->n_pad * sizeof(float));
+  if (e == cudaSuccess)
+    e = launch_ring_resize(*ring, head, *cur, next, ticks, dim, h->n, h->n_pad, stop, ~uint64_t(0), nullptr);
+  if (e == cudaSuccess) e = cudaMemset(head, 0, size_t(h->n) * sizeof(uint32_t));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    cudaFree(next);
+    return fail(UPKIE_B200_ECUDA, std::string(what) + cudaGetErrorString(e));
+  }
+  cudaFree(*ring);
+  *ring = next;
+  *cur = ticks;
   return UPKIE_B200_OK;
 }
 }  // namespace
 
 int upkie_b200_set_action_delay(void* handle, const UpkieActionDelay* spec) {
+  return upkie_b200_set_action_delay_ticks(handle, spec, 1);
+}
+
+int upkie_b200_set_action_delay_ticks(void* handle, const UpkieActionDelay* spec, uint32_t max_ticks) {
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
   if (!spec) {
@@ -1449,10 +1491,15 @@ int upkie_b200_set_action_delay(void* handle, const UpkieActionDelay* spec) {
     h->delay_high = 0;
     return UPKIE_B200_OK;
   }
-  if (const char* why = action_delay_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  if (max_ticks == 0 || max_ticks > UPKIE_MAX_DELAY_TICKS)
+    return fail(UPKIE_B200_EINVAL, "set_action_delay: max_ticks outside 1 .. UPKIE_MAX_DELAY_TICKS");
+  if (const char* why = action_delay_spec_error(*spec, h->P, max_ticks)) return fail(UPKIE_B200_EINVAL, why);
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
   if (alloc_delay_state(h)) return UPKIE_B200_ECUDA;
+  if (resize_ring(h, &h->delay_command, h->delay_head, &h->delay_ticks, int(max_ticks), UPKIE_ACT_DIM, 1,
+                  "action delay history: "))
+    return UPKIE_B200_ECUDA;
   if (!h->delay_dev) CUDA_TRY(cudaMalloc(&h->delay_dev, sizeof(ActionDelay)));
   ActionDelay A;
   std::memset(&A, 0, sizeof(A));
@@ -1461,6 +1508,8 @@ int upkie_b200_set_action_delay(void* handle, const UpkieActionDelay* spec) {
   A.delay = h->delay_delay;
   A.command = h->delay_command;
   A.stride = h->n_pad;
+  A.ticks = h->delay_ticks;
+  A.head = h->delay_head;
   CUDA_TRY(cudaMemcpy(h->delay_dev, &A, sizeof(A), cudaMemcpyHostToDevice));
   CUDA_TRY(cudaDeviceSynchronize());
   h->delay_high = spec->substeps_high;
@@ -1481,7 +1530,11 @@ int upkie_b200_get_action_delay_state(void* handle, uint32_t* count, uint32_t* d
     CUDA_TRY(cudaMemsetAsync(count, 0, bytes, s));
     CUDA_TRY(cudaMemsetAsync(delay, 0, bytes, s));
   }
-  CUDA_TRY(launch_command_rows(h->delay_command, h->n, h->n_pad, command, s));
+  if (h->delay_command)  // the previous tick's command: age 0 of the history
+    CUDA_TRY(launch_ring_rows(h->delay_command, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad, 1, command,
+                              s));
+  else
+    CUDA_TRY(launch_command_rows(nullptr, h->n, h->n_pad, command, s));
   return UPKIE_B200_OK;
 }
 
@@ -1495,7 +1548,31 @@ int upkie_b200_set_action_delay_state(void* handle, const uint32_t* count, const
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
   CUDA_TRY(cudaMemcpyAsync(h->delay_count, count, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(h->delay_delay, delay, bytes, cudaMemcpyDeviceToDevice, s));
-  CUDA_TRY(launch_command_cols(command, h->n, h->n_pad, h->delay_command, s));
+  CUDA_TRY(launch_ring_cols(command, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad, 1, h->delay_command,
+                            s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_action_delay_history(void* handle, float* commands, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !commands) return fail(UPKIE_B200_EINVAL, "get_action_delay_history: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (h->delay_command)
+    CUDA_TRY(launch_ring_rows(h->delay_command, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad,
+                              h->delay_ticks, commands, s));
+  else
+    CUDA_TRY(launch_command_rows(nullptr, h->n, h->n_pad, commands, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_action_delay_history(void* handle, const float* commands, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !commands) return fail(UPKIE_B200_EINVAL, "set_action_delay_history: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (alloc_delay_state(h)) return UPKIE_B200_ECUDA;
+  CUDA_TRY(launch_ring_cols(commands, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad, h->delay_ticks,
+                            h->delay_command, static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 
@@ -1506,28 +1583,75 @@ int alloc_sense_state(Handle* h) {
   if (h->sense_count) return UPKIE_B200_OK;
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
   const size_t row_bytes = size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float);
-  uint32_t *count = nullptr, *delay = nullptr;
+  uint32_t *count = nullptr, *delay = nullptr, *head = nullptr;
   float* rows = nullptr;
   cudaError_t e = cudaDeviceSynchronize();  // the state of the steps in flight
   if (e == cudaSuccess) e = cudaMalloc(&count, bytes);
   if (e == cudaSuccess) e = cudaMalloc(&delay, bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&head, bytes);
   if (e == cudaSuccess) e = cudaMalloc(&rows, row_bytes);
   if (e == cudaSuccess) e = cudaMemset(count, 0, bytes);
   if (e == cudaSuccess) e = cudaMemset(delay, 0, bytes);
+  if (e == cudaSuccess) e = cudaMemset(head, 0, bytes);
   if (e == cudaSuccess) e = cudaMemcpy(rows, h->state, row_bytes, cudaMemcpyDeviceToDevice);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
-    cudaFree(count); cudaFree(delay); cudaFree(rows);
+    cudaFree(count); cudaFree(delay); cudaFree(head); cudaFree(rows);
     return fail(UPKIE_B200_ECUDA, std::string("observation delay state: ") + cudaGetErrorString(e));
   }
   h->sense_count = count;
   h->sense_delay = delay;
+  h->sense_head = head;
   h->sense_rows = rows;
+  h->sense_ticks = 1;
   return UPKIE_B200_OK;
 }
 }  // namespace
 
 int upkie_b200_set_observation_delay(void* handle, const UpkieObservationDelay* spec) {
+  return upkie_b200_set_observation_delay_ticks(handle, spec, 1);
+}
+
+namespace {
+// the snapshot history of depth `ticks` (1: none, the sensed rows are the newest snapshot): the newest min(ticks, K)
+// snapshots in age order, the ages added copies of the oldest
+int resize_sense_history(Handle* h, int ticks) {
+  if (ticks == h->sense_ticks) return UPKIE_B200_OK;
+  const char* what = "observation delay history: ";
+  if (ticks == 1) {  // the newest snapshot's sensed columns become the sensed rows
+    uint64_t sensed = 0;
+    for (int k = 0; k < UPKIE_STATE_DIM; ++k)
+      if (obs_delay_sensed(k)) sensed |= uint64_t(1) << k;
+    cudaError_t e = launch_ring_resize(h->sense_hist, h->sense_head, h->sense_ticks, h->sense_rows, 1, UPKIE_STATE_DIM,
+                                       h->n, h->n_pad, 0, sensed, nullptr);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) return fail(UPKIE_B200_ECUDA, std::string(what) + cudaGetErrorString(e));
+    cudaFree(h->sense_hist);
+    h->sense_hist = nullptr;
+    h->sense_ticks = 1;
+    return UPKIE_B200_OK;
+  }
+  if (h->sense_ticks == 1) {  // every snapshot of the new ring starts as a copy of the sensed rows
+    float* hist = nullptr;
+    cudaError_t e = cudaMalloc(&hist, size_t(ticks) * UPKIE_STATE_DIM * h->n_pad * sizeof(float));
+    if (e == cudaSuccess)
+      e = launch_ring_resize(h->sense_rows, nullptr, 1, hist, ticks, UPKIE_STATE_DIM, h->n, h->n_pad, 0, ~uint64_t(0),
+                             nullptr);
+    if (e == cudaSuccess) e = cudaMemset(h->sense_head, 0, size_t(h->n) * sizeof(uint32_t));
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();
+    if (e != cudaSuccess) {
+      cudaFree(hist);
+      return fail(UPKIE_B200_ECUDA, std::string(what) + cudaGetErrorString(e));
+    }
+    h->sense_hist = hist;
+    h->sense_ticks = ticks;
+    return UPKIE_B200_OK;
+  }
+  return resize_ring(h, &h->sense_hist, h->sense_head, &h->sense_ticks, ticks, UPKIE_STATE_DIM, 0, what);
+}
+}  // namespace
+
+int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationDelay* spec, uint32_t max_ticks) {
   Handle* h = as_handle(handle);
   if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
   if (!spec) {
@@ -1536,16 +1660,23 @@ int upkie_b200_set_observation_delay(void* handle, const UpkieObservationDelay* 
     h->sense_high = 0;
     return UPKIE_B200_OK;
   }
-  if (const char* why = obs_delay_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  if (max_ticks == 0 || max_ticks > UPKIE_MAX_DELAY_TICKS)
+    return fail(UPKIE_B200_EINVAL, "set_observation_delay: max_ticks outside 1 .. UPKIE_MAX_DELAY_TICKS");
+  if (const char* why = obs_delay_spec_error(*spec, h->P, max_ticks)) return fail(UPKIE_B200_EINVAL, why);
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
   const bool allocated = h->sense_rows != nullptr;
   if (alloc_sense_state(h)) return UPKIE_B200_ECUDA;  // a first allocation fills the rows from the state
+  if (resize_sense_history(h, int(max_ticks))) return UPKIE_B200_ECUDA;
   if (allocated && !h->P.obs_delay) {
-    // turned on again: the sensors did not follow the robot while the delay was off, so the rows start from the
-    // current state (its IMU velocity is what the next snapshot differentiates against); counters and delays stay
+    // turned on again: the sensors did not follow the robot while the delay was off, so the rows (and every snapshot
+    // of a history) start from the current state (its IMU velocity is what the next snapshot differentiates against);
+    // counters and delays stay
     CUDA_TRY(cudaMemcpy(h->sense_rows, h->state, size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float),
                         cudaMemcpyDeviceToDevice));
+    if (h->sense_hist)
+      CUDA_TRY(launch_ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad,
+                                  0, ~uint64_t(0), nullptr));
   }
   if (!h->sense_dev) CUDA_TRY(cudaMalloc(&h->sense_dev, sizeof(ObsDelay)));
   ObsDelay O;
@@ -1555,6 +1686,9 @@ int upkie_b200_set_observation_delay(void* handle, const UpkieObservationDelay* 
   O.delay = h->sense_delay;
   O.rows = h->sense_rows;
   O.stride = h->n_pad;
+  O.ticks = h->sense_ticks;
+  O.hist = h->sense_hist;
+  O.head = h->sense_head;
   CUDA_TRY(cudaMemcpy(h->sense_dev, &O, sizeof(O), cudaMemcpyHostToDevice));
   CUDA_TRY(cudaDeviceSynchronize());
   h->sense_high = spec->substeps_high;
@@ -1593,6 +1727,33 @@ int upkie_b200_set_observation_delay_state(void* handle, const uint32_t* count, 
   CUDA_TRY(cudaMemcpyAsync(h->sense_count, count, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(h->sense_delay, delay, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(launch_sensed_cols(rows, h->n, h->n_pad, h->sense_rows, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_observation_delay_history(void* handle, float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !rows) return fail(UPKIE_B200_EINVAL, "get_observation_delay_history: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (h->sense_hist)
+    CUDA_TRY(launch_ring_rows(h->sense_hist, h->sense_head, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad,
+                              h->sense_ticks, rows, s));
+  else  // depth 1: the sensed rows are the newest snapshot (as get_observation_delay_state)
+    CUDA_TRY(launch_sensed_rows(h->sense_rows ? h->sense_rows : h->state, h->n, h->n_pad, rows, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_observation_delay_history(void* handle, const float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !rows) return fail(UPKIE_B200_EINVAL, "set_observation_delay_history: invalid argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (alloc_sense_state(h)) return UPKIE_B200_ECUDA;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (h->sense_hist)
+    CUDA_TRY(launch_ring_cols(rows, h->sense_head, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad, h->sense_ticks,
+                              h->sense_hist, s));
+  else
+    CUDA_TRY(launch_sensed_cols(rows, h->n, h->n_pad, h->sense_rows, s));
   return UPKIE_B200_OK;
 }
 

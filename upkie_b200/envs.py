@@ -511,13 +511,24 @@ def push_randomization_spec(spec: Optional[dict], model: Model, dt: float) -> Op
     return out
 
 
+def _check_max_delay_ticks(max_ticks) -> int:
+    """``max_ticks`` of a delay as an int in ``1 .. MAX_DELAY_TICKS``, or ``UpkieException``"""
+    if isinstance(max_ticks, (bool, np.bool_)) or not isinstance(max_ticks, (int, np.integer)):
+        raise UpkieException(f"max_ticks: expected an integer, got {max_ticks!r}")
+    if not 1 <= int(max_ticks) <= _abi.MAX_DELAY_TICKS:
+        raise UpkieException(f"max_ticks: expected 1 <= max_ticks <= {_abi.MAX_DELAY_TICKS}, got {max_ticks}")
+    return int(max_ticks)
+
+
 def action_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool = False,
-                      joint_limits: Union[bool, int] = True) -> Optional[Tuple[int, int]]:
+                      joint_limits: Union[bool, int] = True, max_ticks: int = 1) -> Optional[Tuple[int, int]]:
     """``(substeps_low, substeps_high)`` (``UpkieSim.set_action_delay``) from an action delay in seconds: a float, or a
     ``(low, high)`` pair from which every reset draws an env's delay. Rounded to the nearest substep of ``dt /
     nb_substeps`` (halves up). Raises ``UpkieException`` on a negative or non-finite bound, ``low > high``, a delay
-    of more than one tick (``nb_substeps`` substeps), ``spine_mode`` (which models the spine's own lag) and no joint
+    of more than ``max_ticks`` ticks (``max_ticks * nb_substeps`` substeps; ``max_ticks`` from 1 to
+    ``MAX_DELAY_TICKS``, the history the delay keeps), ``spine_mode`` (which models the spine's own lag) and no joint
     limits (the delay runs in the kernels with joint-limit rows)."""
+    max_ticks = _check_max_delay_ticks(max_ticks)
     if delay is None:
         return None
     if isinstance(delay, (int, float, np.integer, np.floating)):
@@ -539,19 +550,24 @@ def action_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool = Fal
         raise UpkieException("action_delay: needs joint_limits (the delay runs in the kernels with joint-limit rows)")
     substep = dt / int(nb_substeps)
     lo_s, hi_s = (int(np.floor(x / substep + 0.5)) for x in (lo, hi))
-    if hi_s > int(nb_substeps):
+    if max_ticks == 1 and hi_s > int(nb_substeps):
         raise UpkieException(f"action_delay: {hi} s is more than one tick ({nb_substeps} substeps of {substep} s)")
+    if hi_s > max_ticks * int(nb_substeps):
+        raise UpkieException(f"action_delay: {hi} s is more than max_ticks = {max_ticks} ticks ({nb_substeps} substeps "
+                             f"of {substep} s each)")
     return lo_s, hi_s
 
 
 def observation_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool = False,
                            joint_limits: Union[bool, int] = True,
-                           body_contacts: Union[bool, int] = False) -> Optional[Tuple[int, int]]:
+                           body_contacts: Union[bool, int] = False, max_ticks: int = 1) -> Optional[Tuple[int, int]]:
     """``(substeps_low, substeps_high)`` (``UpkieSim.set_observation_delay``) from an observation delay in seconds: a
     float, or a ``(low, high)`` pair from which every reset draws an env's delay. Rounded to the nearest substep of
     ``dt / nb_substeps`` (halves up). Raises ``UpkieException`` on a negative or non-finite bound, ``low > high``, a
-    delay of more than one tick (``nb_substeps`` substeps), ``spine_mode`` (which models the spine's own lag), no joint
+    delay of more than ``max_ticks`` ticks (``max_ticks * nb_substeps`` substeps; ``max_ticks`` from 1 to
+    ``MAX_DELAY_TICKS``, the history the delay keeps), ``spine_mode`` (which models the spine's own lag), no joint
     limits (the delay runs in the kernels with joint-limit rows) and ``body_contacts`` (no such kernels)."""
+    max_ticks = _check_max_delay_ticks(max_ticks)
     if delay is None:
         return None
     if isinstance(delay, (int, float, np.integer, np.floating)):
@@ -577,8 +593,11 @@ def observation_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool 
         raise UpkieException("observation_delay: body_contacts has no observation-delay kernels")
     substep = dt / int(nb_substeps)
     lo_s, hi_s = (int(np.floor(x / substep + 0.5)) for x in (lo, hi))
-    if hi_s > int(nb_substeps):
+    if max_ticks == 1 and hi_s > int(nb_substeps):
         raise UpkieException(f"observation_delay: {hi} s is more than one tick ({nb_substeps} substeps of {substep} s)")
+    if hi_s > max_ticks * int(nb_substeps):
+        raise UpkieException(f"observation_delay: {hi} s is more than max_ticks = {max_ticks} ticks ({nb_substeps} substeps "
+                             f"of {substep} s each)")
     return lo_s, hi_s
 
 
@@ -621,17 +640,27 @@ class B200VectorEnv(VectorEnv):
     restarts the schedules of the envs it resets. ``set_push_randomization`` changes or (``None``) stops them.
 
     ``action_delay`` (seconds, a float or a ``(low, high)`` range, see ``action_delay_spec``) delays each env's servo
-    command by a number of substeps drawn at every reset of that env, up to one tick: the substeps before it run the
+    command by a number of substeps drawn at every reset of that env, up to one tick (or ``max_delay_ticks``): the substeps before it run the
     command of the previous tick, and the first ones of an episode run with the servos stopped. The draws are keyed on
     the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets.
     ``set_action_delay`` changes or (``None``) stops it from each env's next reset.
 
     ``observation_delay`` (seconds, a float or a ``(low, high)`` range, see ``observation_delay_spec``) makes each env
     observe its robot a number of substeps before the end of the tick, drawn at every reset of that env, up to one
-    tick: the observation (and ``base_velocity``'s, through its gyropod rows) describes the robot at that instant,
+    tick (or ``max_delay_ticks``): the observation (and ``base_velocity``'s, through its gyropod rows) describes the robot at that instant,
     while terminations and resets judge the true state; the observation of a reset is undelayed. The draws are keyed on
     the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets.
     ``set_observation_delay`` changes or (``None``) stops it from each env's next reset.
+
+    ``max_delay_ticks`` (1 to ``MAX_DELAY_TICKS``, default 1) is the history both delays keep, in ticks: with it each
+    delay may reach ``max_delay_ticks`` ticks instead of one (at ``frequency=1000.0`` a tick is one substep, so the
+    default caps each delay at 1 ms). A delay of ``q`` whole ticks and ``r`` substeps runs the command of ``q`` ticks
+    earlier from substep ``r``, and reports what a delay of ``r`` substeps reported ``q`` ticks earlier (the state of
+    the last reset for the ticks before it). ``set_action_delay`` and ``set_observation_delay`` take the same depth.
+    Under an observation delay of a tick or more, the first ticks of an episode report its post-reset state, whose
+    measured torques a reset leaves as the previous episode ended them (its zero-torque substep does not write them, as
+    for the undelayed reset observation): ``reset(seed=s)`` of a used env then reproduces the physics and every later
+    observation, but not those first torque readings; a fresh env reproduces them too.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -669,6 +698,7 @@ class B200VectorEnv(VectorEnv):
         push_randomization: Optional[dict] = None,
         action_delay: Optional[Union[float, Tuple[float, float]]] = None,
         observation_delay: Optional[Union[float, Tuple[float, float]]] = None,
+        max_delay_ticks: int = 1,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -710,11 +740,12 @@ class B200VectorEnv(VectorEnv):
             config = _abi.UpkieSimConfig.from_buffer_copy(config)
             config.max_episode_steps = max_episode_steps
         self.config = config
+        self.max_delay_ticks = _check_max_delay_ticks(max_delay_ticks)
         delay_spec = action_delay_spec(action_delay, 1.0 / frequency, config.nb_substeps, bool(config.spine_mode),
-                                       config.joint_limits)  # validated before any device is touched
+                                       config.joint_limits, self.max_delay_ticks)  # validated before any device is touched
         sense_spec = observation_delay_spec(observation_delay, 1.0 / frequency, config.nb_substeps,
-                                            bool(config.spine_mode), config.joint_limits,
-                                            config.body_contacts)  # validated before any device is touched
+                                            bool(config.spine_mode), config.joint_limits, config.body_contacts,
+                                            self.max_delay_ticks)  # validated before any device is touched
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -764,9 +795,11 @@ class B200VectorEnv(VectorEnv):
         if push_spec is not None:
             self.sim.set_push_randomization(push_spec)
         if delay_spec is not None:
-            self.sim.set_action_delay(*delay_spec)  # before the first reset, which draws every env's delay
+            # before the first reset, which draws every env's delay
+            self.sim.set_action_delay(*delay_spec, max_ticks=self.max_delay_ticks)
         if sense_spec is not None:
-            self.sim.set_observation_delay(*sense_spec)  # before the first reset, which draws every env's delay
+            # before the first reset, which draws every env's delay
+            self.sim.set_observation_delay(*sense_spec, max_ticks=self.max_delay_ticks)
 
     def set_reset_randomization(self, spec: Optional[dict]) -> None:
         """Redraw the parameters ``spec`` names at every later reset of an env (``reset_randomization_spec``);
@@ -782,16 +815,22 @@ class B200VectorEnv(VectorEnv):
         """Delay the servo commands by ``delay`` seconds, a float or a ``(low, high)`` range (``action_delay_spec``);
         ``None`` turns the delay off. A new range takes effect at each env's next reset."""
         spec = action_delay_spec(delay, self.dt, self.config.nb_substeps, bool(self.config.spine_mode),
-                                 self.config.joint_limits)
-        self.sim.set_action_delay(*(spec if spec is not None else (None,)))
+                                 self.config.joint_limits, self.max_delay_ticks)
+        if spec is None:
+            self.sim.set_action_delay(None)
+        else:
+            self.sim.set_action_delay(*spec, max_ticks=self.max_delay_ticks)
 
     def set_observation_delay(self, delay) -> None:
         """Observe each robot ``delay`` seconds before the end of the tick, a float or a ``(low, high)`` range
         (``observation_delay_spec``); ``None`` turns the delay off. A new range takes effect at each env's next
         reset."""
         spec = observation_delay_spec(delay, self.dt, self.config.nb_substeps, bool(self.config.spine_mode),
-                                      self.config.joint_limits, self.config.body_contacts)
-        self.sim.set_observation_delay(*(spec if spec is not None else (None,)))
+                                      self.config.joint_limits, self.config.body_contacts, self.max_delay_ticks)
+        if spec is None:
+            self.sim.set_observation_delay(None)
+        else:
+            self.sim.set_observation_delay(*spec, max_ticks=self.max_delay_ticks)
 
     # ------------------------------------------------------------------
     def get_neutral_action(self) -> dict:

@@ -186,20 +186,40 @@ class UpkieSim:
         self._check_tensor(timer, (self.n,), torch.int32, "timer")
         check(lib().upkie_b200_set_push_state(self._h, _ptr(count), _ptr(timer), self._stream()))
 
-    def set_action_delay(self, low: Optional[int], high: Optional[int] = None) -> None:
+    def set_action_delay(self, low: Optional[int], high: Optional[int] = None, max_ticks: int = 1) -> None:
         """While a range is set, every env applies its servo command ``d`` substeps into each tick, ``low <= d <= high
         <= nb_substeps``: the substeps before ``d`` run the command of its previous tick. Each reset of the env draws a
         new ``d`` (keyed on the auto-reset seed and the env's counter, ``include/upkie_b200.h``) and stops the servos
         until the first command takes over. ``high`` defaults to ``low``; ``None`` turns the delay off. Setting a range
-        draws nothing: it takes effect at each env's next reset."""
+        draws nothing: it takes effect at each env's next reset.
+
+        ``max_ticks`` (1 .. ``MAX_DELAY_TICKS``) is the history of commands each env keeps, in ticks: ``high`` may then
+        reach ``max_ticks * nb_substeps``, and a delay ``d = q * nb_substeps + r`` (``1 <= r <= nb_substeps``) runs the
+        command of ``q`` ticks earlier from substep ``r`` on and the one before it until then. A change of depth keeps
+        the history in age order, truncated or extended with stop rows."""
         if low is None:
             check(lib().upkie_b200_set_action_delay(self._h, None))
             self._action_delay = None
             return
         spec = _abi.UpkieActionDelay(int(low), int(low if high is None else high))
-        check(lib().upkie_b200_set_action_delay(self._h, C.byref(spec)))
+        check(lib().upkie_b200_set_action_delay_ticks(self._h, C.byref(spec), int(max_ticks)))
         self._action_delay = (spec.substeps_low, spec.substeps_high)
+        self._action_delay_ticks = int(max_ticks)
         self._delay_state_set = True  # the handle holds a state from now on
+
+    def get_action_delay_history(self) -> torch.Tensor:
+        """``[max_ticks, N, 6, 6]`` the servo commands of each env's last ``max_ticks`` ticks, the newest first (stop
+        rows before the env's last reset)."""
+        out = torch.empty((getattr(self, "_action_delay_ticks", 1), self.n, _abi.NJ, len(_abi.ACT_KEYS)),
+                          dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_action_delay_history(self._h, _ptr(out), self._stream()))
+        return out
+
+    def set_action_delay_history(self, commands: torch.Tensor) -> None:
+        self._check_tensor(commands, (getattr(self, "_action_delay_ticks", 1), self.n, _abi.NJ, len(_abi.ACT_KEYS)),
+                           name="commands")
+        check(lib().upkie_b200_set_action_delay_history(self._h, _ptr(commands), self._stream()))
+        self._delay_state_set = True
 
     def get_action_delay_state(self):
         """Per-env action-delay state ``(count[N], delay[N], command[N, 6, 6])``: the draw counters (int32 bits of
@@ -219,21 +239,41 @@ class UpkieSim:
                                                       self._stream()))
         self._delay_state_set = True
 
-    def set_observation_delay(self, low: Optional[int], high: Optional[int] = None) -> None:
+    def set_observation_delay(self, low: Optional[int], high: Optional[int] = None, max_ticks: int = 1) -> None:
         """While a range is set, everything a step reports about each env's sensors (its observation, ``spine_obs``,
         ``final_obs`` and the final spine observation) describes the robot ``d`` substeps before the end of the tick,
         ``low <= d <= high <= nb_substeps``; the IMU acceleration differentiates consecutive snapshots. Terminations,
         resets and ``get_state`` read the true state. Each reset of the env draws a new ``d`` (keyed on the auto-reset
         seed and the env's counter, ``include/upkie_b200.h``) and is observed undelayed. ``high`` defaults to ``low``;
-        ``None`` turns the delay off. Setting a range draws nothing: it takes effect at each env's next reset."""
+        ``None`` turns the delay off. Setting a range draws nothing: it takes effect at each env's next reset.
+
+        ``max_ticks`` (1 .. ``MAX_DELAY_TICKS``) is the history of snapshots each env keeps, in ticks: ``high`` may then
+        reach ``max_ticks * nb_substeps``, and a delay ``d = q * nb_substeps + r`` (``1 <= r <= nb_substeps``) reports
+        what a delay of ``r`` reported ``q`` ticks earlier, the post-reset state for the ticks before the env's last
+        reset. A change of depth keeps the history in age order, truncated or extended with copies of the oldest."""
         if low is None:
             check(lib().upkie_b200_set_observation_delay(self._h, None))
             self._observation_delay = None
             return
         spec = _abi.UpkieObservationDelay(int(low), int(low if high is None else high))
-        check(lib().upkie_b200_set_observation_delay(self._h, C.byref(spec)))
+        check(lib().upkie_b200_set_observation_delay_ticks(self._h, C.byref(spec), int(max_ticks)))
         self._observation_delay = (spec.substeps_low, spec.substeps_high)
+        self._observation_delay_ticks = int(max_ticks)
         self._sense_state_set = True  # the handle holds a state from now on
+
+    def get_observation_delay_history(self) -> torch.Tensor:
+        """``[max_ticks, N, STATE_DIM]`` the sensor snapshots of each env's last ``max_ticks`` ticks, the newest first
+        (``get_state`` layout, the sensed columns; the post-reset state before the env's last reset). At depth 1 the
+        sensed rows of ``get_observation_delay_state``."""
+        out = torch.empty((getattr(self, "_observation_delay_ticks", 1), self.n, _abi.STATE_DIM), dtype=torch.float32,
+                          device=self.device)
+        check(lib().upkie_b200_get_observation_delay_history(self._h, _ptr(out), self._stream()))
+        return out
+
+    def set_observation_delay_history(self, rows: torch.Tensor) -> None:
+        self._check_tensor(rows, (getattr(self, "_observation_delay_ticks", 1), self.n, _abi.STATE_DIM), name="rows")
+        check(lib().upkie_b200_set_observation_delay_history(self._h, _ptr(rows), self._stream()))
+        self._sense_state_set = True
 
     def get_observation_delay_state(self):
         """Per-env observation-delay state ``(count[N], delay[N], rows[N, STATE_DIM])``: the draw counters (int32 bits
@@ -624,7 +664,7 @@ class UpkieSim:
         delay_count, delay_delay, delay_command = self.get_action_delay_state()
         sense_count, sense_delay, sense_rows = self.get_observation_delay_state()
         force, local_mask = getattr(self, "_external", (None, 0))
-        return {
+        sd = {
             "reset_randomization": None if spec is None else bytes(spec),  # the UpkieResetRandomization in force
             "draws": self.get_draws(),  # per-env draw counters of the reset randomisation
             "push_randomization": None if push is None else bytes(push),  # the UpkiePushRandomization in force
@@ -638,13 +678,26 @@ class UpkieSim:
             # per-env observation-delay state: draw counters, delays, sensed state rows
             "observation_delay_count": sense_count, "observation_delay_delay": sense_delay,
             "observation_delay_rows": sense_rows,
+        }
+        # delays of more than one tick: the depth and the history of each (absent at depth 1, as before the histories
+        # existed), also while the delay is off: the handle keeps its history for a later spec of the same depth
+        delay_ticks = getattr(self, "_action_delay_ticks", 1)
+        if delay_ticks > 1:
+            sd["action_delay_ticks"] = delay_ticks
+            sd["action_delay_history"] = self.get_action_delay_history()
+        sense_ticks = getattr(self, "_observation_delay_ticks", 1)
+        if sense_ticks > 1:
+            sd["observation_delay_ticks"] = sense_ticks
+            sd["observation_delay_history"] = self.get_observation_delay_history()
+        sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
             "elapsed": elapsed,  # steps since each env's last reset (the time limit's counts)
             "friction": friction, "inertia_eps": eps, "external_force": force, "external_local_mask": local_mask,
             "env_params": env_params,  # per-env parameter table, None = the config's values
             "autoreset": getattr(self, "_autoreset", (AUTORESET_DISABLED, 0, 0)),
-        }
+        })
+        return sd
 
     def load_state_dict(self, sd: dict) -> None:
         dev = self.device
@@ -689,7 +742,13 @@ class UpkieSim:
                             zeros if timer is None else timer.to(dev).contiguous())
         # a checkpoint written before the action delay existed loads as "off, counters 0, delays 0" (and stop rows)
         delay = sd.get("action_delay")
-        self.set_action_delay(*(delay if delay is not None else (None,)))
+        delay_ticks = int(sd.get("action_delay_ticks", 1))  # a checkpoint without a history is depth 1
+        if delay is None:
+            if delay_ticks != getattr(self, "_action_delay_ticks", 1):  # the depth of a delay that is off: set with a spec that draws nothing, then off
+                self.set_action_delay(0, 0, max_ticks=delay_ticks)
+            self.set_action_delay(None)
+        else:
+            self.set_action_delay(*delay, max_ticks=delay_ticks)
         count, delay_d, command = (sd.get(k) for k in ("action_delay_count", "action_delay_delay",
                                                        "action_delay_command"))
         stop = stop_commands(self.n, dev)
@@ -701,10 +760,18 @@ class UpkieSim:
             self.set_action_delay_state(zeros if count is None else count.to(dev).contiguous(),
                                         zeros if delay_d is None else delay_d.to(dev).contiguous(),
                                         stop if command is None else command.to(dev).contiguous())
+        if sd.get("action_delay_history") is not None:
+            self.set_action_delay_history(sd["action_delay_history"].to(dev).contiguous())
         # a checkpoint written before the observation delay existed loads as "off, counters 0, delays 0" (and the
         # state as the sensed rows)
         sense = sd.get("observation_delay")
-        self.set_observation_delay(*(sense if sense is not None else (None,)))
+        sense_ticks = int(sd.get("observation_delay_ticks", 1))
+        if sense is None:
+            if sense_ticks != getattr(self, "_observation_delay_ticks", 1):  # as the action delay's (the state and the history are restored below)
+                self.set_observation_delay(0, 0, max_ticks=sense_ticks)
+            self.set_observation_delay(None)
+        else:
+            self.set_observation_delay(*sense, max_ticks=sense_ticks)
         count, delay_d, rows = (sd.get(k) for k in ("observation_delay_count", "observation_delay_delay",
                                                     "observation_delay_rows"))
         state = sd["state"].to(dev)
@@ -715,6 +782,8 @@ class UpkieSim:
             self.set_observation_delay_state(zeros if count is None else count.to(dev).contiguous(),
                                              zeros if delay_d is None else delay_d.to(dev).contiguous(),
                                              state.contiguous() if rows is None else rows.to(dev).contiguous())
+        if sd.get("observation_delay_history") is not None:
+            self.set_observation_delay_history(sd["observation_delay_history"].to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
