@@ -88,6 +88,29 @@ def ncu_rows(rep):
     return out
 
 
+# H100: 256 KB of L1 + shared memory per SM, shared-memory carveout steps in KB, 1 KB reserved per block; the
+# headline launch: one 256-thread block per SM (255 registers), one 36-float action tile row per thread
+SM_L1_SMEM_KB = 256
+CARVEOUTS_KB = [0, 8, 16, 32, 64, 100, 132, 164, 196, 228]
+BLOCK = 256
+
+
+def l1_budget(text):
+    """the local-memory frame of a block against the L1 its smallest carveout leaves (launch_k_step: one tile buffer
+    per warp when the block steps one tile, the carveout preference cudaSharedmemCarveoutMaxL1)"""
+    frames = [int(v, 16) for v in re.findall(r"(?:IADD3|VIADD)\s+R1, R1, -0x([0-9a-f]+)", text)]
+    frame = max(frames) if frames else 0
+    ldl = len(re.findall(r"\bLDL\b", text))
+    stl = len(re.findall(r"\bSTL\b", text))
+    smem_kb = BLOCK * 36 * 4 / 1024 + 1
+    carve = next(c for c in CARVEOUTS_KB if c >= smem_kb)
+    l1_kb = SM_L1_SMEM_KB - carve
+    need_kb = frame * BLOCK / 1024
+    print(f"frame {frame} B x {BLOCK} threads = {need_kb:.0f} KB vs L1 left {l1_kb} KB (block {smem_kb:.0f} KB of "
+          f"shared memory -> {carve} KB carveout): {'fits' if need_kb <= l1_kb else 'does NOT fit'}; "
+          f"{ldl} LDL, {stl} STL")
+
+
 def main():
     args = [a for a in sys.argv[1:]]
     rep = None
@@ -102,11 +125,20 @@ def main():
         del args[k:k + 2]
     want = args[0] if args else "k_stepILi0ELi1ELi2ELi1E"
     dyn = ncu_rows(rep) if rep else None
+    # every step unit compiles step_unit.cu, so the cubins cuobjdump extracts from the library share one file name and
+    # overwrite each other: extract them from the unit objects next to the library (build.py's build/) when they exist
+    objdir = os.path.join(os.path.dirname(os.path.abspath(lib)), "build")
+    objs = sorted(os.path.join(objdir, f) for f in os.listdir(objdir) if f.endswith(".o")) if os.path.isdir(objdir) else []
     with tempfile.TemporaryDirectory() as tmp:
-        subprocess.run(["cuobjdump", "-xelf", "all", lib], cwd=tmp, check=True, stdout=subprocess.DEVNULL)
+        cubins = []
+        for k, src in enumerate(objs or [lib]):
+            d = os.path.join(tmp, str(k))
+            os.makedirs(d)
+            subprocess.run(["cuobjdump", "-xelf", "all", src], cwd=d, check=True, stdout=subprocess.DEVNULL)
+            cubins += [os.path.join(d, c) for c in sorted(os.listdir(d))]
         text = None
-        for cubin in sorted(os.listdir(tmp)):
-            dis = subprocess.run(["nvdisasm", "--print-line-info-inline", os.path.join(tmp, cubin)],
+        for cubin in cubins:
+            dis = subprocess.run(["nvdisasm", "--print-line-info-inline", cubin],
                                  capture_output=True, text=True).stdout
             m = re.search(r"^\.text\.(\S*" + re.escape(want) + r"\S*):", dis, re.M)
             if m:
@@ -187,6 +219,7 @@ def main():
                     dyn_stall[bucket][h] += v
             total += 1
     print(f"{total} static instructions ({sum(packed.values())} packed f32x2)")
+    l1_budget(text)
     if dyn is None:
         print(f"{'instr':>6s} {'share':>6s} {'f32x2':>6s}  bucket")
         for bucket, c in sorted(counts.items(), key=lambda kv: (not kv[0].startswith("substep"), -kv[1])):

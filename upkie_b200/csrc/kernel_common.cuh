@@ -98,6 +98,7 @@ struct StepArgs {
   int i0, cnt, n_pad, block;
   int compact_obs;      // TILE=1, servos: observation rows [6][3] (position, velocity, torque) instead of [6][5]
   int grid;             // TILE=1: number of persistent blocks (0 = one block per tile)
+  int smem_carveout;    // preferred shared-memory carveout of the kernel, % of the maximum (-1: the driver's choice)
   float* state;
   const float* action;
   float* obs;

@@ -8,6 +8,10 @@
 //       (step_unit.cu, build.py, DESIGN.md section 4).
 #pragma once
 
+#include <map>
+#include <mutex>
+#include <utility>
+
 #include "kernel_common.cuh"
 
 namespace upkie_b200 {
@@ -127,8 +131,9 @@ __device__ __forceinline__ float* obs_delay_report(const ObsDelay& O, uint32_t s
 }
 
 // ---- one env tick of the robot `tid` --------------------------------------------------
-// `tile4` is this warp's staging tile (TILE=1): on entry it holds the warp's 32 action rows when
-// `full` (prefetched by the caller), and it is reused to transpose the observation rows on the way out.
+// `tile4` is this warp's staging tile (TILE >= 1): on entry it holds the warp's 32 action rows when
+// `full` (prefetched by the caller), during the substeps each lane's clamped row, and it is reused to transpose the
+// observation rows on the way out.
 // HIST (the delay families' k_step_hist kernels): a delay keeps a history of more than one tick; compiled out of k_step
 template <int MODE, int AUTORESET, int FAMILY, int TILE, bool HIST = false>
 __device__ __forceinline__ void step_env(
@@ -258,7 +263,8 @@ __device__ __forceinline__ void step_env(
   }
   // action delay (F.delay kernels, P.action_delay set: a uniform branch). A tick swaps this tick's command into the
   // env's column of the command buffer and enters its substeps with the previous one in `a`; substep `dly` loads the
-  // new one back (action_delay_substep), so that one row is held in registers. A next-step reset draws and holds the
+  // new one back (action_delay_substep) into the row the substeps read (the tile row for TILE >= 1, below), so that one
+  // row is held per lane. A next-step reset draws and holds the
   // stop row instead; its reset substep never switches.
   // The buffer's address and stride are read into registers once and the row goes through global-space accesses:
   // reached through the generic pointers of the device block, every store of the row could alias the block, and each
@@ -307,6 +313,17 @@ __device__ __forceinline__ void step_env(
 #pragma unroll
       for (int c = 0; c < UPKIE_ACT_DIM; ++c) a[c] = prev[c];
     }
+  }
+  // TILE >= 1: the row the substeps read (torque law, action delay, spine cycle) is the lane's own row of the warp's
+  // tile, written here whole (9 x 16 B at a stride of 9 float4: conflict-free) whether the row came from the tile or
+  // from global memory, instead of a 36-float register array that ptxas spills to the local-memory frame and reloads in
+  // every substep. The tile is next used by the observation transpose after the substep loop. TILE = 0: the registers.
+  float* arow = a;
+  if (TILE) {
+    float4* row = tile4 + lane * (UPKIE_ACT_DIM / 4);
+#pragma unroll
+    for (int k = 0; k < UPKIE_ACT_DIM / 4; ++k) row[k] = make_float4(a[4 * k], a[4 * k + 1], a[4 * k + 2], a[4 * k + 3]);
+    arow = reinterpret_cast<float*>(row);
   }
   // observation delay (F.sense kernels, P.obs_delay set: a uniform branch). A lane with delay `sdl` stores the sensed
   // fields of its state at the end of substep nb_substeps - sdl - 1 (before the loop for sdl = nb_substeps, after the
@@ -368,7 +385,7 @@ __device__ __forceinline__ void step_env(
 #endif
     if (sub < nsub) {
       if (delaying) {
-        action_delay_substep(sub, dly, a, [&](int c) {
+        action_delay_substep(sub, dly, arow, [&](int c) {
           const ActionDelay& A = *P.action_delay;
           return __ldcg(A.command + dsec + size_t(c) * size_t(A.stride) + size_t(i));
         });
@@ -378,13 +395,13 @@ __device__ __forceinline__ void step_env(
                           size_t(P.body_rec_stride)};
       if (spine) {
         if (resetting && sub == 2) spine_assemble_observation(S, L);
-        spine_cycle(P, S, L, a, resetting, eps, mu, WarpAny(), PhaseSync(), P.joint_limits >= 1 ? P.joint_limits : 1, br,
+        spine_cycle(P, S, L, arow, resetting, eps, mu, WarpAny(), PhaseSync(), P.joint_limits >= 1 ? P.joint_limits : 1, br,
                     i);
       } else {
         // F.limits: the device's two limit modes (1 and 0 alias to 3 there, see physics_substep_paired), spelled as
         // a choice between two nonzero constants so that the compiler drops servo_substep's limits == 0 branches, a
         // second and third inlined copy of the substep that these kernels never run
-        servo_substep(P, S, a, resetting, eps, mu, WarpAny(), PhaseSync(), F.extras ? &nz : nullptr, sub,
+        servo_substep(P, S, arow, resetting, eps, mu, WarpAny(), PhaseSync(), F.extras ? &nz : nullptr, sub,
                       (F.extras && ext) ? &xf : nullptr, F.limits ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
                       pushing ? &pu : nullptr);
       }
@@ -533,6 +550,8 @@ __device__ __forceinline__ void step_env(
 #pragma unroll
     for (int k = 0; k < UPKIE_LAG_DIM; ++k) lag[size_t(k) * n_pad + i] = lr[k];
   }
+  // TILE >= 1: every lane is past its last read of its action row before the observation rows overwrite the tile
+  if (TILE) __syncwarp();
   if (MODE == MODE_SERVOS) {
     float o[UPKIE_OBS_DIM];
     float tq[6];
@@ -721,7 +740,9 @@ __device__ __forceinline__ void step_tiles(const SimParams& P, int i0, int n, in
   extern __shared__ float4 s_tile[];
   constexpr int kRow4 = 32 * UPKIE_ACT_DIM / 4;  // float4 per warp tile
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-  float4* buf[2] = {s_tile + warp * kRow4, s_tile + (nwarps + warp) * kRow4};
+  // the warp's tile of buffer b, computed from the shared-memory symbol where it is used so that the compiler sees
+  // shared-memory accesses (LDS / STS) and not generic ones
+  auto buf = [&](int b) { return s_tile + (b * nwarps + warp) * kRow4; };
   const int ntiles = (n - i0 + blockDim.x - 1) / blockDim.x;
   // a warp's rows are prefetched when all 32 envs exist and the rows are 16 B aligned
   auto warp_full = [&](int t) { return (coalesce & 1) && (i0 + t * int(blockDim.x) + warp * 32 + 32 <= n); };
@@ -735,11 +756,11 @@ __device__ __forceinline__ void step_tiles(const SimParams& P, int i0, int n, in
     cp_async_commit();
   };
   int t = blockIdx.x, it = 0;
-  if (t < ntiles) prefetch(t, buf[0]);
+  if (t < ntiles) prefetch(t, buf(0));
   for (; t < ntiles; t += gridDim.x, ++it) {
     const int nt = t + gridDim.x;
     if (nt < ntiles) {
-      prefetch(nt, buf[(it + 1) & 1]);
+      prefetch(nt, buf((it + 1) & 1));
       cp_async_wait<1>();
     } else {
       cp_async_wait<0>();
@@ -750,7 +771,7 @@ __device__ __forceinline__ void step_tiles(const SimParams& P, int i0, int n, in
     }
     step_env<MODE, AUTORESET, FAMILY, TILE, HIST>(P, i0 + t * blockDim.x + threadIdx.x, n, n_pad, state, action, obs,
                                          reward, terminated, truncated, eps_all, mu_all, err, done_prev, episode, tick,
-                                         seed, env_offset, ext, ext_local, buf[it & 1], warp_full(t),
+                                         seed, env_offset, ext, ext_local, buf(it & 1), warp_full(t),
                                          (coalesce & 2) != 0, TILE == 2 ? &peers : nullptr, lag);
     __syncwarp();  // the tile is free again before the next prefetch lands in it
   }
@@ -795,25 +816,50 @@ k_step_hist(const __grid_constant__ SimParams P, int i0, int n, int n_pad, float
                                                  ext_local, coalesce, peers, lag);
 }
 
+// The shared-memory attributes of a step kernel on the current device: the opt-in above 48 KB of dynamic shared memory,
+// and the preferred carveout (a percentage of the maximum; < 0 leaves the choice to the driver). They belong to a
+// kernel on a device, so each is set on the first launch of the kernel there and again only when it changes: a
+// cudaFuncSetAttribute per launch would be a driver call on every tick.
+inline cudaError_t step_kernel_attributes(const void* kernel, int smem, int carveout) {
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  static std::mutex m;
+  static std::map<std::pair<const void*, int>, std::pair<int, int>> set;  // (kernel, device) -> (smem, carveout)
+  const std::lock_guard<std::mutex> lock(m);
+  const auto key = std::make_pair(kernel, dev);
+  const auto it = set.find(key);
+  if (it != set.end() && it->second == std::make_pair(smem, carveout)) return cudaSuccess;
+  if (smem > 48 * 1024) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e == cudaSuccess && carveout >= 0)
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
+  if (e == cudaSuccess) set[key] = std::make_pair(smem, carveout);
+  return e;
+}
+
 template <int TILE, int MODE, int AUTORESET, int FAMILY>
 cudaError_t launch_k_step(const StepArgs& a) {
   const int tiles = (a.cnt + a.block - 1) / a.block;
   const int grid = (TILE && a.grid > 0 && a.grid < tiles) ? a.grid : tiles;
-  const size_t smem = TILE ? size_t(2) * (a.block / 32) * 32 * UPKIE_ACT_DIM * sizeof(float) : 0;
+  // One tile buffer per warp when every block steps one tile (grid == tiles: the headline and every launch that is not
+  // persistent), two when blocks walk several tiles (the persistent host-buffer launch), for the cp.async prefetch of
+  // the next tile. step_tiles touches the second buffer only for a tile t + gridDim.x < ntiles, which exists exactly
+  // when grid < tiles. One buffer of a 256-thread block is 36 KB, so the block fits the 64 KB carveout and leaves 192 KB
+  // of L1 to the kernel's local-memory frame (DESIGN.md section 4).
+  const int nbuf = grid < tiles ? 2 : 1;
+  const int smem = TILE ? nbuf * (a.block / 32) * 32 * UPKIE_ACT_DIM * int(sizeof(float)) : 0;
   // the tile path needs 16 B aligned rows of 32 envs
   const int aligned =
       ((reinterpret_cast<uintptr_t>(a.action) | reinterpret_cast<uintptr_t>(a.obs)) & 15) == 0 && (a.i0 % 32) == 0;
   const int coalesce = (aligned ? 1 : 0) | ((TILE && a.compact_obs) ? 2 : 0);  // bit 0 tile path, bit 1 compact rows
-  // a 256-thread block's two tile buffers take 72 KB: above 48 KB of dynamic shared memory a kernel must opt in (per
-  // device, so on every launch)
   auto kernel = k_step<MODE, AUTORESET, FAMILY, TILE>;
   if constexpr (step_family_traits(FAMILY).delay && TILE != 2) {
     if (a.history) kernel = k_step_hist<MODE, AUTORESET, FAMILY, TILE>;
   }
-  if (smem > 48 * 1024) {
-    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) return e;
-  }
+  // the carveout: a.smem_carveout, by default cudaSharedmemCarveoutMaxL1 (the driver then rounds up only as far as the
+  // block's shared memory needs, and the rest of the SM's 256 KB stays L1)
+  const cudaError_t e = step_kernel_attributes(reinterpret_cast<const void*>(kernel), smem, a.smem_carveout);
+  if (e != cudaSuccess) return e;
   kernel<<<grid, a.block, smem, a.stream>>>(
       *a.P, a.i0, a.i0 + a.cnt, a.n_pad, a.state, a.action, a.obs, a.reward, a.terminated, a.truncated, a.eps, a.mu,
       a.err, a.done_prev, a.episode, a.tick, a.seed, a.env_offset, a.ext, a.ext_local, coalesce, a.peers, a.lag);

@@ -79,6 +79,7 @@ struct Handle {
   int host_block = 128;          // zero-copy step: persistent blocks of 4 warps, one per SM: ~3.5 tiles per block at
   int host_blocks_per_sm = 1;    // 65536 envs, so PCIe reads of tile k+1 overlap the compute of tile k
   int zero_copy = 2;             // pinned host buffers: 0 staged copies, 1 kernel reads+writes host memory, 2 hybrid
+  int smem_carveout = cudaSharedmemCarveoutMaxL1;  // step kernels' preferred carveout, % (-1: the driver's choice)
   // host-buffer staging (allocated on first use)
   float *h_act = nullptr, *h_obs = nullptr, *h_rew = nullptr;
   uint8_t *h_term = nullptr, *h_trunc = nullptr;
@@ -396,6 +397,7 @@ int step_range(Handle* h, int mode, int i0, int cnt, const float* action, float*
   a.block = (tile && persistent) ? h->host_block : pick_block(h, cnt);
   a.grid = (tile && persistent) ? h->num_sms * h->host_blocks_per_sm : 0;
   a.compact_obs = compact ? 1 : 0;
+  a.smem_carveout = h->smem_carveout;
   a.state = h->state;
   a.action = action;
   a.obs = obs;
@@ -657,6 +659,12 @@ int upkie_b200_create(const UpkieModel* model, const UpkieSimConfig* config, int
     if (v >= 1 && v <= 8) h->host_blocks_per_sm = v;
   }
   if (const char* b = std::getenv("UPKIE_B200_ZERO_COPY")) h->zero_copy = std::atoi(b);  // developer knob: 0, 1, 2
+  // developer knob (tools/l1_budget.py): the step kernels' preferred shared-memory carveout, a percentage of the
+  // maximum, or -1 to leave it to the driver. The attribute belongs to the kernel: it outlives the handle in the process
+  if (const char* b = std::getenv("UPKIE_STEP_SMEM_CARVEOUT")) {
+    const int v = std::atoi(b);
+    if (v >= -1 && v <= 100) h->smem_carveout = v;
+  }
   if (const char* b = std::getenv("UPKIE_B200_HOST_SPLIT")) {  // developer knob: "0.4,0.4,0.2"
     h->host_split_n = 0;
     const char* p = b;
