@@ -2,7 +2,7 @@
 //
 // action_delay.cpp -- TEST INFRASTRUCTURE. The CPU build of the action delay's draw, reset and delayed tick
 // (sim_core.cuh action_delay_draw / action_delay_reset / action_delay_substep, the code the step kernels and
-// action_delay.cu inline). Built by tests/test_action_delay_cpu.py; never loaded by the product.
+// k_reset inline). Built by tests/test_action_delay_cpu.py; never loaded by the product.
 #include "hostsim.cpp"
 
 extern "C" {

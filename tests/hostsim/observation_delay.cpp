@@ -2,7 +2,7 @@
 //
 // observation_delay.cpp -- TEST INFRASTRUCTURE. The CPU build of the observation delay's draw, snapshot and sensed
 // state (sim_core.cuh obs_delay_draw / obs_delay_reset, params.h obs_delay_snapshot / obs_delay_sensed_state, the code
-// the step kernels and observation_delay.cu inline), of its spec's validation and of the family choice with a spec set
+// the step kernels and k_reset inline), of its spec's validation and of the family choice with a spec set
 // (step_family.h). Built by tests/test_observation_delay_cpu.py; never loaded by the product.
 #include "hostsim.cpp"
 #include "../../upkie_b200/csrc/step_family.h"

@@ -2,7 +2,7 @@
 //
 // pushes.cpp -- TEST INFRASTRUCTURE. The CPU build of the push randomisation's draw and schedule (sim_core.cuh
 // push_draw / push_force / push_step / push_restart / push_last_force / push_reset, the code the step kernels and
-// pushes.cu inline). Built by tests/test_push_randomization_cpu.py; never loaded by the product.
+// k_reset inline). Built by tests/test_push_randomization_cpu.py; never loaded by the product.
 #include "hostsim.cpp"
 
 extern "C" {

@@ -44,18 +44,14 @@ UNITS = [
     StepUnit("step_device_table", 0, (FAM_TABLE,), 0),
     StepUnit("step_host_table", 1, (FAM_TABLE,), 0),
     "base_velocity.cu",
-    "reset_randomization.cu",
-    "pushes.cu",
     StepUnit("step_device_push", 0, (FAM_PUSH,), 0),
     StepUnit("step_host_push", 1, (FAM_PUSH,), 0),
     StepUnit("step_device_body_push", 0, (FAM_BODY_PUSH,), 1),
     StepUnit("step_host_body_push", 1, (FAM_BODY_PUSH,), 1),
-    "action_delay.cu",
     StepUnit("step_device_delay", 0, (FAM_DELAY,), 0),
     StepUnit("step_host_delay", 1, (FAM_DELAY,), 0),
     StepUnit("step_device_body_delay", 0, (FAM_BODY_DELAY,), 1),
     StepUnit("step_host_body_delay", 1, (FAM_BODY_DELAY,), 1),
-    "observation_delay.cu",
     StepUnit("step_device_sense", 0, (FAM_SENSE,), 0),
     StepUnit("step_host_sense", 1, (FAM_SENSE,), 0),
 ]

@@ -124,38 +124,5 @@ struct StepArgs {
 template <int TILE, int FAMILY>
 cudaError_t launch_step(const StepArgs& a);
 cudaError_t launch_push_rows(const PeerPtrs& pp, int n, cudaStream_t stream);  // step_unit.cu, TILE=2: flush of a rollout's last rows
-// reset_randomization.cu: the handle-side kernels of reset randomisation (upkie_b200_set_reset_randomization)
-cudaError_t launch_reset_rand(const ResetRand* R, int n, const uint8_t* mask, uint64_t seed, uint64_t env_offset,
-                              cudaStream_t stream);  // draw of the envs an upkie_b200_reset takes, before k_reset
-cudaError_t launch_get_randomization(const SimParams& P, int n, const float* mu, const float* eps, float* friction,
-                                     float* inertia_eps, cudaStream_t stream);
-cudaError_t launch_fill(int n, float* out, float v, cudaStream_t stream);
-cudaError_t launch_env_params_from_config(const SimParams& P, int n, int n_pad, float* table, cudaStream_t stream);
-// pushes.cu: the handle-side kernels of push randomisation (upkie_b200_set_push_randomization)
-cudaError_t launch_push_reset(const PushRand* R, int n, const uint8_t* mask, uint64_t seed, uint64_t env_offset,
-                              cudaStream_t stream);  // the envs an upkie_b200_reset takes restart, before k_reset
-cudaError_t launch_push_forces(const PushRand* R, int n, uint64_t seed, uint64_t env_offset, float* force,
-                               cudaStream_t stream);  // R null: zeros
-// action_delay.cu: the handle-side kernels of action-delay randomisation (upkie_b200_set_action_delay)
-cudaError_t launch_action_delay_reset(const ActionDelay* A, int n, const uint8_t* mask, uint64_t seed,
-                                      uint64_t env_offset, cudaStream_t stream);  // before k_reset
-// command rows [n][UPKIE_ACT_DIM] <-> the buffer's columns [UPKIE_ACT_DIM][stride]; a null source gives stop rows
-cudaError_t launch_command_rows(const float* cols, int n, int stride, float* rows, cudaStream_t stream);
-cudaError_t launch_command_cols(const float* rows, int n, int stride, float* cols, cudaStream_t stream);
-// observation_delay.cu: the handle-side kernels of observation-delay randomisation (upkie_b200_set_observation_delay)
-cudaError_t launch_obs_delay_reset(const ObsDelay* O, int n, int n_pad, const float* state, const uint8_t* mask,
-                                   uint64_t seed, uint64_t env_offset, cudaStream_t stream);  // after k_reset
-// sensed rows [n][UPKIE_STATE_DIM] <-> the buffer's columns [UPKIE_STATE_DIM][stride]
-cudaError_t launch_sensed_rows(const float* cols, int n, int stride, float* rows, cudaStream_t stream);
-cudaError_t launch_sensed_cols(const float* rows, int n, int stride, float* cols, cudaStream_t stream);
-// (action_delay.cu) the delay histories, rings [K][dim][stride] whose next write is row head[i] (null: 0), in age order:
-// rows [ages][n][dim] <-> ages 0 .. ages - 1 (0 the newest); and a ring copied into one of another depth, row 0 its next
-// write, the ages it adds stop rows (stop) or copies of the oldest, `columns` the mask of the columns copied
-cudaError_t launch_ring_rows(const float* ring, const uint32_t* head, int ticks, int dim, int n, int stride, int ages,
-                             float* rows, cudaStream_t stream);
-cudaError_t launch_ring_cols(const float* rows, const uint32_t* head, int ticks, int dim, int n, int stride, int ages,
-                             float* ring, cudaStream_t stream);
-cudaError_t launch_ring_resize(const float* src, const uint32_t* head, int src_ticks, float* dst, int dst_ticks,
-                               int dim, int n, int stride, int stop, uint64_t columns, cudaStream_t stream);
 
 }  // namespace upkie_b200

@@ -1791,7 +1791,7 @@ UPKIE_HD void push_last_force(const UpkiePushRandomization& s, uint64_t seed, ui
   if (t > d.gap && t <= d.gap + d.duration) push_force(s, seed, g, k, d, f);
 }
 
-// An explicit reset of env i (k_push_reset, upkie_b200_reset)
+// An explicit reset of env i (k_reset, upkie_b200_reset)
 UPKIE_HD void push_reset(const PushRand& R, uint64_t seed, uint64_t g, int i) {
   const PushDraw d = push_draw(R.spec, seed, g, R.count[i]);
   uint32_t k = R.count[i], t = R.timer[i];
@@ -1883,7 +1883,7 @@ UPKIE_HD ObsDelayRows obs_delay_rows(uint32_t d, uint32_t nb, uint32_t ticks, ui
   return {delay_ring_row(head, ticks, 0u), (head + ticks - s.q) % ticks, s.r};
 }
 
-// A reset of env i (the step kernels' fused resets, k_action_delay_reset): the next draw, and the stop row as the
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, and the stop row as the
 // previous command. The block's fields are copied before the first store, which the compiler cannot tell apart from
 // the block itself.
 UPKIE_HD void action_delay_reset(const ActionDelay& A, uint64_t seed, uint64_t g, int i) {
@@ -1953,7 +1953,7 @@ UPKIE_HD void imu_velocity(const SimParams& P, const RobotState& S, float v[3]) 
   for (int i = 0; i < 3; ++i) v[i] = S.linvel[i] + w[i];
 }
 
-// A reset of env i (the step kernels' fused resets, k_obs_delay_reset): the next draw. The caller then copies the
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw. The caller then copies the
 // post-reset state into the sensed row. The block's fields are copied before the first store, as action_delay_reset.
 UPKIE_HD void obs_delay_reset(const ObsDelay& O, uint64_t seed, uint64_t g, int i) {
   const UpkieObservationDelay spec = O.spec;

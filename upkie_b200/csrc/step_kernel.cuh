@@ -62,7 +62,7 @@ __device__ __forceinline__ void store_final_obs(const SimParams& P, const RobotS
 }
 
 // The pre-reset state of env `i`, stashed before the same-step auto-reset overwrites it (upkie_b200_final_spine_obs
-// turns it into the spine observation the env would have returned, k_final_spine_obs): the step's number in the mark
+// turns it into the spine observation the env would have returned, k_spine_obs): the step's number in the mark
 // row, the state, and in spine mode the lag record. Per-thread stores on the reset branch only.
 template <bool SPINE>
 __device__ __forceinline__ void store_final_state(const SimParams& P, const RobotState& S, const SpineLag& L, int n_pad,
@@ -78,7 +78,7 @@ __device__ __forceinline__ void store_final_state(const SimParams& P, const Robo
 }
 
 // Reset randomisation, same-step auto-reset with the stash requested: the pre-reset values of the parameter-table
-// columns k_final_spine_obs reads (torque measurement noise and IMU uncertainty), read before the reset's draw
+// columns k_spine_obs reads (torque measurement noise and IMU uncertainty), read before the reset's draw
 // overwrites them, in the stash rows after the state (and lag) rows
 template <bool SPINE>
 __device__ __forceinline__ void store_final_params(const SimParams& P, int n_pad, int i) {
@@ -474,7 +474,7 @@ __device__ __forceinline__ void step_env(
         // neither the reset below nor the rest of the tick writes tick[i] (written above, before the physics) or the
         // parameter table, so the stash and those give the rows k_spine_obs would have returned without the reset (a
         // reset randomisation draw overwrites the table at the end of the tick, and the stash then also holds the
-        // pre-reset columns k_final_spine_obs reads, store_final_params)
+        // pre-reset columns k_spine_obs reads, store_final_params)
         if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
       }
       if (F.reset_rand && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);

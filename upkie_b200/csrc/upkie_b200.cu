@@ -8,9 +8,9 @@
 //                  articulated-body dynamics, wheel-ground contact solve,
 //                  semi-implicit integration), observation, termination; optional
 //                  fused auto-reset.
-//   k_reset        masked reset: set state, one physics substep, observe.
-//   k_spine_obs / k_reset_obs / k_get_state / k_set_state   layout helpers.
-//   k_final_spine_obs   spine observations of the same-step auto-resets' terminal step, from the step kernel's stash.
+//   k_reset        masked reset: set state, one physics substep, observe; the randomisations' per-env state restarts.
+//   k_spine_obs    spine observations of the state, or of the same-step auto-resets' terminal step from the stash.
+//   k_ring_copy    rows <-> struct-of-arrays columns of every per-env buffer, and the delay histories.
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -21,8 +21,10 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <new>
 #include <string>
+#include <utility>
 
 #include "mpc.cuh"
 #include "base_velocity.cuh"
@@ -139,14 +141,20 @@ Handle* as_handle(void* h) {
 }
 
 // ---- masked reset ------------------------------------------------------------------
+// The envs the reset takes (mask, NULL = all) restart from `init_state` rows or from a sampled state (keyed on `seed`,
+// `env_offset`), and the per-env state of every randomisation the handle runs restarts with them, in the per-lane
+// functions of the step kernels' fused resets. Those draws are keyed on the auto-reset's seed and env offset
+// (`rand_seed`, `rand_offset`), whatever init rows the reset takes.
 __global__ void __launch_bounds__(128)
 k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict__ state,
         const uint8_t* __restrict__ mask, const float* __restrict__ init_state, const float* __restrict__ eps_all,
         const float* __restrict__ mu_all, uint32_t* __restrict__ err, uint8_t* __restrict__ done_prev,
-        uint32_t* __restrict__ episode, uint64_t seed, uint64_t env_offset, float* __restrict__ lag) {
+        uint32_t* __restrict__ episode, uint64_t seed, uint64_t env_offset, float* __restrict__ lag,
+        uint64_t rand_seed, uint64_t rand_offset) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   if (mask && !mask[i]) return;
+  const uint64_t g = rand_offset + uint64_t(i);
   RobotState S;
   load_state(state, n_pad, i, S);
   float epsv[6];
@@ -156,7 +164,26 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
     for (int k = 0; k < 6; ++k) epsv[k] = eps_all[size_t(i) * 6 + k];
     eps = epsv;
   }
-  const float mu = mu_all ? mu_all[i] : P.friction;
+  float mu = mu_all ? mu_all[i] : P.friction;
+  // reset randomisation (the handle then holds eps_all and mu_all): the reset substep runs with the drawn epsilons and
+  // friction, taken from the draw in registers and not read back from eps_all and mu_all (the reset substep reads no
+  // parameter table)
+  if (P.reset_rand) {
+    const ResetRand& R = *P.reset_rand;
+    float v[UPKIE_RR_DIM];
+    reset_rand_draw(R.spec, rand_seed, g, R.draws[i] + 1u, v);
+    const uint64_t cols = R.spec.columns;
+#pragma unroll
+    for (int b = 0; b < 6; ++b)
+      if ((cols >> (UPKIE_RR_INERTIA + b)) & 1u) epsv[b] = v[UPKIE_RR_INERTIA + b];
+    if ((cols >> UPKIE_RR_FRICTION) & 1u) mu = v[UPKIE_RR_FRICTION];
+    reset_rand_store(R, i, v);
+  }
+  if (P.push) push_reset(*P.push, rand_seed, g, i);  // a new schedule
+  if (P.action_delay) {  // the next delay, and the stop row as every previous command (the ring head stays)
+    action_delay_reset(*P.action_delay, rand_seed, g, i);
+    action_delay_fill_history(*P.action_delay, i);
+  }
   float init[UPKIE_INIT_DIM];
   if (init_state) {
 #pragma unroll
@@ -180,13 +207,28 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
   err[i] = 0;
   done_prev[i] = 0;
   P.elapsed[i] = 0;
+  if (P.obs_delay) {
+    // the next delay, and the post-reset state as the sensed row and every snapshot: the reset is observed undelayed
+    const ObsDelay& O = *P.obs_delay;
+    obs_delay_reset(O, rand_seed, g, i);
+    float r[UPKIE_STATE_DIM];
+    state_to_row(S, r);
+    float* const col = O.rows + size_t(i);
+    for (int k = 0; k < UPKIE_STATE_DIM; ++k) col[size_t(k) * size_t(O.stride)] = r[k];
+    if (O.ticks > 1) obs_delay_fill_history(O, i, r);
+  }
 }
 
+// The spine observation rows of the states `state` (and in spine mode the lag records `lag`), with the noise keys of
+// the step that produced them (tick[i]). `mark` set: the envs whose mark is `gen` only, the rows of the others are left
+// as they are (upkie_b200_final_spine_obs: the pre-reset states that the same-step auto-resets of step `gen` stashed,
+// store_final_state; neither the reset nor the rest of the step writes tick[i]).
 __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ state,
-                            const uint32_t* __restrict__ tick, uint64_t env_offset, float* __restrict__ out,
-                            const float* __restrict__ lag) {
+                            const float* __restrict__ lag, const uint32_t* __restrict__ mark, uint32_t gen,
+                            const uint32_t* __restrict__ tick, uint64_t env_offset, float* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  if (mark && mark[i] != gen) return;
   float o[UPKIE_SPINE_DIM];
   const NoiseCtx nz{env_offset + uint64_t(i), tick[i]};  // same draw as the step that produced this state
   if (P.spine_mode && lag) {
@@ -199,36 +241,6 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
   } else {
     RobotState S;
     load_state(state, n_pad, i, S);
-    float tq[6];
-    measured_torques(P, S, &nz, tq, i);
-    spine_observation(P, S, o, tq);
-  }
-  apply_imu_uncertainty(P, nz, o, i);
-#pragma unroll
-  for (int k = 0; k < UPKIE_SPINE_DIM; ++k) out[size_t(i) * UPKIE_SPINE_DIM + k] = o[k];
-}
-
-// The spine observation rows of the envs that reset in step `gen` (same-step auto-reset), from the states they stashed
-// before the reset (store_final_state): k_spine_obs's device functions in its order, with the same noise keys (tick[i],
-// which the reset leaves alone) and the same column of the parameter table. The rows of the other envs are left as
-// they are.
-__global__ void k_final_spine_obs(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ stash,
-                                  uint32_t gen, const uint32_t* __restrict__ tick, uint64_t env_offset,
-                                  float* __restrict__ out, int spine) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  if (reinterpret_cast<const uint32_t*>(stash + size_t(kFinalMarkRow) * n_pad)[i] != gen) return;
-  float o[UPKIE_SPINE_DIM];
-  const NoiseCtx nz{env_offset + uint64_t(i), tick[i]};
-  if (spine) {
-    float lr[UPKIE_LAG_DIM];
-    for (int k = 0; k < UPKIE_LAG_DIM; ++k) lr[k] = stash[size_t(kFinalLagRow + k) * n_pad + i];
-    SpineLag L;
-    lag_from_row(lr, L);
-    spine_observation_from_lag(P, L, o);
-  } else {
-    RobotState S;
-    load_state(stash + size_t(kFinalStateRow) * n_pad, n_pad, i, S);
     float tq[6];
     measured_torques(P, S, &nz, tq, i);
     spine_observation(P, S, o, tq);
@@ -273,39 +285,139 @@ __global__ void k_reset_obs(const __grid_constant__ SimParams P, int n, int n_pa
   }
 }
 
-// SoA <-> AoS state transposes
-__global__ void k_get_state(int n, int n_pad, const float* __restrict__ state, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  for (int k = 0; k < UPKIE_STATE_DIM; ++k) out[size_t(i) * UPKIE_STATE_DIM + k] = state[size_t(k) * n_pad + i];
-}
-__global__ void k_set_state(int n, int n_pad, float* __restrict__ state, const float* __restrict__ in) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  for (int k = 0; k < UPKIE_STATE_DIM; ++k) state[size_t(k) * n_pad + i] = in[size_t(i) * UPKIE_STATE_DIM + k];
-}
-// per-env parameter table: validation of the caller's rows [n][UPKIE_EP_DIM] (env_row_flags OR-ed into *flags), and
-// the rows <-> struct-of-arrays transposes; without a table the rows read back the config's values
+// validation of the caller's rows [n][UPKIE_EP_DIM] of a per-env parameter table (env_row_flags OR-ed into *flags)
 __global__ void k_env_params_check(int n, const float* __restrict__ rows, uint32_t* __restrict__ flags) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t f = env_row_flags(rows + size_t(i) * UPKIE_EP_DIM);
   if (f) atomicOr(flags, f);
 }
-__global__ void k_env_params_copy(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict__ table,
-                                  float* __restrict__ rows, int to_rows) {
+
+// Every env's row of the config's parameter values (what the envs run without a table), as out[i * istride + k *
+// kstride]: a table [UPKIE_EP_DIM][n_pad] (1, n_pad) or rows [n][UPKIE_EP_DIM] (UPKIE_EP_DIM, 1)
+__global__ void k_env_params_from_config(const __grid_constant__ SimParams P, int n, int istride, int kstride,
+                                         float* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  for (int k = 0; k < UPKIE_EP_DIM; ++k) {
-    if (!to_rows) table[size_t(k) * n_pad + i] = rows[size_t(i) * UPKIE_EP_DIM + k];
-    else rows[size_t(i) * UPKIE_EP_DIM + k] = table ? table[size_t(k) * n_pad + i] : config_env_param(P, k);
+  for (int k = 0; k < UPKIE_EP_DIM; ++k) out[size_t(i) * istride + size_t(k) * kstride] = config_env_param(P, k);
+}
+
+// The action delay's stop row as every env's command, out[i * istride + c * cstride]: the columns of the command buffer
+// [UPKIE_ACT_DIM][n_pad] (1, n_pad) or rows [n][UPKIE_ACT_DIM] (UPKIE_ACT_DIM, 1)
+__global__ void k_stop_rows(int n, int istride, int cstride, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  for (int c = 0; c < UPKIE_ACT_DIM; ++c) out[size_t(i) * istride + size_t(c) * cstride] = action_delay_stop_value(c);
+}
+
+__global__ void k_fill(int n, float* __restrict__ out, float v) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = v;
+}
+
+// Rows [ages][n][dim] <-> ages 0 .. ages - 1 (0 the newest) of the rings [ticks][dim][stride] whose next write is row
+// head[i] (head null: row 0). At ticks = ages = 1, the transpose of rows [n][dim] and the struct-of-arrays columns
+// [dim][stride] of every per-env buffer.
+__global__ void k_ring_copy(float* __restrict__ ring, const uint32_t* __restrict__ head, int ticks, int dim, int n,
+                            int stride, int ages, float* __restrict__ rows, int to_rows) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t h = head ? head[i] : 0u;
+  for (int a = 0; a < ages; ++a) {
+    float* const col = ring + size_t(delay_ring_row(h, uint32_t(ticks), uint32_t(a))) * dim * stride + size_t(i);
+    float* const row = rows + (size_t(a) * n + i) * dim;
+    for (int k = 0; k < dim; ++k) {
+      if (to_rows) row[k] = col[size_t(k) * stride];
+      else col[size_t(k) * stride] = row[k];
+    }
   }
 }
-__global__ void k_set_ext(int n, int n_pad, float* __restrict__ ext, const float* __restrict__ in) {
+
+// the rings `src` [src_ticks][dim][stride] (next write head[i], null: 0) into `dst` [dst_ticks][dim][stride] in age
+// order, with row 0 of dst the next write: the ages beyond src_ticks are stop rows (stop) or copies of the oldest;
+// columns = a mask of the columns copied (bit k, 64 bits at most), all of them for ~0
+__global__ void k_ring_resize(const float* __restrict__ src, const uint32_t* __restrict__ head, int src_ticks,
+                              float* __restrict__ dst, int dst_ticks, int dim, int n, int stride, int stop,
+                              uint64_t columns) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  for (int k = 0; k < 3 * UPKIE_NB; ++k) ext[size_t(k) * n_pad + i] = in[size_t(i) * 3 * UPKIE_NB + k];
+  const uint32_t h = head ? head[i] : 0u;
+  for (int a = 0; a < dst_ticks; ++a) {
+    const int sa = a < src_ticks ? a : src_ticks - 1;
+    const float* const s = src + size_t(delay_ring_row(h, uint32_t(src_ticks), uint32_t(sa))) * dim * stride + i;
+    float* const d = dst + size_t(delay_ring_row(0u, uint32_t(dst_ticks), uint32_t(a))) * dim * stride + i;
+    for (int k = 0; k < dim; ++k)
+      if ((columns >> k) & 1u) d[size_t(k) * stride] = (stop && a >= src_ticks) ? action_delay_stop_value(k) : s[size_t(k) * stride];
+  }
 }
+
+// the push force of each env's last step, from its schedule state (R null: no spec, zeros)
+__global__ void k_push_forces(const PushRand* __restrict__ R, int n, uint64_t seed, uint64_t env_offset,
+                              float* __restrict__ force) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float f[3] = {0.f, 0.f, 0.f};
+  if (R) push_last_force(R->spec, seed, env_offset + uint64_t(i), R->count[i], R->timer[i], f);
+  for (int k = 0; k < 3; ++k) force[size_t(i) * 3 + k] = f[k];
+}
+
+int grid_of(int n) { return (n + 127) / 128; }
+
+// rows [ages][n][dim] of the rings `ring` (ring_rows) or the other way (ring_cols), k_ring_copy; the defaults are the
+// plain transpose of rows [n][dim] and columns [dim][stride]
+cudaError_t ring_rows(const float* ring, int dim, int n, int stride, float* rows, cudaStream_t s,
+                      const uint32_t* head = nullptr, int ticks = 1, int ages = 1) {
+  k_ring_copy<<<grid_of(n), 128, 0, s>>>(const_cast<float*>(ring), head, ticks, dim, n, stride, ages, rows, 1);
+  return cudaGetLastError();
+}
+cudaError_t ring_cols(const float* rows, int dim, int n, int stride, float* ring, cudaStream_t s,
+                      const uint32_t* head = nullptr, int ticks = 1, int ages = 1) {
+  k_ring_copy<<<grid_of(n), 128, 0, s>>>(ring, head, ticks, dim, n, stride, ages, const_cast<float*>(rows), 0);
+  return cudaGetLastError();
+}
+
+cudaError_t ring_resize(const float* src, const uint32_t* head, int src_ticks, float* dst, int dst_ticks, int dim,
+                        int n, int stride, int stop, uint64_t columns, cudaStream_t s) {
+  k_ring_resize<<<grid_of(n), 128, 0, s>>>(src, head, src_ticks, dst, dst_ticks, dim, n, stride, stop, columns);
+  return cudaGetLastError();
+}
+
+cudaError_t stop_rows(int n, int istride, int cstride, float* out, cudaStream_t s) {
+  k_stop_rows<<<grid_of(n), 128, 0, s>>>(n, istride, cstride, out);
+  return cudaGetLastError();
+}
+
+cudaError_t env_params_from_config(const SimParams& P, int n, int istride, int kstride, float* out, cudaStream_t s) {
+  k_env_params_from_config<<<grid_of(n), 128, 0, s>>>(P, n, istride, kstride, out);
+  return cudaGetLastError();
+}
+
+cudaError_t fill(int n, float* out, float v, cudaStream_t s) {
+  k_fill<<<grid_of(n), 128, 0, s>>>(n, out, v);
+  return cudaGetLastError();
+}
+
+// a per-env buffer the handle may never have allocated, copied into `dst` (src null: zeros)
+cudaError_t copy_or_zero(void* dst, const void* src, size_t bytes, cudaStream_t s) {
+  return src ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s) : cudaMemsetAsync(dst, 0, bytes, s);
+}
+
+// Per-env buffers {&pointer, bytes}, allocated and zeroed, all of them or none: on a failure the ones allocated are
+// freed and every pointer is null again
+cudaError_t alloc_zeroed(std::initializer_list<std::pair<void**, size_t>> bufs) {
+  cudaError_t e = cudaSuccess;
+  for (const auto& b : bufs) {
+    if (e == cudaSuccess) e = cudaMalloc(b.first, b.second);
+    if (e == cudaSuccess) e = cudaMemset(*b.first, 0, b.second);
+  }
+  if (e != cudaSuccess)
+    for (const auto& b : bufs) {
+      cudaFree(*b.first);
+      *b.first = nullptr;
+    }
+  return e;
+}
+
 __global__ void k_init_state(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict__ state) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_pad) return;
@@ -846,8 +958,7 @@ int upkie_b200_set_env_params(void* handle, const float* rows, void* stream) {
     CUDA_TRY(cudaMemsetAsync(h->env_params, 0, bytes, s));
   }
   CUDA_TRY(cudaDeviceSynchronize());  // launches in flight on other streams may still read the previous table
-  k_env_params_copy<<<(h->n + 127) / 128, 128, 0, s>>>(h->P, h->n, h->n_pad, h->env_params, const_cast<float*>(rows), 0);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(ring_cols(rows, UPKIE_EP_DIM, h->n, h->n_pad, h->env_params, s));
   CUDA_TRY(cudaStreamSynchronize(s));
   h->env_param_flags = flags;
   h->P.env_params = h->env_params;
@@ -878,7 +989,7 @@ int upkie_b200_set_reset_randomization(void* handle, const UpkieResetRandomizati
   if (!h->env_params) {
     CUDA_TRY(cudaMalloc(&h->env_params, size_t(UPKIE_EP_DIM) * h->n_pad * sizeof(float)));
     CUDA_TRY(cudaMemset(h->env_params, 0, size_t(UPKIE_EP_DIM) * h->n_pad * sizeof(float)));
-    CUDA_TRY(launch_env_params_from_config(h->P, h->n, h->n_pad, h->env_params, nullptr));
+    CUDA_TRY(env_params_from_config(h->P, h->n, 1, h->n_pad, h->env_params, nullptr));
     h->env_param_flags = h->config_flags;
     h->P.env_params = h->env_params;
     h->P.env_params_stride = h->n_pad;
@@ -889,7 +1000,7 @@ int upkie_b200_set_reset_randomization(void* handle, const UpkieResetRandomizati
   }
   if (!h->mu) {
     CUDA_TRY(cudaMalloc(&h->mu, size_t(h->n) * sizeof(float)));
-    CUDA_TRY(launch_fill(h->n, h->mu, h->P.friction, nullptr));
+    CUDA_TRY(fill(h->n, h->mu, h->P.friction, nullptr));
   }
   if (!h->draws) {
     CUDA_TRY(cudaMalloc(&h->draws, size_t(h->n) * sizeof(uint32_t)));
@@ -918,10 +1029,7 @@ int upkie_b200_get_draws(void* handle, uint32_t* draws, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !draws) return fail(UPKIE_B200_EINVAL, "get_draws: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
-  if (h->draws) CUDA_TRY(cudaMemcpyAsync(draws, h->draws, bytes, cudaMemcpyDeviceToDevice, s));
-  else CUDA_TRY(cudaMemsetAsync(draws, 0, bytes, s));
+  CUDA_TRY(copy_or_zero(draws, h->draws, size_t(h->n) * sizeof(uint32_t), static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 
@@ -940,7 +1048,11 @@ int upkie_b200_get_randomization(void* handle, float* friction, float* inertia_e
   if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
   if (!friction && !inertia_eps) return UPKIE_B200_OK;
   CUDA_TRY(cudaSetDevice(h->device));
-  CUDA_TRY(launch_get_randomization(h->P, h->n, h->mu, h->eps, friction, inertia_eps, static_cast<cudaStream_t>(stream)));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // without buffers, the nominal values: the config's friction and zero epsilons
+  if (friction && h->mu) CUDA_TRY(cudaMemcpyAsync(friction, h->mu, size_t(h->n) * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  else if (friction) CUDA_TRY(fill(h->n, friction, h->P.friction, s));
+  if (inertia_eps) CUDA_TRY(copy_or_zero(inertia_eps, h->eps, size_t(h->n) * 6 * sizeof(float), s));
   return UPKIE_B200_OK;
 }
 
@@ -948,9 +1060,10 @@ int upkie_b200_get_env_params(void* handle, float* rows, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !rows) return fail(UPKIE_B200_EINVAL, "get_env_params: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  k_env_params_copy<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad,
-                                                                                        h->env_params, rows, 1);
-  CUDA_TRY(cudaGetLastError());
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // without a table, the config's values
+  if (h->env_params) CUDA_TRY(ring_rows(h->env_params, UPKIE_EP_DIM, h->n, h->n_pad, rows, s));
+  else CUDA_TRY(env_params_from_config(h->P, h->n, UPKIE_EP_DIM, 1, rows, s));
   return UPKIE_B200_OK;
 }
 
@@ -999,23 +1112,9 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
   h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int rblock = 128;
-  const int grid = (h->n + rblock - 1) / rblock;
-  // reset randomisation: the envs this reset takes draw first, keyed on the auto-reset's seed and env offset whatever
-  // init rows the reset takes; k_reset then runs the reset substep with the drawn epsilons and friction
-  if (h->P.reset_rand) CUDA_TRY(launch_reset_rand(h->rr_dev, h->n, mask, h->seed, h->env_offset, s));
-  // push randomisation: the envs this reset takes start a new schedule
-  if (h->P.push) CUDA_TRY(launch_push_reset(h->push_dev, h->n, mask, h->seed, h->env_offset, s));
-  // action delay: the envs this reset takes draw their next delay and hold the stop row
-  if (h->P.action_delay)
-    CUDA_TRY(launch_action_delay_reset(h->delay_dev, h->n, mask, h->seed, h->env_offset, s));
-  k_reset<<<grid, rblock, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
-                                    h->done_prev, h->episode, seed, env_offset, h->lag);
+  k_reset<<<grid_of(h->n), 128, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
+                                        h->done_prev, h->episode, seed, env_offset, h->lag, h->seed, h->env_offset);
   CUDA_TRY(cudaGetLastError());
-  // observation delay: the envs this reset takes draw their next delay, and their sensed rows become the post-reset
-  // state (the reset's observation is undelayed)
-  if (h->P.obs_delay)
-    CUDA_TRY(launch_obs_delay_reset(h->sense_dev, h->n, h->n_pad, h->state, mask, h->seed, h->env_offset, s));
   // a reset sampled on the device counts an episode: it is not one the base-velocity post step has to carry out
   if (!init_state)
     CUDA_TRY(cudaMemcpyAsync(h->bv_episode, h->episode, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
@@ -1211,7 +1310,8 @@ int upkie_b200_spine_obs(void* handle, float* out, void* stream) {
   CUDA_TRY(cudaSetDevice(h->device));
   // observation delay: the spine observation of the sensed states
   const float* state = h->P.obs_delay ? h->sense_rows : h->state;
-  k_spine_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, state, h->tick, h->env_offset, out, h->lag);
+  k_spine_obs<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, state, h->lag, nullptr,
+                                                                            0u, h->tick, h->env_offset, out);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1226,14 +1326,18 @@ int upkie_b200_final_spine_obs(void* handle, float* out, void* stream) {
   SimParams P = h->P;
   if (h->final_params) {
     // reset randomisation: the resets of that step redrew the table, the stash holds its pre-reset columns
-    // UPKIE_EP_MEAS_NOISE .. UPKIE_EP_DIM - 1 (the only ones k_final_spine_obs reads): the launch's table is the stash,
+    // UPKIE_EP_MEAS_NOISE .. UPKIE_EP_DIM - 1 (the only ones k_spine_obs reads): the launch's table is the stash,
     // shifted so that column k of env i is stash row (first parameter row + k - UPKIE_EP_MEAS_NOISE)
     const int row0 = h->lag ? kFinalRowsSpine : kFinalRows;
     P.env_params = h->final_state + size_t(row0 - UPKIE_EP_MEAS_NOISE) * h->n_pad;
     P.env_params_stride = h->n_pad;
   }
-  k_final_spine_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-      P, h->n, h->n_pad, h->final_state, h->final_gen, h->tick, h->env_offset, out, h->lag ? 1 : 0);
+  const float* stash = h->final_state;
+  k_spine_obs<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+      P, h->n, h->n_pad, stash + size_t(kFinalStateRow) * h->n_pad,
+      h->lag ? stash + size_t(kFinalLagRow) * h->n_pad : nullptr,
+      reinterpret_cast<const uint32_t*>(stash + size_t(kFinalMarkRow) * h->n_pad), h->final_gen, h->tick,
+      h->env_offset, out);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1255,8 +1359,7 @@ int upkie_b200_get_state(void* handle, float* state, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !state) return fail(UPKIE_B200_EINVAL, "get_state: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  k_get_state<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->state, state);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(ring_rows(h->state, UPKIE_STATE_DIM, h->n, h->n_pad, state, static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 
@@ -1265,41 +1368,26 @@ int upkie_b200_set_state(void* handle, const float* state, void* stream) {
   if (!h || !state) return fail(UPKIE_B200_EINVAL, "set_state: invalid argument");
   h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
-  k_set_state<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->state, state);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(ring_cols(state, UPKIE_STATE_DIM, h->n, h->n_pad, h->state, static_cast<cudaStream_t>(stream)));
   // observation delay: the sensors see the state set, without a lag behind it (every snapshot of a history too)
   if (h->P.obs_delay) {
     CUDA_TRY(cudaMemcpyAsync(h->sense_rows, h->state, size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float),
                              cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
     if (h->sense_hist)
-      CUDA_TRY(launch_ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad,
-                                  0, ~uint64_t(0), static_cast<cudaStream_t>(stream)));
+      CUDA_TRY(ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad, 0,
+                           ~uint64_t(0), static_cast<cudaStream_t>(stream)));
   }
   return UPKIE_B200_OK;
-}
-
-__global__ void k_lag_copy(int n, int n_pad, float* __restrict__ lag, float* __restrict__ rows, int to_rows) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  for (int k = 0; k < UPKIE_LAG_DIM; ++k) {
-    if (to_rows) rows[size_t(i) * UPKIE_LAG_DIM + k] = lag[size_t(k) * n_pad + i];
-    else lag[size_t(k) * n_pad + i] = rows[size_t(i) * UPKIE_LAG_DIM + k];
-  }
-}
-
-__global__ void k_body_rec_rows(int n, int n_pad, const float* __restrict__ rec, float* __restrict__ rows) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  for (int k = 0; k < UPKIE_BODY_REC_DIM; ++k) rows[size_t(i) * UPKIE_BODY_REC_DIM + k] = rec ? rec[size_t(k) * n_pad + i] : 0.f;
 }
 
 int upkie_b200_get_body_contacts(void* handle, float* rows, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !rows) return fail(UPKIE_B200_EINVAL, "get_body_contacts: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  k_body_rec_rows<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(
-      h->n, h->n_pad, h->P.body_contacts ? h->body_rec : nullptr, rows);
-  CUDA_TRY(cudaGetLastError());
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // without body contacts, zeros
+  if (h->P.body_rec) CUDA_TRY(ring_rows(h->P.body_rec, UPKIE_BODY_REC_DIM, h->n, h->n_pad, rows, s));
+  else CUDA_TRY(cudaMemsetAsync(rows, 0, size_t(h->n) * UPKIE_BODY_REC_DIM * sizeof(float), s));
   return UPKIE_B200_OK;
 }
 
@@ -1308,8 +1396,7 @@ int upkie_b200_get_lag(void* handle, float* lag_rows, void* stream) {
   if (!h || !lag_rows) return fail(UPKIE_B200_EINVAL, "get_lag: invalid argument");
   if (!h->lag) return fail(UPKIE_B200_EINVAL, "get_lag: the handle was not created with spine_mode");
   CUDA_TRY(cudaSetDevice(h->device));
-  k_lag_copy<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->lag, lag_rows, 1);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(ring_rows(h->lag, UPKIE_LAG_DIM, h->n, h->n_pad, lag_rows, static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 int upkie_b200_set_lag(void* handle, const float* lag_rows, void* stream) {
@@ -1318,8 +1405,7 @@ int upkie_b200_set_lag(void* handle, const float* lag_rows, void* stream) {
   if (!h->lag) return fail(UPKIE_B200_EINVAL, "set_lag: the handle was not created with spine_mode");
   h->final_valid = false;  // the stashed states no longer belong to the last step
   CUDA_TRY(cudaSetDevice(h->device));
-  k_lag_copy<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->n, h->n_pad, h->lag, const_cast<float*>(lag_rows), 0);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(ring_cols(lag_rows, UPKIE_LAG_DIM, h->n, h->n_pad, h->lag, static_cast<cudaStream_t>(stream)));
   return UPKIE_B200_OK;
 }
 
@@ -1344,8 +1430,7 @@ int upkie_b200_set_external_forces(void* handle, const float* force, uint32_t lo
     CUDA_TRY(cudaMalloc(&h->ext, size_t(3 * UPKIE_NB) * h->n_pad * sizeof(float)));
     CUDA_TRY(cudaMemsetAsync(h->ext, 0, size_t(3 * UPKIE_NB) * h->n_pad * sizeof(float), s));
   }
-  k_set_ext<<<(h->n + 127) / 128, 128, 0, s>>>(h->n, h->n_pad, h->ext, force);
-  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(ring_cols(force, 3 * UPKIE_NB, h->n, h->n_pad, h->ext, s));
   return UPKIE_B200_OK;
 }
 
@@ -1354,10 +1439,8 @@ namespace {
 int alloc_push_state(Handle* h) {
   if (h->push_count) return UPKIE_B200_OK;
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
-  CUDA_TRY(cudaMalloc(&h->push_count, bytes));
-  CUDA_TRY(cudaMalloc(&h->push_timer, bytes));
-  CUDA_TRY(cudaMemset(h->push_count, 0, bytes));
-  CUDA_TRY(cudaMemset(h->push_timer, 0, bytes));
+  CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->push_count), bytes},
+                         {reinterpret_cast<void**>(&h->push_timer), bytes}}));
   return UPKIE_B200_OK;
 }
 }  // namespace
@@ -1402,7 +1485,9 @@ int upkie_b200_get_push_forces(void* handle, float* force, void* stream) {
   Handle* h = as_handle(handle);
   if (!h || !force) return fail(UPKIE_B200_EINVAL, "get_push_forces: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  CUDA_TRY(launch_push_forces(h->P.push, h->n, h->seed, h->env_offset, force, static_cast<cudaStream_t>(stream)));
+  k_push_forces<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P.push, h->n, h->seed, h->env_offset,
+                                                                              force);
+  CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
 
@@ -1412,13 +1497,8 @@ int upkie_b200_get_push_state(void* handle, uint32_t* count, uint32_t* timer, vo
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
-  if (h->push_count) {
-    CUDA_TRY(cudaMemcpyAsync(count, h->push_count, bytes, cudaMemcpyDeviceToDevice, s));
-    CUDA_TRY(cudaMemcpyAsync(timer, h->push_timer, bytes, cudaMemcpyDeviceToDevice, s));
-  } else {
-    CUDA_TRY(cudaMemsetAsync(count, 0, bytes, s));
-    CUDA_TRY(cudaMemsetAsync(timer, 0, bytes, s));
-  }
+  CUDA_TRY(copy_or_zero(count, h->push_count, bytes, s));
+  CUDA_TRY(copy_or_zero(timer, h->push_timer, bytes, s));
   return UPKIE_B200_OK;
 }
 
@@ -1440,25 +1520,14 @@ namespace {
 int alloc_delay_state(Handle* h) {
   if (h->delay_count) return UPKIE_B200_OK;
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
-  uint32_t *count = nullptr, *delay = nullptr, *head = nullptr;
-  float* command = nullptr;
-  cudaError_t e = cudaMalloc(&count, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&delay, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&head, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&command, size_t(UPKIE_ACT_DIM) * h->n_pad * sizeof(float));
-  if (e == cudaSuccess) e = cudaMemset(count, 0, bytes);
-  if (e == cudaSuccess) e = cudaMemset(delay, 0, bytes);
-  if (e == cudaSuccess) e = cudaMemset(head, 0, bytes);
-  if (e == cudaSuccess) e = launch_command_cols(nullptr, h->n, h->n_pad, command, nullptr);
+  cudaError_t e = alloc_zeroed({{reinterpret_cast<void**>(&h->delay_count), bytes},
+                                {reinterpret_cast<void**>(&h->delay_delay), bytes},
+                                {reinterpret_cast<void**>(&h->delay_head), bytes},
+                                {reinterpret_cast<void**>(&h->delay_command),
+                                 size_t(UPKIE_ACT_DIM) * h->n_pad * sizeof(float)}});
+  if (e == cudaSuccess) e = stop_rows(h->n, 1, h->n_pad, h->delay_command, nullptr);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    cudaFree(count); cudaFree(delay); cudaFree(head); cudaFree(command);
-    return fail(UPKIE_B200_ECUDA, std::string("action delay state: ") + cudaGetErrorString(e));
-  }
-  h->delay_count = count;
-  h->delay_delay = delay;
-  h->delay_head = head;
-  h->delay_command = command;
+  if (e != cudaSuccess) return fail(UPKIE_B200_ECUDA, std::string("action delay state: ") + cudaGetErrorString(e));
   h->delay_ticks = 1;
   return UPKIE_B200_OK;
 }
@@ -1472,7 +1541,7 @@ int resize_ring(Handle* h, float** ring, uint32_t* head, int* cur, int ticks, in
   float* next = nullptr;
   cudaError_t e = cudaMalloc(&next, size_t(ticks) * dim * h->n_pad * sizeof(float));
   if (e == cudaSuccess)
-    e = launch_ring_resize(*ring, head, *cur, next, ticks, dim, h->n, h->n_pad, stop, ~uint64_t(0), nullptr);
+    e = ring_resize(*ring, head, *cur, next, ticks, dim, h->n, h->n_pad, stop, ~uint64_t(0), nullptr);
   if (e == cudaSuccess) e = cudaMemset(head, 0, size_t(h->n) * sizeof(uint32_t));
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
   if (e != cudaSuccess) {
@@ -1531,18 +1600,12 @@ int upkie_b200_get_action_delay_state(void* handle, uint32_t* count, uint32_t* d
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
-  if (h->delay_count) {
-    CUDA_TRY(cudaMemcpyAsync(count, h->delay_count, bytes, cudaMemcpyDeviceToDevice, s));
-    CUDA_TRY(cudaMemcpyAsync(delay, h->delay_delay, bytes, cudaMemcpyDeviceToDevice, s));
-  } else {
-    CUDA_TRY(cudaMemsetAsync(count, 0, bytes, s));
-    CUDA_TRY(cudaMemsetAsync(delay, 0, bytes, s));
-  }
+  CUDA_TRY(copy_or_zero(count, h->delay_count, bytes, s));
+  CUDA_TRY(copy_or_zero(delay, h->delay_delay, bytes, s));
   if (h->delay_command)  // the previous tick's command: age 0 of the history
-    CUDA_TRY(launch_ring_rows(h->delay_command, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad, 1, command,
-                              s));
+    CUDA_TRY(ring_rows(h->delay_command, UPKIE_ACT_DIM, h->n, h->n_pad, command, s, h->delay_head, h->delay_ticks, 1));
   else
-    CUDA_TRY(launch_command_rows(nullptr, h->n, h->n_pad, command, s));
+    CUDA_TRY(stop_rows(h->n, UPKIE_ACT_DIM, 1, command, s));
   return UPKIE_B200_OK;
 }
 
@@ -1556,8 +1619,7 @@ int upkie_b200_set_action_delay_state(void* handle, const uint32_t* count, const
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
   CUDA_TRY(cudaMemcpyAsync(h->delay_count, count, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(h->delay_delay, delay, bytes, cudaMemcpyDeviceToDevice, s));
-  CUDA_TRY(launch_ring_cols(command, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad, 1, h->delay_command,
-                            s));
+  CUDA_TRY(ring_cols(command, UPKIE_ACT_DIM, h->n, h->n_pad, h->delay_command, s, h->delay_head, h->delay_ticks, 1));
   return UPKIE_B200_OK;
 }
 
@@ -1567,10 +1629,10 @@ int upkie_b200_get_action_delay_history(void* handle, float* commands, void* str
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (h->delay_command)
-    CUDA_TRY(launch_ring_rows(h->delay_command, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad,
-                              h->delay_ticks, commands, s));
+    CUDA_TRY(ring_rows(h->delay_command, UPKIE_ACT_DIM, h->n, h->n_pad, commands, s, h->delay_head, h->delay_ticks,
+                       h->delay_ticks));
   else
-    CUDA_TRY(launch_command_rows(nullptr, h->n, h->n_pad, commands, s));
+    CUDA_TRY(stop_rows(h->n, UPKIE_ACT_DIM, 1, commands, s));
   return UPKIE_B200_OK;
 }
 
@@ -1579,8 +1641,8 @@ int upkie_b200_set_action_delay_history(void* handle, const float* commands, voi
   if (!h || !commands) return fail(UPKIE_B200_EINVAL, "set_action_delay_history: invalid argument");
   CUDA_TRY(cudaSetDevice(h->device));
   if (alloc_delay_state(h)) return UPKIE_B200_ECUDA;
-  CUDA_TRY(launch_ring_cols(commands, h->delay_head, h->delay_ticks, UPKIE_ACT_DIM, h->n, h->n_pad, h->delay_ticks,
-                            h->delay_command, static_cast<cudaStream_t>(stream)));
+  CUDA_TRY(ring_cols(commands, UPKIE_ACT_DIM, h->n, h->n_pad, h->delay_command, static_cast<cudaStream_t>(stream),
+                     h->delay_head, h->delay_ticks, h->delay_ticks));
   return UPKIE_B200_OK;
 }
 
@@ -1591,26 +1653,15 @@ int alloc_sense_state(Handle* h) {
   if (h->sense_count) return UPKIE_B200_OK;
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
   const size_t row_bytes = size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float);
-  uint32_t *count = nullptr, *delay = nullptr, *head = nullptr;
-  float* rows = nullptr;
   cudaError_t e = cudaDeviceSynchronize();  // the state of the steps in flight
-  if (e == cudaSuccess) e = cudaMalloc(&count, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&delay, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&head, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&rows, row_bytes);
-  if (e == cudaSuccess) e = cudaMemset(count, 0, bytes);
-  if (e == cudaSuccess) e = cudaMemset(delay, 0, bytes);
-  if (e == cudaSuccess) e = cudaMemset(head, 0, bytes);
-  if (e == cudaSuccess) e = cudaMemcpy(rows, h->state, row_bytes, cudaMemcpyDeviceToDevice);
+  if (e == cudaSuccess)
+    e = alloc_zeroed({{reinterpret_cast<void**>(&h->sense_count), bytes},
+                      {reinterpret_cast<void**>(&h->sense_delay), bytes},
+                      {reinterpret_cast<void**>(&h->sense_head), bytes},
+                      {reinterpret_cast<void**>(&h->sense_rows), row_bytes}});
+  if (e == cudaSuccess) e = cudaMemcpy(h->sense_rows, h->state, row_bytes, cudaMemcpyDeviceToDevice);
   if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    cudaFree(count); cudaFree(delay); cudaFree(head); cudaFree(rows);
-    return fail(UPKIE_B200_ECUDA, std::string("observation delay state: ") + cudaGetErrorString(e));
-  }
-  h->sense_count = count;
-  h->sense_delay = delay;
-  h->sense_head = head;
-  h->sense_rows = rows;
+  if (e != cudaSuccess) return fail(UPKIE_B200_ECUDA, std::string("observation delay state: ") + cudaGetErrorString(e));
   h->sense_ticks = 1;
   return UPKIE_B200_OK;
 }
@@ -1630,8 +1681,8 @@ int resize_sense_history(Handle* h, int ticks) {
     uint64_t sensed = 0;
     for (int k = 0; k < UPKIE_STATE_DIM; ++k)
       if (obs_delay_sensed(k)) sensed |= uint64_t(1) << k;
-    cudaError_t e = launch_ring_resize(h->sense_hist, h->sense_head, h->sense_ticks, h->sense_rows, 1, UPKIE_STATE_DIM,
-                                       h->n, h->n_pad, 0, sensed, nullptr);
+    cudaError_t e = ring_resize(h->sense_hist, h->sense_head, h->sense_ticks, h->sense_rows, 1, UPKIE_STATE_DIM, h->n,
+                                h->n_pad, 0, sensed, nullptr);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) return fail(UPKIE_B200_ECUDA, std::string(what) + cudaGetErrorString(e));
     cudaFree(h->sense_hist);
@@ -1643,8 +1694,7 @@ int resize_sense_history(Handle* h, int ticks) {
     float* hist = nullptr;
     cudaError_t e = cudaMalloc(&hist, size_t(ticks) * UPKIE_STATE_DIM * h->n_pad * sizeof(float));
     if (e == cudaSuccess)
-      e = launch_ring_resize(h->sense_rows, nullptr, 1, hist, ticks, UPKIE_STATE_DIM, h->n, h->n_pad, 0, ~uint64_t(0),
-                             nullptr);
+      e = ring_resize(h->sense_rows, nullptr, 1, hist, ticks, UPKIE_STATE_DIM, h->n, h->n_pad, 0, ~uint64_t(0), nullptr);
     if (e == cudaSuccess) e = cudaMemset(h->sense_head, 0, size_t(h->n) * sizeof(uint32_t));
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
     if (e != cudaSuccess) {
@@ -1683,8 +1733,8 @@ int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationD
     CUDA_TRY(cudaMemcpy(h->sense_rows, h->state, size_t(UPKIE_STATE_DIM) * h->n_pad * sizeof(float),
                         cudaMemcpyDeviceToDevice));
     if (h->sense_hist)
-      CUDA_TRY(launch_ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad,
-                                  0, ~uint64_t(0), nullptr));
+      CUDA_TRY(ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad, 0,
+                           ~uint64_t(0), nullptr));
   }
   if (!h->sense_dev) CUDA_TRY(cudaMalloc(&h->sense_dev, sizeof(ObsDelay)));
   ObsDelay O;
@@ -1711,15 +1761,10 @@ int upkie_b200_get_observation_delay_state(void* handle, uint32_t* count, uint32
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
-  if (h->sense_count) {
-    CUDA_TRY(cudaMemcpyAsync(count, h->sense_count, bytes, cudaMemcpyDeviceToDevice, s));
-    CUDA_TRY(cudaMemcpyAsync(delay, h->sense_delay, bytes, cudaMemcpyDeviceToDevice, s));
-  } else {
-    CUDA_TRY(cudaMemsetAsync(count, 0, bytes, s));
-    CUDA_TRY(cudaMemsetAsync(delay, 0, bytes, s));
-  }
+  CUDA_TRY(copy_or_zero(count, h->sense_count, bytes, s));
+  CUDA_TRY(copy_or_zero(delay, h->sense_delay, bytes, s));
   // a handle without a state: the current state, what its first spec would fill the rows with
-  CUDA_TRY(launch_sensed_rows(h->sense_rows ? h->sense_rows : h->state, h->n, h->n_pad, rows, s));
+  CUDA_TRY(ring_rows(h->sense_rows ? h->sense_rows : h->state, UPKIE_STATE_DIM, h->n, h->n_pad, rows, s));
   return UPKIE_B200_OK;
 }
 
@@ -1734,7 +1779,7 @@ int upkie_b200_set_observation_delay_state(void* handle, const uint32_t* count, 
   const size_t bytes = size_t(h->n) * sizeof(uint32_t);
   CUDA_TRY(cudaMemcpyAsync(h->sense_count, count, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(h->sense_delay, delay, bytes, cudaMemcpyDeviceToDevice, s));
-  CUDA_TRY(launch_sensed_cols(rows, h->n, h->n_pad, h->sense_rows, s));
+  CUDA_TRY(ring_cols(rows, UPKIE_STATE_DIM, h->n, h->n_pad, h->sense_rows, s));
   return UPKIE_B200_OK;
 }
 
@@ -1744,10 +1789,10 @@ int upkie_b200_get_observation_delay_history(void* handle, float* rows, void* st
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (h->sense_hist)
-    CUDA_TRY(launch_ring_rows(h->sense_hist, h->sense_head, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad,
-                              h->sense_ticks, rows, s));
+    CUDA_TRY(ring_rows(h->sense_hist, UPKIE_STATE_DIM, h->n, h->n_pad, rows, s, h->sense_head, h->sense_ticks,
+                       h->sense_ticks));
   else  // depth 1: the sensed rows are the newest snapshot (as get_observation_delay_state)
-    CUDA_TRY(launch_sensed_rows(h->sense_rows ? h->sense_rows : h->state, h->n, h->n_pad, rows, s));
+    CUDA_TRY(ring_rows(h->sense_rows ? h->sense_rows : h->state, UPKIE_STATE_DIM, h->n, h->n_pad, rows, s));
   return UPKIE_B200_OK;
 }
 
@@ -1758,10 +1803,10 @@ int upkie_b200_set_observation_delay_history(void* handle, const float* rows, vo
   if (alloc_sense_state(h)) return UPKIE_B200_ECUDA;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (h->sense_hist)
-    CUDA_TRY(launch_ring_cols(rows, h->sense_head, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad, h->sense_ticks,
-                              h->sense_hist, s));
+    CUDA_TRY(ring_cols(rows, UPKIE_STATE_DIM, h->n, h->n_pad, h->sense_hist, s, h->sense_head, h->sense_ticks,
+                       h->sense_ticks));
   else
-    CUDA_TRY(launch_sensed_cols(rows, h->n, h->n_pad, h->sense_rows, s));
+    CUDA_TRY(ring_cols(rows, UPKIE_STATE_DIM, h->n, h->n_pad, h->sense_rows, s));
   return UPKIE_B200_OK;
 }
 
