@@ -812,6 +812,52 @@ int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationD
 int upkie_b200_get_observation_delay_history(void* handle, float* rows, void* stream);
 int upkie_b200_set_observation_delay_history(void* handle, const float* rows, void* stream);
 
+/* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
+ * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last
+ * K substeps of chosen columns of its spine observation, as a HistoryObserver in the spine's observer pipeline reports
+ * its vector of the last `size` values of a key (HistoryObserver::read_value pushes each cycle's value to the front).
+ * At 1 kHz, where a tick is one substep, it is plain per-tick frame stacking.
+ * Spec: `count` = C columns of the spine observation row (UPKIE_SP_*, 0 .. UPKIE_SPINE_DIM - 1), 1 <= C <=
+ * UPKIE_MAX_HISTORY_CHANNELS, and `size` = K entries, 1 <= K <= UPKIE_MAX_HISTORY.
+ * - After a step, entry 0 (the newest) holds each column as it was after the tick's last substep, and entry k as it
+ *   was k substeps earlier; entries cross tick boundaries when K > nb_substeps. Newest first, as HistoryObserver.
+ * - Every column has the arithmetic of upkie_b200_spine_obs applied to the state after that substep, except two:
+ *   the IMU linear and raw accelerations differentiate the IMU velocity over one substep dt / nb_substeps, as a 1 kHz
+ *   spine does (the tick's own observation keeps its difference over dt), and the servo torques are those applied in
+ *   the substep, without measurement noise. No IMU uncertainty is added.
+ * - Under an observation delay of d substeps, entry 0 is the instant the observation reports, d substeps before the
+ *   end of the tick, and the window moves back with it: entry 0 then equals the delayed spine observation's columns
+ *   (but for the two exceptions above). The ring holds K + max_ticks * nb_substeps entries, max_ticks the observation
+ *   delay's depth (1 without upkie_b200_set_observation_delay_ticks).
+ * - Every reset of an env (fused next-step or same-step auto-reset, upkie_b200_reset with or without a mask) fills all
+ *   of that env's entries with its post-reset observation's columns (IMU acceleration: the reset's); the other envs
+ *   keep theirs. The reference's HistoryObserver keeps its vector across a spine reset: here a new episode starts
+ *   without the previous episode's samples. A new spec, upkie_b200_set_state, and a change of the ring's size (a new
+ *   observation-delay depth, a new nb_substeps) fill every env's entries from the current state in the same way.
+ * - The history records only: observations, rewards, terminations, truncations, final_obs, the final spine
+ *   observation, the state and every draw are those of the same handle without a history. It runs in the kernels of
+ *   the observation delay (FAM_SENSE), so it needs joint_limits != 0 and is rejected with spine_mode (whose spine
+ *   reports lagged replies) and with body_contacts; the in-kernel rollout transports reject a handle with a history.
+ * upkie_b200_set_history: NULL turns it off (the ring is freed once the device is idle); an invalid spec returns
+ * UPKIE_B200_EINVAL and keeps the previous one. upkie_b200_set_config rejects joint_limits = 0 and body_contacts while
+ * a history is set. The set call waits for the device. upkie_b200_get_history: out[N][K][C] (device pointer), env i's
+ * entries newest first; without a history, UPKIE_B200_EINVAL. Checkpoints: upkie_b200_get_history_state /
+ * set_history_state copy the whole ring in age order, rows[ticks][N][C] with ticks = upkie_b200_history_entries (age 0
+ * the entry the last substep wrote); the ring's head is implied by the age order. */
+#define UPKIE_MAX_HISTORY 64
+#define UPKIE_MAX_HISTORY_CHANNELS 16
+typedef struct UpkieHistory {
+  uint32_t size;                                /* K, entries reported */
+  uint32_t count;                               /* C, columns */
+  int32_t columns[UPKIE_MAX_HISTORY_CHANNELS];  /* UPKIE_SP_* columns, the first `count` used */
+} UpkieHistory;
+int upkie_b200_set_history(void* handle, const UpkieHistory* spec);
+int upkie_b200_get_history(void* handle, float* out, void* stream);
+int upkie_b200_history_entries(void* handle, int* ticks);
+int upkie_b200_get_history_state(void* handle, float* rows, void* stream);
+int upkie_b200_set_history_state(void* handle, const float* rows, void* stream);
+
 /* Number of step-kernel launches issued through this handle since create
  * (bench.py's `gpu_launches`). */
 int upkie_b200_launch_count(void* handle, uint64_t* count);

@@ -401,6 +401,21 @@ class UpkieObservationDelay(C.Structure):
     ]
 
 
+MAX_HISTORY = 64  # UPKIE_MAX_HISTORY: the most entries an observation history reports
+MAX_HISTORY_CHANNELS = 16  # UPKIE_MAX_HISTORY_CHANNELS: the most spine columns it records
+
+
+class UpkieHistory(C.Structure):
+    """``UpkieHistory`` of include/upkie_b200.h: the spine-observation columns an observation history records
+    (``SP_*``, the first ``count`` of ``columns``) and the entries it reports (``size``)."""
+
+    _fields_ = [
+        ("size", C.c_uint32),
+        ("count", C.c_uint32),
+        ("columns", C.c_int32 * MAX_HISTORY_CHANNELS),
+    ]
+
+
 def default_mpc_config() -> UpkieMpcConfig:
     """``MPCBalancer.__init__`` defaults (``mpc_balancer.py:168-181``)."""
     c = UpkieMpcConfig()

@@ -59,6 +59,11 @@ SYMBOLS = {
     "upkie_b200_set_observation_delay_ticks": (C.c_int, [_vp, C.POINTER(_abi.UpkieObservationDelay), C.c_uint32]),
     "upkie_b200_get_observation_delay_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_set_observation_delay_history": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_history": (C.c_int, [_vp, C.POINTER(_abi.UpkieHistory)]),
+    "upkie_b200_get_history": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_history_entries": (C.c_int, [_vp, C.POINTER(C.c_int)]),
+    "upkie_b200_get_history_state": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_history_state": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_reset": (C.c_int, [_vp, _vp, _vp, C.c_uint64, C.c_uint64, _vp]),
     "upkie_b200_step_servos": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_step_gyropod": (C.c_int, [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp, _vp]),

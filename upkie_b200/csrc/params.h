@@ -266,6 +266,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.push = nullptr;
   P.action_delay = nullptr;
   P.obs_delay = nullptr;
+  P.history = nullptr;
   return 0;
 }
 
@@ -373,6 +374,21 @@ inline const char* obs_delay_spec_error(const UpkieObservationDelay& s, const Si
     return "set_observation_delay: needs joint_limits != 0 (the delay runs in a copy of the table kernels)";
   if (P.spine_mode) return "set_observation_delay: spine_mode models the spine's own lag";
   if (P.body_contacts) return "set_observation_delay: body_contacts has no observation-delay kernels";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses a history spec (upkie_b200_set_history), null when it takes it
+inline const char* history_spec_error(const UpkieHistory& s, const SimParams& P) {
+  if (s.count < 1 || s.count > UPKIE_MAX_HISTORY_CHANNELS)
+    return "set_history: count outside 1 .. UPKIE_MAX_HISTORY_CHANNELS";
+  if (s.size < 1 || s.size > UPKIE_MAX_HISTORY) return "set_history: size outside 1 .. UPKIE_MAX_HISTORY";
+  for (uint32_t c = 0; c < s.count; ++c)
+    if (s.columns[c] < 0 || s.columns[c] >= UPKIE_SPINE_DIM)
+      return "set_history: a column outside 0 .. UPKIE_SPINE_DIM - 1";
+  if (P.joint_limits == 0)
+    return "set_history: needs joint_limits != 0 (the history runs in the observation-delay kernels)";
+  if (P.spine_mode) return "set_history: spine_mode reports the spine's lagged replies, which the history does not record";
+  if (P.body_contacts) return "set_history: body_contacts has no observation-history kernels";
   return nullptr;
 }
 

@@ -144,6 +144,9 @@ struct SimParams {
   // observation-delay randomisation (upkie_b200_set_observation_delay): the handle's device block, null = off. Read by
   // the step kernels of FAM_SENSE (step_family.h) only. Appended last, as action_delay above.
   const struct ObsDelay* obs_delay;
+  // spine-rate observation history (upkie_b200_set_history): the handle's device block, null = off. Read by the step
+  // kernels of FAM_SENSE (step_family.h) and k_reset only. Appended last, as obs_delay above.
+  const struct History* history;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -1970,6 +1973,119 @@ UPKIE_HD void obs_delay_fill_history(const ObsDelay& O, int i, const float r[UPK
   const size_t stride = size_t(O.stride);
   for (int s = 0; s < O.ticks; ++s)
     for (int k = 0; k < UPKIE_STATE_DIM; ++k) col[(size_t(s) * UPKIE_STATE_DIM + k) * stride] = r[k];
+}
+
+// ---- spine-rate observation history (upkie_b200_set_history, HistoryObserver.h) ----
+// The handle's device block: the spec and the ring. ring [ticks][count][stride], env i in column i: each entry holds
+// the `count` selected columns of the env's spine observation after one substep, and head[i] is the entry the env's
+// next substep writes. Every step moves every env's head on by nb_substeps, a resetting env's included (its reset
+// refills the whole ring), and nothing else moves them: all envs sit on the same entry, and a warp's stores are
+// coalesced rows (the rule of delay_ring_advance).
+struct History {
+  int size;    // K, the entries a read reports
+  int count;   // C, the columns of an entry
+  int ticks;   // entries of the ring: K + (the observation delay's depth) * nb_substeps
+  int stride;
+  int acc;     // 1: some column is an IMU acceleration, which the substeps differentiate
+  int columns[UPKIE_MAX_HISTORY_CHANNELS];
+  float* ring;
+  uint32_t* head;
+};
+
+// Whether spine column `col` is an IMU acceleration (linear or raw)
+UPKIE_HD constexpr bool history_acc_column(int col) {
+  return col >= UPKIE_SP_IMU_LINACC && col < UPKIE_SP_IMU_RAWACC + 3;
+}
+
+// t[k] of a short array for a runtime k, as unrolled selects (an indexed read would put the array in local memory)
+template <int N>
+UPKIE_HD float history_pick(const float (&t)[N], int k) {
+  float v = t[0];
+#pragma unroll
+  for (int j = 1; j < N; ++j) v = k == j ? t[j] : v;
+  return v;
+}
+
+// Column `col` of the spine observation of S (spine_observation's arithmetic, that column only), with `acc` as the
+// IMU acceleration and the commanded torques without measurement noise
+UPKIE_HD float history_value(const SimParams& P, const RobotState& S, const float acc[3], int col) {
+  if (col >= UPKIE_SP_BASE_LINVEL && col < UPKIE_SP_PITCH) return history_pick(S.linvel, col - UPKIE_SP_BASE_LINVEL);
+  if (col == UPKIE_SP_PITCH) return base_pitch(S);
+  if (col == UPKIE_SP_CONTACT) return S.contact;
+  if (col >= UPKIE_SP_SERVO && col < UPKIE_SP_ODOM_POS) {
+    const int j = (col - UPKIE_SP_SERVO) / UPKIE_OBS_KEYS, key = (col - UPKIE_SP_SERVO) % UPKIE_OBS_KEYS;
+    if (key == UPKIE_OBS_POSITION) return history_pick(S.q, j);
+    if (key == UPKIE_OBS_VELOCITY) return history_pick(S.qd, j);
+    if (key == UPKIE_OBS_TORQUE) return history_pick(S.torque, j);
+    return key == UPKIE_OBS_TEMPERATURE ? 42.0f : 18.0f;
+  }
+  const float signed_radius = P.left_sign * P.wheel_radius;
+  if (col == UPKIE_SP_ODOM_POS) return 0.5f * (S.q[2] - S.q[5]) * signed_radius;
+  if (col == UPKIE_SP_ODOM_VEL) return 0.5f * (S.qd[2] - S.qd[5]) * signed_radius;
+  float R[9];
+  quat_to_rot(S.quat, R);
+  if (col < UPKIE_SP_BASE_LINVEL) {
+    float om_b[3];
+    rot_tmul(R, S.angvel, om_b);
+    return history_pick(om_b, col - UPKIE_SP_BASE_ANGVEL);
+  }
+  if (col < UPKIE_SP_IMU_QUAT) return history_pick(R, col - UPKIE_SP_ROT);
+  float Riw[9];
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+      Riw[3 * i + j] = R[3 * i + 0] * P.Rbi[3 * j + 0] + R[3 * i + 1] * P.Rbi[3 * j + 1] + R[3 * i + 2] * P.Rbi[3 * j + 2];
+  if (col < UPKIE_SP_IMU_ANGVEL) {
+    float Ria[9];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+      Ria[j] = Riw[j];
+      Ria[3 + j] = -Riw[3 + j];
+      Ria[6 + j] = -Riw[6 + j];
+    }
+    float q[4];
+    quat_from_rot(Ria, q);
+    return history_pick(q, col - UPKIE_SP_IMU_QUAT);
+  }
+  float t[3];
+  if (col < UPKIE_SP_IMU_LINACC) {
+    rot_tmul(Riw, S.angvel, t);
+    return history_pick(t, col - UPKIE_SP_IMU_ANGVEL);
+  }
+  if (col < UPKIE_SP_IMU_RAWACC) {
+    rot_tmul(Riw, acc, t);
+    return history_pick(t, col - UPKIE_SP_IMU_LINACC);
+  }
+  const float praw[3] = {acc[0], acc[1], acc[2] + 9.81f};
+  rot_tmul(Riw, praw, t);
+  return history_pick(t, col - UPKIE_SP_IMU_RAWACC);
+}
+
+// One entry of env i's ring, `e`: the columns of S with IMU acceleration `acc`, column(c) the spine column of channel c
+// (the CPU build's record of a substep; the step kernels' history_substep stores the same values)
+template <typename Column>
+UPKIE_HD void history_store(const History& H, const SimParams& P, const RobotState& S, const float acc[3], uint32_t e,
+                            int i, Column column) {
+  float* const col = H.ring + size_t(e) * size_t(H.count) * size_t(H.stride) + size_t(i);
+  for (int c = 0; c < H.count; ++c) col[size_t(c) * size_t(H.stride)] = history_value(P, S, acc, column(c));
+}
+
+// A reset of env i (both fused auto-resets, k_reset), a new spec or a state set: every entry of the ring becomes the
+// columns of S, the IMU acceleration that of the state (what the observation of S reports)
+UPKIE_HD void history_fill(const History& H, const SimParams& P, const RobotState& S, int i) {
+  float* const col = H.ring + size_t(i);
+  const size_t stride = size_t(H.stride), entry = size_t(H.count) * stride;
+  for (int c = 0; c < H.count; ++c) {
+    const float v = history_value(P, S, S.imu_acc, H.columns[c]);
+    for (int e = 0; e < H.ticks; ++e) col[size_t(e) * entry + size_t(c) * stride] = v;
+  }
+}
+
+// The ring entry of history entry k (0 the newest) of an env whose next write is entry `head`, observed `d` substeps
+// before the end of the tick (the observation delay in force; 0 without one)
+UPKIE_HD uint32_t history_entry(uint32_t head, uint32_t ticks, uint32_t d, uint32_t k) {
+  return (head + 2u * ticks - 1u - d - k) % ticks;
 }
 
 }  // namespace upkie_b200

@@ -130,6 +130,32 @@ __device__ __forceinline__ float* obs_delay_report(const ObsDelay& O, uint32_t s
   return row;
 }
 
+// The observation history (F.sense kernels, P.history set): one substep's entry `e` of the lane's ring column, with the
+// IMU velocity differentiated over the substep against `vel` (updated in place) when `acc`; and the fill of the whole
+// column with the columns of S. Out of line: the calls pass a copy of the state, and the kernel's own arithmetic is
+// compiled (and its products contracted) as without the history.
+__device__ __noinline__ void history_substep(const SimParams& P, const RobotState S, float* vel, float* e,
+                                             size_t stride, int count, bool acc) {
+  float a[3] = {0.f, 0.f, 0.f};
+  if (acc) {
+    float v[3];
+    imu_velocity(P, S, v);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      a[k] = (v[k] - vel[k]) * P.inv_h;  // one substep, as a 1 kHz spine differentiates
+      vel[k] = v[k];
+    }
+  }
+  for (int c = 0; c < count; ++c) __stcg(e + size_t(c) * stride, history_value(P, S, a, __ldg(P.history->columns + c)));
+}
+__device__ __noinline__ void history_fill_lane(const SimParams& P, const RobotState S, float* col, size_t stride,
+                                               int count, uint32_t ticks) {
+  for (int c = 0; c < count; ++c) {
+    const float v = history_value(P, S, S.imu_acc, __ldg(P.history->columns + c));
+    for (uint32_t e = 0; e < ticks; ++e) __stcg(col + (size_t(e) * size_t(count) + size_t(c)) * stride, v);
+  }
+}
+
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE >= 1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), during the substeps each lane's clamped row, and it is reused to transpose the
@@ -377,6 +403,29 @@ __device__ __forceinline__ void step_env(
     imu_velocity(P, S, v);
     obs_delay_snapshot(P, S, v, sense_load, sense_store);
   }
+  // spine-rate observation history (F.sense kernels, P.history set: a uniform branch). Each substep of a lane that does
+  // not reset stores the selected spine columns of its state into ring entry (head + sub) % ticks, differentiating the
+  // IMU velocity over the substep against the previous substep's, kept in the lane's frame (the tick starts from the
+  // velocity the last observation update stored). A lane that resets fills its whole ring after the tick instead. The
+  // ring's address, stride and shape are read into registers once, and the columns through the read-only path (the
+  // block is not written while a step runs).
+  const bool recording = F.sense && P.history;
+  float* hring = nullptr;
+  size_t hstride = 0;
+  uint32_t hhead = 0, hticks = 1;
+  int hcount = 0;
+  bool hacc = false;
+  float hvel[3] = {S.prev_imu_vel[0], S.prev_imu_vel[1], S.prev_imu_vel[2]};
+  bool refill = resetting;  // this tick resets the lane: its ring is filled with the post-reset columns
+  if (recording) {
+    const History& H = *P.history;
+    hring = H.ring + size_t(i);
+    hstride = size_t(H.stride);
+    hticks = uint32_t(H.ticks);
+    hcount = H.count;
+    hacc = H.acc != 0;
+    hhead = __ldcg(H.head + i);
+  }
   if (spine && !resetting) spine_assemble_observation(S, L);  // the first cycle's observation (Spine.cpp:126-131)
   const int nloop = (AUTORESET == AUTORESET_NEXT_STEP && spine && P.nb_substeps < 3) ? 3 : P.nb_substeps;
   for (int sub = 0; sub < nloop; ++sub) {
@@ -411,6 +460,9 @@ __device__ __forceinline__ void step_env(
         imu_velocity(P, S, v);
         obs_delay_snapshot(P, S, v, sense_load, sense_store);
       }
+      if (recording && !resetting && live)
+        history_substep(P, S, hvel, hring + size_t((hhead + uint32_t(sub)) % hticks) * size_t(hcount) * hstride,
+                        hstride, hcount, hacc);
     } else {
 #pragma unroll
       for (int k = 0; k < kPhaseSyncs; ++k) PhaseSync()();
@@ -487,6 +539,7 @@ __device__ __forceinline__ void step_env(
       // the terminal step was observed under its delay; the reset is observed undelayed, with a new draw
       if (sensing && live) obs_delay_reset(*P.obs_delay, seed, env_offset + uint64_t(i), i);
       elapsed = 0;
+      refill = true;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
       float init[UPKIE_INIT_DIM];
@@ -504,6 +557,12 @@ __device__ __forceinline__ void step_env(
   }
 
   if (live) store_state(state, n_pad, i, S);
+  // the history: a reset fills the lane's ring from its post-reset state (the true state, here in S), and every lane's
+  // head moves on by the tick's substeps
+  if (recording && live) {
+    if (refill) history_fill_lane(P, S, hring, hstride, hcount, hticks);
+    __stcg(P.history->head + i, (hhead + uint32_t(P.nb_substeps)) % hticks);
+  }
   if (sensing) {
     // K > 1: the sensed row becomes the report, and the end of the tick works on it as for one tick
     if (HIST && !resetting && P.obs_delay->ticks > 1) scol = obs_delay_report(*P.obs_delay, srep, i, live);

@@ -11,6 +11,7 @@
 //   k_reset        masked reset: set state, one physics substep, observe; the randomisations' per-env state restarts.
 //   k_spine_obs    spine observations of the state, or of the same-step auto-resets' terminal step from the stash.
 //   k_ring_copy    rows <-> struct-of-arrays columns of every per-env buffer, and the delay histories.
+//   k_history_read / k_history_fill   the observation history's entries of each env / its ring filled from the state.
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -126,6 +127,13 @@ struct Handle {
   int sense_ticks = 1;             // the history depth (upkie_b200_set_observation_delay_ticks)
   float* sense_hist = nullptr;     // sense_ticks > 1: [sense_ticks][UPKIE_STATE_DIM][n_pad], a ring of snapshots
   uint32_t* sense_head = nullptr;  // the ring row each env's next tick writes
+  // spine-rate observation history (upkie_b200_set_history): the device block P.history points to while a spec is set,
+  // and its ring [hist_ticks][spec.count][n_pad] and per-env heads (allocated with the spec, freed when it is turned off)
+  History* hist_dev = nullptr;
+  UpkieHistory hist_spec = {};
+  int hist_ticks = 0;
+  float* hist_ring = nullptr;
+  uint32_t* hist_head = nullptr;
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -217,6 +225,37 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
     for (int k = 0; k < UPKIE_STATE_DIM; ++k) col[size_t(k) * size_t(O.stride)] = r[k];
     if (O.ticks > 1) obs_delay_fill_history(O, i, r);
   }
+  if (P.history) history_fill(*P.history, P, S, i);  // a new episode's history starts from its post-reset columns
+}
+
+// The observation history of every env, out[n][size][count], entries newest first: the window ends `d` substeps
+// before the end of the tick, the env's observation delay when one is set (clamped as the step kernels clamp it)
+__global__ void k_history_read(const __grid_constant__ SimParams P, const History* __restrict__ H, int n,
+                               float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t ticks = uint32_t(H->ticks), size = uint32_t(H->size), count = uint32_t(H->count);
+  uint32_t d = 0;
+  if (P.obs_delay) {
+    const uint32_t cap = uint32_t(P.obs_delay->ticks > 1 ? P.obs_delay->ticks : 1) * uint32_t(P.nb_substeps);
+    d = min(P.obs_delay->delay[i], cap);
+    d = min(d, ticks - size);
+  }
+  const uint32_t head = H->head[i];
+  for (uint32_t k = 0; k < size; ++k) {
+    const float* const e = H->ring + size_t(history_entry(head, ticks, d, k)) * count * size_t(H->stride) + size_t(i);
+    for (uint32_t c = 0; c < count; ++c) out[(size_t(i) * size + k) * count + c] = e[size_t(c) * size_t(H->stride)];
+  }
+}
+
+// Every env's history filled from its state (a new spec, set_state, a new ring size)
+__global__ void k_history_fill(const __grid_constant__ SimParams P, const History* __restrict__ H, int n, int n_pad,
+                               const float* __restrict__ state) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  RobotState S;
+  load_state(state, n_pad, i, S);
+  history_fill(*H, P, S, i);
 }
 
 // The spine observation rows of the states `state` (and in spine mode the lag records `lag`), with the noise keys of
@@ -718,6 +757,52 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
   return UPKIE_B200_OK;
 }
 
+// The entries the observation history's ring holds: K, and the deepest observation delay the handle may draw
+int history_ticks(const Handle* h) {
+  return int(h->hist_spec.size) + (h->sense_ticks > 1 ? h->sense_ticks : 1) * h->P.nb_substeps;
+}
+
+// The observation history of the spec h->hist_spec: its device block, ring (history_ticks entries) and heads, every
+// entry filled from the current state. Waits for the device.
+int history_build(Handle* h) {
+  const UpkieHistory& spec = h->hist_spec;
+  const int ticks = history_ticks(h);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the ring
+  h->P.history = nullptr;
+  cudaFree(h->hist_ring);
+  h->hist_ring = nullptr;
+  CUDA_TRY(cudaMalloc(&h->hist_ring, size_t(ticks) * spec.count * h->n_pad * sizeof(float)));
+  if (!h->hist_head) CUDA_TRY(cudaMalloc(&h->hist_head, size_t(h->n) * sizeof(uint32_t)));
+  CUDA_TRY(cudaMemset(h->hist_head, 0, size_t(h->n) * sizeof(uint32_t)));
+  if (!h->hist_dev) CUDA_TRY(cudaMalloc(&h->hist_dev, sizeof(History)));
+  History H;
+  std::memset(&H, 0, sizeof(H));
+  H.size = int(spec.size);
+  H.count = int(spec.count);
+  H.ticks = ticks;
+  H.stride = h->n_pad;
+  for (uint32_t c = 0; c < spec.count; ++c) {
+    H.columns[c] = spec.columns[c];
+    if (history_acc_column(spec.columns[c])) H.acc = 1;
+  }
+  H.ring = h->hist_ring;
+  H.head = h->hist_head;
+  CUDA_TRY(cudaMemcpy(h->hist_dev, &H, sizeof(H), cudaMemcpyHostToDevice));
+  h->hist_ticks = ticks;
+  h->P.history = h->hist_dev;
+  k_history_fill<<<grid_of(h->n), 128>>>(h->P, h->hist_dev, h->n, h->n_pad, h->state);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaDeviceSynchronize());
+  return UPKIE_B200_OK;
+}
+
+// After a change of nb_substeps or of the observation delay's depth: a ring of the new size, filled from the state
+int history_resize(Handle* h) {
+  if (!h->P.history || history_ticks(h) == h->hist_ticks) return UPKIE_B200_OK;
+  return history_build(h);
+}
+
 }  // namespace
 
 // ---- C ABI ----------------------------------------------------------------------------
@@ -849,6 +934,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->delay_head);
   cudaFree(h->sense_dev); cudaFree(h->sense_count); cudaFree(h->sense_delay); cudaFree(h->sense_rows);
   cudaFree(h->sense_hist); cudaFree(h->sense_head);
+  cudaFree(h->hist_dev); cudaFree(h->hist_ring); cudaFree(h->hist_head);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -888,6 +974,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: nb_substeps below the observation delay's substeps_high");
   if (h->P.obs_delay && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no observation-delay kernels");
+  if (h->P.history && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: the observation history needs joint_limits != 0");
+  if (h->P.history && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no observation-history kernels");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -907,6 +997,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.push = h->P.push;              // and the push randomisation
   P.action_delay = h->P.action_delay;  // and the action delay
   P.obs_delay = h->P.obs_delay;        // and the observation delay
+  P.history = h->P.history;            // and the observation history
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -918,7 +1009,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   // kernels read the parameter block by value at launch: steps already enqueued keep the old one
   h->P = P;
   h->config_flags = config_flags;
-  return UPKIE_B200_OK;
+  return history_resize(h);  // a new nb_substeps changes the ring's size
 }
 
 int upkie_b200_set_env_params(void* handle, const float* rows, void* stream) {
@@ -1377,6 +1468,12 @@ int upkie_b200_set_state(void* handle, const float* state, void* stream) {
       CUDA_TRY(ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad, 0,
                            ~uint64_t(0), static_cast<cudaStream_t>(stream)));
   }
+  // the observation history restarts from the state set
+  if (h->P.history) {
+    k_history_fill<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->P.history, h->n, h->n_pad,
+                                                                                 h->state);
+    CUDA_TRY(cudaGetLastError());
+  }
   return UPKIE_B200_OK;
 }
 
@@ -1751,7 +1848,7 @@ int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationD
   CUDA_TRY(cudaDeviceSynchronize());
   h->sense_high = spec->substeps_high;
   h->P.obs_delay = h->sense_dev;
-  return UPKIE_B200_OK;
+  return history_resize(h);  // a new depth changes the observation history's ring
 }
 
 int upkie_b200_get_observation_delay_state(void* handle, uint32_t* count, uint32_t* delay, float* rows, void* stream) {
@@ -1807,6 +1904,64 @@ int upkie_b200_set_observation_delay_history(void* handle, const float* rows, vo
                        h->sense_ticks));
   else
     CUDA_TRY(ring_cols(rows, UPKIE_STATE_DIM, h->n, h->n_pad, h->sense_rows, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_history(void* handle, const UpkieHistory* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    if (h->P.history) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the ring
+      h->P.history = nullptr;
+      cudaFree(h->hist_ring);
+      cudaFree(h->hist_head);
+      h->hist_ring = nullptr;
+      h->hist_head = nullptr;
+      h->hist_ticks = 0;
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = history_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  h->hist_spec = *spec;
+  return history_build(h);
+}
+
+int upkie_b200_get_history(void* handle, float* out, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !out) return fail(UPKIE_B200_EINVAL, "get_history: invalid argument");
+  if (!h->P.history) return fail(UPKIE_B200_EINVAL, "get_history: no history is set (upkie_b200_set_history)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  k_history_read<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->P.history, h->n, out);
+  CUDA_TRY(cudaGetLastError());
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_history_entries(void* handle, int* ticks) {
+  Handle* h = as_handle(handle);
+  if (!h || !ticks) return fail(UPKIE_B200_EINVAL, "history_entries: invalid argument");
+  *ticks = h->P.history ? h->hist_ticks : 0;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_history_state(void* handle, float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !rows) return fail(UPKIE_B200_EINVAL, "get_history_state: invalid argument");
+  if (!h->P.history) return fail(UPKIE_B200_EINVAL, "get_history_state: no history is set (upkie_b200_set_history)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(ring_rows(h->hist_ring, int(h->hist_spec.count), h->n, h->n_pad, rows, static_cast<cudaStream_t>(stream),
+                     h->hist_head, h->hist_ticks, h->hist_ticks));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_history_state(void* handle, const float* rows, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !rows) return fail(UPKIE_B200_EINVAL, "set_history_state: invalid argument");
+  if (!h->P.history) return fail(UPKIE_B200_EINVAL, "set_history_state: no history is set (upkie_b200_set_history)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(ring_cols(rows, int(h->hist_spec.count), h->n, h->n_pad, h->hist_ring, static_cast<cudaStream_t>(stream),
+                     h->hist_head, h->hist_ticks, h->hist_ticks));
   return UPKIE_B200_OK;
 }
 

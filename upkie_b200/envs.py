@@ -163,14 +163,21 @@ class SpineObservations:
     ``obs[i]`` returns the reference's nested dictionary for env ``i``
     (``pybullet_backend.py:325-331``); ``obs.array`` the flat ``[N, 62]`` array,
     ``obs.tensor`` the same rows as a CUDA tensor (no host copy).
+
+    With an observation history (``B200VectorEnv(history=...)``), ``obs.history`` is the batched ``[N, K, C]`` CUDA
+    tensor of ``UpkieSim.get_history`` and ``obs[i]`` has a ``"history"`` subtree in ``HistoryObserver``'s layout (the
+    key path of each recorded value holds its ``K`` values, newest first), fetched and stale-checked like ``.tensor``.
     """
 
     _key = "info['spine_observation']"
 
-    def __init__(self, sim: UpkieSim):
+    def __init__(self, sim: UpkieSim, history_layout: Optional[list] = None):
         self._sim = sim
         self._tensor = None
         self._array = None
+        self._history_layout = history_layout  # [(key path, first column in the history, shape)], None = no history
+        self._history = None
+        self._history_array = None
         self._stamp = sim.launches  # step kernels launched so far: identifies the tick this object belongs to
 
     def _fetch(self) -> torch.Tensor:
@@ -193,11 +200,33 @@ class SpineObservations:
             self._array = self.tensor.cpu().numpy()
         return self._array
 
+    def _check_stamp(self) -> None:
+        if self._sim.launches != self._stamp:
+            # the simulator has moved on: fetching now would silently return a LATER tick's history
+            raise UpkieRuntimeError(
+                f"{self._key} is fetched lazily and the simulator has been stepped since this step: "
+                "read it (e.g. `.history`) before calling step() again")
+
+    @property
+    def history(self) -> torch.Tensor:
+        """``[N, K, C]`` the observation history of every env (``UpkieSim.get_history``), newest entry first."""
+        if self._history_layout is None:
+            raise UpkieException(f"{self._key}: the env records no history (B200VectorEnv(history=...))")
+        if self._history is None:
+            self._check_stamp()
+            self._history = self._sim.get_history()
+        return self._history
+
     def __len__(self):
         return self._sim.n
 
     def __getitem__(self, i: int) -> dict:
-        return spine_row_to_dict(self.array[i])
+        d = spine_row_to_dict(self.array[i])
+        if self._history_layout is not None:
+            if self._history_array is None:
+                self._history_array = self.history.cpu().numpy()
+            d["history"] = history_to_dict(self._history_layout, self._history_array[i])
+        return d
 
 
 class FinalSpineObservations(SpineObservations):
@@ -207,6 +236,9 @@ class FinalSpineObservations(SpineObservations):
     mask are stale."""
 
     _key = "info['final_info']['spine_observation']"
+
+    def __init__(self, sim: UpkieSim):
+        super().__init__(sim)  # no history: the terminal step's history is not kept
 
     def _fetch(self) -> torch.Tensor:
         return self._sim.final_spine_obs()
@@ -238,6 +270,87 @@ def spine_row_to_dict(r: np.ndarray) -> dict:
         },
         "wheel_odometry": {"position": float(r[A.SP_ODOM_POS]), "velocity": float(r[A.SP_ODOM_VEL])},
     }
+
+
+# The spine observation's keys (spine_row_to_dict's table) as key path -> (first column, shape of the value): the
+# history records these columns, a vector or matrix key all of its columns
+def _history_keys() -> dict:
+    A = _abi
+    keys = {
+        ("base_orientation", "angular_velocity"): (A.SP_BASE_ANGVEL, (3,)),
+        ("base_orientation", "linear_velocity"): (A.SP_BASE_LINVEL, (3,)),
+        ("base_orientation", "pitch"): (A.SP_PITCH, ()),
+        ("base_orientation", "rotation_base_to_world"): (A.SP_ROT, (3, 3)),
+        ("floor_contact", "contact"): (A.SP_CONTACT, ()),
+        ("imu", "orientation"): (A.SP_IMU_QUAT, (4,)),
+        ("imu", "angular_velocity"): (A.SP_IMU_ANGVEL, (3,)),
+        ("imu", "linear_acceleration"): (A.SP_IMU_LINACC, (3,)),
+        ("imu", "raw_linear_acceleration"): (A.SP_IMU_RAWACC, (3,)),
+        ("wheel_odometry", "position"): (A.SP_ODOM_POS, ()),
+        ("wheel_odometry", "velocity"): (A.SP_ODOM_VEL, ()),
+    }
+    for j, name in enumerate(A.JOINT_NAMES):
+        for k, key in enumerate(A.OBS_KEYS):
+            keys[("servo", name, key)] = (A.SP_SERVO + j * len(A.OBS_KEYS) + k, ())
+    return keys
+
+
+_CONSTANT_KEYS = ("temperature", "voltage")  # servo keys the simulation reports as constants
+
+
+def history_spec(keys, size: int = 1, spine_mode: bool = False, joint_limits: int = 3,
+                 body_contacts: bool = False) -> Optional[Tuple[list, int, list]]:
+    """``(columns, size, layout)`` of an observation history from key paths of the spine observation dictionary,
+    e.g. ``("imu", "angular_velocity")``, ``("base_orientation", "pitch")``, ``("servo", "left_wheel", "velocity")``
+    (tuples, or strings with ``/`` between the keys). A vector key records its 3 (or 4) columns, the rotation matrix its
+    9. ``layout`` lists ``(key path, first column in the history, shape)``. None for ``keys=None``. Raises on an unknown
+    key, a constant servo key (temperature, voltage), more than ``MAX_HISTORY_CHANNELS`` columns, a size outside 1 ..
+    ``MAX_HISTORY``, and the configurations the history does not run in, before any device is touched."""
+    if keys is None:
+        return None
+    if isinstance(keys, (str, tuple)):
+        keys = [keys]
+    table = _history_keys()
+    columns, layout = [], []
+    for key in keys:
+        path = tuple(key.strip("/").split("/")) if isinstance(key, str) else tuple(key)
+        if len(path) == 3 and path[0] == "servo" and path[2] in _CONSTANT_KEYS:
+            raise UpkieException(f"history: {'/'.join(path)} is a constant of the simulation, not a measurement")
+        if path not in table:
+            raise UpkieException(f"history: unknown key {'/'.join(map(str, path))} of the spine observation")
+        col, shape = table[path]
+        layout.append((path, len(columns), shape))
+        columns.extend(range(col, col + int(np.prod(shape, dtype=int))))
+    if not 1 <= len(columns) <= _abi.MAX_HISTORY_CHANNELS:
+        raise UpkieException(f"history: 1 to {_abi.MAX_HISTORY_CHANNELS} columns, the keys give {len(columns)}")
+    if int(size) != size or not 1 <= size <= _abi.MAX_HISTORY:
+        raise UpkieException(f"history_size must be an integer in [1, {_abi.MAX_HISTORY}], got {size!r}")
+    if spine_mode:
+        raise UpkieException("history: spine_mode reports the spine's lagged replies, which the history does not record")
+    if not joint_limits:
+        raise UpkieException("history: needs joint_limits (the history runs in the kernels with joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("history: body_contacts has no observation-history kernels")
+    return columns, int(size), layout
+
+
+def history_to_dict(layout: list, h: np.ndarray) -> dict:
+    """One env's history ``h[K, C]`` as the ``observation["history"]`` subtree of the reference's HistoryObserver: each
+    key path holds the list of its ``K`` values, newest first."""
+    out: dict = {}
+    for path, c0, shape in layout:
+        node = out
+        for key in path[:-1]:
+            node = node.setdefault(key, {})
+        size = int(np.prod(shape, dtype=int))
+        vals = h[:, c0 : c0 + size].astype(float)
+        if path == ("floor_contact", "contact"):
+            node[path[-1]] = [bool(v > 0.5) for v in vals[:, 0]]
+        elif shape == ():
+            node[path[-1]] = [float(v) for v in vals[:, 0]]
+        else:
+            node[path[-1]] = [v.reshape(shape).tolist() for v in vals]
+    return out
 
 
 def _check_max_episode_steps(value) -> int:
@@ -661,6 +774,15 @@ class B200VectorEnv(VectorEnv):
     measured torques a reset leaves as the previous episode ended them (its zero-torque substep does not write them, as
     for the undelayed reset observation): ``reset(seed=s)`` of a used env then reproduces the physics and every later
     observation, but not those first torque readings; a fresh env reproduces them too.
+
+    ``history`` (key paths of the spine observation, see ``history_spec``) with ``history_size=K`` records those keys
+    after every physics substep, as a ``HistoryObserver`` in the spine's pipeline records them every 1 kHz cycle:
+    ``info["spine_observation"].history`` is the ``[N, K, C]`` CUDA tensor and ``info["spine_observation"][i]["history"]``
+    the reference's ``observation["history"]`` subtree, newest first. Entry 0 is the instant the observation reports
+    (under an observation delay too); the IMU accelerations differentiate over one substep and the torques carry no
+    measurement noise. Each reset of an env fills its history with the post-reset values (the reference keeps it across
+    a spine reset). The terminal step of a same-step reset keeps no history. ``set_history`` changes or (``None``)
+    stops it. The history changes no other output.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -699,6 +821,8 @@ class B200VectorEnv(VectorEnv):
         action_delay: Optional[Union[float, Tuple[float, float]]] = None,
         observation_delay: Optional[Union[float, Tuple[float, float]]] = None,
         max_delay_ticks: int = 1,
+        history=None,
+        history_size: int = 1,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -746,6 +870,8 @@ class B200VectorEnv(VectorEnv):
         sense_spec = observation_delay_spec(observation_delay, 1.0 / frequency, config.nb_substeps,
                                             bool(config.spine_mode), config.joint_limits, config.body_contacts,
                                             self.max_delay_ticks)  # validated before any device is touched
+        hist_spec = history_spec(history, history_size, bool(config.spine_mode), config.joint_limits,
+                                 bool(config.body_contacts))  # validated before any device is touched
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -800,6 +926,26 @@ class B200VectorEnv(VectorEnv):
         if sense_spec is not None:
             # before the first reset, which draws every env's delay
             self.sim.set_observation_delay(*sense_spec, max_ticks=self.max_delay_ticks)
+        self._history_layout = None
+        if hist_spec is not None:
+            self.sim.set_history(hist_spec[0], hist_spec[1])
+            self._history_layout = hist_spec[2]
+
+    def set_history(self, keys, size: int = 1) -> None:
+        """Record the spine-observation ``keys`` (``history_spec``) after every substep and report the last ``size``
+        in ``info["spine_observation"]``; ``None`` turns the history off. Every env's history restarts from its
+        current state."""
+        spec = history_spec(keys, size, bool(self.config.spine_mode), self.config.joint_limits,
+                            bool(self.config.body_contacts))
+        if spec is None:
+            self.sim.set_history(None)
+            self._history_layout = None
+        else:
+            self.sim.set_history(spec[0], spec[1])
+            self._history_layout = spec[2]
+
+    def _spine_observations(self) -> "SpineObservations":
+        return SpineObservations(self.sim, self._history_layout)
 
     def set_reset_randomization(self, spec: Optional[dict]) -> None:
         """Redraw the parameters ``spec`` names at every later reset of an env (``reset_randomization_spec``);
@@ -991,7 +1137,7 @@ class B200VectorEnv(VectorEnv):
             mask=torch.from_numpy(mask).to(dev) if mask is not None else None,
             init_state=torch.from_numpy(rows).to(dev),
         )
-        info = {"spine_observation": SpineObservations(self.sim)}
+        info = {"spine_observation": self._spine_observations()}
         if self.env_type == "base_velocity":
             # UpkieBaseVelocity.reset (upkie_base_velocity.py:137-162) of the reset envs: MPC reset, x = y = 0, zero
             # observation; the other envs keep their state and their last observation
@@ -1041,7 +1187,7 @@ class B200VectorEnv(VectorEnv):
                                                              final_state=self._same_step())
             else:
                 obs18, term, trunc = *self.sim.step_servos_host_compact(a), hb["trunc"]
-            info = {"spine_observation": SpineObservations(self.sim)}
+            info = {"spine_observation": self._spine_observations()}
             if self.copy:
                 obs18 = obs18.copy()
                 self._add_final_obs(info, term, trunc, fin, lambda f: self._servo_obs_dict(f.copy(), cache=False))
@@ -1058,7 +1204,7 @@ class B200VectorEnv(VectorEnv):
                 rew = self.sim._host_buffers()["rew"]
             else:
                 obs, rew, term, trunc = self.sim.step_gyropod_host(a)
-        info = {"spine_observation": SpineObservations(self.sim)}
+        info = {"spine_observation": self._spine_observations()}
         if self.copy:
             self._add_final_obs(info, term, trunc, fin, np.copy)
             return obs.copy(), rew.copy(), term.view(np.bool_).copy(), trunc.view(np.bool_).copy(), info
@@ -1109,7 +1255,7 @@ class B200VectorEnv(VectorEnv):
             obs, rew, term, trunc = self._base_velocity_step(action, fin)
         else:
             obs, rew, term, trunc = self.sim.step_pendulum(action, final_obs=fin, final_state=same)
-        info = {"spine_observation": SpineObservations(self.sim)}
+        info = {"spine_observation": self._spine_observations()}
         # same-step mode: one host synchronisation per step decides whether some env reset
         self._add_final_obs(info, term, trunc, fin, lambda f: f)
         return obs, rew, term, trunc, info

@@ -8,14 +8,14 @@ device memory and streams only; all arithmetic happens in the sm_90a kernels).
 """
 
 import ctypes as C
-from typing import Optional
+from typing import Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import _abi
 from ._lib import check, lib
-from .exceptions import UpkieRuntimeError
+from .exceptions import UpkieException, UpkieRuntimeError
 from .model import Model, default_model
 
 AUTORESET_DISABLED, AUTORESET_NEXT_STEP, AUTORESET_SAME_STEP = 0, 1, 2
@@ -293,6 +293,62 @@ class UpkieSim:
         check(lib().upkie_b200_set_observation_delay_state(self._h, _ptr(count), _ptr(delay), _ptr(rows),
                                                            self._stream()))
         self._sense_state_set = True
+
+    def set_history(self, columns: Optional[Sequence[int]], size: int = 1) -> None:
+        """Record each env's spine-observation ``columns`` (``_abi.SP_*``, 1 to ``MAX_HISTORY_CHANNELS`` of them) after
+        every substep, and report the last ``size`` (1 to ``MAX_HISTORY``) through ``get_history``: the spine's
+        ``HistoryObserver`` (``upkie/cpp/observers/HistoryObserver.h``) at the substep rate. Entry 0 is the observed
+        instant (the end of the tick, or the observation delay's snapshot), entry k is k substeps earlier. The IMU
+        accelerations differentiate over one substep, the torques are the applied ones without measurement noise. Each
+        reset of an env fills its entries with its post-reset columns; a new spec and ``set_state`` fill every env's.
+        ``None`` turns it off. The history records only: every other output of a step is unchanged."""
+        if columns is None:
+            check(lib().upkie_b200_set_history(self._h, None))
+            self._history = None
+            return
+        cols = [int(c) for c in columns]
+        if not 1 <= len(cols) <= _abi.MAX_HISTORY_CHANNELS:
+            raise UpkieException(f"set_history: 1 to {_abi.MAX_HISTORY_CHANNELS} columns, got {len(cols)}")
+        spec = _abi.UpkieHistory(int(size), len(cols))
+        for k, c in enumerate(cols):
+            spec.columns[k] = c
+        check(lib().upkie_b200_set_history(self._h, C.byref(spec)))
+        self._history = (tuple(cols), int(size))
+
+    @property
+    def history_spec(self) -> Optional[Tuple[Tuple[int, ...], int]]:
+        """``(columns, size)`` of the history in force, or None."""
+        return getattr(self, "_history", None)
+
+    def get_history(self) -> torch.Tensor:
+        """``[N, size, C]`` the history's entries of every env, newest first (``set_history``)."""
+        cols, size = self._require_history()
+        out = torch.empty((self.n, size, len(cols)), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_history(self._h, _ptr(out), self._stream()))
+        return out
+
+    def _require_history(self):
+        if self.history_spec is None:
+            raise UpkieException("no observation history is set (set_history)")
+        return self.history_spec
+
+    def history_entries(self) -> int:
+        """Entries of the history's ring: ``size`` plus the deepest observation delay, in substeps (0: no history)."""
+        t = C.c_int(0)
+        check(lib().upkie_b200_history_entries(self._h, C.byref(t)))
+        return int(t.value)
+
+    def get_history_state(self) -> torch.Tensor:
+        """``[history_entries(), N, C]`` the whole ring in age order, 0 the entry the last substep wrote (checkpoints)."""
+        cols, _ = self._require_history()
+        out = torch.empty((self.history_entries(), self.n, len(cols)), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_history_state(self._h, _ptr(out), self._stream()))
+        return out
+
+    def set_history_state(self, rows: torch.Tensor) -> None:
+        cols, _ = self._require_history()
+        self._check_tensor(rows, (self.history_entries(), self.n, len(cols)), name="rows")
+        check(lib().upkie_b200_set_history_state(self._h, _ptr(rows), self._stream()))
 
     def set_external_forces(self, force: Optional[torch.Tensor] = None, local_mask: int = 0) -> None:
         """``force[N, 7, 3]`` newtons at the centres of mass of the 7 bodies, applied on every substep of
@@ -689,6 +745,10 @@ class UpkieSim:
         if sense_ticks > 1:
             sd["observation_delay_ticks"] = sense_ticks
             sd["observation_delay_history"] = self.get_observation_delay_history()
+        # the observation history: (columns, size) and its ring in age order (absent without one)
+        if self.history_spec is not None:
+            sd["history"] = self.history_spec
+            sd["history_ring"] = self.get_history_state()
         sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
@@ -784,6 +844,12 @@ class UpkieSim:
                                              state.contiguous() if rows is None else rows.to(dev).contiguous())
         if sd.get("observation_delay_history") is not None:
             self.set_observation_delay_history(sd["observation_delay_history"].to(dev).contiguous())
+        # the observation history after the observation delay, whose depth sizes its ring; a checkpoint without one
+        # turns it off
+        hist = sd.get("history")
+        self.set_history(None if hist is None else hist[0], 1 if hist is None else hist[1])
+        if hist is not None:
+            self.set_history_state(sd["history_ring"].to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
