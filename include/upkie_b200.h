@@ -812,6 +812,48 @@ int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationD
 int upkie_b200_get_observation_delay_history(void* handle, float* rows, void* stream);
 int upkie_b200_set_observation_delay_history(void* handle, const float* rows, void* stream);
 
+/* ---- Servo reply dropouts (upkie/cpp/observers/observe_servos.cpp:32-52) ---------------------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. The spine refreshes a servo's observation
+ * only from a reply that arrived intact: a reply that is lost (or reports a NaN torque) writes nothing, and the servo's
+ * position, velocity and torque keep the values of its last good reply. While a spec is set:
+ * - Draw per reset: at every reset of env i (both fused auto-resets, upkie_b200_reset with or without a mask) its loss
+ *   probability p_i ~ U(prob_low, prob_high) is drawn. Draw law: a per-env counter k, +1 at every reset; draw k of the
+ *   env of global index g = env_offset + i is Philox4x32-10 with key seed (upkie_b200_set_autoreset) and counter
+ *   (g, 2^59 | k << 4), whose word w0 gives p_i = min(low + fl(fl(high - low) * u(w0)), high), u(w) = (w >> 8) / 2^24.
+ * - Loss per cycle: every substep is one 1 kHz spine cycle. In substep s of the env's tick t (the per-env tick counter
+ *   of upkie_b200_get_counters after the step), the reply of servo j of joint_mask is lost when u(w) < p_i, w word
+ *   j % 4 of Philox4x32-10 with key seed and counter (g, 2^59 | 2^58 | t << 20 | s << 1 | j / 4). The tag bits 59 and
+ *   58 keep these counters apart from the initial states ((episode << 2) | b, below 2^34), the reset randomisation
+ *   (bit 63), the pushes (62), the action delay (61) and the observation delay (60); s < 2^19.
+ * - A received reply latches the servo's q_j, qd_j and commanded torque after that substep; a lost one latches
+ *   nothing. Every servo-derived output reports the latched triple: the [6][5] and compact [6][3] servo rows, the servo
+ *   block of upkie_b200_spine_obs and of the final spine observation and the wheel odometry built from them, the
+ *   gyropod and pendulum rows (whose p and pdot are odometry), final_obs, reset_obs, and the servo and odometry columns
+ *   of every entry of an observation history. Torque measurement noise is added to the latched torque as it is added
+ *   to the true one. Under an observation delay the snapshot takes the values latched at the delayed instant.
+ * - Not affected: the physics, terminated, truncated, the auto-resets, the gyropod's leg targets and
+ *   upkie_b200_get_state. Every reply of a reset's cycles arrives, so a reset latches the post-reset state.
+ * - Off is free: with the spec off, or prob_high = 0, every output equals the same handle's without a spec.
+ * Setting a spec draws nothing: each env keeps its probability (0 on a handle that never had a spec) until its next
+ * reset. A spec set while the feature is off latches the current state; replacing a spec in force keeps the latched
+ * values of the servos both masks hold and latches the current state of the servos it adds; NULL turns it off (the per-env state is freed once the device is idle). upkie_b200_set_state latches the
+ * state set. Per-env state (get/set_servo_dropout_state, for checkpoints; device pointers): count[N], prob[N] and
+ * held[N][18], the latched [joint][position, velocity, torque] of each env; UPKIE_B200_EINVAL without a spec.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: prob_low < 0, prob_low > prob_high, prob_high > 1, a
+ * joint_mask of zero or with bits above 5, joint_limits == 0 and body_contacts (it runs in the observation-delay
+ * kernels), spine_mode (whose spine reports its own replies). upkie_b200_set_config rejects joint_limits = 0 and
+ * body_contacts while a spec is set; the in-kernel rollout transports reject a handle with one. The set call waits for
+ * the device. */
+typedef struct UpkieServoDropout {
+  float prob_low, prob_high; /* range of each env's per-cycle reply loss probability */
+  uint32_t joint_mask;       /* bit j: servo j (UPKIE_NJ order) may lose replies */
+  uint32_t reserved;         /* 0 */
+} UpkieServoDropout;
+int upkie_b200_set_servo_dropout(void* handle, const UpkieServoDropout* spec);
+int upkie_b200_get_servo_dropout_state(void* handle, uint32_t* count, float* prob, float* held, void* stream);
+int upkie_b200_set_servo_dropout_state(void* handle, const uint32_t* count, const float* prob, const float* held,
+                                       void* stream);
+
 /* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
  * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
  * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last

@@ -401,6 +401,21 @@ class UpkieObservationDelay(C.Structure):
     ]
 
 
+class UpkieServoDropout(C.Structure):
+    """``UpkieServoDropout`` of include/upkie_b200.h: the range each env's per-cycle servo reply loss probability is
+    drawn from at its resets, and the servos (bit j, ``NJ`` order) whose replies may be lost."""
+
+    _fields_ = [
+        ("prob_low", C.c_float),
+        ("prob_high", C.c_float),
+        ("joint_mask", C.c_uint32),
+        ("reserved", C.c_uint32),
+    ]
+
+
+SERVO_HELD_DIM = 18  # the held rows of an env under servo dropouts: [joint][position, velocity, torque]
+
+
 MAX_HISTORY = 64  # UPKIE_MAX_HISTORY: the most entries an observation history reports
 MAX_HISTORY_CHANNELS = 16  # UPKIE_MAX_HISTORY_CHANNELS: the most spine columns it records
 

@@ -59,6 +59,9 @@ SYMBOLS = {
     "upkie_b200_set_observation_delay_ticks": (C.c_int, [_vp, C.POINTER(_abi.UpkieObservationDelay), C.c_uint32]),
     "upkie_b200_get_observation_delay_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_set_observation_delay_history": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_servo_dropout": (C.c_int, [_vp, C.POINTER(_abi.UpkieServoDropout)]),
+    "upkie_b200_get_servo_dropout_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
+    "upkie_b200_set_servo_dropout_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_set_history": (C.c_int, [_vp, C.POINTER(_abi.UpkieHistory)]),
     "upkie_b200_get_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_history_entries": (C.c_int, [_vp, C.POINTER(C.c_int)]),

@@ -267,6 +267,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.action_delay = nullptr;
   P.obs_delay = nullptr;
   P.history = nullptr;
+  P.servo_dropout = nullptr;
   return 0;
 }
 
@@ -389,6 +390,19 @@ inline const char* history_spec_error(const UpkieHistory& s, const SimParams& P)
     return "set_history: needs joint_limits != 0 (the history runs in the observation-delay kernels)";
   if (P.spine_mode) return "set_history: spine_mode reports the spine's lagged replies, which the history does not record";
   if (P.body_contacts) return "set_history: body_contacts has no observation-history kernels";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses a servo-dropout spec (upkie_b200_set_servo_dropout), null when it takes it
+inline const char* servo_dropout_spec_error(const UpkieServoDropout& s, const SimParams& P) {
+  if (!(s.prob_low >= 0.f) || !(s.prob_low <= s.prob_high) || !(s.prob_high <= 1.f))
+    return "set_servo_dropout: 0 <= prob_low <= prob_high <= 1 required";
+  if (s.joint_mask == 0 || (s.joint_mask >> UPKIE_NJ) != 0)
+    return "set_servo_dropout: joint_mask must select servos of bits 0 .. 5, at least one";
+  if (P.joint_limits == 0)
+    return "set_servo_dropout: needs joint_limits != 0 (the dropouts run in the observation-delay kernels)";
+  if (P.spine_mode) return "set_servo_dropout: spine_mode reports the spine's own servo replies";
+  if (P.body_contacts) return "set_servo_dropout: body_contacts has no servo-dropout kernels";
   return nullptr;
 }
 

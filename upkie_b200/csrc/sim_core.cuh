@@ -147,6 +147,9 @@ struct SimParams {
   // spine-rate observation history (upkie_b200_set_history): the handle's device block, null = off. Read by the step
   // kernels of FAM_SENSE (step_family.h) and k_reset only. Appended last, as obs_delay above.
   const struct History* history;
+  // servo reply dropouts (upkie_b200_set_servo_dropout): the handle's device block, null = off. Read by the step kernels
+  // of FAM_SENSE (step_family.h), k_reset, k_spine_obs and k_reset_obs only. Appended last, as history above.
+  const struct ServoDropout* servo_dropout;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -2086,6 +2089,89 @@ UPKIE_HD void history_fill(const History& H, const SimParams& P, const RobotStat
 // before the end of the tick (the observation delay in force; 0 without one)
 UPKIE_HD uint32_t history_entry(uint32_t head, uint32_t ticks, uint32_t d, uint32_t k) {
   return (head + 2u * ticks - 1u - d - k) % ticks;
+}
+
+// ---- servo reply dropouts (upkie_b200_set_servo_dropout, observe_servos.cpp:32-52) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw, prob[i] = p_i, and held = the latched [joint][position, velocity, torque] of each env,
+// [kServoHeldRows][stride] structure-of-arrays like the state, env i in column i.
+constexpr int kServoHeldRows = 18;
+struct ServoDropout {
+  UpkieServoDropout spec;
+  uint32_t* count;
+  float* prob;
+  float* held;
+  int stride;
+};
+
+// bit 59 of the high counter word, the per-reset draws of p_i: never set by sample_init_state ((episode << 2) | b,
+// episode < 2^32), the noise ((tick << 10) | (slot << 1) | b, tick < 2^32), the reset randomisation (bit 63), the
+// pushes (bit 62), the action delay (bit 61) or the observation delay (bit 60), whose draw numbers stay below bit 36.
+// Bits 59 and 58 together: the per-cycle losses, (tick << 20) | (sub << 1) | b below bit 52.
+constexpr uint64_t kServoDropoutTag = uint64_t(1) << 59;
+constexpr uint64_t kServoLossTag = kServoDropoutTag | (uint64_t(1) << 58);
+
+// Draw k of the env of global index g: its loss probability, push_value's exact form
+UPKIE_HD float servo_dropout_draw(const UpkieServoDropout& s, uint64_t seed, uint64_t g, uint32_t k) {
+  const Philox4 r = philox4x32_10(g, kServoDropoutTag | (uint64_t(k) << 4), seed);
+  return push_value(r.v[0], s.prob_low, s.prob_high);
+}
+
+// The servos of `mask` whose reply is lost in substep `sub` of the env's tick `tick` (bit j: servo j), each with
+// probability p. A block of four servos none of which may lose a reply, or p <= 0, draws nothing.
+UPKIE_HD uint32_t servo_dropout_lost(uint32_t mask, float p, uint64_t seed, uint64_t g, uint32_t tick, uint32_t sub) {
+  uint32_t lost = 0;
+  if (!(p > 0.f)) return lost;
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    if (!((mask >> (4 * b)) & 0xFu)) continue;
+    const Philox4 r = philox4x32_10(g, kServoLossTag | (uint64_t(tick) << 20) | (uint64_t(sub) << 1) | uint64_t(b), seed);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int j = 4 * b + k;
+      if (j < UPKIE_NJ && ((mask >> j) & 1u) && u01(r.v[k]) < p) lost |= 1u << j;
+    }
+  }
+  return lost;
+}
+
+// One spine cycle: the servos of `mask` whose reply was not lost (`lost`) latch their triple after the substep,
+// store(row, value). The held rows then always hold each masked servo's last received triple.
+template <typename Store>
+UPKIE_HD void servo_dropout_hold(const RobotState& S, uint32_t mask, uint32_t lost, Store store) {
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!((mask >> j) & 1u) || ((lost >> j) & 1u)) continue;
+    store(3 * j, S.q[j]);
+    store(3 * j + 1, S.qd[j]);
+    store(3 * j + 2, S.torque[j]);
+  }
+}
+
+// The observed state of S at an instant whose replies `lost` lost: those servos report their held triple, load(row)
+template <typename Load>
+UPKIE_HD void servo_dropout_view(RobotState& S, uint32_t lost, Load load) {
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!((lost >> j) & 1u)) continue;
+    S.q[j] = load(3 * j);
+    S.qd[j] = load(3 * j + 1);
+    S.torque[j] = load(3 * j + 2);
+  }
+}
+
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, and the post-reset state S latched. The
+// block's fields are copied before the first store, as action_delay_reset.
+UPKIE_HD void servo_dropout_reset(const ServoDropout& D, uint64_t seed, uint64_t g, int i, const RobotState& S) {
+  const UpkieServoDropout spec = D.spec;
+  uint32_t* const count = D.count;
+  float* const prob = D.prob;
+  float* const col = D.held + size_t(i);
+  const size_t stride = size_t(D.stride);
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  prob[i] = servo_dropout_draw(spec, seed, g, k);
+  servo_dropout_hold(S, ~0u, 0u, [&](int r, float v) { col[size_t(r) * stride] = v; });
 }
 
 }  // namespace upkie_b200

@@ -25,7 +25,7 @@ enum {
   FAM_BODY_PUSH = 7,  // FAM_BODY + push randomisation
   FAM_DELAY = 8,      // FAM_PUSH + action delay
   FAM_BODY_DELAY = 9, // FAM_BODY_PUSH + action delay
-  FAM_SENSE = 10,     // FAM_DELAY + observation delay + observation history
+  FAM_SENSE = 10,     // FAM_DELAY + observation delay + observation history + servo reply dropouts
   kNumFamilies = 11
 };
 
@@ -39,7 +39,8 @@ struct StepFamily {
   bool body;        // body-contact record (BodyRecOut); units built with UPKIE_BODY_CONTACTS_BUILD 1
   bool push;        // the push schedule
   bool delay;       // the action delay: previous command rows, per-env delays
-  bool sense;       // the observation delay: sensed state rows, per-env delays; the observation history's ring
+  bool sense;       // the observation delay: sensed state rows, per-env delays; the observation history's ring; the
+                    // servo dropouts' held rows
 };
 
 UPKIE_HD constexpr StepFamily step_family_traits(int family) {
@@ -91,6 +92,8 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "observation delay has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.history)
     no = "the observation history has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
+  else if (in_kernel && P.servo_dropout)
+    no = "servo dropouts have no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.max_episode_steps > 0)
     no = "max_episode_steps has no in-kernel rollout transport: it does not carry truncated (use upkie_b200_step with "
          "compact rows)";
@@ -112,15 +115,21 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "observation history needs joint_limits != 0";
   else if (P.history && P.body_contacts)
     no = "observation history has no body-contact kernels";
+  else if (P.servo_dropout && P.spine_mode)
+    no = "servo dropouts: spine_mode reports the spine's own servo replies";
+  else if (P.servo_dropout && P.joint_limits == 0)
+    no = "servo dropouts need joint_limits != 0";
+  else if (P.servo_dropout && P.body_contacts)
+    no = "servo dropouts have no body-contact kernels";
   if (no) {
     *why = no;
     return -1;
   }
   if (P.spine_mode) return FAM_SPINE;
   // the observation-delay family carries the action delay and the pushes too (runtime-uniform branches on
-  // P.action_delay and P.push), and the observation history (P.history, the same rule); the set calls reject spine
-  // mode, no limits and body contacts
-  if (P.obs_delay || P.history) return FAM_SENSE;
+  // P.action_delay and P.push), the observation history (P.history) and the servo dropouts (P.servo_dropout), by the
+  // same rule; the set calls reject spine mode, no limits and body contacts
+  if (P.obs_delay || P.history || P.servo_dropout) return FAM_SENSE;
   // the delay families carry the pushes too (a runtime-uniform branch on P.push); the set calls reject spine mode and
   // no limits
   if (P.action_delay) return P.body_contacts ? FAM_BODY_DELAY : FAM_DELAY;

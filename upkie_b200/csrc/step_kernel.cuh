@@ -134,8 +134,14 @@ __device__ __forceinline__ float* obs_delay_report(const ObsDelay& O, uint32_t s
 // IMU velocity differentiated over the substep against `vel` (updated in place) when `acc`; and the fill of the whole
 // column with the columns of S. Out of line: the calls pass a copy of the state, and the kernel's own arithmetic is
 // compiled (and its products contracted) as without the history.
-__device__ __noinline__ void history_substep(const SimParams& P, const RobotState S, float* vel, float* e,
-                                             size_t stride, int count, bool acc) {
+// Under servo dropouts the servos of `lost` report env i's held triple, as the observation does.
+__device__ __noinline__ void history_substep(const SimParams& P, RobotState S, float* vel, float* e,
+                                             size_t stride, int count, bool acc, uint32_t lost, int i) {
+  if (lost) {
+    const ServoDropout& D = *P.servo_dropout;
+    const float* const held = D.held + size_t(i);
+    servo_dropout_view(S, lost, [&](int r) { return __ldcg(held + size_t(r) * size_t(D.stride)); });
+  }
   float a[3] = {0.f, 0.f, 0.f};
   if (acc) {
     float v[3];
@@ -154,6 +160,48 @@ __device__ __noinline__ void history_fill_lane(const SimParams& P, const RobotSt
     const float v = history_value(P, S, S.imu_acc, __ldg(P.history->columns + c));
     for (uint32_t e = 0; e < ticks; ++e) __stcg(col + (size_t(e) * size_t(count) + size_t(c)) * stride, v);
   }
+}
+
+// The servo dropouts (F.sense kernels, P.servo_dropout set). dropout_cycle: one spine cycle of env i, the end of
+// substep `sub` of its tick, whose servo triples are `R`: the servos of the mask whose reply is lost (the result,
+// servo_dropout_lost), and the triple of every masked servo received now latched into the env's column of the held
+// rows. dropout_sense: the servos of `lost` (those of the mask) in the sensed row `scol` of an observation-delay
+// snapshot take their held triple. Out of line, as history_substep; the cycle takes the 18 servo values only, and
+// reads the spec and p_i from the device block itself, so that the substep loop carries no dropout state but the
+// last cycle's losses.
+struct ServoReplies {
+  float q[UPKIE_NJ], qd[UPKIE_NJ], tau[UPKIE_NJ];
+};
+__device__ __noinline__ uint32_t dropout_cycle(const SimParams& P, const ServoReplies R, int i, uint64_t seed, uint64_t g,
+                                               uint32_t tick, int sub) {
+  const ServoDropout& D = *P.servo_dropout;
+  const uint32_t mask = D.spec.joint_mask;
+  const uint32_t lost = servo_dropout_lost(mask, __ldcg(D.prob + i), seed, g, tick, uint32_t(sub));
+  float* const held = D.held + size_t(i);
+  const size_t stride = size_t(D.stride);
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!((mask >> j) & 1u) || ((lost >> j) & 1u)) continue;
+    __stcg(held + size_t(3 * j) * stride, R.q[j]);
+    __stcg(held + size_t(3 * j + 1) * stride, R.qd[j]);
+    __stcg(held + size_t(3 * j + 2) * stride, R.tau[j]);
+  }
+  return lost;
+}
+__device__ __noinline__ void dropout_sense(const SimParams& P, uint32_t lost, int i, float* scol, size_t sstride) {
+  const ServoDropout& D = *P.servo_dropout;
+  const float* const held = D.held + size_t(i);
+  const size_t stride = size_t(D.stride);
+  lost &= D.spec.joint_mask;
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!((lost >> j) & 1u)) continue;
+    __stcg(scol + size_t(UPKIE_ST_Q + j) * sstride, __ldcg(held + size_t(3 * j) * stride));
+    __stcg(scol + size_t(UPKIE_ST_QD + j) * sstride, __ldcg(held + size_t(3 * j + 1) * stride));
+    __stcg(scol + size_t(UPKIE_ST_TORQUE + j) * sstride, __ldcg(held + size_t(3 * j + 2) * stride));
+  }
+}
+__device__ __noinline__ void dropout_reset_lane(const SimParams& P, const RobotState S, uint64_t seed, uint64_t g,
+                                                int i) {
+  servo_dropout_reset(*P.servo_dropout, seed, g, i, S);
 }
 
 // ---- one env tick of the robot `tid` --------------------------------------------------
@@ -396,12 +444,27 @@ __device__ __forceinline__ void step_env(
       sdl = min(__ldcg(O.delay + i), uint32_t(P.nb_substeps));
     }
   }
+  // servo reply dropouts (F.sense kernels, P.servo_dropout set: a uniform branch). Each substep of a lane that does
+  // not reset is one spine cycle (dropout_cycle): it draws which masked servos lose their reply, and latches the triple
+  // of every masked servo received into the env's column of the held rows, so that the held rows always hold each
+  // masked servo's last received triple. An instant whose cycle lost replies (`dcur`, the last cycle's losses) reads
+  // those servos back from the held rows: an observation-delay snapshot, a history entry, the observation after the
+  // tick. A lane that resets loses nothing, and latches its post-reset state after the tick with its next draw.
+  const bool dropping = F.sense && P.servo_dropout;
+  uint32_t dcur = 0;
+  bool dreset = resetting;  // this tick resets the lane: it latches its post-reset state
+  auto dheld = [&](int r) {
+    const ServoDropout& D = *P.servo_dropout;
+    return __ldcg(D.held + size_t(r) * size_t(D.stride) + size_t(i));
+  };
   auto sense_load = [&](int k) { return __ldcg(scol + size_t(k) * sstride); };
   auto sense_store = [&](int k, float v) { __stcg(scol + size_t(k) * sstride, v); };
   if (sensing && live && sdl == uint32_t(P.nb_substeps)) {  // the state at the start of the tick
     float v[3];
     imu_velocity(P, S, v);
     obs_delay_snapshot(P, S, v, sense_load, sense_store);
+    // the end of the last tick: every servo reports what the held rows latched then
+    if (dropping) dropout_sense(P, ~0u, i, scol, sstride);
   }
   // spine-rate observation history (F.sense kernels, P.history set: a uniform branch). Each substep of a lane that does
   // not reset stores the selected spine columns of its state into ring entry (head + sub) % ticks, differentiating the
@@ -454,15 +517,26 @@ __device__ __forceinline__ void step_env(
                       (F.extras && ext) ? &xf : nullptr, F.limits ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
                       pushing ? &pu : nullptr);
       }
+      if (dropping && !resetting && live) {
+        ServoReplies R;
+#pragma unroll
+        for (int j = 0; j < UPKIE_NJ; ++j) {
+          R.q[j] = S.q[j];
+          R.qd[j] = S.qd[j];
+          R.tau[j] = S.torque[j];
+        }
+        dcur = dropout_cycle(P, R, i, seed, env_offset + uint64_t(i), nz.tick, sub);
+      }
       // the end of substep nb_substeps - sdl - 1 (0 < sdl < nb_substeps)
       if (sensing && live && sdl != 0 && uint32_t(sub) + sdl + 1u == uint32_t(P.nb_substeps)) {
         float v[3];
         imu_velocity(P, S, v);
         obs_delay_snapshot(P, S, v, sense_load, sense_store);
+        if (dropping && dcur) dropout_sense(P, dcur, i, scol, sstride);
       }
       if (recording && !resetting && live)
         history_substep(P, S, hvel, hring + size_t((hhead + uint32_t(sub)) % hticks) * size_t(hcount) * hstride,
-                        hstride, hcount, hacc);
+                        hstride, hcount, hacc, dcur, i);
     } else {
 #pragma unroll
       for (int k = 0; k < kPhaseSyncs; ++k) PhaseSync()();
@@ -470,7 +544,10 @@ __device__ __forceinline__ void step_env(
   }
   if (!spine) observe_update(P, S);  // spine mode: the cycles read the IMU
   // sdl = 0: the end of the tick, with the IMU velocity observe_update just computed
-  if (sensing && live && sdl == 0) obs_delay_snapshot(P, S, S.prev_imu_vel, sense_load, sense_store);
+  if (sensing && live && sdl == 0) {
+    obs_delay_snapshot(P, S, S.prev_imu_vel, sense_load, sense_store);
+    if (dropping && dcur) dropout_sense(P, dcur, i, scol, sstride);
+  }
   if (resetting) {
     reset_wrapper_state(S);
   } else {
@@ -521,6 +598,15 @@ __device__ __forceinline__ void step_env(
         fin_yaw_vel = S.yaw_vel;
       }
       if (!(F.sense && sensing)) {
+        // servo dropouts: the terminal step's observation and stash report the latched servos. The reset below keeps
+        // the commanded torques (its substep commands none), so the true ones are put back after the stores.
+        float dtrue[UPKIE_NJ];
+        if (F.sense && dropping && dcur) {
+#pragma unroll
+          for (int j = 0; j < UPKIE_NJ; ++j) dtrue[j] = S.torque[j];
+          servo_dropout_view(S, dcur, dheld);
+          if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
+        }
         if (P.final_obs && live)
           store_final_obs<MODE, spine>(P, S, L, o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
         // neither the reset below nor the rest of the tick writes tick[i] (written above, before the physics) or the
@@ -528,6 +614,10 @@ __device__ __forceinline__ void step_env(
         // reset randomisation draw overwrites the table at the end of the tick, and the stash then also holds the
         // pre-reset columns k_spine_obs reads, store_final_params)
         if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
+        if (F.sense && dropping && dcur) {
+#pragma unroll
+          for (int j = 0; j < UPKIE_NJ; ++j) S.torque[j] = dtrue[j];
+        }
       }
       if (F.reset_rand && P.reset_rand && P.final_state && live) store_final_params<spine>(P, n_pad, i);
       if (pushing) push_restart(push_k, push_t, push_end);  // the terminal step ran under its push; a new schedule
@@ -540,6 +630,7 @@ __device__ __forceinline__ void step_env(
       if (sensing && live) obs_delay_reset(*P.obs_delay, seed, env_offset + uint64_t(i), i);
       elapsed = 0;
       refill = true;
+      dreset = true;
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
       float init[UPKIE_INIT_DIM];
@@ -563,6 +654,8 @@ __device__ __forceinline__ void step_env(
     if (refill) history_fill_lane(P, S, hring, hstride, hcount, hticks);
     __stcg(P.history->head + i, (hhead + uint32_t(P.nb_substeps)) % hticks);
   }
+  // the dropouts: a reset latches the lane's post-reset state (the true state, here in S) and draws its next p_i
+  if (dropping && live && dreset) dropout_reset_lane(P, S, seed, env_offset + uint64_t(i), i);
   if (sensing) {
     // K > 1: the sensed row becomes the report, and the end of the tick works on it as for one tick
     if (HIST && !resetting && P.obs_delay->ticks > 1) scol = obs_delay_report(*P.obs_delay, srep, i, live);
@@ -575,7 +668,7 @@ __device__ __forceinline__ void step_env(
       S.yaw = fin_yaw;
       S.yaw_vel = fin_yaw_vel;
       obs_delay_sensed_state(S, sense_load);
-      if (MODE != MODE_SERVOS && sdl != 0) gyropod_obs(P, S, fin_o6);
+      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0)) gyropod_obs(P, S, fin_o6);  // (a dropout patched the snapshot)
       if (P.final_obs && live)
         store_final_obs<MODE, spine>(P, S, L, fin_o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
       if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
@@ -592,7 +685,7 @@ __device__ __forceinline__ void step_env(
           if (!obs_delay_sensed(k)) sense_store(k, r[k]);
       }
       obs_delay_sensed_state(S, sense_load);
-      if (MODE != MODE_SERVOS && sdl != 0) gyropod_obs(P, S, o6);
+      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0)) gyropod_obs(P, S, o6);
     }
     if ((resetting || fin_pending) && live) {
       // a reset in this tick: the sensed row becomes a copy of the post-reset state, the observation is undelayed
@@ -602,6 +695,12 @@ __device__ __forceinline__ void step_env(
       for (int k = 0; k < UPKIE_STATE_DIM; ++k) sense_store(k, r[k]);
       if (HIST && P.obs_delay->ticks > 1) obs_delay_fill_history(*P.obs_delay, i, r);  // and so does every snapshot
     }
+  }
+  // the dropouts without an observation delay: the observation after a tick that did not reset reports the latched
+  // servos (the true state is stored above)
+  if (F.sense && dropping && !sensing && !dreset && dcur) {
+    servo_dropout_view(S, dcur, dheld);
+    if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
   }
   if (spine && live) {
     float lr[UPKIE_LAG_DIM];

@@ -12,6 +12,8 @@
 //   k_spine_obs    spine observations of the state, or of the same-step auto-resets' terminal step from the stash.
 //   k_ring_copy    rows <-> struct-of-arrays columns of every per-env buffer, and the delay histories.
 //   k_history_read / k_history_fill   the observation history's entries of each env / its ring filled from the state.
+// The servo dropouts' held rows take no kernel of their own: k_reset latches, k_ring_copy copies them for checkpoints,
+// and a new spec or set_state latches the state with device copies of its rows (servo_dropout_latch).
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -134,6 +136,13 @@ struct Handle {
   int hist_ticks = 0;
   float* hist_ring = nullptr;
   uint32_t* hist_head = nullptr;
+  // servo reply dropouts (upkie_b200_set_servo_dropout): the device block P.servo_dropout points to while a spec is set,
+  // and the per-env state it points to (allocated with the first spec, freed when it is turned off)
+  ServoDropout* drop_dev = nullptr;
+  uint32_t* drop_count = nullptr;
+  float* drop_prob = nullptr;
+  float* drop_held = nullptr;  // [kServoHeldRows][n_pad]
+  uint32_t drop_mask = 0;      // joint_mask of the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -226,6 +235,15 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
     if (O.ticks > 1) obs_delay_fill_history(O, i, r);
   }
   if (P.history) history_fill(*P.history, P, S, i);  // a new episode's history starts from its post-reset columns
+  if (P.servo_dropout) servo_dropout_reset(*P.servo_dropout, rand_seed, g, i, S);  // a new p_i, the reset latched
+}
+
+// Servo dropouts without an observation delay: the observed state of S, every servo of the mask reporting its held
+// triple (the held rows latch every servo after a tick's last substep that received it, so this is the state for them)
+__device__ void servo_dropout_observed(const SimParams& P, int i, RobotState& S) {
+  if (!P.servo_dropout || P.obs_delay) return;
+  const ServoDropout& D = *P.servo_dropout;
+  servo_dropout_view(S, D.spec.joint_mask, [&](int r) { return D.held[size_t(r) * size_t(D.stride) + size_t(i)]; });
 }
 
 // The observation history of every env, out[n][size][count], entries newest first: the window ends `d` substeps
@@ -280,6 +298,7 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
   } else {
     RobotState S;
     load_state(state, n_pad, i, S);
+    if (!mark) servo_dropout_observed(P, i, S);  // (the stash holds the terminal step's observed state)
     float tq[6];
     measured_torques(P, S, &nz, tq, i);
     spine_observation(P, S, o, tq);
@@ -296,6 +315,7 @@ __global__ void k_reset_obs(const __grid_constant__ SimParams P, int n, int n_pa
   if (i >= n) return;
   RobotState S;
   load_state(state, n_pad, i, S);
+  servo_dropout_observed(P, i, S);
   if (obs_dim == UPKIE_OBS_DIM && P.spine_mode && lag) {
     for (int j = 0; j < 6; ++j) {
       float* o = out + size_t(i) * UPKIE_OBS_DIM + j * 5;
@@ -797,6 +817,23 @@ int history_build(Handle* h) {
   return UPKIE_B200_OK;
 }
 
+// Servo dropouts: the held rows of the servos of `joints` (bit j) latch every env's current state (a new spec, a mask
+// that gains servos, set_state): the state's position, velocity and torque rows of joint j into held rows 3j, 3j + 1,
+// 3j + 2
+cudaError_t servo_dropout_latch(Handle* h, uint32_t joints, cudaStream_t s) {
+  const int src[3] = {UPKIE_ST_Q, UPKIE_ST_QD, UPKIE_ST_TORQUE};
+  const size_t row = size_t(h->n_pad) * sizeof(float);
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!((joints >> j) & 1u)) continue;
+    for (int k = 0; k < 3; ++k) {
+      const cudaError_t e = cudaMemcpyAsync(h->drop_held + size_t(3 * j + k) * h->n_pad,
+                                            h->state + size_t(src[k] + j) * h->n_pad, row, cudaMemcpyDeviceToDevice, s);
+      if (e != cudaSuccess) return e;
+    }
+  }
+  return cudaSuccess;
+}
+
 // After a change of nb_substeps or of the observation delay's depth: a ring of the new size, filled from the state
 int history_resize(Handle* h) {
   if (!h->P.history || history_ticks(h) == h->hist_ticks) return UPKIE_B200_OK;
@@ -935,6 +972,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->sense_dev); cudaFree(h->sense_count); cudaFree(h->sense_delay); cudaFree(h->sense_rows);
   cudaFree(h->sense_hist); cudaFree(h->sense_head);
   cudaFree(h->hist_dev); cudaFree(h->hist_ring); cudaFree(h->hist_head);
+  cudaFree(h->drop_dev); cudaFree(h->drop_count); cudaFree(h->drop_prob); cudaFree(h->drop_held);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -978,6 +1016,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: the observation history needs joint_limits != 0");
   if (h->P.history && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no observation-history kernels");
+  if (h->P.servo_dropout && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: servo dropouts need joint_limits != 0");
+  if (h->P.servo_dropout && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no servo-dropout kernels");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -998,6 +1040,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.action_delay = h->P.action_delay;  // and the action delay
   P.obs_delay = h->P.obs_delay;        // and the observation delay
   P.history = h->P.history;            // and the observation history
+  P.servo_dropout = h->P.servo_dropout;  // and the servo dropouts
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -1468,6 +1511,8 @@ int upkie_b200_set_state(void* handle, const float* state, void* stream) {
       CUDA_TRY(ring_resize(h->state, nullptr, 1, h->sense_hist, h->sense_ticks, UPKIE_STATE_DIM, h->n, h->n_pad, 0,
                            ~uint64_t(0), static_cast<cudaStream_t>(stream)));
   }
+  // the servo dropouts latch the state set
+  if (h->P.servo_dropout) CUDA_TRY(servo_dropout_latch(h, ~0u, static_cast<cudaStream_t>(stream)));
   // the observation history restarts from the state set
   if (h->P.history) {
     k_history_fill<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->P.history, h->n, h->n_pad,
@@ -1904,6 +1949,83 @@ int upkie_b200_set_observation_delay_history(void* handle, const float* rows, vo
                        h->sense_ticks));
   else
     CUDA_TRY(ring_cols(rows, UPKIE_STATE_DIM, h->n, h->n_pad, h->sense_rows, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_servo_dropout(void* handle, const UpkieServoDropout* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    if (h->P.servo_dropout) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the per-env state
+      h->P.servo_dropout = nullptr;
+      cudaFree(h->drop_count);
+      cudaFree(h->drop_prob);
+      cudaFree(h->drop_held);
+      h->drop_count = nullptr;
+      h->drop_prob = nullptr;
+      h->drop_held = nullptr;
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = servo_dropout_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
+  // the servos the held rows have not followed latch the current state: every servo when the feature is switched on
+  // (zero counters and probabilities), the servos a replaced spec adds to the mask (the kernels latch masked servos
+  // only, so an unmasked servo's rows hold its last reset)
+  uint32_t latch = ~0u;
+  if (!h->P.servo_dropout) {
+    const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+    CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->drop_count), bytes},
+                           {reinterpret_cast<void**>(&h->drop_prob), bytes},
+                           {reinterpret_cast<void**>(&h->drop_held), size_t(kServoHeldRows) * h->n_pad * sizeof(float)}}));
+  } else {
+    latch = spec->joint_mask & ~h->drop_mask;
+  }
+  CUDA_TRY(servo_dropout_latch(h, latch, nullptr));
+  h->drop_mask = spec->joint_mask;
+  if (!h->drop_dev) CUDA_TRY(cudaMalloc(&h->drop_dev, sizeof(ServoDropout)));
+  ServoDropout D;
+  std::memset(&D, 0, sizeof(D));
+  D.spec = *spec;
+  D.count = h->drop_count;
+  D.prob = h->drop_prob;
+  D.held = h->drop_held;
+  D.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->drop_dev, &D, sizeof(D), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->P.servo_dropout = h->drop_dev;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_servo_dropout_state(void* handle, uint32_t* count, float* prob, float* held, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !prob || !held) return fail(UPKIE_B200_EINVAL, "get_servo_dropout_state: invalid argument");
+  if (!h->P.servo_dropout)
+    return fail(UPKIE_B200_EINVAL, "get_servo_dropout_state: no servo dropouts are set (upkie_b200_set_servo_dropout)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  CUDA_TRY(cudaMemcpyAsync(count, h->drop_count, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(prob, h->drop_prob, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_rows(h->drop_held, kServoHeldRows, h->n, h->n_pad, held, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_servo_dropout_state(void* handle, const uint32_t* count, const float* prob, const float* held,
+                                       void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !prob || !held) return fail(UPKIE_B200_EINVAL, "set_servo_dropout_state: invalid argument");
+  if (!h->P.servo_dropout)
+    return fail(UPKIE_B200_EINVAL, "set_servo_dropout_state: no servo dropouts are set (upkie_b200_set_servo_dropout)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t bytes = size_t(h->n) * sizeof(uint32_t);
+  CUDA_TRY(cudaMemcpyAsync(h->drop_count, count, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(h->drop_prob, prob, bytes, cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_cols(held, kServoHeldRows, h->n, h->n_pad, h->drop_held, s));
   return UPKIE_B200_OK;
 }
 

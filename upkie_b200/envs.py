@@ -714,6 +714,47 @@ def observation_delay_spec(delay, dt: float, nb_substeps: int, spine_mode: bool 
     return lo_s, hi_s
 
 
+def servo_dropout_spec(prob, joints=None, spine_mode: bool = False, joint_limits: Union[bool, int] = True,
+                       body_contacts: Union[bool, int] = False) -> Optional[_abi.UpkieServoDropout]:
+    """``UpkieServoDropout`` (``UpkieSim.set_servo_dropout``) from a per-cycle reply loss probability: a float, or a
+    ``(low, high)`` pair from which every reset draws an env's probability, and the names of the servos that may lose
+    replies (``joints``, ``JOINT_NAMES``; None: all six). Raises ``UpkieException`` on a bound outside [0, 1] or not a
+    number, ``low > high``, an unknown or empty joint list, ``spine_mode`` (whose spine reports its own replies), no
+    joint limits and ``body_contacts`` (the dropouts run in the kernels of the observation delay)."""
+    if prob is None:
+        return None
+    if isinstance(prob, (int, float, np.integer, np.floating)):
+        lo, hi = prob, prob
+    else:
+        try:
+            lo, hi = prob
+        except (TypeError, ValueError):
+            raise UpkieException(f"servo_dropout: expected a probability or a (low, high) pair, got {prob!r}") from None
+    try:
+        lo, hi = float(lo), float(hi)
+    except (TypeError, ValueError):
+        raise UpkieException(f"servo_dropout: expected probabilities, got ({lo!r}, {hi!r})") from None
+    if not 0.0 <= lo <= hi <= 1.0:
+        raise UpkieException(f"servo_dropout: expected probabilities 0 <= low <= high <= 1, got ({lo}, {hi})")
+    names = _abi.JOINT_NAMES if joints is None else list(joints)
+    unknown = [j for j in names if j not in _abi.JOINT_NAMES]
+    if unknown:
+        raise UpkieException(f"servo_dropout_joints: unknown joint(s) {unknown}, expected names of {_abi.JOINT_NAMES}")
+    if not names:
+        raise UpkieException("servo_dropout_joints: at least one joint")
+    if spine_mode:
+        raise UpkieException("servo_dropout: spine_mode reports the spine's own servo replies; the dropouts are not "
+                             "available there")
+    if not joint_limits:
+        raise UpkieException("servo_dropout: needs joint_limits (the dropouts run in the kernels with joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("servo_dropout: body_contacts has no servo-dropout kernels")
+    mask = 0
+    for j in names:
+        mask |= 1 << _abi.JOINT_NAMES.index(j)
+    return _abi.UpkieServoDropout(lo, hi, mask, 0)
+
+
 class B200VectorEnv(VectorEnv):
     """N Upkie environments stepped by one kernel launch per ``step()``.
 
@@ -783,6 +824,14 @@ class B200VectorEnv(VectorEnv):
     measurement noise. Each reset of an env fills its history with the post-reset values (the reference keeps it across
     a spine reset). The terminal step of a same-step reset keeps no history. ``set_history`` changes or (``None``)
     stops it. The history changes no other output.
+
+    ``servo_dropout`` (a probability, or a ``(low, high)`` range, see ``servo_dropout_spec``) loses each reply of the
+    servos ``servo_dropout_joints`` (names, default all six) in each 1 kHz spine cycle with a probability drawn at every
+    reset of the env, as the spine skips a reply that did not arrive intact (``observe_servos.cpp``): a servo whose reply
+    is lost reports the position, velocity and torque of its last received one, in the observation of every env type
+    (the gyropod and pendulum wheel odometry too), the spine observation and the history. The physics, terminations
+    and ``get_state`` see the true state. The draws are keyed on the seed of ``reset(seed=s)``, which also restarts the
+    draw counters of the envs it resets. ``set_servo_dropout`` changes or (``None``) stops it.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -823,6 +872,8 @@ class B200VectorEnv(VectorEnv):
         max_delay_ticks: int = 1,
         history=None,
         history_size: int = 1,
+        servo_dropout: Optional[Union[float, Tuple[float, float]]] = None,
+        servo_dropout_joints: Optional[Sequence[str]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -872,6 +923,8 @@ class B200VectorEnv(VectorEnv):
                                             self.max_delay_ticks)  # validated before any device is touched
         hist_spec = history_spec(history, history_size, bool(config.spine_mode), config.joint_limits,
                                  bool(config.body_contacts))  # validated before any device is touched
+        drop_spec = servo_dropout_spec(servo_dropout, servo_dropout_joints, bool(config.spine_mode),
+                                       config.joint_limits, config.body_contacts)  # validated before any device
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -930,6 +983,20 @@ class B200VectorEnv(VectorEnv):
         if hist_spec is not None:
             self.sim.set_history(hist_spec[0], hist_spec[1])
             self._history_layout = hist_spec[2]
+        if drop_spec is not None:
+            # before the first reset, which draws every env's probability
+            self.sim.set_servo_dropout(drop_spec.prob_low, drop_spec.prob_high, servo_dropout_joints)
+
+    def set_servo_dropout(self, prob, joints=None) -> None:
+        """Lose the replies of the servos ``joints`` (names, None: all) with a per-cycle probability ``prob``, a float
+        or a ``(low, high)`` range (``servo_dropout_spec``); ``None`` turns the dropouts off. A new range takes effect
+        at each env's next reset."""
+        spec = servo_dropout_spec(prob, joints, bool(self.config.spine_mode), self.config.joint_limits,
+                                  self.config.body_contacts)
+        if spec is None:
+            self.sim.set_servo_dropout(None)
+        else:
+            self.sim.set_servo_dropout(spec.prob_low, spec.prob_high, joints)
 
     def set_history(self, keys, size: int = 1) -> None:
         """Record the spine-observation ``keys`` (``history_spec``) after every substep and report the last ``size``
@@ -1126,6 +1193,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_observation_delay_state(count, delay, rows)
+            if self.sim.servo_dropout_spec is not None:
+                # so are the servo dropouts
+                count, prob, held = self.sim.get_servo_dropout_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_servo_dropout_state(count, prob, held)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

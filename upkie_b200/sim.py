@@ -294,6 +294,52 @@ class UpkieSim:
                                                            self._stream()))
         self._sense_state_set = True
 
+    def set_servo_dropout(self, low: Optional[float], high: Optional[float] = None,
+                          joints: Optional[Sequence[str]] = None) -> None:
+        """While a range is set, each reply of the servos ``joints`` (names, None: all six) is lost in each substep (a
+        1 kHz spine cycle) with each env's probability ``p ~ U(low, high)``, drawn at every reset of the env (keyed on
+        the auto-reset seed and the env's counter, ``include/upkie_b200.h``). A servo whose reply is lost reports the
+        position, velocity and torque of its last received reply in every observation, ``spine_obs`` (its wheel
+        odometry too), the final observations and the history; the physics, terminations and ``get_state`` see the
+        true state. ``high`` defaults to ``low``; ``None`` turns the dropouts off. Setting a range draws nothing: it
+        takes effect at each env's next reset."""
+        if low is None:
+            check(lib().upkie_b200_set_servo_dropout(self._h, None))
+            self._servo_dropout = None
+            return
+        names = _abi.JOINT_NAMES if joints is None else list(joints)
+        unknown = [j for j in names if j not in _abi.JOINT_NAMES]
+        if unknown:
+            raise UpkieException(f"set_servo_dropout: unknown joint(s) {unknown}")
+        mask = sum(1 << _abi.JOINT_NAMES.index(j) for j in set(names))
+        spec = _abi.UpkieServoDropout(float(low), float(low if high is None else high), mask, 0)
+        check(lib().upkie_b200_set_servo_dropout(self._h, C.byref(spec)))
+        self._servo_dropout = (spec.prob_low, spec.prob_high, mask)
+
+    @property
+    def servo_dropout_spec(self) -> Optional[Tuple[float, float, int]]:
+        """``(prob_low, prob_high, joint_mask)`` of the servo dropouts in force, or None."""
+        return getattr(self, "_servo_dropout", None)
+
+    def get_servo_dropout_state(self):
+        """Per-env servo-dropout state ``(count[N], prob[N], held[N, 6, 3])``: the draw counters (int32 bits of
+        uint32), the loss probabilities and the latched ``[joint][position, velocity, torque]``."""
+        if self.servo_dropout_spec is None:
+            raise UpkieException("no servo dropouts are set (set_servo_dropout)")
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        prob = torch.empty(self.n, dtype=torch.float32, device=self.device)
+        held = torch.empty((self.n, _abi.NJ, 3), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_servo_dropout_state(self._h, _ptr(count), _ptr(prob), _ptr(held), self._stream()))
+        return count, prob, held
+
+    def set_servo_dropout_state(self, count: torch.Tensor, prob: torch.Tensor, held: torch.Tensor) -> None:
+        if self.servo_dropout_spec is None:
+            raise UpkieException("no servo dropouts are set (set_servo_dropout)")
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(prob, (self.n,), name="prob")
+        self._check_tensor(held, (self.n, _abi.NJ, 3), name="held")
+        check(lib().upkie_b200_set_servo_dropout_state(self._h, _ptr(count), _ptr(prob), _ptr(held), self._stream()))
+
     def set_history(self, columns: Optional[Sequence[int]], size: int = 1) -> None:
         """Record each env's spine-observation ``columns`` (``_abi.SP_*``, 1 to ``MAX_HISTORY_CHANNELS`` of them) after
         every substep, and report the last ``size`` (1 to ``MAX_HISTORY``) through ``get_history``: the spine's
@@ -749,6 +795,11 @@ class UpkieSim:
         if self.history_spec is not None:
             sd["history"] = self.history_spec
             sd["history_ring"] = self.get_history_state()
+        # the servo dropouts: (prob_low, prob_high, joint_mask) and the per-env state (absent without a spec)
+        if self.servo_dropout_spec is not None:
+            sd["servo_dropout"] = self.servo_dropout_spec
+            sd["servo_dropout_count"], sd["servo_dropout_prob"], sd["servo_dropout_held"] = \
+                self.get_servo_dropout_state()
         sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
@@ -850,6 +901,14 @@ class UpkieSim:
         self.set_history(None if hist is None else hist[0], 1 if hist is None else hist[1])
         if hist is not None:
             self.set_history_state(sd["history_ring"].to(dev).contiguous())
+        # the servo dropouts; a checkpoint without them (or written before they existed) turns them off
+        drop = sd.get("servo_dropout")
+        if drop is None:
+            self.set_servo_dropout(None)
+        else:
+            self.set_servo_dropout(drop[0], drop[1], [n for j, n in enumerate(_abi.JOINT_NAMES) if (drop[2] >> j) & 1])
+            self.set_servo_dropout_state(*(sd[k].to(dev).contiguous() for k in (
+                "servo_dropout_count", "servo_dropout_prob", "servo_dropout_held")))
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
