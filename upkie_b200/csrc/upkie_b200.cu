@@ -677,9 +677,16 @@ int step_host(Handle* h, int mode, const float* action, float* obs, float* rewar
   const size_t n = size_t(h->n);
   const size_t act_dim = mode == MODE_SERVOS ? UPKIE_ACT_DIM : (mode == MODE_GYROPOD ? 2 : 1);
   const size_t obs_dim = mode == MODE_SERVOS ? (compact ? 18 : UPKIE_OBS_DIM) : (mode == MODE_GYROPOD ? 6 : 4);
+  // The kernels move a row with vector accesses: the servo action row as float4 and the gyropod one as float2, the
+  // observation rows as float2 and the pendulum's as float4. A pinned buffer short of that alignment (a float32 view
+  // that starts 4 bytes into its allocation, say) is staged like a pageable one rather than used in place.
+  auto aligned_to = [](const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; };
+  const uintptr_t act_align = mode == MODE_SERVOS ? 16 : (mode == MODE_GYROPOD ? 8 : 4);
+  const uintptr_t obs_align = mode == MODE_PENDULUM ? 16 : 8;
   // reward / truncated are constants of the reference (0.0 and false): callers may pass NULL for them
-  const bool pin_in = mapped(action) != nullptr;
-  const bool pin_out = mapped(obs) && (!reward || mapped(reward)) && mapped(term) && (!trunc || mapped(trunc));
+  const bool pin_in = mapped(action) != nullptr && aligned_to(action, act_align);
+  const bool pin_out = mapped(obs) && aligned_to(obs, obs_align) && (!reward || mapped(reward)) && mapped(term) &&
+                       (!trunc || mapped(trunc));
   if (!pin_in) std::memcpy(h->h_act, action, n * act_dim * sizeof(float));
   const float* src_act = pin_in ? action : h->h_act;
   float* dst_obs = pin_out ? obs : h->h_obs;
