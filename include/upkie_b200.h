@@ -854,6 +854,48 @@ int upkie_b200_get_servo_dropout_state(void* handle, uint32_t* count, float* pro
 int upkie_b200_set_servo_dropout_state(void* handle, const uint32_t* count, const float* prob, const float* held,
                                        void* stream);
 
+/* ---- IMU mounting misalignment (upkie/cpp/observers/BaseOrientation.h:29-35,106-112) ---------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. The spine derives the base orientation, its
+ * angular velocity and rotation_base_to_world from the IMU through a fixed rotation_base_to_imu; a board mounted
+ * slightly off its nominal pose rotates every one of those readings by the mounting error. While a spec is set:
+ * - Draw per reset: at every reset of env i (both fused auto-resets, upkie_b200_reset with or without a mask or host
+ *   rows) three angles are drawn. Draw law: a per-env counter k, +1 at every reset; draw k of the env of global index
+ *   g = env_offset + i is Philox4x32-10 with key seed (upkie_b200_set_autoreset) and counter (g, 2^57 | k << 4), whose
+ *   words w0, w1, w2 give roll, pitch and yaw = min(low + fl(fl(high - low) * u(w)), high), u(w) = (w >> 8) / 2^24 (the
+ *   servo dropouts' map). Tag bit 57 keeps these counters apart from the initial states (below 2^34), the reset
+ *   randomisation (bit 63), the pushes (62), the action delay (61), the observation delay (60) and the servo dropouts
+ *   (59, 59 | 58). The env keeps its misalignment as the unit quaternion e_i (w, x, y, z) of
+ *   E_i = Rz(yaw) Ry(pitch) Rx(roll), a rotation in the base frame.
+ * - Model: the true IMU frame is the nominal one rotated by E_i, and the pipeline still assumes the nominal mounting.
+ *   Every orientation-derived observation is that of a robot whose base orientation is R E_i instead of R, everything
+ *   else unchanged: base_orientation.pitch, base_orientation.angular_velocity ((R E)^T omega), rotation_base_to_world,
+ *   imu.orientation, imu.angular_velocity, imu.linear_acceleration, imu.raw_linear_acceleration, and the gyropod and
+ *   pendulum pitch and pitch rate, in the step's rows, upkie_b200_spine_obs, the final observation and final spine
+ *   observation, reset_obs and every entry of an observation history. IMU bias and noise (UPKIE_EP_IMU_*) are then
+ *   added in the true IMU frame as without a misalignment. Under an observation delay the misalignment is applied to
+ *   the sensed snapshot when the observation is built. A same-step terminal step's final observation and final spine
+ *   observation use the terminal episode's e_i, the reset observation the new one.
+ * - Not affected: the physics, terminated, truncated and the auto-resets (a fall is the simulator's judgement, as for
+ *   the observation delay), base_orientation.linear_velocity (world frame), the world-frame UPKIE_ST_IMU_ACC state
+ *   column, the servo rows and the wheel odometry, upkie_b200_get_state, contacts and push forces.
+ * Setting a spec draws nothing: each env keeps its e_i (the identity on a handle that never had a spec) until its next
+ * reset; NULL turns the feature off (the per-env state is freed once the device is idle). upkie_b200_set_state and
+ * explicit resets need nothing else: e_i depends on the draws only. Per-env state (get/set_imu_misalignment_state, for
+ * checkpoints and for fixed offsets chosen by the caller; device pointers): count[N] and quat[N][4];
+ * UPKIE_B200_EINVAL without a spec, or when a quaternion is not unit within 1e-5.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: a bound that is not finite, low > high, |bound| > pi/4 (a
+ * misalignment, not a remount), spine_mode (whose spine models its own IMU), joint_limits == 0 and body_contacts (it
+ * runs in the observation-delay kernels). upkie_b200_set_config rejects joint_limits = 0 and body_contacts while a spec
+ * is set; the in-kernel rollout transports reject a handle with one. The set call waits for the device. */
+typedef struct UpkieImuMisalignment {
+  float roll_low, roll_high;   /* radians, about the base x axis */
+  float pitch_low, pitch_high; /* radians, about the base y axis */
+  float yaw_low, yaw_high;     /* radians, about the base z axis */
+} UpkieImuMisalignment;
+int upkie_b200_set_imu_misalignment(void* handle, const UpkieImuMisalignment* spec);
+int upkie_b200_get_imu_misalignment_state(void* handle, uint32_t* count, float* quat, void* stream);
+int upkie_b200_set_imu_misalignment_state(void* handle, const uint32_t* count, const float* quat, void* stream);
+
 /* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
  * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
  * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last

@@ -416,6 +416,20 @@ class UpkieServoDropout(C.Structure):
 SERVO_HELD_DIM = 18  # the held rows of an env under servo dropouts: [joint][position, velocity, torque]
 
 
+class UpkieImuMisalignment(C.Structure):
+    """``UpkieImuMisalignment`` of include/upkie_b200.h: the ranges, in radians, of the roll, pitch and yaw of the IMU
+    mounting error each env draws at its resets (E = Rz(yaw) Ry(pitch) Rx(roll), a rotation in the base frame)."""
+
+    _fields_ = [
+        ("roll_low", C.c_float),
+        ("roll_high", C.c_float),
+        ("pitch_low", C.c_float),
+        ("pitch_high", C.c_float),
+        ("yaw_low", C.c_float),
+        ("yaw_high", C.c_float),
+    ]
+
+
 MAX_HISTORY = 64  # UPKIE_MAX_HISTORY: the most entries an observation history reports
 MAX_HISTORY_CHANNELS = 16  # UPKIE_MAX_HISTORY_CHANNELS: the most spine columns it records
 

@@ -62,6 +62,9 @@ SYMBOLS = {
     "upkie_b200_set_servo_dropout": (C.c_int, [_vp, C.POINTER(_abi.UpkieServoDropout)]),
     "upkie_b200_get_servo_dropout_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_set_servo_dropout_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp]),
+    "upkie_b200_set_imu_misalignment": (C.c_int, [_vp, C.POINTER(_abi.UpkieImuMisalignment)]),
+    "upkie_b200_get_imu_misalignment_state": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_set_imu_misalignment_state": (C.c_int, [_vp, _vp, _vp, _vp]),
     "upkie_b200_set_history": (C.c_int, [_vp, C.POINTER(_abi.UpkieHistory)]),
     "upkie_b200_get_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_history_entries": (C.c_int, [_vp, C.POINTER(C.c_int)]),

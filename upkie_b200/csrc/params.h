@@ -268,6 +268,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.obs_delay = nullptr;
   P.history = nullptr;
   P.servo_dropout = nullptr;
+  P.imu_misalign = nullptr;
   return 0;
 }
 
@@ -403,6 +404,22 @@ inline const char* servo_dropout_spec_error(const UpkieServoDropout& s, const Si
     return "set_servo_dropout: needs joint_limits != 0 (the dropouts run in the observation-delay kernels)";
   if (P.spine_mode) return "set_servo_dropout: spine_mode reports the spine's own servo replies";
   if (P.body_contacts) return "set_servo_dropout: body_contacts has no servo-dropout kernels";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses an IMU-misalignment spec (upkie_b200_set_imu_misalignment), null when it takes
+// it: every bound finite, low <= high and |bound| <= pi/4 (a misalignment, not a remount)
+inline const char* imu_misalignment_spec_error(const UpkieImuMisalignment& s, const SimParams& P) {
+  const float b[6] = {s.roll_low, s.roll_high, s.pitch_low, s.pitch_high, s.yaw_low, s.yaw_high};
+  for (int k = 0; k < 6; ++k)
+    if (!(b[k] >= -0.78539816f && b[k] <= 0.78539816f))
+      return "set_imu_misalignment: every bound must be finite and within [-pi/4, pi/4] radians";
+  for (int k = 0; k < 6; k += 2)
+    if (!(b[k] <= b[k + 1])) return "set_imu_misalignment: low <= high required for roll, pitch and yaw";
+  if (P.joint_limits == 0)
+    return "set_imu_misalignment: needs joint_limits != 0 (the misalignment runs in the observation-delay kernels)";
+  if (P.spine_mode) return "set_imu_misalignment: spine_mode models its spine's own IMU";
+  if (P.body_contacts) return "set_imu_misalignment: body_contacts has no IMU-misalignment kernels";
   return nullptr;
 }
 

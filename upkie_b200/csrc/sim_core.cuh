@@ -150,6 +150,9 @@ struct SimParams {
   // servo reply dropouts (upkie_b200_set_servo_dropout): the handle's device block, null = off. Read by the step kernels
   // of FAM_SENSE (step_family.h), k_reset, k_spine_obs and k_reset_obs only. Appended last, as history above.
   const struct ServoDropout* servo_dropout;
+  // IMU mounting misalignment (upkie_b200_set_imu_misalignment): the handle's device block, null = off. Read by the step
+  // kernels of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs and k_history_fill only. Appended last.
+  const struct ImuMisalign* imu_misalign;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -2172,6 +2175,85 @@ UPKIE_HD void servo_dropout_reset(const ServoDropout& D, uint64_t seed, uint64_t
   count[i] = k;
   prob[i] = servo_dropout_draw(spec, seed, g, k);
   servo_dropout_hold(S, ~0u, 0u, [&](int r, float v) { col[size_t(r) * stride] = v; });
+}
+
+// ---- IMU mounting misalignment (upkie_b200_set_imu_misalignment, BaseOrientation.h:29-35,106-112) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw, and quat = the unit quaternion e_i (w, x, y, z) of the env's misalignment, a rotation in the base
+// frame, [4][stride] structure-of-arrays like the state, env i in column i.
+struct ImuMisalign {
+  UpkieImuMisalignment spec;
+  uint32_t* count;
+  float* quat;
+  int stride;
+};
+
+// bit 57 of the high counter word, the per-reset draws of e_i: never set by sample_init_state (below 2^34), the noise
+// (below bit 42), the reset randomisation (bit 63), the pushes (62), the action delay (61), the observation delay (60)
+// or the servo dropouts (59, and 59 | 58), whose draw numbers stay below bit 36
+constexpr uint64_t kImuMisalignTag = uint64_t(1) << 57;
+
+struct Quat4 {
+  float q[4];  // w, x, y, z
+};
+
+// The unit quaternion of Rz(yaw) Ry(pitch) Rx(roll)
+UPKIE_HD Quat4 imu_misalign_quat(float roll, float pitch, float yaw) {
+  const float cr = cosf(0.5f * roll), sr = sinf(0.5f * roll);
+  const float cp = cosf(0.5f * pitch), sp = sinf(0.5f * pitch);
+  const float cy = cosf(0.5f * yaw), sy = sinf(0.5f * yaw);
+  Quat4 e;
+  e.q[0] = cr * cp * cy + sr * sp * sy;
+  e.q[1] = sr * cp * cy - cr * sp * sy;
+  e.q[2] = cr * sp * cy + sr * cp * sy;
+  e.q[3] = cr * cp * sy - sr * sp * cy;
+  return e;
+}
+
+// Draw k of the env of global index g: words 0, 1, 2 give roll, pitch and yaw, push_value's exact form (the map of the
+// servo dropouts), and the result is the quaternion of the misalignment they make
+UPKIE_HD Quat4 imu_misalign_draw(const UpkieImuMisalignment& s, uint64_t seed, uint64_t g, uint32_t k) {
+  const Philox4 r = philox4x32_10(g, kImuMisalignTag | (uint64_t(k) << 4), seed);
+  return imu_misalign_quat(push_value(r.v[0], s.roll_low, s.roll_high), push_value(r.v[1], s.pitch_low, s.pitch_high),
+                           push_value(r.v[2], s.yaw_low, s.yaw_high));
+}
+
+// The observed state of S under the misalignment e: its base orientation becomes R E (quat <- quat (x) e), so that
+// every orientation-derived observation is that of an IMU tilted by E while the pipeline assumes the nominal mounting.
+// Nothing else changes: the twist is world-frame and the IMU acceleration of the state is world-frame too. The identity
+// leaves S bit for bit (the product would turn a -0 component into +0); returns whether S changed.
+UPKIE_HD bool imu_misalign_view(RobotState& S, const Quat4& e) {
+  if (e.q[1] == 0.f && e.q[2] == 0.f && e.q[3] == 0.f) return false;
+  const float w = S.quat[0], x = S.quat[1], y = S.quat[2], z = S.quat[3];
+  S.quat[0] = w * e.q[0] - x * e.q[1] - y * e.q[2] - z * e.q[3];
+  S.quat[1] = w * e.q[1] + x * e.q[0] + y * e.q[3] - z * e.q[2];
+  S.quat[2] = w * e.q[2] - x * e.q[3] + y * e.q[0] + z * e.q[1];
+  S.quat[3] = w * e.q[3] + x * e.q[2] - y * e.q[1] + z * e.q[0];
+  return true;
+}
+
+// Env i's misalignment, load(row) of its column
+template <typename Load>
+UPKIE_HD Quat4 imu_misalign_load(Load load) {
+  Quat4 e;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) e.q[r] = load(r);
+  return e;
+}
+
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, stored; the new e_i. The block's fields
+// are copied before the first store, as servo_dropout_reset.
+UPKIE_HD Quat4 imu_misalign_reset(const ImuMisalign& M, uint64_t seed, uint64_t g, int i) {
+  const UpkieImuMisalignment spec = M.spec;
+  uint32_t* const count = M.count;
+  float* const col = M.quat + size_t(i);
+  const size_t stride = size_t(M.stride);
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  const Quat4 e = imu_misalign_draw(spec, seed, g, k);
+#pragma unroll
+  for (int r = 0; r < 4; ++r) col[size_t(r) * stride] = e.q[r];
+  return e;
 }
 
 }  // namespace upkie_b200

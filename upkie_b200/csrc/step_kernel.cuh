@@ -134,9 +134,10 @@ __device__ __forceinline__ float* obs_delay_report(const ObsDelay& O, uint32_t s
 // IMU velocity differentiated over the substep against `vel` (updated in place) when `acc`; and the fill of the whole
 // column with the columns of S. Out of line: the calls pass a copy of the state, and the kernel's own arithmetic is
 // compiled (and its products contracted) as without the history.
-// Under servo dropouts the servos of `lost` report env i's held triple, as the observation does.
+// Under servo dropouts the servos of `lost` report env i's held triple, as the observation does; under an IMU
+// misalignment the columns are read through the env's `em` (after the IMU velocity, which is the true IMU's).
 __device__ __noinline__ void history_substep(const SimParams& P, RobotState S, float* vel, float* e,
-                                             size_t stride, int count, bool acc, uint32_t lost, int i) {
+                                             size_t stride, int count, bool acc, uint32_t lost, int i, const Quat4 em) {
   if (lost) {
     const ServoDropout& D = *P.servo_dropout;
     const float* const held = D.held + size_t(i);
@@ -152,10 +153,12 @@ __device__ __noinline__ void history_substep(const SimParams& P, RobotState S, f
       vel[k] = v[k];
     }
   }
+  imu_misalign_view(S, em);
   for (int c = 0; c < count; ++c) __stcg(e + size_t(c) * stride, history_value(P, S, a, __ldg(P.history->columns + c)));
 }
-__device__ __noinline__ void history_fill_lane(const SimParams& P, const RobotState S, float* col, size_t stride,
-                                               int count, uint32_t ticks) {
+__device__ __noinline__ void history_fill_lane(const SimParams& P, RobotState S, float* col, size_t stride,
+                                               int count, uint32_t ticks, const Quat4 em) {
+  imu_misalign_view(S, em);
   for (int c = 0; c < count; ++c) {
     const float v = history_value(P, S, S.imu_acc, __ldg(P.history->columns + c));
     for (uint32_t e = 0; e < ticks; ++e) __stcg(col + (size_t(e) * size_t(count) + size_t(c)) * stride, v);
@@ -202,6 +205,19 @@ __device__ __noinline__ void dropout_sense(const SimParams& P, uint32_t lost, in
 __device__ __noinline__ void dropout_reset_lane(const SimParams& P, const RobotState S, uint64_t seed, uint64_t g,
                                                 int i) {
   servo_dropout_reset(*P.servo_dropout, seed, g, i, S);
+}
+
+// The IMU misalignment (F.sense kernels, P.imu_misalign set): env i's e_i, loaded once per lane (coherent loads: a
+// lane that resets stores its next draw in the same launch), and a reset's next draw, stored (out of line, as
+// dropout_reset_lane: the Philox rounds and the trigonometry are not inlined into the kernel twice)
+__device__ __forceinline__ Quat4 tilt_load_lane(const SimParams& P, int i) {
+  const ImuMisalign& M = *P.imu_misalign;
+  const float* const col = M.quat + size_t(i);
+  const size_t stride = size_t(M.stride);
+  return imu_misalign_load([&](int r) { return __ldcg(col + size_t(r) * stride); });
+}
+__device__ __noinline__ Quat4 tilt_reset_lane(const SimParams& P, uint64_t seed, uint64_t g, int i) {
+  return imu_misalign_reset(*P.imu_misalign, seed, g, i);
 }
 
 // ---- one env tick of the robot `tid` --------------------------------------------------
@@ -457,6 +473,20 @@ __device__ __forceinline__ void step_env(
     const ServoDropout& D = *P.servo_dropout;
     return __ldcg(D.held + size_t(r) * size_t(D.stride) + size_t(i));
   };
+  // IMU mounting misalignment (F.sense kernels, P.imu_misalign set: a uniform branch). `em` is the lane's e_i: loaded
+  // once, or drawn here by a next-step reset and at the same-step reset below. Every observation of the tick is built
+  // from a copy of the state whose orientation is read through it (imu_misalign_view): the history entries, the
+  // same-step final observation and stash (the terminal episode's e_i), and the observation. The physics, the
+  // terminations and the stored state keep the true orientation. Without the feature `em` is the identity, which
+  // imu_misalign_view leaves out.
+  const bool tilting = F.sense && P.imu_misalign;
+  Quat4 em{{1.f, 0.f, 0.f, 0.f}};
+  if constexpr (F.sense) {
+    if (tilting) {
+      if (!resetting) em = tilt_load_lane(P, i);
+      else if (live) em = tilt_reset_lane(P, seed, env_offset + uint64_t(i), i);
+    }
+  }
   auto sense_load = [&](int k) { return __ldcg(scol + size_t(k) * sstride); };
   auto sense_store = [&](int k, float v) { __stcg(scol + size_t(k) * sstride, v); };
   if (sensing && live && sdl == uint32_t(P.nb_substeps)) {  // the state at the start of the tick
@@ -536,7 +566,7 @@ __device__ __forceinline__ void step_env(
       }
       if (recording && !resetting && live)
         history_substep(P, S, hvel, hring + size_t((hhead + uint32_t(sub)) % hticks) * size_t(hcount) * hstride,
-                        hstride, hcount, hacc, dcur, i);
+                        hstride, hcount, hacc, dcur, i, em);
     } else {
 #pragma unroll
       for (int k = 0; k < kPhaseSyncs; ++k) PhaseSync()();
@@ -584,6 +614,7 @@ __device__ __forceinline__ void step_env(
 
   bool fin_pending = false;  // F.sense, same-step reset: the terminal observation is stashed after the tick
   float fin_o6[6], fin_yaw = 0.f, fin_yaw_vel = 0.f;
+  const Quat4 fin_e = em;  // the terminal episode's misalignment (a same-step reset draws the next one into em)
   if (AUTORESET == AUTORESET_SAME_STEP) {
     if (term || trunc) {
       if constexpr (F.sense) {
@@ -606,6 +637,11 @@ __device__ __forceinline__ void step_env(
           for (int j = 0; j < UPKIE_NJ; ++j) dtrue[j] = S.torque[j];
           servo_dropout_view(S, dcur, dheld);
           if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
+        }
+        // the misalignment: they report the terminal episode's sensed orientation (the reset below overwrites the
+        // orientation whole, reset_pose)
+        if constexpr (F.sense) {
+          if (tilting && imu_misalign_view(S, em) && MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
         }
         if (P.final_obs && live)
           store_final_obs<MODE, spine>(P, S, L, o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
@@ -631,6 +667,9 @@ __device__ __forceinline__ void step_env(
       elapsed = 0;
       refill = true;
       dreset = true;
+      if constexpr (F.sense) {
+        if (tilting && live) em = tilt_reset_lane(P, seed, env_offset + uint64_t(i), i);  // the new episode's e_i
+      }
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
       float init[UPKIE_INIT_DIM];
@@ -651,7 +690,7 @@ __device__ __forceinline__ void step_env(
   // the history: a reset fills the lane's ring from its post-reset state (the true state, here in S), and every lane's
   // head moves on by the tick's substeps
   if (recording && live) {
-    if (refill) history_fill_lane(P, S, hring, hstride, hcount, hticks);
+    if (refill) history_fill_lane(P, S, hring, hstride, hcount, hticks, em);
     __stcg(P.history->head + i, (hhead + uint32_t(P.nb_substeps)) % hticks);
   }
   // the dropouts: a reset latches the lane's post-reset state (the true state, here in S) and draws its next p_i
@@ -668,7 +707,9 @@ __device__ __forceinline__ void step_env(
       S.yaw = fin_yaw;
       S.yaw_vel = fin_yaw_vel;
       obs_delay_sensed_state(S, sense_load);
-      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0)) gyropod_obs(P, S, fin_o6);  // (a dropout patched the snapshot)
+      const bool ftilt = tilting && imu_misalign_view(S, fin_e);  // the terminal episode's sensed orientation
+      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0 || ftilt))
+        gyropod_obs(P, S, fin_o6);  // (a dropout patched the snapshot, or the orientation is the sensed one)
       if (P.final_obs && live)
         store_final_obs<MODE, spine>(P, S, L, fin_o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
       if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
@@ -701,6 +742,11 @@ __device__ __forceinline__ void step_env(
   if (F.sense && dropping && !sensing && !dreset && dcur) {
     servo_dropout_view(S, dcur, dheld);
     if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
+  }
+  // the misalignment: the gyropod and pendulum rows report the sensed orientation of the state they are built from,
+  // the snapshot under an observation delay (the true state is stored above; UpkieServos rows hold no orientation)
+  if constexpr (F.sense && MODE != MODE_SERVOS) {
+    if (tilting && imu_misalign_view(S, em)) gyropod_obs(P, S, o6);
   }
   if (spine && live) {
     float lr[UPKIE_LAG_DIM];

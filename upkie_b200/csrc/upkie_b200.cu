@@ -14,6 +14,8 @@
 //   k_history_read / k_history_fill   the observation history's entries of each env / its ring filled from the state.
 // The servo dropouts' held rows take no kernel of their own: k_reset latches, k_ring_copy copies them for checkpoints,
 // and a new spec or set_state latches the state with device copies of its rows (servo_dropout_latch).
+// The IMU misalignment takes none either: k_reset draws, k_ring_copy copies its quaternions for checkpoints, and
+// k_spine_obs, k_reset_obs and k_history_fill read the orientation through it (imu_misalign_observed).
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -21,6 +23,7 @@
 
 #include <cuda_runtime.h>
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -28,6 +31,7 @@
 #include <new>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "mpc.cuh"
 #include "base_velocity.cuh"
@@ -143,6 +147,11 @@ struct Handle {
   float* drop_prob = nullptr;
   float* drop_held = nullptr;  // [kServoHeldRows][n_pad]
   uint32_t drop_mask = 0;      // joint_mask of the spec in force
+  // IMU mounting misalignment (upkie_b200_set_imu_misalignment): the device block P.imu_misalign points to while a spec
+  // is set, and the per-env state it points to (allocated with the first spec, freed when it is turned off)
+  ImuMisalign* tilt_dev = nullptr;
+  uint32_t* tilt_count = nullptr;
+  float* tilt_quat = nullptr;  // [4][n_pad], e_i (w, x, y, z)
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -234,8 +243,23 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
     for (int k = 0; k < UPKIE_STATE_DIM; ++k) col[size_t(k) * size_t(O.stride)] = r[k];
     if (O.ticks > 1) obs_delay_fill_history(O, i, r);
   }
-  if (P.history) history_fill(*P.history, P, S, i);  // a new episode's history starts from its post-reset columns
+  // the misalignment's next draw, before the history: the new episode is observed through it
+  Quat4 e{{1.f, 0.f, 0.f, 0.f}};
+  if (P.imu_misalign) e = imu_misalign_reset(*P.imu_misalign, rand_seed, g, i);
+  if (P.history) {  // a new episode's history starts from its post-reset columns
+    RobotState V = S;
+    imu_misalign_view(V, e);
+    history_fill(*P.history, P, V, i);
+  }
   if (P.servo_dropout) servo_dropout_reset(*P.servo_dropout, rand_seed, g, i, S);  // a new p_i, the reset latched
+}
+
+// The IMU misalignment: the observed orientation of S, read through env i's e_i (the state or a sensed row: under an
+// observation delay the misalignment is applied to the snapshot when the observation is built)
+__device__ void imu_misalign_observed(const SimParams& P, int i, RobotState& S) {
+  if (!P.imu_misalign) return;
+  const ImuMisalign& M = *P.imu_misalign;
+  imu_misalign_view(S, imu_misalign_load([&](int r) { return M.quat[size_t(r) * size_t(M.stride) + size_t(i)]; }));
 }
 
 // Servo dropouts without an observation delay: the observed state of S, every servo of the mask reporting its held
@@ -273,6 +297,7 @@ __global__ void k_history_fill(const __grid_constant__ SimParams P, const Histor
   if (i >= n) return;
   RobotState S;
   load_state(state, n_pad, i, S);
+  imu_misalign_observed(P, i, S);
   history_fill(*H, P, S, i);
 }
 
@@ -298,7 +323,10 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
   } else {
     RobotState S;
     load_state(state, n_pad, i, S);
-    if (!mark) servo_dropout_observed(P, i, S);  // (the stash holds the terminal step's observed state)
+    if (!mark) {  // (the stash holds the terminal step's observed state)
+      servo_dropout_observed(P, i, S);
+      imu_misalign_observed(P, i, S);
+    }
     float tq[6];
     measured_torques(P, S, &nz, tq, i);
     spine_observation(P, S, o, tq);
@@ -316,6 +344,7 @@ __global__ void k_reset_obs(const __grid_constant__ SimParams P, int n, int n_pa
   RobotState S;
   load_state(state, n_pad, i, S);
   servo_dropout_observed(P, i, S);
+  imu_misalign_observed(P, i, S);
   if (obs_dim == UPKIE_OBS_DIM && P.spine_mode && lag) {
     for (int j = 0; j < 6; ++j) {
       float* o = out + size_t(i) * UPKIE_OBS_DIM + j * 5;
@@ -980,6 +1009,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->sense_hist); cudaFree(h->sense_head);
   cudaFree(h->hist_dev); cudaFree(h->hist_ring); cudaFree(h->hist_head);
   cudaFree(h->drop_dev); cudaFree(h->drop_count); cudaFree(h->drop_prob); cudaFree(h->drop_held);
+  cudaFree(h->tilt_dev); cudaFree(h->tilt_count); cudaFree(h->tilt_quat);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -1027,6 +1057,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: servo dropouts need joint_limits != 0");
   if (h->P.servo_dropout && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no servo-dropout kernels");
+  if (h->P.imu_misalign && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: IMU misalignment needs joint_limits != 0");
+  if (h->P.imu_misalign && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no IMU-misalignment kernels");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -1048,6 +1082,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.obs_delay = h->P.obs_delay;        // and the observation delay
   P.history = h->P.history;            // and the observation history
   P.servo_dropout = h->P.servo_dropout;  // and the servo dropouts
+  P.imu_misalign = h->P.imu_misalign;    // and the IMU misalignment
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -2033,6 +2068,79 @@ int upkie_b200_set_servo_dropout_state(void* handle, const uint32_t* count, cons
   CUDA_TRY(cudaMemcpyAsync(h->drop_count, count, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(cudaMemcpyAsync(h->drop_prob, prob, bytes, cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(ring_cols(held, kServoHeldRows, h->n, h->n_pad, h->drop_held, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_imu_misalignment(void* handle, const UpkieImuMisalignment* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    if (h->P.imu_misalign) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the per-env state
+      h->P.imu_misalign = nullptr;
+      cudaFree(h->tilt_count);
+      cudaFree(h->tilt_quat);
+      h->tilt_count = nullptr;
+      h->tilt_quat = nullptr;
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = imu_misalignment_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
+  if (!h->P.imu_misalign) {
+    // switched on: zero counters, and the identity as every env's misalignment until its next reset
+    CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->tilt_count), size_t(h->n) * sizeof(uint32_t)},
+                           {reinterpret_cast<void**>(&h->tilt_quat), size_t(4) * h->n_pad * sizeof(float)}}));
+    CUDA_TRY(fill(h->n, h->tilt_quat, 1.f, nullptr));
+  }
+  if (!h->tilt_dev) CUDA_TRY(cudaMalloc(&h->tilt_dev, sizeof(ImuMisalign)));
+  ImuMisalign M;
+  std::memset(&M, 0, sizeof(M));
+  M.spec = *spec;
+  M.count = h->tilt_count;
+  M.quat = h->tilt_quat;
+  M.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->tilt_dev, &M, sizeof(M), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->P.imu_misalign = h->tilt_dev;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_imu_misalignment_state(void* handle, uint32_t* count, float* quat, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !quat) return fail(UPKIE_B200_EINVAL, "get_imu_misalignment_state: invalid argument");
+  if (!h->P.imu_misalign)
+    return fail(UPKIE_B200_EINVAL,
+                "get_imu_misalignment_state: no IMU misalignment is set (upkie_b200_set_imu_misalignment)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemcpyAsync(count, h->tilt_count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_rows(h->tilt_quat, 4, h->n, h->n_pad, quat, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_imu_misalignment_state(void* handle, const uint32_t* count, const float* quat, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !quat) return fail(UPKIE_B200_EINVAL, "set_imu_misalignment_state: invalid argument");
+  if (!h->P.imu_misalign)
+    return fail(UPKIE_B200_EINVAL,
+                "set_imu_misalignment_state: no IMU misalignment is set (upkie_b200_set_imu_misalignment)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // every quaternion must be a rotation: read back (after the caller's work on the stream) and checked here
+  std::vector<float> q(size_t(h->n) * 4);
+  CUDA_TRY(cudaMemcpyAsync(q.data(), quat, q.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (int i = 0; i < h->n; ++i) {
+    const double w = q[4 * i], x = q[4 * i + 1], y = q[4 * i + 2], z = q[4 * i + 3];
+    const double norm = std::sqrt(w * w + x * x + y * y + z * z);
+    if (!(std::fabs(norm - 1.0) <= 1e-5))
+      return fail(UPKIE_B200_EINVAL, "set_imu_misalignment_state: every quaternion must be unit (within 1e-5)");
+  }
+  CUDA_TRY(cudaMemcpyAsync(h->tilt_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_cols(quat, 4, h->n, h->n_pad, h->tilt_quat, s));
   return UPKIE_B200_OK;
 }
 

@@ -755,6 +755,63 @@ def servo_dropout_spec(prob, joints=None, spine_mode: bool = False, joint_limits
     return _abi.UpkieServoDropout(lo, hi, mask, 0)
 
 
+_IMU_MISALIGNMENT_MAX = np.float32(np.pi / 4)  # the largest |bound| (the C check compares float32 values)
+
+
+def imu_misalignment_spec(misalignment, spine_mode: bool = False, joint_limits: Union[bool, int] = True,
+                          body_contacts: Union[bool, int] = False) -> Optional[_abi.UpkieImuMisalignment]:
+    """``UpkieImuMisalignment`` (``UpkieSim.set_imu_misalignment``) from a dict with any of the keys ``roll``,
+    ``pitch`` and ``yaw`` (radians), each a fixed angle or a ``(low, high)`` range every reset draws the env's angle
+    from; a missing key is 0. Raises ``UpkieException`` on an unknown key, a bound that is not a finite number, ``low >
+    high``, ``|bound| > pi/4`` (a misalignment, not a remount), ``spine_mode`` (whose spine models its own IMU), no
+    joint limits and ``body_contacts`` (the misalignment runs in the kernels of the observation delay)."""
+    if misalignment is None:
+        return None
+    if not isinstance(misalignment, dict):
+        raise UpkieException(f"imu_misalignment: expected a dict of roll / pitch / yaw ranges, got {misalignment!r}")
+    unknown = sorted(set(misalignment) - {"roll", "pitch", "yaw"})
+    if unknown:
+        raise UpkieException(f"imu_misalignment: unknown key(s) {unknown}, expected roll, pitch and yaw")
+    bounds = []
+    for key in ("roll", "pitch", "yaw"):
+        r = misalignment.get(key, 0.0)
+        if isinstance(r, (int, float, np.integer, np.floating)):
+            lo, hi = r, r
+        else:
+            try:
+                lo, hi = r
+            except (TypeError, ValueError):
+                raise UpkieException(f"imu_misalignment: {key}: expected an angle or a (low, high) pair, got {r!r}") \
+                    from None
+        try:
+            lo, hi = np.float32(lo), np.float32(hi)
+        except (TypeError, ValueError):
+            raise UpkieException(f"imu_misalignment: {key}: expected angles, got ({lo!r}, {hi!r})") from None
+        if not (np.isfinite(lo) and np.isfinite(hi)) or max(abs(lo), abs(hi)) > _IMU_MISALIGNMENT_MAX:
+            raise UpkieException(f"imu_misalignment: {key}: expected finite angles within [-pi/4, pi/4] radians, got "
+                                 f"({lo}, {hi})")
+        if lo > hi:
+            raise UpkieException(f"imu_misalignment: {key}: expected low <= high, got ({lo}, {hi})")
+        bounds += [float(lo), float(hi)]
+    if spine_mode:
+        raise UpkieException("imu_misalignment: spine_mode models its spine's own IMU; the misalignment is not "
+                             "available there")
+    if not joint_limits:
+        raise UpkieException("imu_misalignment: needs joint_limits (the misalignment runs in the kernels with "
+                             "joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("imu_misalignment: body_contacts has no IMU-misalignment kernels")
+    return _abi.UpkieImuMisalignment(*bounds)
+
+
+def _set_imu_misalignment(sim, spec: Optional[_abi.UpkieImuMisalignment]) -> None:
+    if spec is None:
+        sim.set_imu_misalignment(None)
+    else:
+        sim.set_imu_misalignment((spec.roll_low, spec.roll_high), (spec.pitch_low, spec.pitch_high),
+                                 (spec.yaw_low, spec.yaw_high))
+
+
 class B200VectorEnv(VectorEnv):
     """N Upkie environments stepped by one kernel launch per ``step()``.
 
@@ -832,6 +889,14 @@ class B200VectorEnv(VectorEnv):
     (the gyropod and pendulum wheel odometry too), the spine observation and the history. The physics, terminations
     and ``get_state`` see the true state. The draws are keyed on the seed of ``reset(seed=s)``, which also restarts the
     draw counters of the envs it resets. ``set_servo_dropout`` changes or (``None``) stops it.
+
+    ``imu_misalignment`` (a dict of ``roll`` / ``pitch`` / ``yaw`` angles or ``(low, high)`` ranges in radians, see
+    ``imu_misalignment_spec``) mounts each env's IMU off its nominal pose by a rotation drawn at every reset of the env,
+    while the observers still assume the nominal ``rotation_base_to_imu`` (``BaseOrientation.h``): the base pitch, its
+    rate and rotation, the IMU orientation, rates and accelerations that every env type observes (the gyropod and
+    pendulum pitch and pitch rate, the spine observation, the history) are those the tilted IMU reports. The physics,
+    terminations and ``get_state`` see the true state. The draws are keyed on the seed of ``reset(seed=s)``, which also
+    restarts the draw counters of the envs it resets. ``set_imu_misalignment`` changes or (``None``) stops it.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -874,6 +939,7 @@ class B200VectorEnv(VectorEnv):
         history_size: int = 1,
         servo_dropout: Optional[Union[float, Tuple[float, float]]] = None,
         servo_dropout_joints: Optional[Sequence[str]] = None,
+        imu_misalignment: Optional[Dict[str, Union[float, Tuple[float, float]]]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -925,6 +991,8 @@ class B200VectorEnv(VectorEnv):
                                  bool(config.body_contacts))  # validated before any device is touched
         drop_spec = servo_dropout_spec(servo_dropout, servo_dropout_joints, bool(config.spine_mode),
                                        config.joint_limits, config.body_contacts)  # validated before any device
+        tilt_spec = imu_misalignment_spec(imu_misalignment, bool(config.spine_mode), config.joint_limits,
+                                          config.body_contacts)  # validated before any device is touched
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -986,6 +1054,15 @@ class B200VectorEnv(VectorEnv):
         if drop_spec is not None:
             # before the first reset, which draws every env's probability
             self.sim.set_servo_dropout(drop_spec.prob_low, drop_spec.prob_high, servo_dropout_joints)
+        if tilt_spec is not None:
+            _set_imu_misalignment(self.sim, tilt_spec)  # before the first reset, which draws every env's misalignment
+
+    def set_imu_misalignment(self, misalignment) -> None:
+        """Mount each env's IMU off its nominal pose by ``roll`` / ``pitch`` / ``yaw`` angles or ranges (a dict,
+        ``imu_misalignment_spec``); ``None`` turns the misalignment off. New ranges take effect at each env's next
+        reset."""
+        _set_imu_misalignment(self.sim, imu_misalignment_spec(misalignment, bool(self.config.spine_mode),
+                                                              self.config.joint_limits, self.config.body_contacts))
 
     def set_servo_dropout(self, prob, joints=None) -> None:
         """Lose the replies of the servos ``joints`` (names, None: all) with a per-cycle probability ``prob``, a float
@@ -1201,6 +1278,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_servo_dropout_state(count, prob, held)
+            if self.sim.imu_misalignment_spec is not None:
+                # so is the IMU misalignment
+                count, quat = self.sim.get_imu_misalignment_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_imu_misalignment_state(count, quat)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

@@ -340,6 +340,48 @@ class UpkieSim:
         self._check_tensor(held, (self.n, _abi.NJ, 3), name="held")
         check(lib().upkie_b200_set_servo_dropout_state(self._h, _ptr(count), _ptr(prob), _ptr(held), self._stream()))
 
+    def set_imu_misalignment(self, roll: Optional[Tuple[float, float]] = (0.0, 0.0),
+                             pitch: Tuple[float, float] = (0.0, 0.0), yaw: Tuple[float, float] = (0.0, 0.0)) -> None:
+        """While ranges are set, each env's IMU is mounted off its nominal pose by E = Rz(yaw) Ry(pitch) Rx(roll), the
+        three angles (radians) drawn from ``(low, high)`` ranges at every reset of the env (keyed on the auto-reset seed
+        and the env's counter, ``include/upkie_b200.h``). Every orientation-derived observation (base pitch, angular
+        velocity and rotation, the IMU orientation, rates and accelerations, the gyropod and pendulum pitch and rate)
+        is that of a base oriented R E instead of R; the physics, terminations and ``get_state`` see the true state.
+        ``roll=None`` turns the misalignment off. Setting ranges draws nothing: they take effect at each env's next
+        reset."""
+        if roll is None:
+            check(lib().upkie_b200_set_imu_misalignment(self._h, None))
+            self._imu_misalignment = None
+            return
+        spec = _abi.UpkieImuMisalignment(*(float(v) for r in (roll, pitch, yaw) for v in r))
+        check(lib().upkie_b200_set_imu_misalignment(self._h, C.byref(spec)))
+        self._imu_misalignment = ((spec.roll_low, spec.roll_high), (spec.pitch_low, spec.pitch_high),
+                                  (spec.yaw_low, spec.yaw_high))
+
+    @property
+    def imu_misalignment_spec(self) -> Optional[Tuple[Tuple[float, float], ...]]:
+        """``((roll_low, roll_high), (pitch_low, pitch_high), (yaw_low, yaw_high))`` in force, or None."""
+        return getattr(self, "_imu_misalignment", None)
+
+    def get_imu_misalignment_state(self):
+        """Per-env IMU-misalignment state ``(count[N], quat[N, 4])``: the draw counters (int32 bits of uint32) and each
+        env's misalignment as a unit quaternion (w, x, y, z)."""
+        if self.imu_misalignment_spec is None:
+            raise UpkieException("no IMU misalignment is set (set_imu_misalignment)")
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        quat = torch.empty((self.n, 4), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_imu_misalignment_state(self._h, _ptr(count), _ptr(quat), self._stream()))
+        return count, quat
+
+    def set_imu_misalignment_state(self, count: torch.Tensor, quat: torch.Tensor) -> None:
+        """Set every env's draw counter and misalignment quaternion (w, x, y, z), unit within 1e-5: a checkpoint, or
+        fixed offsets of the caller's choice (kept until each env's next reset)."""
+        if self.imu_misalignment_spec is None:
+            raise UpkieException("no IMU misalignment is set (set_imu_misalignment)")
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(quat, (self.n, 4), name="quat")
+        check(lib().upkie_b200_set_imu_misalignment_state(self._h, _ptr(count), _ptr(quat), self._stream()))
+
     def set_history(self, columns: Optional[Sequence[int]], size: int = 1) -> None:
         """Record each env's spine-observation ``columns`` (``_abi.SP_*``, 1 to ``MAX_HISTORY_CHANNELS`` of them) after
         every substep, and report the last ``size`` (1 to ``MAX_HISTORY``) through ``get_history``: the spine's
@@ -800,6 +842,10 @@ class UpkieSim:
             sd["servo_dropout"] = self.servo_dropout_spec
             sd["servo_dropout_count"], sd["servo_dropout_prob"], sd["servo_dropout_held"] = \
                 self.get_servo_dropout_state()
+        # the IMU misalignment: its ranges and the per-env state (absent without a spec)
+        if self.imu_misalignment_spec is not None:
+            sd["imu_misalignment"] = self.imu_misalignment_spec
+            sd["imu_misalignment_count"], sd["imu_misalignment_quat"] = self.get_imu_misalignment_state()
         sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
@@ -909,6 +955,14 @@ class UpkieSim:
             self.set_servo_dropout(drop[0], drop[1], [n for j, n in enumerate(_abi.JOINT_NAMES) if (drop[2] >> j) & 1])
             self.set_servo_dropout_state(*(sd[k].to(dev).contiguous() for k in (
                 "servo_dropout_count", "servo_dropout_prob", "servo_dropout_held")))
+        # the IMU misalignment; a checkpoint without one (or written before it existed) turns it off
+        tilt = sd.get("imu_misalignment")
+        if tilt is None:
+            self.set_imu_misalignment(None)
+        else:
+            self.set_imu_misalignment(*tilt)
+            self.set_imu_misalignment_state(*(sd[k].to(dev).contiguous() for k in (
+                "imu_misalignment_count", "imu_misalignment_quat")))
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
