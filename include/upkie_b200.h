@@ -896,6 +896,61 @@ int upkie_b200_set_imu_misalignment(void* handle, const UpkieImuMisalignment* sp
 int upkie_b200_get_imu_misalignment_state(void* handle, uint32_t* count, float* quat, void* stream);
 int upkie_b200_set_imu_misalignment_state(void* handle, const uint32_t* count, const float* quat, void* stream);
 
+/* ---- Servo encoder zero offsets (pi3hat_spine.cpp:181-236, moteus/QueryResult.h:33-39) --------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. The hip and knee servos are zeroed by hand
+ * (upkie_tool rezero); each servo then reports its encoder position, and its position loop tracks targets in that same
+ * frame. A leg zeroed off by delta reports every position shifted by delta and lands every target shifted by it.
+ * While a spec is set:
+ * - Draw per reset: at every reset of env i (both fused auto-resets, upkie_b200_reset with or without a mask or host
+ *   rows) an offset per joint is drawn. Draw law: a per-env counter k, +1 at every reset; draw k of the env of global
+ *   index g = env_offset + i is Philox4x32-10 with key seed (upkie_b200_set_autoreset) and counters
+ *   (g, 2^56 | k << 4 | b), b = 0, 1; word j % 4 of block b = j / 4 gives delta_ij = min(low + fl(fl(high - low) *
+ *   u(w)), high), u(w) = (w >> 8) / 2^24 (the servo dropouts' map). Every joint's word is drawn whatever the mask, and a
+ *   joint outside joint_mask gets exactly 0, so that changing the mask changes no other joint's draw. Tag bit 56 keeps
+ *   these counters apart from the initial states (below 2^34), the noise (below bit 42), the reset randomisation (bit
+ *   63), the pushes (62), the action delay (61), the observation delay (60), the servo dropouts (59, 59 | 58) and the
+ *   IMU misalignment (57).
+ * - Model: the servo frame is the joint frame shifted by delta, q_servo = q + delta. Everything the agent and the
+ *   wrapper exchange with the servos is in the servo frame:
+ *   - reported positions are q_j + delta_ij: the [6][5] and compact [6][3] servo rows, the servo block of
+ *     upkie_b200_spine_obs and of the final spine observation, the wheel odometry position (wheels in the mask), the
+ *     gyropod and pendulum p, final_obs, reset_obs, and the servo-position and odometry columns of every entry of an
+ *     observation history;
+ *   - executed position targets are target - delta_ij, after the action clamps (which stay in the servo frame); a NaN
+ *     target stays NaN;
+ *   - the gyropod, pendulum and base-velocity leg targets (UPKIE_ST_LEG_TARGET) are servo-frame values: a reset sets
+ *     them from the reported positions q + delta with the new episode's offsets, and they decay toward the servo zero,
+ *     so that the legs settle at the physical angle -delta.
+ * - Not affected: velocities and torques (torque measurement noise included), the joint-limit rows (on the true q),
+ *   terminated, truncated and the auto-resets, and the q of upkie_b200_get_state, whose leg-target columns hold the
+ *   servo-frame targets above.
+ * - Episode boundaries: a same-step terminal step's final observation and final spine observation use the terminal
+ *   episode's offsets, the reset observation and the history refilled at the reset the new ones.
+ * - Composition: the offset is applied last, when an observation is built: under an observation delay to the delayed
+ *   snapshot, under servo dropouts to the latched values. The dropouts' held rows, the observation-delay rows and
+ *   their get/set state keep true joint values. The action-delay buffers (and get/set_action_delay_history) hold the
+ *   commands as the agent sent them; the shift applies to the row the substeps execute.
+ * - Off is free: with the spec off, or low = high = 0, every output is bit for bit the same handle's without a spec.
+ * Setting a spec draws nothing: each env keeps its offsets (zeros on a handle that never had a spec) until its next
+ * reset; a spec that replaces another zeroes the offsets of the joints it drops from the mask; NULL turns the feature
+ * off (the per-env state is freed once the device is idle). Per-env state (get/set_encoder_offset_state, for
+ * checkpoints and for fixed offsets measured on a robot; device pointers): count[N] and offset[N][6];
+ * UPKIE_B200_EINVAL without a spec, for a value that is not finite or |value| > 0.5, and for a nonzero value of a joint
+ * outside the mask.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: a bound that is not finite, low > high, |bound| > 0.5 rad (a
+ * calibration error, not a remount), a joint_mask of zero or with bits above 5, spine_mode (whose spine reports its
+ * own servos), joint_limits == 0 and body_contacts (it runs in the observation-delay kernels).
+ * upkie_b200_set_config rejects joint_limits = 0 and body_contacts while a spec is set; the in-kernel rollout
+ * transports reject a handle with one. The set call waits for the device. */
+typedef struct UpkieEncoderOffset {
+  float low, high;     /* radians, range of each joint's zero offset */
+  uint32_t joint_mask; /* bit j: joint j (UPKIE_NJ order) has an offset */
+  uint32_t reserved;   /* 0 */
+} UpkieEncoderOffset;
+int upkie_b200_set_encoder_offset(void* handle, const UpkieEncoderOffset* spec);
+int upkie_b200_get_encoder_offset_state(void* handle, uint32_t* count, float* offset, void* stream);
+int upkie_b200_set_encoder_offset_state(void* handle, const uint32_t* count, const float* offset, void* stream);
+
 /* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
  * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
  * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last

@@ -430,6 +430,21 @@ class UpkieImuMisalignment(C.Structure):
     ]
 
 
+class UpkieEncoderOffset(C.Structure):
+    """``UpkieEncoderOffset`` of include/upkie_b200.h: the range, in radians, of the encoder zero offset each joint of
+    ``joint_mask`` draws at every reset of its env (the servo frame is the joint frame shifted by it)."""
+
+    _fields_ = [
+        ("low", C.c_float),
+        ("high", C.c_float),
+        ("joint_mask", C.c_uint32),
+        ("reserved", C.c_uint32),
+    ]
+
+
+ENCODER_OFFSET_DEFAULT_JOINTS = ("left_hip", "left_knee", "right_hip", "right_knee")  # zeroed by hand on the robot
+
+
 MAX_HISTORY = 64  # UPKIE_MAX_HISTORY: the most entries an observation history reports
 MAX_HISTORY_CHANNELS = 16  # UPKIE_MAX_HISTORY_CHANNELS: the most spine columns it records
 

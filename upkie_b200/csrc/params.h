@@ -269,6 +269,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.history = nullptr;
   P.servo_dropout = nullptr;
   P.imu_misalign = nullptr;
+  P.encoder_offset = nullptr;
   return 0;
 }
 
@@ -420,6 +421,21 @@ inline const char* imu_misalignment_spec_error(const UpkieImuMisalignment& s, co
     return "set_imu_misalignment: needs joint_limits != 0 (the misalignment runs in the observation-delay kernels)";
   if (P.spine_mode) return "set_imu_misalignment: spine_mode models its spine's own IMU";
   if (P.body_contacts) return "set_imu_misalignment: body_contacts has no IMU-misalignment kernels";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses an encoder-offset spec (upkie_b200_set_encoder_offset), null when it takes it:
+// both bounds finite, low <= high and |bound| <= 0.5 rad (a calibration error, not a remount), and a mask of joints
+inline const char* encoder_offset_spec_error(const UpkieEncoderOffset& s, const SimParams& P) {
+  if (!(s.low >= -0.5f && s.low <= 0.5f) || !(s.high >= -0.5f && s.high <= 0.5f))
+    return "set_encoder_offset: both bounds must be finite and within [-0.5, 0.5] radians";
+  if (!(s.low <= s.high)) return "set_encoder_offset: low <= high required";
+  if (s.joint_mask == 0 || (s.joint_mask >> UPKIE_NJ) != 0)
+    return "set_encoder_offset: joint_mask must select joints of bits 0 .. 5, at least one";
+  if (P.joint_limits == 0)
+    return "set_encoder_offset: needs joint_limits != 0 (the offsets run in the observation-delay kernels)";
+  if (P.spine_mode) return "set_encoder_offset: spine_mode reports the spine's own servos";
+  if (P.body_contacts) return "set_encoder_offset: body_contacts has no encoder-offset kernels";
   return nullptr;
 }
 

@@ -153,6 +153,9 @@ struct SimParams {
   // IMU mounting misalignment (upkie_b200_set_imu_misalignment): the handle's device block, null = off. Read by the step
   // kernels of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs and k_history_fill only. Appended last.
   const struct ImuMisalign* imu_misalign;
+  // servo encoder zero offsets (upkie_b200_set_encoder_offset): the handle's device block, null = off. Read by the step
+  // kernels of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs and k_history_fill only. Appended last.
+  const struct EncoderOffset* encoder_offset;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -2254,6 +2257,95 @@ UPKIE_HD Quat4 imu_misalign_reset(const ImuMisalign& M, uint64_t seed, uint64_t 
 #pragma unroll
   for (int r = 0; r < 4; ++r) col[size_t(r) * stride] = e.q[r];
   return e;
+}
+
+// ---- Servo encoder zero offsets (upkie_b200_set_encoder_offset, pi3hat_spine.cpp:181-236) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw, and offset = delta_i, the encoder zero offset of each joint in radians, [UPKIE_NJ][stride]
+// structure-of-arrays like the state, env i in column i.
+struct EncoderOffset {
+  UpkieEncoderOffset spec;
+  uint32_t* count;
+  float* offset;
+  int stride;
+};
+
+// bit 56 of the high counter word, the per-reset draws of delta_i, (k << 4) | b below bit 36: never set by
+// sample_init_state (below 2^34), the noise (below bit 42), the reset randomisation (bit 63), the pushes (62), the
+// action delay (61), the observation delay (60), the servo dropouts (59, and 59 | 58, below bit 52 otherwise) or the
+// IMU misalignment (57)
+constexpr uint64_t kEncoderOffsetTag = uint64_t(1) << 56;
+
+struct Offset6 {
+  float d[UPKIE_NJ];
+};
+
+// Draw k of the env of global index g: word j % 4 of the block of counter j / 4 gives joint j's offset, push_value's
+// exact form (the map of the servo dropouts). Every joint's word is drawn whatever the mask, and a joint outside it
+// gets 0, so that the mask changes no other joint's draw.
+UPKIE_HD Offset6 encoder_offset_draw(const UpkieEncoderOffset& s, uint64_t seed, uint64_t g, uint32_t k) {
+  Offset6 o;
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    const Philox4 r = philox4x32_10(g, kEncoderOffsetTag | (uint64_t(k) << 4) | uint64_t(b), seed);
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const int j = 4 * b + w;
+      if (j < UPKIE_NJ) o.d[j] = ((s.joint_mask >> j) & 1u) ? push_value(r.v[w], s.low, s.high) : 0.f;
+    }
+  }
+  return o;
+}
+
+// The observed state of S under the offsets d: every servo reports its position in its own frame, q_j + delta_j.
+// A zero offset leaves q_j bit for bit (the sum would turn a -0 into +0). Returns whether a wheel position changed (the
+// odometry that the gyropod and pendulum rows report).
+UPKIE_HD bool encoder_offset_view(RobotState& S, const Offset6& d) {
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j)
+    if (d.d[j] != 0.f) S.q[j] += d.d[j];
+  return d.d[2] != 0.f || d.d[5] != 0.f;
+}
+
+// The position targets of the servo command `a` (servo frame, after clamp_servo_action) as the joints execute them,
+// target - delta_j. A NaN target stays NaN; a zero offset leaves the target as it is.
+UPKIE_HD void encoder_offset_command(float a[UPKIE_ACT_DIM], const Offset6& d) {
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j)
+    if (d.d[j] != 0.f) a[j * UPKIE_ACT_KEYS + UPKIE_ACT_POSITION] -= d.d[j];
+}
+
+// The gyropod and pendulum leg targets a reset sets (reset_wrapper_state: the true hip and knee positions) made the
+// reported ones, q + delta: the wrapper holds servo-frame targets
+UPKIE_HD void encoder_offset_leg_targets(RobotState& S, const Offset6& d) {
+  const int leg_joint[4] = {0, 1, 3, 4};
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (d.d[leg_joint[k]] != 0.f) S.leg_target[k] += d.d[leg_joint[k]];
+}
+
+// Env i's offsets, load(row) of its column
+template <typename Load>
+UPKIE_HD Offset6 encoder_offset_load(Load load) {
+  Offset6 o;
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) o.d[j] = load(j);
+  return o;
+}
+
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, stored; the new delta_i. The block's
+// fields are copied before the first store, as servo_dropout_reset.
+UPKIE_HD Offset6 encoder_offset_reset(const EncoderOffset& E, uint64_t seed, uint64_t g, int i) {
+  const UpkieEncoderOffset spec = E.spec;
+  uint32_t* const count = E.count;
+  float* const col = E.offset + size_t(i);
+  const size_t stride = size_t(E.stride);
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  const Offset6 o = encoder_offset_draw(spec, seed, g, k);
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) col[size_t(j) * stride] = o.d[j];
+  return o;
 }
 
 }  // namespace upkie_b200

@@ -135,9 +135,11 @@ __device__ __forceinline__ float* obs_delay_report(const ObsDelay& O, uint32_t s
 // column with the columns of S. Out of line: the calls pass a copy of the state, and the kernel's own arithmetic is
 // compiled (and its products contracted) as without the history.
 // Under servo dropouts the servos of `lost` report env i's held triple, as the observation does; under an IMU
-// misalignment the columns are read through the env's `em` (after the IMU velocity, which is the true IMU's).
+// misalignment the columns are read through the env's `em` (after the IMU velocity, which is the true IMU's), and under
+// encoder offsets through its `eo`.
 __device__ __noinline__ void history_substep(const SimParams& P, RobotState S, float* vel, float* e,
-                                             size_t stride, int count, bool acc, uint32_t lost, int i, const Quat4 em) {
+                                             size_t stride, int count, bool acc, uint32_t lost, int i, const Quat4 em,
+                                             const Offset6 eo) {
   if (lost) {
     const ServoDropout& D = *P.servo_dropout;
     const float* const held = D.held + size_t(i);
@@ -154,11 +156,13 @@ __device__ __noinline__ void history_substep(const SimParams& P, RobotState S, f
     }
   }
   imu_misalign_view(S, em);
+  encoder_offset_view(S, eo);
   for (int c = 0; c < count; ++c) __stcg(e + size_t(c) * stride, history_value(P, S, a, __ldg(P.history->columns + c)));
 }
 __device__ __noinline__ void history_fill_lane(const SimParams& P, RobotState S, float* col, size_t stride,
-                                               int count, uint32_t ticks, const Quat4 em) {
+                                               int count, uint32_t ticks, const Quat4 em, const Offset6 eo) {
   imu_misalign_view(S, em);
+  encoder_offset_view(S, eo);
   for (int c = 0; c < count; ++c) {
     const float v = history_value(P, S, S.imu_acc, __ldg(P.history->columns + c));
     for (uint32_t e = 0; e < ticks; ++e) __stcg(col + (size_t(e) * size_t(count) + size_t(c)) * stride, v);
@@ -218,6 +222,18 @@ __device__ __forceinline__ Quat4 tilt_load_lane(const SimParams& P, int i) {
 }
 __device__ __noinline__ Quat4 tilt_reset_lane(const SimParams& P, uint64_t seed, uint64_t g, int i) {
   return imu_misalign_reset(*P.imu_misalign, seed, g, i);
+}
+
+// The encoder offsets (F.sense kernels, P.encoder_offset set): env i's delta_i, loaded once per lane (coherent loads,
+// as tilt_load_lane), and a reset's next draw, stored (out of line, as tilt_reset_lane)
+__device__ __forceinline__ Offset6 offset_load_lane(const SimParams& P, int i) {
+  const EncoderOffset& E = *P.encoder_offset;
+  const float* const col = E.offset + size_t(i);
+  const size_t stride = size_t(E.stride);
+  return encoder_offset_load([&](int j) { return __ldcg(col + size_t(j) * stride); });
+}
+__device__ __noinline__ Offset6 offset_reset_lane(const SimParams& P, uint64_t seed, uint64_t g, int i) {
+  return encoder_offset_reset(*P.encoder_offset, seed, g, i);
 }
 
 // ---- one env tick of the robot `tid` --------------------------------------------------
@@ -404,6 +420,26 @@ __device__ __forceinline__ void step_env(
       for (int c = 0; c < UPKIE_ACT_DIM; ++c) a[c] = prev[c];
     }
   }
+  // servo encoder zero offsets (F.sense kernels, P.encoder_offset set: a uniform branch). `eo` is the lane's delta_i:
+  // loaded once, or drawn here by a next-step reset and at the same-step reset below. The substeps execute the position
+  // targets of the servo frame in the joint frame, target - delta: the row entering the tick here (after the clamps and
+  // the action-delay swap, whose buffer keeps the commands as sent) and the row the delay's switch substep loads. A
+  // reset's leg targets are the reported positions, and every observation of the tick is built from a copy of the state
+  // whose positions are read through `eo` (encoder_offset_view), after the dropout and misalignment views: the history
+  // entries, the same-step final observation and stash (the terminal episode's delta_i), and the observation. Without
+  // the feature `eo` is zero, which every use leaves out.
+  const bool offsetting = F.sense && P.encoder_offset;
+  Offset6 eo{{0.f, 0.f, 0.f, 0.f, 0.f, 0.f}};
+  if constexpr (F.sense) {
+    if (offsetting) {
+      if (!resetting) {
+        eo = offset_load_lane(P, i);
+        encoder_offset_command(a, eo);
+      } else if (live) {
+        eo = offset_reset_lane(P, seed, env_offset + uint64_t(i), i);
+      }
+    }
+  }
   // TILE >= 1: the row the substeps read (torque law, action delay, spine cycle) is the lane's own row of the warp's
   // tile, written here whole (9 x 16 B at a stride of 9 float4: conflict-free) whether the row came from the tile or
   // from global memory, instead of a 36-float register array that ptxas spills to the local-memory frame and reloads in
@@ -531,6 +567,9 @@ __device__ __forceinline__ void step_env(
           const ActionDelay& A = *P.action_delay;
           return __ldcg(A.command + dsec + size_t(c) * size_t(A.stride) + size_t(i));
         });
+        if constexpr (F.sense) {
+          if (offsetting && uint32_t(sub) == dly) encoder_offset_command(arow, eo);  // the new command, executed
+        }
       }
       // the body-ground contacts of the tick's last substep go to the handle's record (F.body kernels)
       const BodyRecOut br{(F.body && P.body_rec && live && sub == nsub - 1) ? P.body_rec + i : nullptr,
@@ -566,7 +605,7 @@ __device__ __forceinline__ void step_env(
       }
       if (recording && !resetting && live)
         history_substep(P, S, hvel, hring + size_t((hhead + uint32_t(sub)) % hticks) * size_t(hcount) * hstride,
-                        hstride, hcount, hacc, dcur, i, em);
+                        hstride, hcount, hacc, dcur, i, em, eo);
     } else {
 #pragma unroll
       for (int k = 0; k < kPhaseSyncs; ++k) PhaseSync()();
@@ -580,6 +619,9 @@ __device__ __forceinline__ void step_env(
   }
   if (resetting) {
     reset_wrapper_state(S);
+    if constexpr (F.sense) {
+      if (offsetting) encoder_offset_leg_targets(S, eo);  // the new episode's reported leg positions
+    }
   } else {
     e |= state_sanity(S);
     if (MODE != MODE_SERVOS) {
@@ -615,6 +657,7 @@ __device__ __forceinline__ void step_env(
   bool fin_pending = false;  // F.sense, same-step reset: the terminal observation is stashed after the tick
   float fin_o6[6], fin_yaw = 0.f, fin_yaw_vel = 0.f;
   const Quat4 fin_e = em;  // the terminal episode's misalignment (a same-step reset draws the next one into em)
+  const Offset6 fin_eo = eo;  // and its encoder offsets
   if (AUTORESET == AUTORESET_SAME_STEP) {
     if (term || trunc) {
       if constexpr (F.sense) {
@@ -642,6 +685,8 @@ __device__ __forceinline__ void step_env(
         // orientation whole, reset_pose)
         if constexpr (F.sense) {
           if (tilting && imu_misalign_view(S, em) && MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
+          // the encoder offsets: its reported positions (the reset below overwrites q whole, reset_pose)
+          if (offsetting && encoder_offset_view(S, eo) && MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
         }
         if (P.final_obs && live)
           store_final_obs<MODE, spine>(P, S, L, o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
@@ -669,6 +714,7 @@ __device__ __forceinline__ void step_env(
       dreset = true;
       if constexpr (F.sense) {
         if (tilting && live) em = tilt_reset_lane(P, seed, env_offset + uint64_t(i), i);  // the new episode's e_i
+        if (offsetting && live) eo = offset_reset_lane(P, seed, env_offset + uint64_t(i), i);  // and delta_i
       }
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
@@ -682,6 +728,9 @@ __device__ __forceinline__ void step_env(
                           size_t(P.body_rec_stride)};
       if (spine) reset_robot_spine(P, S, L, init, eps, mu, WarpAny(), P.joint_limits, br);
       else reset_robot(P, S, init, eps, mu, WarpAny(), F.limits ? P.joint_limits : 0, br);
+      if constexpr (F.sense) {
+        if (offsetting) encoder_offset_leg_targets(S, eo);  // the new episode's reported leg positions
+      }
       if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
     }
   }
@@ -690,7 +739,7 @@ __device__ __forceinline__ void step_env(
   // the history: a reset fills the lane's ring from its post-reset state (the true state, here in S), and every lane's
   // head moves on by the tick's substeps
   if (recording && live) {
-    if (refill) history_fill_lane(P, S, hring, hstride, hcount, hticks, em);
+    if (refill) history_fill_lane(P, S, hring, hstride, hcount, hticks, em, eo);
     __stcg(P.history->head + i, (hhead + uint32_t(P.nb_substeps)) % hticks);
   }
   // the dropouts: a reset latches the lane's post-reset state (the true state, here in S) and draws its next p_i
@@ -708,7 +757,9 @@ __device__ __forceinline__ void step_env(
       S.yaw_vel = fin_yaw_vel;
       obs_delay_sensed_state(S, sense_load);
       const bool ftilt = tilting && imu_misalign_view(S, fin_e);  // the terminal episode's sensed orientation
-      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0 || ftilt))
+      bool fodo = false;
+      if constexpr (F.sense) fodo = offsetting && encoder_offset_view(S, fin_eo);  // and its reported positions
+      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0 || ftilt || fodo))
         gyropod_obs(P, S, fin_o6);  // (a dropout patched the snapshot, or the orientation is the sensed one)
       if (P.final_obs && live)
         store_final_obs<MODE, spine>(P, S, L, fin_o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
@@ -747,6 +798,11 @@ __device__ __forceinline__ void step_env(
   // the snapshot under an observation delay (the true state is stored above; UpkieServos rows hold no orientation)
   if constexpr (F.sense && MODE != MODE_SERVOS) {
     if (tilting && imu_misalign_view(S, em)) gyropod_obs(P, S, o6);
+  }
+  // the encoder offsets: every row reports the positions of the servo frame (the wheels' as the gyropod and pendulum
+  // odometry)
+  if constexpr (F.sense) {
+    if (offsetting && encoder_offset_view(S, eo) && MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
   }
   if (spine && live) {
     float lr[UPKIE_LAG_DIM];

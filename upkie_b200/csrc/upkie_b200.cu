@@ -15,7 +15,9 @@
 // The servo dropouts' held rows take no kernel of their own: k_reset latches, k_ring_copy copies them for checkpoints,
 // and a new spec or set_state latches the state with device copies of its rows (servo_dropout_latch).
 // The IMU misalignment takes none either: k_reset draws, k_ring_copy copies its quaternions for checkpoints, and
-// k_spine_obs, k_reset_obs and k_history_fill read the orientation through it (imu_misalign_observed).
+// k_spine_obs, k_reset_obs and k_history_fill read the orientation through it (imu_misalign_observed). Neither do the
+// encoder offsets: k_reset draws and shifts the leg targets, and the same three kernels read the servo positions
+// through them (encoder_offset_observed).
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -152,6 +154,12 @@ struct Handle {
   ImuMisalign* tilt_dev = nullptr;
   uint32_t* tilt_count = nullptr;
   float* tilt_quat = nullptr;  // [4][n_pad], e_i (w, x, y, z)
+  // servo encoder zero offsets (upkie_b200_set_encoder_offset): the device block P.encoder_offset points to while a spec
+  // is set, and the per-env state it points to (allocated with the first spec, freed when it is turned off)
+  EncoderOffset* enc_dev = nullptr;
+  uint32_t* enc_count = nullptr;
+  float* enc_offset = nullptr;  // [UPKIE_NJ][n_pad], delta_i
+  uint32_t enc_mask = 0;        // joint_mask of the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -229,6 +237,12 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
   } else {
     reset_robot(P, S, init, eps, mu, WarpAny(), P.joint_limits, br);
   }
+  // the encoder offsets' next draw: the new episode's leg targets are its reported leg positions
+  Offset6 d{{0.f, 0.f, 0.f, 0.f, 0.f, 0.f}};
+  if (P.encoder_offset) {
+    d = encoder_offset_reset(*P.encoder_offset, rand_seed, g, i);
+    encoder_offset_leg_targets(S, d);
+  }
   store_state(state, n_pad, i, S);
   err[i] = 0;
   done_prev[i] = 0;
@@ -249,6 +263,7 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
   if (P.history) {  // a new episode's history starts from its post-reset columns
     RobotState V = S;
     imu_misalign_view(V, e);
+    encoder_offset_view(V, d);
     history_fill(*P.history, P, V, i);
   }
   if (P.servo_dropout) servo_dropout_reset(*P.servo_dropout, rand_seed, g, i, S);  // a new p_i, the reset latched
@@ -260,6 +275,14 @@ __device__ void imu_misalign_observed(const SimParams& P, int i, RobotState& S) 
   if (!P.imu_misalign) return;
   const ImuMisalign& M = *P.imu_misalign;
   imu_misalign_view(S, imu_misalign_load([&](int r) { return M.quat[size_t(r) * size_t(M.stride) + size_t(i)]; }));
+}
+
+// The encoder offsets: the reported servo positions of S, read through env i's delta_i (the state or a sensed row, as
+// imu_misalign_observed)
+__device__ void encoder_offset_observed(const SimParams& P, int i, RobotState& S) {
+  if (!P.encoder_offset) return;
+  const EncoderOffset& E = *P.encoder_offset;
+  encoder_offset_view(S, encoder_offset_load([&](int j) { return E.offset[size_t(j) * size_t(E.stride) + size_t(i)]; }));
 }
 
 // Servo dropouts without an observation delay: the observed state of S, every servo of the mask reporting its held
@@ -298,6 +321,7 @@ __global__ void k_history_fill(const __grid_constant__ SimParams P, const Histor
   RobotState S;
   load_state(state, n_pad, i, S);
   imu_misalign_observed(P, i, S);
+  encoder_offset_observed(P, i, S);
   history_fill(*H, P, S, i);
 }
 
@@ -326,6 +350,7 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
     if (!mark) {  // (the stash holds the terminal step's observed state)
       servo_dropout_observed(P, i, S);
       imu_misalign_observed(P, i, S);
+      encoder_offset_observed(P, i, S);
     }
     float tq[6];
     measured_torques(P, S, &nz, tq, i);
@@ -345,6 +370,7 @@ __global__ void k_reset_obs(const __grid_constant__ SimParams P, int n, int n_pa
   load_state(state, n_pad, i, S);
   servo_dropout_observed(P, i, S);
   imu_misalign_observed(P, i, S);
+  encoder_offset_observed(P, i, S);
   if (obs_dim == UPKIE_OBS_DIM && P.spine_mode && lag) {
     for (int j = 0; j < 6; ++j) {
       float* o = out + size_t(i) * UPKIE_OBS_DIM + j * 5;
@@ -1010,6 +1036,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->hist_dev); cudaFree(h->hist_ring); cudaFree(h->hist_head);
   cudaFree(h->drop_dev); cudaFree(h->drop_count); cudaFree(h->drop_prob); cudaFree(h->drop_held);
   cudaFree(h->tilt_dev); cudaFree(h->tilt_count); cudaFree(h->tilt_quat);
+  cudaFree(h->enc_dev); cudaFree(h->enc_count); cudaFree(h->enc_offset);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -1061,6 +1088,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: IMU misalignment needs joint_limits != 0");
   if (h->P.imu_misalign && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no IMU-misalignment kernels");
+  if (h->P.encoder_offset && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: encoder offsets need joint_limits != 0");
+  if (h->P.encoder_offset && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no encoder-offset kernels");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -1083,6 +1114,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.history = h->P.history;            // and the observation history
   P.servo_dropout = h->P.servo_dropout;  // and the servo dropouts
   P.imu_misalign = h->P.imu_misalign;    // and the IMU misalignment
+  P.encoder_offset = h->P.encoder_offset;  // and the encoder offsets
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -2141,6 +2173,85 @@ int upkie_b200_set_imu_misalignment_state(void* handle, const uint32_t* count, c
   }
   CUDA_TRY(cudaMemcpyAsync(h->tilt_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(ring_cols(quat, 4, h->n, h->n_pad, h->tilt_quat, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_encoder_offset(void* handle, const UpkieEncoderOffset* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    if (h->P.encoder_offset) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the per-env state
+      h->P.encoder_offset = nullptr;
+      cudaFree(h->enc_count);
+      cudaFree(h->enc_offset);
+      h->enc_count = nullptr;
+      h->enc_offset = nullptr;
+      h->enc_mask = 0;
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = encoder_offset_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
+  if (!h->P.encoder_offset) {
+    // switched on: zero counters, and zero offsets until each env's next reset
+    CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->enc_count), size_t(h->n) * sizeof(uint32_t)},
+                           {reinterpret_cast<void**>(&h->enc_offset), size_t(UPKIE_NJ) * h->n_pad * sizeof(float)}}));
+  } else {
+    // a replacement: the joints it drops from the mask have no offset from now on
+    for (int j = 0; j < UPKIE_NJ; ++j)
+      if (((h->enc_mask & ~spec->joint_mask) >> j) & 1u)
+        CUDA_TRY(cudaMemset(h->enc_offset + size_t(j) * h->n_pad, 0, size_t(h->n_pad) * sizeof(float)));
+  }
+  if (!h->enc_dev) CUDA_TRY(cudaMalloc(&h->enc_dev, sizeof(EncoderOffset)));
+  EncoderOffset E;
+  std::memset(&E, 0, sizeof(E));
+  E.spec = *spec;
+  E.count = h->enc_count;
+  E.offset = h->enc_offset;
+  E.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->enc_dev, &E, sizeof(E), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->P.encoder_offset = h->enc_dev;
+  h->enc_mask = spec->joint_mask;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_encoder_offset_state(void* handle, uint32_t* count, float* offset, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !offset) return fail(UPKIE_B200_EINVAL, "get_encoder_offset_state: invalid argument");
+  if (!h->P.encoder_offset)
+    return fail(UPKIE_B200_EINVAL, "get_encoder_offset_state: no encoder offsets are set (upkie_b200_set_encoder_offset)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemcpyAsync(count, h->enc_count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_rows(h->enc_offset, UPKIE_NJ, h->n, h->n_pad, offset, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_encoder_offset_state(void* handle, const uint32_t* count, const float* offset, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !offset) return fail(UPKIE_B200_EINVAL, "set_encoder_offset_state: invalid argument");
+  if (!h->P.encoder_offset)
+    return fail(UPKIE_B200_EINVAL, "set_encoder_offset_state: no encoder offsets are set (upkie_b200_set_encoder_offset)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // every offset must be a calibration error of a joint of the mask: read back (after the caller's work on the
+  // stream) and checked here
+  std::vector<float> d(size_t(h->n) * UPKIE_NJ);
+  CUDA_TRY(cudaMemcpyAsync(d.data(), offset, d.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (size_t k = 0; k < d.size(); ++k) {
+    if (!(std::fabs(d[k]) <= 0.5f))
+      return fail(UPKIE_B200_EINVAL, "set_encoder_offset_state: every offset must be finite and within [-0.5, 0.5] "
+                                     "radians");
+    if (d[k] != 0.f && !((h->enc_mask >> (k % UPKIE_NJ)) & 1u))
+      return fail(UPKIE_B200_EINVAL, "set_encoder_offset_state: a joint outside joint_mask must have a zero offset");
+  }
+  CUDA_TRY(cudaMemcpyAsync(h->enc_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_cols(offset, UPKIE_NJ, h->n, h->n_pad, h->enc_offset, s));
   return UPKIE_B200_OK;
 }
 

@@ -804,6 +804,61 @@ def imu_misalignment_spec(misalignment, spine_mode: bool = False, joint_limits: 
     return _abi.UpkieImuMisalignment(*bounds)
 
 
+_ENCODER_OFFSET_MAX = np.float32(0.5)  # the largest |bound|, radians (the C check compares float32 values)
+
+
+def encoder_offset_spec(offset, joints=None, spine_mode: bool = False, joint_limits: Union[bool, int] = True,
+                        body_contacts: Union[bool, int] = False) -> Optional[_abi.UpkieEncoderOffset]:
+    """``UpkieEncoderOffset`` (``UpkieSim.set_encoder_offset``) from a servo encoder zero offset in radians: a bound
+    ``b`` (the range ``(-b, b)``), or a ``(low, high)`` pair from which every reset draws each joint's offset, and the
+    names of the joints that have one (``joints``, ``JOINT_NAMES``; None: the four hip and knee joints, which are zeroed
+    by hand on the robot). Raises ``UpkieException`` on a bound that is not a finite number, ``low > high``, ``|bound| >
+    0.5`` (a calibration error, not a remount), an unknown or empty joint list, ``spine_mode`` (whose spine reports its
+    own servos), no joint limits and ``body_contacts`` (the offsets run in the kernels of the observation delay)."""
+    if offset is None:
+        return None
+    if isinstance(offset, (int, float, np.integer, np.floating)):
+        lo, hi = -abs(offset), abs(offset)
+    else:
+        try:
+            lo, hi = offset
+        except (TypeError, ValueError):
+            raise UpkieException(f"encoder_offset: expected a bound or a (low, high) pair, got {offset!r}") from None
+    try:
+        lo, hi = np.float32(lo), np.float32(hi)
+    except (TypeError, ValueError):
+        raise UpkieException(f"encoder_offset: expected angles, got ({lo!r}, {hi!r})") from None
+    if not (np.isfinite(lo) and np.isfinite(hi)) or max(abs(lo), abs(hi)) > _ENCODER_OFFSET_MAX:
+        raise UpkieException(f"encoder_offset: expected finite angles within [-0.5, 0.5] radians, got ({lo}, {hi})")
+    if lo > hi:
+        raise UpkieException(f"encoder_offset: expected low <= high, got ({lo}, {hi})")
+    names = list(_abi.ENCODER_OFFSET_DEFAULT_JOINTS) if joints is None else list(joints)
+    unknown = [j for j in names if j not in _abi.JOINT_NAMES]
+    if unknown:
+        raise UpkieException(f"encoder_offset_joints: unknown joint(s) {unknown}, expected names of {_abi.JOINT_NAMES}")
+    if not names:
+        raise UpkieException("encoder_offset_joints: at least one joint")
+    if spine_mode:
+        raise UpkieException("encoder_offset: spine_mode reports the spine's own servos; the offsets are not available "
+                             "there")
+    if not joint_limits:
+        raise UpkieException("encoder_offset: needs joint_limits (the offsets run in the kernels with joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("encoder_offset: body_contacts has no encoder-offset kernels")
+    mask = 0
+    for j in names:
+        mask |= 1 << _abi.JOINT_NAMES.index(j)
+    return _abi.UpkieEncoderOffset(float(lo), float(hi), mask, 0)
+
+
+def _set_encoder_offset(sim, spec: Optional[_abi.UpkieEncoderOffset]) -> None:
+    if spec is None:
+        sim.set_encoder_offset(None)
+    else:
+        sim.set_encoder_offset(spec.low, spec.high, [n for j, n in enumerate(_abi.JOINT_NAMES)
+                                                     if (spec.joint_mask >> j) & 1])
+
+
 def _set_imu_misalignment(sim, spec: Optional[_abi.UpkieImuMisalignment]) -> None:
     if spec is None:
         sim.set_imu_misalignment(None)
@@ -897,6 +952,16 @@ class B200VectorEnv(VectorEnv):
     pendulum pitch and pitch rate, the spine observation, the history) are those the tilted IMU reports. The physics,
     terminations and ``get_state`` see the true state. The draws are keyed on the seed of ``reset(seed=s)``, which also
     restarts the draw counters of the envs it resets. ``set_imu_misalignment`` changes or (``None``) stops it.
+
+    ``encoder_offset`` (a bound ``b`` for ``(-b, b)``, or a ``(low, high)`` range in radians, see
+    ``encoder_offset_spec``) zeroes the servos ``encoder_offset_joints`` (names, default the hips and knees) off by an
+    offset drawn per joint at every reset of the env, as a leg rezeroed by hand would be (``pi3hat_spine.cpp``). The
+    servo frame is the joint frame shifted by the offset: every position an env type observes (servo rows, the gyropod
+    and pendulum wheel odometry, the spine observation, the history) is ``q + delta``, every position target lands at
+    ``target - delta``, and the gyropod, pendulum and base-velocity legs hold their servo zero, the physical angle
+    ``-delta``. The physics, terminations and ``get_state``'s q see the true joints. The draws are keyed on the seed of
+    ``reset(seed=s)``, which also restarts the draw counters of the envs it resets. ``set_encoder_offset`` changes or
+    (``None``) stops it.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -940,6 +1005,8 @@ class B200VectorEnv(VectorEnv):
         servo_dropout: Optional[Union[float, Tuple[float, float]]] = None,
         servo_dropout_joints: Optional[Sequence[str]] = None,
         imu_misalignment: Optional[Dict[str, Union[float, Tuple[float, float]]]] = None,
+        encoder_offset: Optional[Union[float, Tuple[float, float]]] = None,
+        encoder_offset_joints: Optional[Sequence[str]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -993,6 +1060,8 @@ class B200VectorEnv(VectorEnv):
                                        config.joint_limits, config.body_contacts)  # validated before any device
         tilt_spec = imu_misalignment_spec(imu_misalignment, bool(config.spine_mode), config.joint_limits,
                                           config.body_contacts)  # validated before any device is touched
+        enc_spec = encoder_offset_spec(encoder_offset, encoder_offset_joints, bool(config.spine_mode),
+                                       config.joint_limits, config.body_contacts)  # validated before any device
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -1056,6 +1125,15 @@ class B200VectorEnv(VectorEnv):
             self.sim.set_servo_dropout(drop_spec.prob_low, drop_spec.prob_high, servo_dropout_joints)
         if tilt_spec is not None:
             _set_imu_misalignment(self.sim, tilt_spec)  # before the first reset, which draws every env's misalignment
+        if enc_spec is not None:
+            _set_encoder_offset(self.sim, enc_spec)  # before the first reset, which draws every env's offsets
+
+    def set_encoder_offset(self, offset, joints=None) -> None:
+        """Zero the servos ``joints`` (names, None: the hips and knees) off by an offset drawn from a bound or a
+        ``(low, high)`` range in radians (``encoder_offset_spec``); ``None`` turns the offsets off. A new range takes
+        effect at each env's next reset; the joints it drops have no offset from now on."""
+        _set_encoder_offset(self.sim, encoder_offset_spec(offset, joints, bool(self.config.spine_mode),
+                                                          self.config.joint_limits, self.config.body_contacts))
 
     def set_imu_misalignment(self, misalignment) -> None:
         """Mount each env's IMU off its nominal pose by ``roll`` / ``pitch`` / ``yaw`` angles or ranges (a dict,
@@ -1286,6 +1364,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_imu_misalignment_state(count, quat)
+            if self.sim.encoder_offset_spec is not None:
+                # so are the encoder offsets
+                count, offset = self.sim.get_encoder_offset_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_encoder_offset_state(count, offset)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

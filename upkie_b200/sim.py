@@ -382,6 +382,54 @@ class UpkieSim:
         self._check_tensor(quat, (self.n, 4), name="quat")
         check(lib().upkie_b200_set_imu_misalignment_state(self._h, _ptr(count), _ptr(quat), self._stream()))
 
+    def set_encoder_offset(self, low: Optional[float], high: Optional[float] = None,
+                           joints: Optional[Sequence[str]] = None) -> None:
+        """While a range is set, each servo of ``joints`` (names, None: the four hip and knee joints) is zeroed off by
+        an offset ``delta ~ U(low, high)`` radians, drawn per joint at every reset of the env (keyed on the auto-reset
+        seed and the env's counter, ``include/upkie_b200.h``). The servo frame is the joint frame shifted by delta:
+        every reported position (the servo rows, ``spine_obs`` and its wheel odometry, the gyropod and pendulum ``p``,
+        the final observations and the history) is ``q + delta``, every position target executes as ``target - delta``,
+        and the gyropod, pendulum and base-velocity leg targets are servo-frame values (a reset sets them to the
+        reported positions). The physics, terminations and ``get_state``'s q see the true joints. ``high`` defaults to
+        ``low``; ``None`` turns the offsets off. Setting a range draws nothing: it takes effect at each env's next
+        reset."""
+        if low is None:
+            check(lib().upkie_b200_set_encoder_offset(self._h, None))
+            self._encoder_offset = None
+            return
+        names = list(_abi.ENCODER_OFFSET_DEFAULT_JOINTS) if joints is None else list(joints)
+        unknown = [j for j in names if j not in _abi.JOINT_NAMES]
+        if unknown:
+            raise UpkieException(f"set_encoder_offset: unknown joint(s) {unknown}")
+        mask = sum(1 << _abi.JOINT_NAMES.index(j) for j in set(names))
+        spec = _abi.UpkieEncoderOffset(float(low), float(low if high is None else high), mask, 0)
+        check(lib().upkie_b200_set_encoder_offset(self._h, C.byref(spec)))
+        self._encoder_offset = (spec.low, spec.high, mask)
+
+    @property
+    def encoder_offset_spec(self) -> Optional[Tuple[float, float, int]]:
+        """``(low, high, joint_mask)`` of the encoder offsets in force, or None."""
+        return getattr(self, "_encoder_offset", None)
+
+    def get_encoder_offset_state(self):
+        """Per-env encoder-offset state ``(count[N], offset[N, 6])``: the draw counters (int32 bits of uint32) and each
+        env's zero offset per joint, in radians."""
+        if self.encoder_offset_spec is None:
+            raise UpkieException("no encoder offsets are set (set_encoder_offset)")
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        offset = torch.empty((self.n, _abi.NJ), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_encoder_offset_state(self._h, _ptr(count), _ptr(offset), self._stream()))
+        return count, offset
+
+    def set_encoder_offset_state(self, count: torch.Tensor, offset: torch.Tensor) -> None:
+        """Set every env's draw counter and zero offsets (finite, within 0.5 rad, zero outside the mask): a checkpoint,
+        or offsets measured on a robot (kept until each env's next reset)."""
+        if self.encoder_offset_spec is None:
+            raise UpkieException("no encoder offsets are set (set_encoder_offset)")
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(offset, (self.n, _abi.NJ), name="offset")
+        check(lib().upkie_b200_set_encoder_offset_state(self._h, _ptr(count), _ptr(offset), self._stream()))
+
     def set_history(self, columns: Optional[Sequence[int]], size: int = 1) -> None:
         """Record each env's spine-observation ``columns`` (``_abi.SP_*``, 1 to ``MAX_HISTORY_CHANNELS`` of them) after
         every substep, and report the last ``size`` (1 to ``MAX_HISTORY``) through ``get_history``: the spine's
@@ -846,6 +894,10 @@ class UpkieSim:
         if self.imu_misalignment_spec is not None:
             sd["imu_misalignment"] = self.imu_misalignment_spec
             sd["imu_misalignment_count"], sd["imu_misalignment_quat"] = self.get_imu_misalignment_state()
+        # the encoder offsets: (low, high, joint_mask) and the per-env state (absent without a spec)
+        if self.encoder_offset_spec is not None:
+            sd["encoder_offset"] = self.encoder_offset_spec
+            sd["encoder_offset_count"], sd["encoder_offset_offset"] = self.get_encoder_offset_state()
         sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
@@ -963,6 +1015,14 @@ class UpkieSim:
             self.set_imu_misalignment(*tilt)
             self.set_imu_misalignment_state(*(sd[k].to(dev).contiguous() for k in (
                 "imu_misalignment_count", "imu_misalignment_quat")))
+        # the encoder offsets; a checkpoint without them (or written before they existed) turns them off
+        enc = sd.get("encoder_offset")
+        if enc is None:
+            self.set_encoder_offset(None)
+        else:
+            self.set_encoder_offset(enc[0], enc[1], [n for j, n in enumerate(_abi.JOINT_NAMES) if (enc[2] >> j) & 1])
+            self.set_encoder_offset_state(*(sd[k].to(dev).contiguous() for k in (
+                "encoder_offset_count", "encoder_offset_offset")))
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
