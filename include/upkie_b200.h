@@ -951,6 +951,75 @@ int upkie_b200_set_encoder_offset(void* handle, const UpkieEncoderOffset* spec);
 int upkie_b200_get_encoder_offset_state(void* handle, uint32_t* count, float* offset, void* stream);
 int upkie_b200_set_encoder_offset_state(void* handle, const uint32_t* count, const float* offset, void* stream);
 
+/* ---- Servo measurement noise (observe_servos.cpp:62-75, pybullet_backend.py:448-466) ------------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. Each servo reply carries the moteus
+ * encoder's estimates of position and velocity, which reach the spine once per cycle; the velocity estimate is visibly
+ * noisy. The torque reply keeps its own noise (UPKIE_EP_MEAS_NOISE). While a spec is set:
+ * - Draw per reset: at every reset of env i (both fused auto-resets, upkie_b200_reset with or without a mask or host
+ *   rows) twelve standard deviations are drawn, columns 0-5 the position noise of joints 0-5 (UPKIE_NJ order), 6-11 the
+ *   velocity noise. Draw law: a per-env counter k, +1 at every reset; draw k of the env of global index
+ *   g = env_offset + i is Philox4x32-10 with key seed (upkie_b200_set_autoreset) and counters (g, 2^55 | k << 4 | b),
+ *   b = 0, 1, 2; word c % 4 of block c / 4 gives sigma_ic = min(low_c + fl(fl(high_c - low_c) * u(w)), high_c),
+ *   u(w) = (w >> 8) / 2^24 (the servo dropouts' map). Every column is drawn whatever the ranges, so that changing one
+ *   joint's range changes no other joint's draw.
+ * - Noise per cycle: every reported position and velocity is the true value plus sigma * n, n a standard normal that
+ *   depends only on (seed, g, the cycle reported, joint, quantity). Cycle s (0 .. nb_substeps - 1) of tick t (the
+ *   per-env tick counter after the step, as the dropout losses use it) draws counters (g, 2^55 | 2^54 | t << 20 |
+ *   s << 2 | b), b = 0, 1, 2; the twelve words pass in pairs through gaussian8's Box-Muller transform (normal c from
+ *   words 2p, 2p + 1 of block c / 4, p = (c % 4) / 2, the cosine for even c). A reset's observation is a cycle of its
+ *   own, (g, 2^55 | 2^54 | 2^53 | k << 2 | b) with the draw counter k after the reset, which every reset advances
+ *   (with host rows too, which do not count an episode): it never coincides with a step cycle, and two resets of an env
+ *   report different normals unless a restart of the counters (a set_servo_noise_state with count 0, as
+ *   B200VectorEnv.reset(seed=s) does) repeats a draw on purpose. A cycle reported twice reports the same value.
+ *   Tag bit 55 keeps these counters apart from the initial states (below 2^34), the noise (below bit 42), the reset
+ *   randomisation (bit 63), the pushes (62), the action delay (61), the observation delay (60), the servo dropouts
+ *   (59, 59 | 58), the IMU misalignment (57) and the encoder offsets (56).
+ * - Where it appears: wherever the encoder offsets appear: the [6][5] and compact [6][3] servo rows, the servo block of
+ *   upkie_b200_spine_obs and of the final spine observation and the wheel odometry built from them, the gyropod and
+ *   pendulum p and pdot, final_obs, reset_obs, and the servo-position, servo-velocity and odometry columns of every
+ *   history entry, each entry with the noise of its own cycle. A ring a reset refills holds the reset observation as
+ *   its newest entry and, as each older entry, the post-reset state with the noise of the cycle that entry stands for.
+ * - Composition: the reported position is fl(fl(q + fl(sigma_q * n_q)) + delta) with the encoder offset delta, the
+ *   velocity fl(qd + fl(sigma_v * n_v)). Under an observation delay the noise is that of the cycle observed, d
+ *   substeps before the tick's last cycle (d = min(delay, K * nb_substeps), K the delay's depth in ticks), applied to
+ *   the snapshot when the observation is built; a snapshot that a reset refilled is reported with the noise of the
+ *   cycle it stands for. Under servo dropouts a lost reply repeats the last received reply as it was received: the
+ *   held rows latch the noisy position and velocity (the reset latches the reset observation's). The gyropod,
+ *   pendulum and base-velocity leg targets a reset sets from the reported hip and knee positions include the reset
+ *   cycle's noise. upkie_b200_spine_obs and upkie_b200_reset_obs report the reset cycle for the envs whose last event
+ *   was a reset, the last step's observed cycle for the others: a per-env mark, 1 after a reset and 0 after a step that
+ *   does not reset (get/set_servo_noise_mark, mark[N] of 0 or 1, for checkpoints; a spec switched on starts every env
+ *   at 0).
+ * - Not affected: the physics (the servo's torque law runs on the true q and qd: this models the reply, not the
+ *   servo's internal estimate), the joint-limit rows, terminated, truncated and the auto-resets, the torques, the q and
+ *   qd of upkie_b200_get_state (whose leg-target columns hold the reset targets above; k_reset does not know the env
+ *   type, so UpkieServos handles carry them too, unused), the observation-delay rows and their get/set state, and
+ *   UPKIE_EP_DIM.
+ * - Off is free: with the spec off, or every high bound 0, every output is bit for bit the same handle's without one.
+ * Setting a spec draws nothing: each env keeps its sigmas (zeros on a handle that never had a spec) until its next
+ * reset; a spec that replaces another zeroes the columns whose high bound is 0; NULL turns the feature off (the per-env
+ * state is freed once the device is idle). Per-env state (get/set_servo_noise_state, for checkpoints; device
+ * pointers): count[N] and sigma[N][12]; UPKIE_B200_EINVAL without a spec, for a sigma that is not finite or negative,
+ * above the caps of every spec (0.1 rad for a position, 5 rad/s for a velocity: a narrower spec leaves each env's
+ * sigmas until its next reset, so the spec in force does not bound them), or nonzero in a column whose high bound is
+ * zero in the spec in force.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: a bound that is not finite, a negative low bound, low > high,
+ * a position high above 0.1 rad or a velocity high above 5 rad/s (a sensor noise, not a broken encoder), spine_mode
+ * (whose spine reports its own servos), joint_limits == 0 and body_contacts (it runs in the observation-delay kernels),
+ * and an observation delay together with servo dropouts (a delayed snapshot does not record which of its replies were
+ * held). upkie_b200_set_config rejects joint_limits = 0 and body_contacts while a spec is set, and
+ * upkie_b200_set_observation_delay(_ticks) and upkie_b200_set_servo_dropout reject the third of the three; the in-kernel
+ * rollout transports reject a handle with a spec. The set call waits for the device. */
+typedef struct UpkieServoNoise {
+  float position_low[6], position_high[6]; /* rad, range of each joint's position noise std (UPKIE_NJ order) */
+  float velocity_low[6], velocity_high[6]; /* rad/s, range of each joint's velocity noise std */
+} UpkieServoNoise;
+int upkie_b200_set_servo_noise(void* handle, const UpkieServoNoise* spec);
+int upkie_b200_get_servo_noise_state(void* handle, uint32_t* count, float* sigma, void* stream);
+int upkie_b200_set_servo_noise_state(void* handle, const uint32_t* count, const float* sigma, void* stream);
+int upkie_b200_get_servo_noise_mark(void* handle, uint8_t* mark, void* stream);
+int upkie_b200_set_servo_noise_mark(void* handle, const uint8_t* mark, void* stream);
+
 /* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
  * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
  * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last

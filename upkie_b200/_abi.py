@@ -430,6 +430,21 @@ class UpkieImuMisalignment(C.Structure):
     ]
 
 
+class UpkieServoNoise(C.Structure):
+    """``UpkieServoNoise`` of include/upkie_b200.h: the ranges of the standard deviations of each joint's position
+    (radians) and velocity (rad/s) measurement noise, drawn per env at every reset (UPKIE_NJ order)."""
+
+    _fields_ = [
+        ("position_low", C.c_float * 6),
+        ("position_high", C.c_float * 6),
+        ("velocity_low", C.c_float * 6),
+        ("velocity_high", C.c_float * 6),
+    ]
+
+
+SERVO_NOISE_MAX = {"position": 0.1, "velocity": 5.0}  # the largest high bound of each quantity (rad, rad/s)
+
+
 class UpkieEncoderOffset(C.Structure):
     """``UpkieEncoderOffset`` of include/upkie_b200.h: the range, in radians, of the encoder zero offset each joint of
     ``joint_mask`` draws at every reset of its env (the servo frame is the joint frame shifted by it)."""

@@ -68,6 +68,11 @@ SYMBOLS = {
     "upkie_b200_set_encoder_offset": (C.c_int, [_vp, C.POINTER(_abi.UpkieEncoderOffset)]),
     "upkie_b200_get_encoder_offset_state": (C.c_int, [_vp, _vp, _vp, _vp]),
     "upkie_b200_set_encoder_offset_state": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_set_servo_noise": (C.c_int, [_vp, C.POINTER(_abi.UpkieServoNoise)]),
+    "upkie_b200_get_servo_noise_state": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_set_servo_noise_state": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_get_servo_noise_mark": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_servo_noise_mark": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_set_history": (C.c_int, [_vp, C.POINTER(_abi.UpkieHistory)]),
     "upkie_b200_get_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_history_entries": (C.c_int, [_vp, C.POINTER(C.c_int)]),

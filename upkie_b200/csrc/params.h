@@ -270,6 +270,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.servo_dropout = nullptr;
   P.imu_misalign = nullptr;
   P.encoder_offset = nullptr;
+  P.servo_noise = nullptr;
   return 0;
 }
 
@@ -436,6 +437,26 @@ inline const char* encoder_offset_spec_error(const UpkieEncoderOffset& s, const 
     return "set_encoder_offset: needs joint_limits != 0 (the offsets run in the observation-delay kernels)";
   if (P.spine_mode) return "set_encoder_offset: spine_mode reports the spine's own servos";
   if (P.body_contacts) return "set_encoder_offset: body_contacts has no encoder-offset kernels";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses a servo-noise spec (upkie_b200_set_servo_noise), null when it takes it: every
+// bound finite, 0 <= low <= high, a position high of at most 0.1 rad and a velocity high of at most 5 rad/s (a sensor
+// noise, not a broken encoder)
+inline const char* servo_noise_spec_error(const UpkieServoNoise& s, const SimParams& P) {
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!(s.position_low[j] >= 0.f && s.position_low[j] <= s.position_high[j] && s.position_high[j] <= 0.1f) ||
+        !(s.velocity_low[j] >= 0.f && s.velocity_low[j] <= s.velocity_high[j] && s.velocity_high[j] <= 5.f))
+      return "set_servo_noise: every range must be finite with 0 <= low <= high, position high <= 0.1 rad and "
+             "velocity high <= 5 rad/s";
+  }
+  if (P.joint_limits == 0)
+    return "set_servo_noise: needs joint_limits != 0 (the noise runs in the observation-delay kernels)";
+  if (P.spine_mode) return "set_servo_noise: spine_mode reports the spine's own servos";
+  if (P.body_contacts) return "set_servo_noise: body_contacts has no servo-noise kernels";
+  if (P.obs_delay && P.servo_dropout)
+    return "set_servo_noise: not with both an observation delay and servo dropouts (a delayed snapshot does not "
+           "record which of its replies were held)";
   return nullptr;
 }
 

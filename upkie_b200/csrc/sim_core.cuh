@@ -156,6 +156,9 @@ struct SimParams {
   // servo encoder zero offsets (upkie_b200_set_encoder_offset): the handle's device block, null = off. Read by the step
   // kernels of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs and k_history_fill only. Appended last.
   const struct EncoderOffset* encoder_offset;
+  // servo measurement noise (upkie_b200_set_servo_noise): the handle's device block, null = off. Read by the step kernels
+  // of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs and k_history_fill only. Appended last.
+  const struct ServoNoise* servo_noise;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -2346,6 +2349,175 @@ UPKIE_HD Offset6 encoder_offset_reset(const EncoderOffset& E, uint64_t seed, uin
 #pragma unroll
   for (int j = 0; j < UPKIE_NJ; ++j) col[size_t(j) * stride] = o.d[j];
   return o;
+}
+
+// ---- Servo measurement noise (upkie_b200_set_servo_noise, observe_servos.cpp:62-75) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw; sigma = the standard deviations of env i, [12][stride] structure-of-arrays like the state (rows 0-5
+// position, 6-11 velocity), env i in column i; fresh[i] = 1 while the observation env i reports is its reset
+// observation (set by a reset, cleared by a step that does not reset), which k_spine_obs and k_reset_obs key on.
+constexpr int kServoNoiseCols = 2 * UPKIE_NJ;
+struct ServoNoise {
+  UpkieServoNoise spec;
+  uint32_t* count;
+  float* sigma;
+  uint8_t* fresh;
+  int stride;
+};
+
+// bit 55 of the high counter word: the per-reset draws of sigma_i, (k << 4) | b below bit 36; with bit 54, the cycles
+// of a step, (t << 20) | (s << 2) | b below bit 52; with bits 54 and 53, the reset observations, (k << 2) | b with the
+// env's draw counter k after the reset (every reset advances it, whether it samples its state or takes host rows).
+// Never set by sample_init_state (below 2^34), the noise (below bit 42), the reset randomisation (bit 63), the pushes
+// (62), the action delay (61), the observation delay (60), the servo dropouts (59, and 59 | 58 below bit 52), the IMU
+// misalignment (57) or the encoder offsets (56).
+constexpr uint64_t kServoNoiseTag = uint64_t(1) << 55;
+constexpr uint64_t kServoNoiseCycleTag = kServoNoiseTag | (uint64_t(1) << 54);
+constexpr uint64_t kServoNoiseResetTag = kServoNoiseCycleTag | (uint64_t(1) << 53);
+
+// The counter word (b = 0) of cycle s of tick t, and of the observation of the reset that made draw k
+UPKIE_HD uint64_t servo_noise_cycle(uint32_t t, uint32_t s) {
+  return kServoNoiseCycleTag | (uint64_t(t) << 20) | (uint64_t(s) << 2);
+}
+UPKIE_HD uint64_t servo_noise_reset_cycle(uint32_t k) { return kServoNoiseResetTag | (uint64_t(k) << 2); }
+
+// The cycle `age` cycles before cycle nb - 1 of tick t (an observation delay of `age` substeps, an older history entry):
+// cycle t * nb + nb - 1 - age of the env's count of cycles, floored into its tick (modulo 2^32 ticks)
+UPKIE_HD uint64_t servo_noise_cycle_before(uint32_t t, uint32_t nb, uint32_t age) {
+  const uint32_t back = age / nb, s = nb - 1u - age % nb;  // cycle s of tick t - back
+  return servo_noise_cycle(t - back, s);
+}
+
+// Draw k of the env of global index g: column c from word c % 4 of the block of counter c / 4 (push_value's exact form,
+// the map of the servo dropouts). Every column is drawn whatever the ranges.
+struct Sigma12 {
+  float s[kServoNoiseCols];
+};
+UPKIE_HD Sigma12 servo_noise_draw(const UpkieServoNoise& spec, uint64_t seed, uint64_t g, uint32_t k) {
+  Sigma12 o;
+#pragma unroll
+  for (int b = 0; b < 3; ++b) {
+    const Philox4 r = philox4x32_10(g, kServoNoiseTag | (uint64_t(k) << 4) | uint64_t(b), seed);
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const int c = 4 * b + w;
+      const float lo = c < UPKIE_NJ ? spec.position_low[c] : spec.velocity_low[c - UPKIE_NJ];
+      const float hi = c < UPKIE_NJ ? spec.position_high[c] : spec.velocity_high[c - UPKIE_NJ];
+      o.s[c] = push_value(r.v[w], lo, hi);
+    }
+  }
+  return o;
+}
+
+// The twelve standard normals of the cycle of counter word `cycle`: gaussian8's Box-Muller transform on the words of
+// three Philox blocks, normal c from block c / 4
+UPKIE_HD void servo_noise_normals(uint64_t seed, uint64_t g, uint64_t cycle, float n[kServoNoiseCols]) {
+#pragma unroll
+  for (int b = 0; b < 3; ++b) {
+    const Philox4 r = philox4x32_10(g, cycle | uint64_t(b), seed);
+#pragma unroll
+    for (int p = 0; p < 2; ++p) {
+      const float u1 = (float(r.v[2 * p] >> 8) + 1.0f) * (1.0f / 16777216.0f);  // (0, 1]
+      const float u2 = u01(r.v[2 * p + 1]);
+      const float rad = sqrtf(-2.0f * logf(u1));
+      float sn, cs;
+      sincosf(6.28318530718f * u2, &sn, &cs);
+      n[4 * b + 2 * p] = rad * cs;
+      n[4 * b + 2 * p + 1] = rad * sn;
+    }
+  }
+}
+
+// What the noise adds to each reported value of one cycle, sigma * n rounded on its own (never contracted into the
+// sum it enters); exactly 0 where sigma is 0. An env whose sigmas are all zero draws nothing.
+struct Noise12 {
+  float d[kServoNoiseCols];
+};
+UPKIE_HD float servo_noise_mul(float s, float n) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rn(s, n);
+#else
+  return s * n;  // ISO C++ mode: g++ does not contract this into an FMA
+#endif
+}
+template <typename Load>
+UPKIE_HD Noise12 servo_noise_increments(Load sigma, uint64_t seed, uint64_t g, uint64_t cycle) {
+  Noise12 o;
+  bool any = false;
+#pragma unroll
+  for (int c = 0; c < kServoNoiseCols; ++c) {
+    o.d[c] = sigma(c);
+    any = any || o.d[c] != 0.f;
+  }
+  if (!any) return o;
+  float n[kServoNoiseCols];
+  servo_noise_normals(seed, g, cycle, n);
+#pragma unroll
+  for (int c = 0; c < kServoNoiseCols; ++c) o.d[c] = o.d[c] != 0.f ? servo_noise_mul(o.d[c], n[c]) : 0.f;
+  return o;
+}
+
+// The reported state of S under the increments d: q_j + d_j, qd_j + d_{6+j}. A zero increment leaves the value bit for
+// bit. Returns whether a wheel's position or velocity changed (the odometry that the gyropod and pendulum rows report).
+UPKIE_HD bool servo_noise_view(RobotState& S, const Noise12& d) {
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (d.d[j] != 0.f) S.q[j] += d.d[j];
+    if (d.d[UPKIE_NJ + j] != 0.f) S.qd[j] += d.d[UPKIE_NJ + j];
+  }
+  return d.d[2] != 0.f || d.d[5] != 0.f || d.d[UPKIE_NJ + 2] != 0.f || d.d[UPKIE_NJ + 5] != 0.f;
+}
+
+// The gyropod and pendulum leg targets a reset sets (reset_wrapper_state: the true hip and knee positions) made the
+// reported ones of the reset observation: applied before encoder_offset_leg_targets, in the order of the view
+UPKIE_HD void servo_noise_leg_targets(RobotState& S, const Noise12& d) {
+  const int leg_joint[4] = {0, 1, 3, 4};
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    if (d.d[leg_joint[k]] != 0.f) S.leg_target[k] += d.d[leg_joint[k]];
+}
+
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, stored, and the env marked as reporting
+// its reset observation; returns the draw's number k, which keys that observation's cycle. The block's fields are
+// copied before the first store, as servo_dropout_reset.
+UPKIE_HD uint32_t servo_noise_reset(const ServoNoise& N, uint64_t seed, uint64_t g, int i) {
+  const UpkieServoNoise spec = N.spec;
+  uint32_t* const count = N.count;
+  float* const col = N.sigma + size_t(i);
+  uint8_t* const fresh = N.fresh;
+  const size_t stride = size_t(N.stride);
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  const Sigma12 o = servo_noise_draw(spec, seed, g, k);
+#pragma unroll
+  for (int c = 0; c < kServoNoiseCols; ++c) col[size_t(c) * stride] = o.s[c];
+  fresh[i] = 1;
+  return k;
+}
+
+// Whether spine column `col` reports a servo position or velocity, or the wheel odometry built from them
+UPKIE_HD constexpr bool history_noise_column(int col) {
+  return (col >= UPKIE_SP_SERVO && col < UPKIE_SP_ODOM_POS &&
+          ((col - UPKIE_SP_SERVO) % UPKIE_OBS_KEYS == UPKIE_OBS_POSITION ||
+           (col - UPKIE_SP_SERVO) % UPKIE_OBS_KEYS == UPKIE_OBS_VELOCITY)) ||
+         col == UPKIE_SP_ODOM_POS || col == UPKIE_SP_ODOM_VEL;
+}
+
+// A ring filled under servo noise (a reset, a new spec or a state set): every entry holds the columns of S with the
+// noise of the cycle it stands for, the newest (age 0) cycle `newest`, the entry of age a >= 1 the cycle a substeps
+// before cycle nb - 1 of tick t; `view` then reads the copy through the other views. `head` is the env's next write.
+template <typename Sigma, typename View, typename Store>
+UPKIE_HD void history_fill_noise(const History& H, const SimParams& P, const RobotState& S, uint32_t head, Sigma sigma,
+                                 uint64_t seed, uint64_t g, uint64_t newest, uint32_t t, View view, Store store) {
+  const uint32_t ticks = uint32_t(H.ticks);
+  for (uint32_t a = 0; a < ticks; ++a) {
+    RobotState V = S;
+    const uint64_t cyc = a == 0 ? newest : servo_noise_cycle_before(t, uint32_t(P.nb_substeps), a);
+    servo_noise_view(V, servo_noise_increments(sigma, seed, g, cyc));
+    view(V);
+    const uint32_t e = (head + 2u * ticks - 1u - a) % ticks;
+    for (int c = 0; c < H.count; ++c) store(e, c, history_value(P, V, V.imu_acc, H.columns[c]));
+  }
 }
 
 }  // namespace upkie_b200

@@ -136,10 +136,22 @@ __device__ __forceinline__ float* obs_delay_report(const ObsDelay& O, uint32_t s
 // compiled (and its products contracted) as without the history.
 // Under servo dropouts the servos of `lost` report env i's held triple, as the observation does; under an IMU
 // misalignment the columns are read through the env's `em` (after the IMU velocity, which is the true IMU's), and under
-// encoder offsets through its `eo`.
+// encoder offsets through its `eo`. Under servo noise the entry reports the noise of cycle `cyc` (first: a lost reply
+// is held as it was received, noise included), drawn only when a column reports a servo position or velocity.
+__device__ __forceinline__ Noise12 noise_load(const SimParams& P, uint64_t seed, uint64_t g, int i, uint64_t cyc) {
+  const ServoNoise& N = *P.servo_noise;
+  const float* const col = N.sigma + size_t(i);
+  const size_t stride = size_t(N.stride);
+  return servo_noise_increments([&](int c) { return __ldcg(col + size_t(c) * stride); }, seed, g, cyc);
+}
 __device__ __noinline__ void history_substep(const SimParams& P, RobotState S, float* vel, float* e,
                                              size_t stride, int count, bool acc, uint32_t lost, int i, const Quat4 em,
-                                             const Offset6 eo) {
+                                             const Offset6 eo, uint64_t seed, uint64_t g, uint64_t cyc) {
+  if (P.servo_noise) {
+    bool servo = false;
+    for (int c = 0; c < count; ++c) servo = servo || history_noise_column(__ldg(P.history->columns + c));
+    if (servo) servo_noise_view(S, noise_load(P, seed, g, i, cyc));
+  }
   if (lost) {
     const ServoDropout& D = *P.servo_dropout;
     const float* const held = D.held + size_t(i);
@@ -160,7 +172,22 @@ __device__ __noinline__ void history_substep(const SimParams& P, RobotState S, f
   for (int c = 0; c < count; ++c) __stcg(e + size_t(c) * stride, history_value(P, S, a, __ldg(P.history->columns + c)));
 }
 __device__ __noinline__ void history_fill_lane(const SimParams& P, RobotState S, float* col, size_t stride,
-                                               int count, uint32_t ticks, const Quat4 em, const Offset6 eo) {
+                                               int count, uint32_t ticks, const Quat4 em, const Offset6 eo,
+                                               uint64_t seed, uint64_t g, int i, uint32_t head, uint64_t newest,
+                                               uint32_t t) {
+  if (P.servo_noise) {  // every entry with the noise of its own cycle (history_fill_noise)
+    const ServoNoise& N = *P.servo_noise;
+    const float* const sg = N.sigma + size_t(i);
+    const size_t nstride = size_t(N.stride);
+    history_fill_noise(
+        *P.history, P, S, head, [&](int c) { return __ldcg(sg + size_t(c) * nstride); }, seed, g, newest, t,
+        [&](RobotState& V) {
+          imu_misalign_view(V, em);
+          encoder_offset_view(V, eo);
+        },
+        [&](uint32_t e, int c, float v) { __stcg(col + (size_t(e) * size_t(count) + size_t(c)) * stride, v); });
+    return;
+  }
   imu_misalign_view(S, em);
   encoder_offset_view(S, eo);
   for (int c = 0; c < count; ++c) {
@@ -179,11 +206,21 @@ __device__ __noinline__ void history_fill_lane(const SimParams& P, RobotState S,
 struct ServoReplies {
   float q[UPKIE_NJ], qd[UPKIE_NJ], tau[UPKIE_NJ];
 };
-__device__ __noinline__ uint32_t dropout_cycle(const SimParams& P, const ServoReplies R, int i, uint64_t seed, uint64_t g,
+__device__ __noinline__ uint32_t dropout_cycle(const SimParams& P, ServoReplies R, int i, uint64_t seed, uint64_t g,
                                                uint32_t tick, int sub) {
   const ServoDropout& D = *P.servo_dropout;
   const uint32_t mask = D.spec.joint_mask;
-  const uint32_t lost = servo_dropout_lost(mask, __ldcg(D.prob + i), seed, g, tick, uint32_t(sub));
+  const float p = __ldcg(D.prob + i);
+  const uint32_t lost = servo_dropout_lost(mask, p, seed, g, tick, uint32_t(sub));
+  // the replies as received: with the cycle's noise. An env that loses no reply (p_i = 0) reads its held rows only
+  // through the tick's last cycle (k_spine_obs), so its earlier cycles latch without drawing.
+  if (P.servo_noise && (p > 0.f || sub + 1 == P.nb_substeps)) {
+    const Noise12 d = noise_load(P, seed, g, i, servo_noise_cycle(tick, uint32_t(sub)));
+    for (int j = 0; j < UPKIE_NJ; ++j) {
+      if (d.d[j] != 0.f) R.q[j] += d.d[j];
+      if (d.d[UPKIE_NJ + j] != 0.f) R.qd[j] += d.d[UPKIE_NJ + j];
+    }
+  }
   float* const held = D.held + size_t(i);
   const size_t stride = size_t(D.stride);
   for (int j = 0; j < UPKIE_NJ; ++j) {
@@ -206,8 +243,9 @@ __device__ __noinline__ void dropout_sense(const SimParams& P, uint32_t lost, in
     __stcg(scol + size_t(UPKIE_ST_TORQUE + j) * sstride, __ldcg(held + size_t(3 * j + 2) * stride));
   }
 }
-__device__ __noinline__ void dropout_reset_lane(const SimParams& P, const RobotState S, uint64_t seed, uint64_t g,
-                                                int i) {
+__device__ __noinline__ void dropout_reset_lane(const SimParams& P, RobotState S, uint64_t seed, uint64_t g, int i,
+                                                uint64_t rcyc) {
+  if (P.servo_noise) servo_noise_view(S, noise_load(P, seed, g, i, rcyc));  // the reset observation's replies
   servo_dropout_reset(*P.servo_dropout, seed, g, i, S);
 }
 
@@ -234,6 +272,16 @@ __device__ __forceinline__ Offset6 offset_load_lane(const SimParams& P, int i) {
 }
 __device__ __noinline__ Offset6 offset_reset_lane(const SimParams& P, uint64_t seed, uint64_t g, int i) {
   return encoder_offset_reset(*P.encoder_offset, seed, g, i);
+}
+
+// The servo noise (F.sense kernels, P.servo_noise set): what one cycle's noise adds to env i's replies (sigma_i loaded
+// with coherent loads, as tilt_load_lane), and a reset's next draw of sigma_i, stored. Out of line, as tilt_reset_lane:
+// the Philox rounds and the Box-Muller transform are not inlined into the kernel at every use.
+__device__ __noinline__ Noise12 noise_lane(const SimParams& P, uint64_t seed, uint64_t g, int i, uint64_t cyc) {
+  return noise_load(P, seed, g, i, cyc);
+}
+__device__ __noinline__ uint32_t noise_reset_lane(const SimParams& P, uint64_t seed, uint64_t g, int i) {
+  return servo_noise_reset(*P.servo_noise, seed, g, i);
 }
 
 // ---- one env tick of the robot `tid` --------------------------------------------------
@@ -347,6 +395,7 @@ __device__ __forceinline__ void step_env(
     for (int k = 0; k < UPKIE_LAG_DIM; ++k) lr[k] = lag[size_t(k) * n_pad + i];
     lag_from_row(lr, L);
   }
+  uint32_t nk = 0;  // F.sense, servo noise: the draw of a reset of this tick (its reset observation's cycle)
   if (resetting) {
     const uint32_t ep = episode[i] + 1u;
     if (live) episode[i] = ep;
@@ -440,6 +489,18 @@ __device__ __forceinline__ void step_env(
       }
     }
   }
+  // servo measurement noise (F.sense kernels, P.servo_noise set: a uniform branch). sigma_i stays in the env's column
+  // (noise_lane loads it): a reset draws the next one here and at the same-step reset below. Every observation of the
+  // tick is built from a copy of the state whose replies carry the noise of the cycle it reports (servo_noise_view,
+  // before the dropout, misalignment and offset views): the history entries (cycle sub of tick t), the replies the
+  // dropouts latch, the observation (cycle nb - 1, or under an observation delay of d substeps the cycle d before it),
+  // the same-step final observation and stash, and a reset's observation, leg targets, latch and history refill (the
+  // reset cycle of its draw). The physics runs on the true replies.
+  const bool noising = F.sense && P.servo_noise;
+  uint32_t dtot = 0;  // the observation delay of a tick that does not reset, in substeps (min(delay, K nb))
+  if constexpr (F.sense) {
+    if (noising && resetting && live) nk = noise_reset_lane(P, seed, env_offset + uint64_t(i), i);
+  }
   // TILE >= 1: the row the substeps read (torque law, action delay, spine cycle) is the lane's own row of the warp's
   // tile, written here whole (9 x 16 B at a stride of 9 float4: conflict-free) whether the row came from the tile or
   // from global memory, instead of a 36-float register array that ptxas spills to the local-memory frame and reloads in
@@ -494,6 +555,10 @@ __device__ __forceinline__ void step_env(
       }
     } else {
       sdl = min(__ldcg(O.delay + i), uint32_t(P.nb_substeps));
+    }
+    if constexpr (F.sense) {
+      if (noising && !resetting)
+        dtot = min(__ldcg(O.delay + i), uint32_t(O.ticks > 1 ? O.ticks : 1) * uint32_t(P.nb_substeps));
     }
   }
   // servo reply dropouts (F.sense kernels, P.servo_dropout set: a uniform branch). Each substep of a lane that does
@@ -605,7 +670,8 @@ __device__ __forceinline__ void step_env(
       }
       if (recording && !resetting && live)
         history_substep(P, S, hvel, hring + size_t((hhead + uint32_t(sub)) % hticks) * size_t(hcount) * hstride,
-                        hstride, hcount, hacc, dcur, i, em, eo);
+                        hstride, hcount, hacc, dcur, i, em, eo, seed, env_offset + uint64_t(i),
+                        servo_noise_cycle(nz.tick, uint32_t(sub)));
     } else {
 #pragma unroll
       for (int k = 0; k < kPhaseSyncs; ++k) PhaseSync()();
@@ -620,7 +686,10 @@ __device__ __forceinline__ void step_env(
   if (resetting) {
     reset_wrapper_state(S);
     if constexpr (F.sense) {
-      if (offsetting) encoder_offset_leg_targets(S, eo);  // the new episode's reported leg positions
+      // the new episode's reported leg positions: the reset observation's noise, then the offsets
+      if (noising)
+        servo_noise_leg_targets(S, noise_lane(P, seed, env_offset + uint64_t(i), i, servo_noise_reset_cycle(nk)));
+      if (offsetting) encoder_offset_leg_targets(S, eo);
     }
   } else {
     e |= state_sanity(S);
@@ -675,6 +744,14 @@ __device__ __forceinline__ void step_env(
         // servo dropouts: the terminal step's observation and stash report the latched servos. The reset below keeps
         // the commanded torques (its substep commands none), so the true ones are put back after the stores.
         float dtrue[UPKIE_NJ];
+        // the servo noise: the replies of the terminal step's last cycle (the reset below overwrites q and qd whole)
+        if constexpr (F.sense) {
+          if (noising &&
+              servo_noise_view(S, noise_lane(P, seed, env_offset + uint64_t(i), i,
+                                             servo_noise_cycle(nz.tick, uint32_t(P.nb_substeps) - 1u))) &&
+              MODE != MODE_SERVOS)
+            gyropod_obs(P, S, o6);
+        }
         if (F.sense && dropping && dcur) {
 #pragma unroll
           for (int j = 0; j < UPKIE_NJ; ++j) dtrue[j] = S.torque[j];
@@ -715,6 +792,7 @@ __device__ __forceinline__ void step_env(
       if constexpr (F.sense) {
         if (tilting && live) em = tilt_reset_lane(P, seed, env_offset + uint64_t(i), i);  // the new episode's e_i
         if (offsetting && live) eo = offset_reset_lane(P, seed, env_offset + uint64_t(i), i);  // and delta_i
+        if (noising && live) nk = noise_reset_lane(P, seed, env_offset + uint64_t(i), i);  // and sigma_i
       }
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;
@@ -729,7 +807,10 @@ __device__ __forceinline__ void step_env(
       if (spine) reset_robot_spine(P, S, L, init, eps, mu, WarpAny(), P.joint_limits, br);
       else reset_robot(P, S, init, eps, mu, WarpAny(), F.limits ? P.joint_limits : 0, br);
       if constexpr (F.sense) {
-        if (offsetting) encoder_offset_leg_targets(S, eo);  // the new episode's reported leg positions
+        // the new episode's reported leg positions
+        if (noising)
+          servo_noise_leg_targets(S, noise_lane(P, seed, env_offset + uint64_t(i), i, servo_noise_reset_cycle(nk)));
+        if (offsetting) encoder_offset_leg_targets(S, eo);
       }
       if (MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
     }
@@ -739,11 +820,18 @@ __device__ __forceinline__ void step_env(
   // the history: a reset fills the lane's ring from its post-reset state (the true state, here in S), and every lane's
   // head moves on by the tick's substeps
   if (recording && live) {
-    if (refill) history_fill_lane(P, S, hring, hstride, hcount, hticks, em, eo);
+    if (refill)
+      history_fill_lane(P, S, hring, hstride, hcount, hticks, em, eo, seed, env_offset + uint64_t(i), i,
+                        (hhead + uint32_t(P.nb_substeps)) % hticks, servo_noise_reset_cycle(nk), nz.tick);
     __stcg(P.history->head + i, (hhead + uint32_t(P.nb_substeps)) % hticks);
   }
   // the dropouts: a reset latches the lane's post-reset state (the true state, here in S) and draws its next p_i
-  if (dropping && live && dreset) dropout_reset_lane(P, S, seed, env_offset + uint64_t(i), i);
+  if (dropping && live && dreset)
+    dropout_reset_lane(P, S, seed, env_offset + uint64_t(i), i, servo_noise_reset_cycle(nk));
+  // the servo noise: the observation of a tick that does not reset is a step cycle's (k_spine_obs, k_reset_obs)
+  if constexpr (F.sense) {
+    if (noising && live && !dreset) P.servo_noise->fresh[i] = 0;
+  }
   if (sensing) {
     // K > 1: the sensed row becomes the report, and the end of the tick works on it as for one tick
     if (HIST && !resetting && P.obs_delay->ticks > 1) scol = obs_delay_report(*P.obs_delay, srep, i, live);
@@ -756,10 +844,15 @@ __device__ __forceinline__ void step_env(
       S.yaw = fin_yaw;
       S.yaw_vel = fin_yaw_vel;
       obs_delay_sensed_state(S, sense_load);
+      bool fnoise = false;  // the noise of the cycle the snapshot stands for
+      if constexpr (F.sense)
+        fnoise = noising && servo_noise_view(S, noise_lane(P, seed, env_offset + uint64_t(i), i,
+                                                           servo_noise_cycle_before(nz.tick, uint32_t(P.nb_substeps),
+                                                                                    dtot)));
       const bool ftilt = tilting && imu_misalign_view(S, fin_e);  // the terminal episode's sensed orientation
       bool fodo = false;
       if constexpr (F.sense) fodo = offsetting && encoder_offset_view(S, fin_eo);  // and its reported positions
-      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0 || ftilt || fodo))
+      if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0 || ftilt || fodo || fnoise))
         gyropod_obs(P, S, fin_o6);  // (a dropout patched the snapshot, or the orientation is the sensed one)
       if (P.final_obs && live)
         store_final_obs<MODE, spine>(P, S, L, fin_o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
@@ -786,6 +879,16 @@ __device__ __forceinline__ void step_env(
 #pragma unroll
       for (int k = 0; k < UPKIE_STATE_DIM; ++k) sense_store(k, r[k]);
       if (HIST && P.obs_delay->ticks > 1) obs_delay_fill_history(*P.obs_delay, i, r);  // and so does every snapshot
+    }
+  }
+  // the servo noise: the replies of the cycle the observation reports, before the dropouts' held replies (which carry
+  // the noise of the cycle that received them)
+  if constexpr (F.sense) {
+    if (noising) {
+      const uint64_t cyc = dreset ? servo_noise_reset_cycle(nk)
+                                  : servo_noise_cycle_before(nz.tick, uint32_t(P.nb_substeps), dtot);
+      if (servo_noise_view(S, noise_lane(P, seed, env_offset + uint64_t(i), i, cyc)) && MODE != MODE_SERVOS)
+        gyropod_obs(P, S, o6);
     }
   }
   // the dropouts without an observation delay: the observation after a tick that did not reset reports the latched

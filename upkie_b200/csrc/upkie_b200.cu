@@ -17,7 +17,8 @@
 // The IMU misalignment takes none either: k_reset draws, k_ring_copy copies its quaternions for checkpoints, and
 // k_spine_obs, k_reset_obs and k_history_fill read the orientation through it (imu_misalign_observed). Neither do the
 // encoder offsets: k_reset draws and shifts the leg targets, and the same three kernels read the servo positions
-// through them (encoder_offset_observed).
+// through them (encoder_offset_observed). Nor does the servo noise: k_reset draws, noises the leg targets, the latch
+// and the history refill, and the same three kernels read the servo replies through it (servo_noise_observed).
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -160,6 +161,13 @@ struct Handle {
   uint32_t* enc_count = nullptr;
   float* enc_offset = nullptr;  // [UPKIE_NJ][n_pad], delta_i
   uint32_t enc_mask = 0;        // joint_mask of the spec in force
+  // servo measurement noise (upkie_b200_set_servo_noise): the device block P.servo_noise points to while a spec is set,
+  // and the per-env state it points to (allocated with the first spec, freed when it is turned off)
+  ServoNoise* noise_dev = nullptr;
+  uint32_t* noise_count = nullptr;
+  float* noise_sigma = nullptr;  // [12][n_pad], sigma_i
+  uint8_t* noise_fresh = nullptr;
+  UpkieServoNoise noise_spec{};  // the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -184,7 +192,7 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
         const uint8_t* __restrict__ mask, const float* __restrict__ init_state, const float* __restrict__ eps_all,
         const float* __restrict__ mu_all, uint32_t* __restrict__ err, uint8_t* __restrict__ done_prev,
         uint32_t* __restrict__ episode, uint64_t seed, uint64_t env_offset, float* __restrict__ lag,
-        uint64_t rand_seed, uint64_t rand_offset) {
+        uint64_t rand_seed, uint64_t rand_offset, const uint32_t* __restrict__ tick) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   if (mask && !mask[i]) return;
@@ -237,7 +245,17 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
   } else {
     reset_robot(P, S, init, eps, mu, WarpAny(), P.joint_limits, br);
   }
-  // the encoder offsets' next draw: the new episode's leg targets are its reported leg positions
+  // the servo noise's and the encoder offsets' next draws: the new episode's leg targets are its reported leg
+  // positions, the reset observation's (the noise, then the offsets)
+  Noise12 nd;
+  uint64_t rcyc = 0;  // the reset observation's cycle, keyed on the new draw
+  if (P.servo_noise) {
+    const ServoNoise& N = *P.servo_noise;
+    rcyc = servo_noise_reset_cycle(servo_noise_reset(N, rand_seed, g, i));
+    nd = servo_noise_increments([&](int c) { return N.sigma[size_t(c) * size_t(N.stride) + size_t(i)]; }, rand_seed, g,
+                                rcyc);
+    servo_noise_leg_targets(S, nd);
+  }
   Offset6 d{{0.f, 0.f, 0.f, 0.f, 0.f, 0.f}};
   if (P.encoder_offset) {
     d = encoder_offset_reset(*P.encoder_offset, rand_seed, g, i);
@@ -261,12 +279,31 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
   Quat4 e{{1.f, 0.f, 0.f, 0.f}};
   if (P.imu_misalign) e = imu_misalign_reset(*P.imu_misalign, rand_seed, g, i);
   if (P.history) {  // a new episode's history starts from its post-reset columns
-    RobotState V = S;
-    imu_misalign_view(V, e);
-    encoder_offset_view(V, d);
-    history_fill(*P.history, P, V, i);
+    const History& H = *P.history;
+    if (P.servo_noise) {  // each entry with the noise of its cycle, the newest the reset observation's
+      const ServoNoise& N = *P.servo_noise;
+      history_fill_noise(
+          H, P, S, H.head[i], [&](int c) { return N.sigma[size_t(c) * size_t(N.stride) + size_t(i)]; }, rand_seed, g,
+          rcyc, tick[i],
+          [&](RobotState& V) {
+            imu_misalign_view(V, e);
+            encoder_offset_view(V, d);
+          },
+          [&](uint32_t en, int c, float v) {
+            H.ring[(size_t(en) * size_t(H.count) + size_t(c)) * size_t(H.stride) + size_t(i)] = v;
+          });
+    } else {
+      RobotState V = S;
+      imu_misalign_view(V, e);
+      encoder_offset_view(V, d);
+      history_fill(H, P, V, i);
+    }
   }
-  if (P.servo_dropout) servo_dropout_reset(*P.servo_dropout, rand_seed, g, i, S);  // a new p_i, the reset latched
+  if (P.servo_dropout) {  // a new p_i, the reset latched (its replies as the reset observation reports them)
+    RobotState V = S;
+    if (P.servo_noise) servo_noise_view(V, nd);
+    servo_dropout_reset(*P.servo_dropout, rand_seed, g, i, V);
+  }
 }
 
 // The IMU misalignment: the observed orientation of S, read through env i's e_i (the state or a sensed row: under an
@@ -283,6 +320,27 @@ __device__ void encoder_offset_observed(const SimParams& P, int i, RobotState& S
   if (!P.encoder_offset) return;
   const EncoderOffset& E = *P.encoder_offset;
   encoder_offset_view(S, encoder_offset_load([&](int j) { return E.offset[size_t(j) * size_t(E.stride) + size_t(i)]; }));
+}
+
+// The servo noise: the replies of S with the noise of the cycle env i reports, its reset observation's (fresh) or the
+// cycle d before the last step's last cycle (d its observation delay, as the step kernels clamp it; the state or a
+// sensed row), before the other views
+__device__ uint64_t servo_noise_reported_cycle(const SimParams& P, int i, const uint32_t* tick) {
+  const ServoNoise& N = *P.servo_noise;
+  if (N.fresh[i]) return servo_noise_reset_cycle(N.count[i]);
+  uint32_t d = 0;
+  if (P.obs_delay) {
+    const uint32_t cap = uint32_t(P.obs_delay->ticks > 1 ? P.obs_delay->ticks : 1) * uint32_t(P.nb_substeps);
+    d = min(P.obs_delay->delay[i], cap);
+  }
+  return servo_noise_cycle_before(tick[i], uint32_t(P.nb_substeps), d);
+}
+__device__ void servo_noise_observed(const SimParams& P, int i, RobotState& S, const uint32_t* tick,
+                                     uint64_t seed, uint64_t g) {
+  if (!P.servo_noise) return;
+  const ServoNoise& N = *P.servo_noise;
+  servo_noise_view(S, servo_noise_increments([&](int c) { return N.sigma[size_t(c) * size_t(N.stride) + size_t(i)]; },
+                                             seed, g, servo_noise_reported_cycle(P, i, tick)));
 }
 
 // Servo dropouts without an observation delay: the observed state of S, every servo of the mask reporting its held
@@ -315,11 +373,27 @@ __global__ void k_history_read(const __grid_constant__ SimParams P, const Histor
 
 // Every env's history filled from its state (a new spec, set_state, a new ring size)
 __global__ void k_history_fill(const __grid_constant__ SimParams P, const History* __restrict__ H, int n, int n_pad,
-                               const float* __restrict__ state) {
+                               const float* __restrict__ state, const uint32_t* __restrict__ tick,
+                               uint64_t seed, uint64_t env_offset) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   RobotState S;
   load_state(state, n_pad, i, S);
+  if (P.servo_noise) {  // each entry with the noise of its cycle, the newest the one the env reports
+    const ServoNoise& N = *P.servo_noise;
+    const uint64_t g = env_offset + uint64_t(i);
+    history_fill_noise(
+        *H, P, S, H->head[i], [&](int c) { return N.sigma[size_t(c) * size_t(N.stride) + size_t(i)]; },
+        seed, g, servo_noise_reported_cycle(P, i, tick), tick[i],
+        [&](RobotState& V) {
+          imu_misalign_observed(P, i, V);
+          encoder_offset_observed(P, i, V);
+        },
+        [&](uint32_t e, int c, float v) {
+          H->ring[(size_t(e) * size_t(H->count) + size_t(c)) * size_t(H->stride) + size_t(i)] = v;
+        });
+    return;
+  }
   imu_misalign_observed(P, i, S);
   encoder_offset_observed(P, i, S);
   history_fill(*H, P, S, i);
@@ -331,7 +405,8 @@ __global__ void k_history_fill(const __grid_constant__ SimParams P, const Histor
 // store_final_state; neither the reset nor the rest of the step writes tick[i]).
 __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ state,
                             const float* __restrict__ lag, const uint32_t* __restrict__ mark, uint32_t gen,
-                            const uint32_t* __restrict__ tick, uint64_t env_offset, float* __restrict__ out) {
+                            const uint32_t* __restrict__ tick, uint64_t env_offset, float* __restrict__ out,
+                            uint64_t seed) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   if (mark && mark[i] != gen) return;
@@ -348,6 +423,7 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
     RobotState S;
     load_state(state, n_pad, i, S);
     if (!mark) {  // (the stash holds the terminal step's observed state)
+      servo_noise_observed(P, i, S, tick, seed, env_offset + uint64_t(i));
       servo_dropout_observed(P, i, S);
       imu_misalign_observed(P, i, S);
       encoder_offset_observed(P, i, S);
@@ -363,11 +439,12 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
 
 __global__ void k_reset_obs(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ state,
                             const uint32_t* __restrict__ tick, uint64_t env_offset, int obs_dim,
-                            float* __restrict__ out, const float* __restrict__ lag) {
+                            float* __restrict__ out, const float* __restrict__ lag, uint64_t seed) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   RobotState S;
   load_state(state, n_pad, i, S);
+  servo_noise_observed(P, i, S, tick, seed, env_offset + uint64_t(i));
   servo_dropout_observed(P, i, S);
   imu_misalign_observed(P, i, S);
   encoder_offset_observed(P, i, S);
@@ -873,7 +950,7 @@ int history_build(Handle* h) {
   CUDA_TRY(cudaMemcpy(h->hist_dev, &H, sizeof(H), cudaMemcpyHostToDevice));
   h->hist_ticks = ticks;
   h->P.history = h->hist_dev;
-  k_history_fill<<<grid_of(h->n), 128>>>(h->P, h->hist_dev, h->n, h->n_pad, h->state);
+  k_history_fill<<<grid_of(h->n), 128>>>(h->P, h->hist_dev, h->n, h->n_pad, h->state, h->tick, h->seed, h->env_offset);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaDeviceSynchronize());
   return UPKIE_B200_OK;
@@ -1037,6 +1114,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->drop_dev); cudaFree(h->drop_count); cudaFree(h->drop_prob); cudaFree(h->drop_held);
   cudaFree(h->tilt_dev); cudaFree(h->tilt_count); cudaFree(h->tilt_quat);
   cudaFree(h->enc_dev); cudaFree(h->enc_count); cudaFree(h->enc_offset);
+  cudaFree(h->noise_dev); cudaFree(h->noise_count); cudaFree(h->noise_sigma); cudaFree(h->noise_fresh);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -1092,6 +1170,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: encoder offsets need joint_limits != 0");
   if (h->P.encoder_offset && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no encoder-offset kernels");
+  if (h->P.servo_noise && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: servo noise needs joint_limits != 0");
+  if (h->P.servo_noise && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no servo-noise kernels");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -1115,6 +1197,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.servo_dropout = h->P.servo_dropout;  // and the servo dropouts
   P.imu_misalign = h->P.imu_misalign;    // and the IMU misalignment
   P.encoder_offset = h->P.encoder_offset;  // and the encoder offsets
+  P.servo_noise = h->P.servo_noise;        // and the servo noise
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -1321,7 +1404,8 @@ int upkie_b200_reset(void* handle, const uint8_t* mask, const float* init_state,
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   k_reset<<<grid_of(h->n), 128, 0, s>>>(h->P, h->n, h->n_pad, h->state, mask, init_state, h->eps, h->mu, h->err,
-                                        h->done_prev, h->episode, seed, env_offset, h->lag, h->seed, h->env_offset);
+                                        h->done_prev, h->episode, seed, env_offset, h->lag, h->seed, h->env_offset,
+                                        h->tick);
   CUDA_TRY(cudaGetLastError());
   // a reset sampled on the device counts an episode: it is not one the base-velocity post step has to carry out
   if (!init_state)
@@ -1519,7 +1603,7 @@ int upkie_b200_spine_obs(void* handle, float* out, void* stream) {
   // observation delay: the spine observation of the sensed states
   const float* state = h->P.obs_delay ? h->sense_rows : h->state;
   k_spine_obs<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, state, h->lag, nullptr,
-                                                                            0u, h->tick, h->env_offset, out);
+                                                                            0u, h->tick, h->env_offset, out, h->seed);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1545,7 +1629,7 @@ int upkie_b200_final_spine_obs(void* handle, float* out, void* stream) {
       P, h->n, h->n_pad, stash + size_t(kFinalStateRow) * h->n_pad,
       h->lag ? stash + size_t(kFinalLagRow) * h->n_pad : nullptr,
       reinterpret_cast<const uint32_t*>(stash + size_t(kFinalMarkRow) * h->n_pad), h->final_gen, h->tick,
-      h->env_offset, out);
+      h->env_offset, out, h->seed);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1558,7 +1642,7 @@ int upkie_b200_reset_obs(void* handle, int obs_dim, float* obs, void* stream) {
   // observation delay: the observation of the sensed states (those of the envs a reset took are the post-reset state;
   // the others report their robot as the last step observed it)
   const float* state = h->P.obs_delay ? h->sense_rows : h->state;
-  k_reset_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, state, h->tick, h->env_offset, obs_dim, obs, h->lag);
+  k_reset_obs<<<(h->n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, state, h->tick, h->env_offset, obs_dim, obs, h->lag, h->seed);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1589,8 +1673,8 @@ int upkie_b200_set_state(void* handle, const float* state, void* stream) {
   if (h->P.servo_dropout) CUDA_TRY(servo_dropout_latch(h, ~0u, static_cast<cudaStream_t>(stream)));
   // the observation history restarts from the state set
   if (h->P.history) {
-    k_history_fill<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->P.history, h->n, h->n_pad,
-                                                                                 h->state);
+    k_history_fill<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+        h->P, h->P.history, h->n, h->n_pad, h->state, h->tick, h->seed, h->env_offset);
     CUDA_TRY(cudaGetLastError());
   }
   return UPKIE_B200_OK;
@@ -1937,6 +2021,9 @@ int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationD
   if (max_ticks == 0 || max_ticks > UPKIE_MAX_DELAY_TICKS)
     return fail(UPKIE_B200_EINVAL, "set_observation_delay: max_ticks outside 1 .. UPKIE_MAX_DELAY_TICKS");
   if (const char* why = obs_delay_spec_error(*spec, h->P, max_ticks)) return fail(UPKIE_B200_EINVAL, why);
+  if (h->P.servo_noise && h->P.servo_dropout)
+    return fail(UPKIE_B200_EINVAL, "set_observation_delay: not with both servo noise and servo dropouts (a delayed "
+                                   "snapshot does not record which of its replies were held)");
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
   const bool allocated = h->sense_rows != nullptr;
@@ -2044,6 +2131,9 @@ int upkie_b200_set_servo_dropout(void* handle, const UpkieServoDropout* spec) {
     return UPKIE_B200_OK;
   }
   if (const char* why = servo_dropout_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  if (h->P.servo_noise && h->P.obs_delay)
+    return fail(UPKIE_B200_EINVAL, "set_servo_dropout: not with both servo noise and an observation delay (a delayed "
+                                   "snapshot does not record which of its replies were held)");
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
   // the servos the held rows have not followed latch the current state: every servo when the feature is switched on
@@ -2252,6 +2342,121 @@ int upkie_b200_set_encoder_offset_state(void* handle, const uint32_t* count, con
   }
   CUDA_TRY(cudaMemcpyAsync(h->enc_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(ring_cols(offset, UPKIE_NJ, h->n, h->n_pad, h->enc_offset, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_servo_noise(void* handle, const UpkieServoNoise* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    if (h->P.servo_noise) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the per-env state
+      h->P.servo_noise = nullptr;
+      cudaFree(h->noise_count);
+      cudaFree(h->noise_sigma);
+      cudaFree(h->noise_fresh);
+      h->noise_count = nullptr;
+      h->noise_sigma = nullptr;
+      h->noise_fresh = nullptr;
+      h->noise_spec = UpkieServoNoise{};
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = servo_noise_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
+  if (!h->P.servo_noise) {
+    // switched on: zero counters, and zero sigmas until each env's next reset
+    CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->noise_count), size_t(h->n) * sizeof(uint32_t)},
+                           {reinterpret_cast<void**>(&h->noise_sigma), size_t(kServoNoiseCols) * h->n_pad * sizeof(float)},
+                           {reinterpret_cast<void**>(&h->noise_fresh), size_t(h->n_pad)}}));
+  } else {
+    // a replacement: the columns whose high bound is 0 have no noise from now on
+    for (int c = 0; c < kServoNoiseCols; ++c) {
+      const float hi = c < UPKIE_NJ ? spec->position_high[c] : spec->velocity_high[c - UPKIE_NJ];
+      if (hi == 0.f) CUDA_TRY(cudaMemset(h->noise_sigma + size_t(c) * h->n_pad, 0, size_t(h->n_pad) * sizeof(float)));
+    }
+  }
+  if (!h->noise_dev) CUDA_TRY(cudaMalloc(&h->noise_dev, sizeof(ServoNoise)));
+  ServoNoise N;
+  std::memset(&N, 0, sizeof(N));
+  N.spec = *spec;
+  N.count = h->noise_count;
+  N.sigma = h->noise_sigma;
+  N.fresh = h->noise_fresh;
+  N.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->noise_dev, &N, sizeof(N), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->P.servo_noise = h->noise_dev;
+  h->noise_spec = *spec;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_servo_noise_state(void* handle, uint32_t* count, float* sigma, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !sigma) return fail(UPKIE_B200_EINVAL, "get_servo_noise_state: invalid argument");
+  if (!h->P.servo_noise)
+    return fail(UPKIE_B200_EINVAL, "get_servo_noise_state: no servo noise is set (upkie_b200_set_servo_noise)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemcpyAsync(count, h->noise_count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_rows(h->noise_sigma, kServoNoiseCols, h->n, h->n_pad, sigma, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_servo_noise_state(void* handle, const uint32_t* count, const float* sigma, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !sigma) return fail(UPKIE_B200_EINVAL, "set_servo_noise_state: invalid argument");
+  if (!h->P.servo_noise)
+    return fail(UPKIE_B200_EINVAL, "set_servo_noise_state: no servo noise is set (upkie_b200_set_servo_noise)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // every sigma must be a sensor noise (the fixed caps of a spec's bounds, not the spec in force: a narrower spec
+  // leaves each env's sigmas until its next reset, and a checkpoint taken before then must load), and zero in the
+  // columns the spec in force turns off: read back (after the caller's work on the stream) and checked here
+  std::vector<float> v(size_t(h->n) * kServoNoiseCols);
+  CUDA_TRY(cudaMemcpyAsync(v.data(), sigma, v.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  const UpkieServoNoise& sp = h->noise_spec;
+  for (size_t k = 0; k < v.size(); ++k) {
+    const int c = int(k % kServoNoiseCols);
+    const float hi = c < UPKIE_NJ ? sp.position_high[c] : sp.velocity_high[c - UPKIE_NJ];
+    if (!(v[k] >= 0.f && v[k] <= (c < UPKIE_NJ ? 0.1f : 5.f)))
+      return fail(UPKIE_B200_EINVAL, "set_servo_noise_state: every sigma must be finite, >= 0, at most 0.1 rad for a "
+                                     "position and 5 rad/s for a velocity");
+    if (v[k] != 0.f && hi == 0.f)
+      return fail(UPKIE_B200_EINVAL, "set_servo_noise_state: a column whose high bound is zero must have a zero sigma");
+  }
+  CUDA_TRY(cudaMemcpyAsync(h->noise_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_cols(sigma, kServoNoiseCols, h->n, h->n_pad, h->noise_sigma, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_servo_noise_mark(void* handle, uint8_t* mark, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !mark) return fail(UPKIE_B200_EINVAL, "get_servo_noise_mark: invalid argument");
+  if (!h->P.servo_noise)
+    return fail(UPKIE_B200_EINVAL, "get_servo_noise_mark: no servo noise is set (upkie_b200_set_servo_noise)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaMemcpyAsync(mark, h->noise_fresh, size_t(h->n), cudaMemcpyDeviceToDevice,
+                           static_cast<cudaStream_t>(stream)));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_servo_noise_mark(void* handle, const uint8_t* mark, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !mark) return fail(UPKIE_B200_EINVAL, "set_servo_noise_mark: invalid argument");
+  if (!h->P.servo_noise)
+    return fail(UPKIE_B200_EINVAL, "set_servo_noise_mark: no servo noise is set (upkie_b200_set_servo_noise)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<uint8_t> m(size_t(h->n));
+  CUDA_TRY(cudaMemcpyAsync(m.data(), mark, m.size(), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (uint8_t x : m)
+    if (x > 1) return fail(UPKIE_B200_EINVAL, "set_servo_noise_mark: every mark must be 0 or 1");
+  CUDA_TRY(cudaMemcpyAsync(h->noise_fresh, mark, m.size(), cudaMemcpyDefault, s));
   return UPKIE_B200_OK;
 }
 

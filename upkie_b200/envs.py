@@ -851,6 +851,83 @@ def encoder_offset_spec(offset, joints=None, spine_mode: bool = False, joint_lim
     return _abi.UpkieEncoderOffset(float(lo), float(hi), mask, 0)
 
 
+def _noise_range(name: str, value):
+    """(low, high) float32 of one servo-noise level: a standard deviation ``s`` or a ``(low, high)`` range"""
+    if isinstance(value, (int, float, np.integer, np.floating)):
+        lo = hi = value
+    else:
+        try:
+            lo, hi = value
+        except (TypeError, ValueError):
+            raise UpkieException(f"servo_noise: {name}: expected a standard deviation or a (low, high) pair, got "
+                                 f"{value!r}") from None
+    try:
+        lo, hi = np.float32(lo), np.float32(hi)
+    except (TypeError, ValueError):
+        raise UpkieException(f"servo_noise: {name}: expected numbers, got ({lo!r}, {hi!r})") from None
+    cap = np.float32(_abi.SERVO_NOISE_MAX[name.split(".")[0]])
+    if not (np.isfinite(lo) and np.isfinite(hi)) or lo < 0 or hi > cap:
+        raise UpkieException(f"servo_noise: {name}: expected finite levels within [0, {cap}], got ({lo}, {hi})")
+    if lo > hi:
+        raise UpkieException(f"servo_noise: {name}: expected low <= high, got ({lo}, {hi})")
+    return lo, hi
+
+
+def servo_noise_spec(noise, spine_mode: bool = False, joint_limits: Union[bool, int] = True,
+                     body_contacts: Union[bool, int] = False, observation_delay: bool = False,
+                     servo_dropout: bool = False) -> Optional[_abi.UpkieServoNoise]:
+    """``UpkieServoNoise`` (``UpkieSim.set_servo_noise``) from a dict with keys ``position`` (radians) and
+    ``velocity`` (rad/s), each a standard deviation ``s`` for every joint, a ``(low, high)`` range from which every
+    reset draws each joint's, or a dict ``{joint: s or (low, high)}`` (``JOINT_NAMES``; the joints it leaves out have
+    no noise). A quantity left out has no noise. Raises ``UpkieException`` on an unknown key or joint, a level that is
+    not a finite number, a negative low, ``low > high``, a position level above 0.1 rad or a velocity level above
+    5 rad/s (a sensor noise, not a broken encoder), ``spine_mode`` (whose spine reports its own servos), no joint limits,
+    ``body_contacts`` (the noise runs in the kernels of the observation delay), and an observation delay together with
+    servo dropouts."""
+    if noise is None:
+        return None
+    if not isinstance(noise, dict):
+        raise UpkieException(f"servo_noise: expected a dict with keys 'position' and 'velocity', got {noise!r}")
+    unknown = [k for k in noise if k not in ("position", "velocity")]
+    if unknown:
+        raise UpkieException(f"servo_noise: unknown key(s) {unknown}, expected 'position' and 'velocity'")
+    spec = _abi.UpkieServoNoise()
+    for name in ("position", "velocity"):
+        value = noise.get(name)
+        lo = np.zeros(_abi.NJ, dtype=np.float32)
+        hi = np.zeros(_abi.NJ, dtype=np.float32)
+        if isinstance(value, dict):
+            bad = [j for j in value if j not in _abi.JOINT_NAMES]
+            if bad:
+                raise UpkieException(f"servo_noise: {name}: unknown joint(s) {bad}, expected names of "
+                                     f"{_abi.JOINT_NAMES}")
+            for j, v in value.items():
+                k = _abi.JOINT_NAMES.index(j)
+                lo[k], hi[k] = _noise_range(f"{name}.{j}", v)
+        elif value is not None:
+            lo[:], hi[:] = _noise_range(name, value)
+        getattr(spec, f"{name}_low")[:] = [float(x) for x in lo]
+        getattr(spec, f"{name}_high")[:] = [float(x) for x in hi]
+    if spine_mode:
+        raise UpkieException("servo_noise: spine_mode reports the spine's own servos; the noise is not available there")
+    if not joint_limits:
+        raise UpkieException("servo_noise: needs joint_limits (the noise runs in the kernels with joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("servo_noise: body_contacts has no servo-noise kernels")
+    if observation_delay and servo_dropout:
+        raise UpkieException("servo_noise: not with both an observation delay and servo dropouts (a delayed snapshot "
+                             "does not record which of its replies were held)")
+    return spec
+
+
+def _set_servo_noise(sim, spec: Optional[_abi.UpkieServoNoise]) -> None:
+    if spec is None:
+        sim.set_servo_noise(None)
+    else:
+        sim.set_servo_noise((list(spec.position_low), list(spec.position_high)),
+                            (list(spec.velocity_low), list(spec.velocity_high)))
+
+
 def _set_encoder_offset(sim, spec: Optional[_abi.UpkieEncoderOffset]) -> None:
     if spec is None:
         sim.set_encoder_offset(None)
@@ -962,6 +1039,15 @@ class B200VectorEnv(VectorEnv):
     ``-delta``. The physics, terminations and ``get_state``'s q see the true joints. The draws are keyed on the seed of
     ``reset(seed=s)``, which also restarts the draw counters of the envs it resets. ``set_encoder_offset`` changes or
     (``None``) stops it.
+
+    ``servo_noise`` (a dict ``{"position": ..., "velocity": ...}``, each a standard deviation, a ``(low, high)`` range
+    or ``{joint: s or (low, high)}``, see ``servo_noise_spec``) adds white noise to every servo position (radians) and
+    velocity (rad/s) reply, at levels drawn per joint at every reset of the env, as the moteus encoder estimates reach
+    the spine (``observe_servos.cpp``). Every position and velocity an env type observes (servo rows, the gyropod and
+    pendulum wheel odometry, the spine observation, the history) carries the noise of the spine cycle it reports; the
+    physics, the torques, terminations and ``get_state`` see the true replies. The draws are keyed on the seed of
+    ``reset(seed=s)``, which also restarts the draw counters of the envs it resets. ``set_servo_noise`` changes or
+    (``None``) stops it.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -1007,6 +1093,7 @@ class B200VectorEnv(VectorEnv):
         imu_misalignment: Optional[Dict[str, Union[float, Tuple[float, float]]]] = None,
         encoder_offset: Optional[Union[float, Tuple[float, float]]] = None,
         encoder_offset_joints: Optional[Sequence[str]] = None,
+        servo_noise: Optional[Dict[str, Any]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -1062,6 +1149,8 @@ class B200VectorEnv(VectorEnv):
                                           config.body_contacts)  # validated before any device is touched
         enc_spec = encoder_offset_spec(encoder_offset, encoder_offset_joints, bool(config.spine_mode),
                                        config.joint_limits, config.body_contacts)  # validated before any device
+        noise_spec = servo_noise_spec(servo_noise, bool(config.spine_mode), config.joint_limits, config.body_contacts,
+                                      sense_spec is not None, drop_spec is not None)  # validated before any device
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -1127,6 +1216,17 @@ class B200VectorEnv(VectorEnv):
             _set_imu_misalignment(self.sim, tilt_spec)  # before the first reset, which draws every env's misalignment
         if enc_spec is not None:
             _set_encoder_offset(self.sim, enc_spec)  # before the first reset, which draws every env's offsets
+        if noise_spec is not None:
+            _set_servo_noise(self.sim, noise_spec)  # before the first reset, which draws every env's levels
+
+    def set_servo_noise(self, noise) -> None:
+        """Add white noise to the servos' position and velocity replies at levels drawn per env (a dict, see
+        ``servo_noise_spec``); ``None`` turns the noise off. New ranges take effect at each env's next reset; the
+        columns whose range they make zero have no noise from now on."""
+        _set_servo_noise(self.sim, servo_noise_spec(noise, bool(self.config.spine_mode), self.config.joint_limits,
+                                                    self.config.body_contacts,
+                                                    getattr(self.sim, "_observation_delay", None) is not None,
+                                                    self.sim.servo_dropout_spec is not None))
 
     def set_encoder_offset(self, offset, joints=None) -> None:
         """Zero the servos ``joints`` (names, None: the hips and knees) off by an offset drawn from a bound or a
@@ -1372,6 +1472,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_encoder_offset_state(count, offset)
+            if self.sim.servo_noise_spec is not None:
+                # so is the servo noise
+                count, sigma = self.sim.get_servo_noise_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_servo_noise_state(count, sigma)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

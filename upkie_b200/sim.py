@@ -430,6 +430,73 @@ class UpkieSim:
         self._check_tensor(offset, (self.n, _abi.NJ), name="offset")
         check(lib().upkie_b200_set_encoder_offset_state(self._h, _ptr(count), _ptr(offset), self._stream()))
 
+    def set_servo_noise(self, position=None, velocity=None) -> None:
+        """While ranges are set, every reported servo position and velocity carries white noise: each reset of an env
+        draws one standard deviation per joint and quantity, ``sigma ~ U(low, high)`` (radians for ``position``, rad/s
+        for ``velocity``, each a ``(low[6], high[6])`` pair in ``JOINT_NAMES`` order; None: no noise on that quantity),
+        and each spine cycle adds ``sigma * n``, n a standard normal keyed on the auto-reset seed, the env and the
+        cycle (``include/upkie_b200.h``). Every output that reports a cycle reports the same noise: the servo rows,
+        ``spine_obs`` and its wheel odometry, the gyropod and pendulum ``p`` / ``pdot``, the final observations and the
+        history. The physics, the torques and ``get_state`` see the true replies. Both None turns the noise off.
+        Setting ranges draws nothing: they take effect at each env's next reset."""
+        if position is None and velocity is None:
+            check(lib().upkie_b200_set_servo_noise(self._h, None))
+            self._servo_noise = None
+            return
+        spec = _abi.UpkieServoNoise()
+        for name, pair in (("position", position), ("velocity", velocity)):
+            lo, hi = ([0.0] * _abi.NJ, [0.0] * _abi.NJ) if pair is None else pair
+            lo = np.asarray(lo, dtype=np.float32).reshape(-1)
+            hi = np.asarray(hi, dtype=np.float32).reshape(-1)
+            if lo.shape != (_abi.NJ,) or hi.shape != (_abi.NJ,):
+                raise UpkieException(f"set_servo_noise: {name} expects (low[6], high[6])")
+            getattr(spec, f"{name}_low")[:] = [float(x) for x in lo]
+            getattr(spec, f"{name}_high")[:] = [float(x) for x in hi]
+        check(lib().upkie_b200_set_servo_noise(self._h, C.byref(spec)))
+        self._servo_noise = ((tuple(spec.position_low), tuple(spec.position_high)),
+                             (tuple(spec.velocity_low), tuple(spec.velocity_high)))
+
+    @property
+    def servo_noise_spec(self):
+        """``((position_low, position_high), (velocity_low, velocity_high))`` of the servo noise in force, or None."""
+        return getattr(self, "_servo_noise", None)
+
+    def get_servo_noise_state(self):
+        """Per-env servo-noise state ``(count[N], sigma[N, 12])``: the draw counters (int32 bits of uint32) and each
+        env's standard deviations, columns 0-5 the joints' position noise (rad), 6-11 their velocity noise (rad/s)."""
+        if self.servo_noise_spec is None:
+            raise UpkieException("no servo noise is set (set_servo_noise)")
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        sigma = torch.empty((self.n, 2 * _abi.NJ), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_servo_noise_state(self._h, _ptr(count), _ptr(sigma), self._stream()))
+        return count, sigma
+
+    def set_servo_noise_state(self, count: torch.Tensor, sigma: torch.Tensor) -> None:
+        """Set every env's draw counter and standard deviations (finite, >= 0, at most 0.1 rad / 5 rad/s, zero in a
+        column whose high bound is zero): a checkpoint, or levels measured on a robot (kept until each env's next
+        reset)."""
+        if self.servo_noise_spec is None:
+            raise UpkieException("no servo noise is set (set_servo_noise)")
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(sigma, (self.n, 2 * _abi.NJ), name="sigma")
+        check(lib().upkie_b200_set_servo_noise_state(self._h, _ptr(count), _ptr(sigma), self._stream()))
+
+    def get_servo_noise_mark(self) -> torch.Tensor:
+        """Per-env mark ``[N]`` (uint8): 1 while the env reports its reset observation (``spine_obs`` and
+        ``reset_obs`` then carry the reset cycle's noise), 0 after a step that did not reset it."""
+        if self.servo_noise_spec is None:
+            raise UpkieException("no servo noise is set (set_servo_noise)")
+        mark = torch.empty(self.n, dtype=torch.uint8, device=self.device)
+        check(lib().upkie_b200_get_servo_noise_mark(self._h, _ptr(mark), self._stream()))
+        return mark
+
+    def set_servo_noise_mark(self, mark: torch.Tensor) -> None:
+        """Set every env's mark (0 or 1, see ``get_servo_noise_mark``): a checkpoint."""
+        if self.servo_noise_spec is None:
+            raise UpkieException("no servo noise is set (set_servo_noise)")
+        self._check_tensor(mark, (self.n,), torch.uint8, "mark")
+        check(lib().upkie_b200_set_servo_noise_mark(self._h, _ptr(mark), self._stream()))
+
     def set_history(self, columns: Optional[Sequence[int]], size: int = 1) -> None:
         """Record each env's spine-observation ``columns`` (``_abi.SP_*``, 1 to ``MAX_HISTORY_CHANNELS`` of them) after
         every substep, and report the last ``size`` (1 to ``MAX_HISTORY``) through ``get_history``: the spine's
@@ -898,6 +965,11 @@ class UpkieSim:
         if self.encoder_offset_spec is not None:
             sd["encoder_offset"] = self.encoder_offset_spec
             sd["encoder_offset_count"], sd["encoder_offset_offset"] = self.get_encoder_offset_state()
+        # the servo noise: its ranges and the per-env state (absent without a spec)
+        if self.servo_noise_spec is not None:
+            sd["servo_noise"] = self.servo_noise_spec
+            sd["servo_noise_count"], sd["servo_noise_sigma"] = self.get_servo_noise_state()
+            sd["servo_noise_mark"] = self.get_servo_noise_mark()
         sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
@@ -921,6 +993,9 @@ class UpkieSim:
         elapsed = torch.zeros(self.n, dtype=torch.int32, device=dev) if elapsed is None else elapsed.to(dev).contiguous()
         check(lib().upkie_b200_set_elapsed(self._h, _ptr(elapsed), self._stream()))
         torch.cuda.current_stream(dev).synchronize()
+        # the servo noise is off while the observation delay and the servo dropouts are restored (a handle with noise
+        # refuses the second of the two), and restored last
+        self.set_servo_noise(None)
         # the buffers a reset randomisation spec writes into are restored with the spec off; a checkpoint written
         # before reset randomisation existed loads as "off, counters 0"
         if getattr(self, "_reset_randomization", None) is not None:
@@ -1023,6 +1098,13 @@ class UpkieSim:
             self.set_encoder_offset(enc[0], enc[1], [n for j, n in enumerate(_abi.JOINT_NAMES) if (enc[2] >> j) & 1])
             self.set_encoder_offset_state(*(sd[k].to(dev).contiguous() for k in (
                 "encoder_offset_count", "encoder_offset_offset")))
+        # the servo noise (off above); a checkpoint without it (or written before it existed) leaves it off
+        noise = sd.get("servo_noise")
+        if noise is not None:
+            self.set_servo_noise(*noise)
+            self.set_servo_noise_state(*(sd[k].to(dev).contiguous() for k in ("servo_noise_count", "servo_noise_sigma")))
+            if sd.get("servo_noise_mark") is not None:
+                self.set_servo_noise_mark(sd["servo_noise_mark"].to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
