@@ -1020,6 +1020,53 @@ int upkie_b200_set_servo_noise_state(void* handle, const uint32_t* count, const 
 int upkie_b200_get_servo_noise_mark(void* handle, uint8_t* mark, void* stream);
 int upkie_b200_set_servo_noise_mark(void* handle, const uint8_t* mark, void* stream);
 
+/* ---- Servo velocity limits (tools/configure_servos:99-104, moteus servo.max_velocity) -----------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. Every Upkie's servos are configured with a
+ * velocity limit (servo.max_velocity: 2 rev/s on the hips and knees, 8 rev/s on the wheels); past it the moteus
+ * firmware reduces its output, which reaches zero at max_velocity + servo.max_velocity_derate. The model implemented
+ * here rests on two assumptions taken from the moteus documentation, not from a source in this project: the derate
+ * band's default of 2 rev/s (UPKIE_VELOCITY_DERATE in upkie_b200.envs), and that only motoring torque is limited.
+ * While a spec is set:
+ * - Draw per reset: at every reset of env i (both fused auto-resets, upkie_b200_reset with or without a mask or host
+ *   rows) a limit per joint is drawn. Draw law: a per-env counter k, +1 at every reset; draw k of the env of global
+ *   index g = env_offset + i is Philox4x32-10 with key seed (upkie_b200_set_autoreset) and counters
+ *   (g, 2^52 | k << 4 | b), b = 0, 1; word j % 4 of block b = j / 4 gives v_ij = min(low_j + fl(fl(high_j - low_j) *
+ *   u(w)), high_j), u(w) = (w >> 8) / 2^24 (the servo dropouts' map). Every joint's word is drawn whatever the mask,
+ *   and a joint outside joint_mask stores exactly 0, so that changing the mask changes no other joint's draw. Tag bit
+ *   52 keeps these counters apart from the initial states (below 2^34), the noise (below bit 42), the reset
+ *   randomisation (bit 63), the pushes (62), the action delay (61), the observation delay (60), the servo dropouts (59,
+ *   59 | 58, below bit 52 otherwise), the IMU misalignment (57), the encoder offsets (56) and the servo noise (55,
+ *   55 | 54 below bit 52, 55 | 54 | 53).
+ * - Law: in every substep, t is the torque of the servo law as without a spec (PD law, joint friction and control
+ *   noise, clipped to +-maximum_torque). For a joint of the mask with |qd| > v_ij (qd the true joint velocity of the
+ *   substep): f = clamp((v_ij + derate_j - |qd|) / derate_j, 0, 1), cap = f * tau_max_j (the model's effort limit),
+ *   and t = min(t, cap) for qd > 0, max(t, -cap) for qd < 0. A torque that brakes the joint passes unchanged, and
+ *   below the limit t is left bit for bit. The derated torque is what the physics integrates and what the torque
+ *   replies report (torque measurement noise added on top of it). External forces and pushes are added after the law,
+ *   the action delay's command is derated like any other, and the zero-torque substep of a reset is untouched.
+ * - Not affected: the observations but the torque, servo noise, encoder offsets and delays (the law runs on the true
+ *   qd), the velocity target clamp (qd_max) and max_coordinate_velocity.
+ * Setting a spec draws nothing: each env keeps the limits of the joints that stay in the mask until its next reset;
+ * the joints a spec adds to the mask (every joint of the first spec) take max_velocity_high until then, and the joints
+ * it drops store 0. NULL turns the feature off (the per-env state is freed once the device is idle). Per-env state
+ * (get/set_velocity_derate_state, for checkpoints and fixed limits; device pointers): count[N] and
+ * max_velocity[N][6] in rad/s; UPKIE_B200_EINVAL without a spec, for a value of a joint of the mask in force that is
+ * not finite or <= 0, and for a nonzero value of a joint outside it.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: a bound that is not finite, max_velocity_low <= 0 or
+ * low > high or derate <= 0 on a joint of the mask, a joint_mask of zero or with bits above 5, reserved != 0,
+ * spine_mode (whose spine applies its own torque law), joint_limits == 0 and body_contacts (it runs in the
+ * observation-delay kernels). upkie_b200_set_config rejects joint_limits = 0 and body_contacts while a spec is set;
+ * the in-kernel rollout transports reject a handle with one. The set call waits for the device. */
+typedef struct UpkieVelocityDerate {
+  float max_velocity_low[6], max_velocity_high[6]; /* rad/s, range of each joint's velocity limit (UPKIE_NJ order) */
+  float derate[6];     /* rad/s, the band past the limit over which the motoring torque falls to zero */
+  uint32_t joint_mask; /* bit j: joint j has a velocity limit */
+  uint32_t reserved;   /* 0 */
+} UpkieVelocityDerate;
+int upkie_b200_set_velocity_derate(void* handle, const UpkieVelocityDerate* spec);
+int upkie_b200_get_velocity_derate_state(void* handle, uint32_t* count, float* max_velocity, void* stream);
+int upkie_b200_set_velocity_derate_state(void* handle, const uint32_t* count, const float* max_velocity, void* stream);
+
 /* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
  * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
  * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last

@@ -9,6 +9,7 @@ action keys ``upkie/envs/upkie_servos.py:98-105``, observation keys
 """
 
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -458,6 +459,26 @@ class UpkieEncoderOffset(C.Structure):
 
 
 ENCODER_OFFSET_DEFAULT_JOINTS = ("left_hip", "left_knee", "right_hip", "right_knee")  # zeroed by hand on the robot
+
+
+RAD_PER_REV = 2.0 * math.pi  # a speed in rev/s (the moteus unit) times this is in rad/s
+# servo.max_velocity_derate, the band past servo.max_velocity over which a moteus servo's output falls to zero: 2 rev/s,
+# the default of the moteus reference documentation as remembered (an assumption: no source in this project states it)
+MOTEUS_MAX_VELOCITY_DERATE = 2.0 * RAD_PER_REV
+
+
+class UpkieVelocityDerate(C.Structure):
+    """``UpkieVelocityDerate`` of include/upkie_b200.h: the range of each joint's velocity limit, drawn per env at every
+    reset, and the band past it over which the servo's motoring torque falls to zero, in rad/s (UPKIE_NJ order;
+    rev/s times 2 pi)."""
+
+    _fields_ = [
+        ("max_velocity_low", C.c_float * 6),
+        ("max_velocity_high", C.c_float * 6),
+        ("derate", C.c_float * 6),
+        ("joint_mask", C.c_uint32),
+        ("reserved", C.c_uint32),
+    ]
 
 
 MAX_HISTORY = 64  # UPKIE_MAX_HISTORY: the most entries an observation history reports

@@ -271,6 +271,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.imu_misalign = nullptr;
   P.encoder_offset = nullptr;
   P.servo_noise = nullptr;
+  P.velocity_derate = nullptr;
   return 0;
 }
 
@@ -457,6 +458,27 @@ inline const char* servo_noise_spec_error(const UpkieServoNoise& s, const SimPar
   if (P.obs_delay && P.servo_dropout)
     return "set_servo_noise: not with both an observation delay and servo dropouts (a delayed snapshot does not "
            "record which of its replies were held)";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses a velocity-limit spec (upkie_b200_set_velocity_derate), null when it takes it:
+// every bound finite, and on a joint of the mask 0 < low <= high and derate > 0
+inline const char* velocity_derate_spec_error(const UpkieVelocityDerate& s, const SimParams& P) {
+  if (s.joint_mask == 0 || (s.joint_mask >> UPKIE_NJ) != 0)
+    return "set_velocity_derate: joint_mask must select joints of bits 0 .. 5, at least one";
+  if (s.reserved != 0) return "set_velocity_derate: reserved must be 0";
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!std::isfinite(s.max_velocity_low[j]) || !std::isfinite(s.max_velocity_high[j]) || !std::isfinite(s.derate[j]))
+      return "set_velocity_derate: every bound must be finite";
+    if (!((s.joint_mask >> j) & 1u)) continue;
+    if (!(s.max_velocity_low[j] > 0.f && s.max_velocity_low[j] <= s.max_velocity_high[j]))
+      return "set_velocity_derate: 0 < max_velocity_low <= max_velocity_high required on every joint of the mask";
+    if (!(s.derate[j] > 0.f)) return "set_velocity_derate: derate > 0 required on every joint of the mask";
+  }
+  if (P.joint_limits == 0)
+    return "set_velocity_derate: needs joint_limits != 0 (the limits run in the observation-delay kernels)";
+  if (P.spine_mode) return "set_velocity_derate: spine_mode applies the spine's own torque law";
+  if (P.body_contacts) return "set_velocity_derate: body_contacts has no velocity-limit kernels";
   return nullptr;
 }
 

@@ -159,6 +159,9 @@ struct SimParams {
   // servo measurement noise (upkie_b200_set_servo_noise): the handle's device block, null = off. Read by the step kernels
   // of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs and k_history_fill only. Appended last.
   const struct ServoNoise* servo_noise;
+  // servo velocity limits (upkie_b200_set_velocity_derate): the handle's device block, null = off. Read by the step
+  // kernels of FAM_SENSE (step_family.h) and k_reset only. Appended last.
+  const struct VelocityDerate* velocity_derate;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -1023,6 +1026,34 @@ UPKIE_HD float joint_torque(float torque_control_kp, float torque_control_kd, fl
   return fminf(fmaxf(torque, -maximum_torque), maximum_torque);
 }
 
+// ---- Servo velocity limits (upkie_b200_set_velocity_derate, tools/configure_servos:99-104) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw, and max_velocity = v_i, each joint's limit in rad/s (0 outside the mask), [UPKIE_NJ][stride]
+// structure-of-arrays like the state, env i in column i. The draws are at the end of this file.
+struct VelocityDerate {
+  UpkieVelocityDerate spec;
+  uint32_t* count;
+  float* max_velocity;
+  int stride;
+};
+
+// The moteus derate of the torque t of a joint at velocity qd under the limit v, the band `derate` and the effort limit
+// tau_max: past v, the torque that drives the joint faster in its direction of motion is capped by f * tau_max, f
+// falling linearly from 1 at v to 0 at v + derate. A braking torque, and any torque at |qd| <= v, is t bit for bit.
+UPKIE_HD float velocity_derate_torque(float t, float qd, float v, float derate, float tau_max) {
+  const float s = fabsf(qd);
+  if (!(s > v)) return t;
+  const float cap = clampf((v + derate - s) / derate, 0.f, 1.f) * tau_max;
+  return qd > 0.f ? fminf(t, cap) : fmaxf(t, -cap);
+}
+
+// Joint j's torque t of env i (its column of V) at velocity qd: derated on a joint of the mask, t otherwise
+UPKIE_HD float velocity_derate_joint(const VelocityDerate& V, int i, int j, float qd, float t, float tau_max) {
+  if (!((V.spec.joint_mask >> j) & 1u)) return t;
+  return velocity_derate_torque(t, qd, V.max_velocity[size_t(j) * size_t(V.stride) + size_t(i)], V.spec.derate[j],
+                                tau_max);
+}
+
 // Derived observation quantities (pybullet_backend.py:333-490). Updates the
 // IMU finite-difference state exactly once per call, as get_spine_observation.
 UPKIE_HD void observe_update(const SimParams& P, RobotState& S) {
@@ -1164,10 +1195,13 @@ UPKIE_HD void servo_substep(const SimParams& P, RobotState& S, const float a[UPK
                             const float* eps, float mu, AnyFn warp_any, SyncFn phase_sync = SyncFn(),
                             const NoiseCtx* nz = nullptr, int sub = 0, const ExtForces* ext = nullptr,
                             int limits = 0, BodyRecOut rec = BodyRecOut{nullptr, 0}, int env = -1,
-                            const ExtPush* push = nullptr) {
+                            const ExtPush* push = nullptr, const VelocityDerate* derate = nullptr,
+                            int derate_env = 0) {
   // `env`: this robot's column of the per-env parameter table; env < 0 (the default, and a constant in the
   // instantiations that never run with a table) compiles the table reads out. Its values are read where they are used, under a uniform branch
   // on the table pointer; the arithmetic is the same for the config's values and the table's.
+  // `derate` (non-null in every lane of a FAM_SENSE launch with velocity limits; a null constant elsewhere, which
+  // compiles the law out): the servo velocity limits of env `derate_env`, read from its column in every substep.
   const bool table = env >= 0 && P.env_params != nullptr;
   float tau[6];
   float noise[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -1185,9 +1219,10 @@ UPKIE_HD void servo_substep(const SimParams& P, RobotState& S, const float a[UPK
   for (int j = 0; j < 6; ++j) {
     const float* aj = a + j * 6;
     const float fr = table ? env_param(P, env, UPKIE_EP_FRICTION + j) : P.joint_friction[j];
-    const float t = joint_torque(kp, kd, fr, S.q[j], S.qd[j], aj[UPKIE_ACT_FEEDFORWARD_TORQUE], aj[UPKIE_ACT_POSITION],
-                                 aj[UPKIE_ACT_VELOCITY], aj[UPKIE_ACT_KP_SCALE], aj[UPKIE_ACT_KD_SCALE],
-                                 aj[UPKIE_ACT_MAXIMUM_TORQUE], noise[j]);
+    float t = joint_torque(kp, kd, fr, S.q[j], S.qd[j], aj[UPKIE_ACT_FEEDFORWARD_TORQUE], aj[UPKIE_ACT_POSITION],
+                           aj[UPKIE_ACT_VELOCITY], aj[UPKIE_ACT_KP_SCALE], aj[UPKIE_ACT_KD_SCALE],
+                           aj[UPKIE_ACT_MAXIMUM_TORQUE], noise[j]);
+    if (derate) t = velocity_derate_joint(*derate, derate_env, j, S.qd[j], t, P.tau_max[j]);
     tau[j] = zero_torque ? 0.f : t;
     if (!zero_torque) S.torque[j] = t;
   }
@@ -2370,7 +2405,7 @@ struct ServoNoise {
 // env's draw counter k after the reset (every reset advances it, whether it samples its state or takes host rows).
 // Never set by sample_init_state (below 2^34), the noise (below bit 42), the reset randomisation (bit 63), the pushes
 // (62), the action delay (61), the observation delay (60), the servo dropouts (59, and 59 | 58 below bit 52), the IMU
-// misalignment (57) or the encoder offsets (56).
+// misalignment (57), the encoder offsets (56) or the velocity limits (52).
 constexpr uint64_t kServoNoiseTag = uint64_t(1) << 55;
 constexpr uint64_t kServoNoiseCycleTag = kServoNoiseTag | (uint64_t(1) << 54);
 constexpr uint64_t kServoNoiseResetTag = kServoNoiseCycleTag | (uint64_t(1) << 53);
@@ -2518,6 +2553,49 @@ UPKIE_HD void history_fill_noise(const History& H, const SimParams& P, const Rob
     const uint32_t e = (head + 2u * ticks - 1u - a) % ticks;
     for (int c = 0; c < H.count; ++c) store(e, c, history_value(P, V, V.imu_acc, H.columns[c]));
   }
+}
+
+// ---- Servo velocity limits: the draws (upkie_b200_set_velocity_derate; the block and the law above servo_substep) ----
+// bit 52 of the high counter word, the per-reset draws of v_i, (k << 4) | b below bit 36: never set by
+// sample_init_state (below 2^34), the noise (below bit 42), the reset randomisation (bit 63), the pushes (62), the
+// action delay (61), the observation delay (60), the servo dropouts (59, and 59 | 58, below bit 52 otherwise), the IMU
+// misalignment (57), the encoder offsets (56) or the servo noise (55, 55 | 54 below bit 52, and 55 | 54 | 53)
+constexpr uint64_t kVelocityDerateTag = uint64_t(1) << 52;
+
+struct Vmax6 {
+  float v[UPKIE_NJ];
+};
+
+// Draw k of the env of global index g: word j % 4 of the block of counter j / 4 gives joint j's limit, push_value's
+// exact form (the map of the servo dropouts). Every joint's word is drawn whatever the mask, and a joint outside it
+// gets 0, so that the mask changes no other joint's draw.
+UPKIE_HD Vmax6 velocity_derate_draw(const UpkieVelocityDerate& s, uint64_t seed, uint64_t g, uint32_t k) {
+  Vmax6 o;
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    const Philox4 r = philox4x32_10(g, kVelocityDerateTag | (uint64_t(k) << 4) | uint64_t(b), seed);
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const int j = 4 * b + w;
+      if (j < UPKIE_NJ)
+        o.v[j] = ((s.joint_mask >> j) & 1u) ? push_value(r.v[w], s.max_velocity_low[j], s.max_velocity_high[j]) : 0.f;
+    }
+  }
+  return o;
+}
+
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, stored. The block's fields are copied
+// before the first store, as servo_dropout_reset.
+UPKIE_HD void velocity_derate_reset(const VelocityDerate& V, uint64_t seed, uint64_t g, int i) {
+  const UpkieVelocityDerate spec = V.spec;
+  uint32_t* const count = V.count;
+  float* const col = V.max_velocity + size_t(i);
+  const size_t stride = size_t(V.stride);
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  const Vmax6 o = velocity_derate_draw(spec, seed, g, k);
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) col[size_t(j) * stride] = o.v[j];
 }
 
 }  // namespace upkie_b200

@@ -26,7 +26,7 @@ enum {
   FAM_DELAY = 8,      // FAM_PUSH + action delay
   FAM_BODY_DELAY = 9, // FAM_BODY_PUSH + action delay
   FAM_SENSE = 10,     // FAM_DELAY + observation delay + observation history + servo reply dropouts + IMU misalignment
-                      // + encoder offsets + servo measurement noise
+                      // + encoder offsets + servo measurement noise + servo velocity limits
   kNumFamilies = 11
 };
 
@@ -101,6 +101,8 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "encoder offsets have no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.servo_noise)
     no = "servo noise has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
+  else if (in_kernel && P.velocity_derate)
+    no = "velocity limits have no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.max_episode_steps > 0)
     no = "max_episode_steps has no in-kernel rollout transport: it does not carry truncated (use upkie_b200_step with "
          "compact rows)";
@@ -146,6 +148,12 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "servo noise needs joint_limits != 0";
   else if (P.servo_noise && P.body_contacts)
     no = "servo noise has no body-contact kernels";
+  else if (P.velocity_derate && P.spine_mode)
+    no = "velocity limits: spine_mode applies the spine's own torque law";
+  else if (P.velocity_derate && P.joint_limits == 0)
+    no = "velocity limits need joint_limits != 0";
+  else if (P.velocity_derate && P.body_contacts)
+    no = "velocity limits have no body-contact kernels";
   if (no) {
     *why = no;
     return -1;
@@ -153,9 +161,11 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
   if (P.spine_mode) return FAM_SPINE;
   // the observation-delay family carries the action delay and the pushes too (runtime-uniform branches on
   // P.action_delay and P.push), the observation history (P.history), the servo dropouts (P.servo_dropout), the IMU
-  // misalignment (P.imu_misalign), the encoder offsets (P.encoder_offset) and the servo noise (P.servo_noise), by the
-  // same rule; the set calls reject spine mode, no limits and body contacts
-  if (P.obs_delay || P.history || P.servo_dropout || P.imu_misalign || P.encoder_offset || P.servo_noise)
+  // misalignment (P.imu_misalign), the encoder offsets (P.encoder_offset), the servo noise (P.servo_noise) and the
+  // servo velocity limits (P.velocity_derate), by the same rule; the set calls reject spine mode, no limits and body
+  // contacts
+  if (P.obs_delay || P.history || P.servo_dropout || P.imu_misalign || P.encoder_offset || P.servo_noise ||
+      P.velocity_derate)
     return FAM_SENSE;
   // the delay families carry the pushes too (a runtime-uniform branch on P.push); the set calls reject spine mode and
   // no limits

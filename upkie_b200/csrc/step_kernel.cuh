@@ -284,6 +284,12 @@ __device__ __noinline__ uint32_t noise_reset_lane(const SimParams& P, uint64_t s
   return servo_noise_reset(*P.servo_noise, seed, g, i);
 }
 
+// The servo velocity limits (F.sense kernels, P.velocity_derate set): a reset's next draw, stored (out of line, as
+// tilt_reset_lane). The substeps read the lane's limits from its column (servo_substep).
+__device__ __noinline__ void derate_reset_lane(const SimParams& P, uint64_t seed, uint64_t g, int i) {
+  velocity_derate_reset(*P.velocity_derate, seed, g, i);
+}
+
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE >= 1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), during the substeps each lane's clamped row, and it is reused to transpose the
@@ -501,6 +507,16 @@ __device__ __forceinline__ void step_env(
   if constexpr (F.sense) {
     if (noising && resetting && live) nk = noise_reset_lane(P, seed, env_offset + uint64_t(i), i);
   }
+  // servo velocity limits (F.sense kernels, P.velocity_derate set: a uniform branch). The torque law of every substep
+  // derates the motoring torque of a joint past its limit (servo_substep, which reads v_i from the env's column), on
+  // the true joint velocity: the row executed whatever its source (the action delay's included), before external
+  // forces and pushes. A reset draws the next v_i here and at the same-step reset below; its zero-torque substep is
+  // untouched. Null outside FAM_SENSE, which compiles the law out.
+  const VelocityDerate* vderate = nullptr;
+  if constexpr (F.sense) {
+    vderate = P.velocity_derate;
+    if (vderate && resetting && live) derate_reset_lane(P, seed, env_offset + uint64_t(i), i);
+  }
   // TILE >= 1: the row the substeps read (torque law, action delay, spine cycle) is the lane's own row of the warp's
   // tile, written here whole (9 x 16 B at a stride of 9 float4: conflict-free) whether the row came from the tile or
   // from global memory, instead of a 36-float register array that ptxas spills to the local-memory frame and reloads in
@@ -649,7 +665,7 @@ __device__ __forceinline__ void step_env(
         // second and third inlined copy of the substep that these kernels never run
         servo_substep(P, S, arow, resetting, eps, mu, WarpAny(), PhaseSync(), F.extras ? &nz : nullptr, sub,
                       (F.extras && ext) ? &xf : nullptr, F.limits ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
-                      pushing ? &pu : nullptr);
+                      pushing ? &pu : nullptr, vderate, i);
       }
       if (dropping && !resetting && live) {
         ServoReplies R;
@@ -793,6 +809,7 @@ __device__ __forceinline__ void step_env(
         if (tilting && live) em = tilt_reset_lane(P, seed, env_offset + uint64_t(i), i);  // the new episode's e_i
         if (offsetting && live) eo = offset_reset_lane(P, seed, env_offset + uint64_t(i), i);  // and delta_i
         if (noising && live) nk = noise_reset_lane(P, seed, env_offset + uint64_t(i), i);  // and sigma_i
+        if (vderate && live) derate_reset_lane(P, seed, env_offset + uint64_t(i), i);       // and v_i
       }
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;

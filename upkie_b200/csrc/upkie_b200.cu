@@ -18,7 +18,8 @@
 // k_spine_obs, k_reset_obs and k_history_fill read the orientation through it (imu_misalign_observed). Neither do the
 // encoder offsets: k_reset draws and shifts the leg targets, and the same three kernels read the servo positions
 // through them (encoder_offset_observed). Nor does the servo noise: k_reset draws, noises the leg targets, the latch
-// and the history refill, and the same three kernels read the servo replies through it (servo_noise_observed).
+// and the history refill, and the same three kernels read the servo replies through it (servo_noise_observed). The
+// servo velocity limits touch the torque law only: k_reset draws, and the step kernels' substeps derate.
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -168,6 +169,12 @@ struct Handle {
   float* noise_sigma = nullptr;  // [12][n_pad], sigma_i
   uint8_t* noise_fresh = nullptr;
   UpkieServoNoise noise_spec{};  // the spec in force
+  // servo velocity limits (upkie_b200_set_velocity_derate): the device block P.velocity_derate points to while a spec
+  // is set, and the per-env state it points to (allocated with the first spec, freed when it is turned off)
+  VelocityDerate* vlim_dev = nullptr;
+  uint32_t* vlim_count = nullptr;
+  float* vlim_max = nullptr;  // [UPKIE_NJ][n_pad], v_i
+  uint32_t vlim_mask = 0;     // joint_mask of the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -256,6 +263,7 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
                                 rcyc);
     servo_noise_leg_targets(S, nd);
   }
+  if (P.velocity_derate) velocity_derate_reset(*P.velocity_derate, rand_seed, g, i);  // the new episode's v_i
   Offset6 d{{0.f, 0.f, 0.f, 0.f, 0.f, 0.f}};
   if (P.encoder_offset) {
     d = encoder_offset_reset(*P.encoder_offset, rand_seed, g, i);
@@ -1115,6 +1123,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->tilt_dev); cudaFree(h->tilt_count); cudaFree(h->tilt_quat);
   cudaFree(h->enc_dev); cudaFree(h->enc_count); cudaFree(h->enc_offset);
   cudaFree(h->noise_dev); cudaFree(h->noise_count); cudaFree(h->noise_sigma); cudaFree(h->noise_fresh);
+  cudaFree(h->vlim_dev); cudaFree(h->vlim_count); cudaFree(h->vlim_max);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -1174,6 +1183,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: servo noise needs joint_limits != 0");
   if (h->P.servo_noise && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no servo-noise kernels");
+  if (h->P.velocity_derate && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: velocity limits need joint_limits != 0");
+  if (h->P.velocity_derate && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no velocity-limit kernels");
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -1198,6 +1211,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.imu_misalign = h->P.imu_misalign;    // and the IMU misalignment
   P.encoder_offset = h->P.encoder_offset;  // and the encoder offsets
   P.servo_noise = h->P.servo_noise;        // and the servo noise
+  P.velocity_derate = h->P.velocity_derate;  // and the velocity limits
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -2457,6 +2471,95 @@ int upkie_b200_set_servo_noise_mark(void* handle, const uint8_t* mark, void* str
   for (uint8_t x : m)
     if (x > 1) return fail(UPKIE_B200_EINVAL, "set_servo_noise_mark: every mark must be 0 or 1");
   CUDA_TRY(cudaMemcpyAsync(h->noise_fresh, mark, m.size(), cudaMemcpyDefault, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_velocity_derate(void* handle, const UpkieVelocityDerate* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    if (h->P.velocity_derate) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the per-env state
+      h->P.velocity_derate = nullptr;
+      cudaFree(h->vlim_count);
+      cudaFree(h->vlim_max);
+      h->vlim_count = nullptr;
+      h->vlim_max = nullptr;
+      h->vlim_mask = 0;
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = velocity_derate_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
+  if (!h->P.velocity_derate) {
+    // switched on: zero counters; every joint of the mask is filled below
+    CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->vlim_count), size_t(h->n) * sizeof(uint32_t)},
+                           {reinterpret_cast<void**>(&h->vlim_max), size_t(UPKIE_NJ) * h->n_pad * sizeof(float)}}));
+  }
+  // the joints the spec drops from the mask have no limit from now on, and those it adds take the range's upper bound
+  // until each env's next reset (a joint of the mask always holds a limit > 0)
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    float* const col = h->vlim_max + size_t(j) * h->n_pad;
+    if (((h->vlim_mask & ~spec->joint_mask) >> j) & 1u)
+      CUDA_TRY(cudaMemset(col, 0, size_t(h->n_pad) * sizeof(float)));
+    if (((spec->joint_mask & ~h->vlim_mask) >> j) & 1u) {
+      k_fill<<<grid_of(h->n), 128>>>(h->n, col, spec->max_velocity_high[j]);
+      CUDA_TRY(cudaGetLastError());
+    }
+  }
+  if (!h->vlim_dev) CUDA_TRY(cudaMalloc(&h->vlim_dev, sizeof(VelocityDerate)));
+  VelocityDerate V;
+  std::memset(&V, 0, sizeof(V));
+  V.spec = *spec;
+  V.count = h->vlim_count;
+  V.max_velocity = h->vlim_max;
+  V.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->vlim_dev, &V, sizeof(V), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->P.velocity_derate = h->vlim_dev;
+  h->vlim_mask = spec->joint_mask;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_velocity_derate_state(void* handle, uint32_t* count, float* max_velocity, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !max_velocity) return fail(UPKIE_B200_EINVAL, "get_velocity_derate_state: invalid argument");
+  if (!h->P.velocity_derate)
+    return fail(UPKIE_B200_EINVAL,
+                "get_velocity_derate_state: no velocity limits are set (upkie_b200_set_velocity_derate)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemcpyAsync(count, h->vlim_count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_rows(h->vlim_max, UPKIE_NJ, h->n, h->n_pad, max_velocity, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_velocity_derate_state(void* handle, const uint32_t* count, const float* max_velocity, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !max_velocity) return fail(UPKIE_B200_EINVAL, "set_velocity_derate_state: invalid argument");
+  if (!h->P.velocity_derate)
+    return fail(UPKIE_B200_EINVAL,
+                "set_velocity_derate_state: no velocity limits are set (upkie_b200_set_velocity_derate)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // every joint of the mask in force must hold a limit, every other joint none: read back (after the caller's work on
+  // the stream) and checked here
+  std::vector<float> v(size_t(h->n) * UPKIE_NJ);
+  CUDA_TRY(cudaMemcpyAsync(v.data(), max_velocity, v.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (size_t k = 0; k < v.size(); ++k) {
+    if ((h->vlim_mask >> (k % UPKIE_NJ)) & 1u) {
+      if (!(v[k] > 0.f && std::isfinite(v[k])))
+        return fail(UPKIE_B200_EINVAL, "set_velocity_derate_state: every limit of a joint of joint_mask must be finite "
+                                       "and > 0");
+    } else if (v[k] != 0.f) {
+      return fail(UPKIE_B200_EINVAL, "set_velocity_derate_state: a joint outside joint_mask must have a zero limit");
+    }
+  }
+  CUDA_TRY(cudaMemcpyAsync(h->vlim_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_cols(max_velocity, UPKIE_NJ, h->n, h->n_pad, h->vlim_max, s));
   return UPKIE_B200_OK;
 }
 

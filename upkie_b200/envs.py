@@ -920,6 +920,109 @@ def servo_noise_spec(noise, spine_mode: bool = False, joint_limits: Union[bool, 
     return spec
 
 
+# The velocity limits every Upkie's servos are configured with (the reference's tools/configure_servos,
+# configure_velocity_limits: servo.max_velocity 2 rev/s on the hips and knees, 8 rev/s on the wheels), and the moteus
+# default derate band of 2 rev/s (an assumption, see _abi.MOTEUS_MAX_VELOCITY_DERATE), in rad/s: a ``velocity_derate``
+# of ``B200VectorEnv``. 12.57 rad/s on the legs, 50.27 rad/s on the wheels (2.51 m/s of ground velocity).
+UPKIE_VELOCITY_DERATE = {
+    "max_velocity": {name: (8.0 if "wheel" in name else 2.0) * _abi.RAD_PER_REV for name in _abi.JOINT_NAMES},
+    "derate": _abi.MOTEUS_MAX_VELOCITY_DERATE,
+}
+
+
+def _positive_range(name: str, value):
+    """(low, high) float32 of one velocity limit: a limit ``v`` or a ``(low, high)`` range, 0 < low <= high"""
+    if isinstance(value, (int, float, np.integer, np.floating)):
+        lo = hi = value
+    else:
+        try:
+            lo, hi = value
+        except (TypeError, ValueError):
+            raise UpkieException(f"velocity_derate: {name}: expected a limit or a (low, high) pair, got {value!r}") \
+                from None
+    try:
+        lo, hi = np.float32(lo), np.float32(hi)
+    except (TypeError, ValueError):
+        raise UpkieException(f"velocity_derate: {name}: expected numbers, got ({lo!r}, {hi!r})") from None
+    if not (np.isfinite(lo) and np.isfinite(hi)) or not lo > 0:
+        raise UpkieException(f"velocity_derate: {name}: expected finite limits > 0 rad/s, got ({lo}, {hi})")
+    if lo > hi:
+        raise UpkieException(f"velocity_derate: {name}: expected low <= high, got ({lo}, {hi})")
+    return lo, hi
+
+
+def velocity_derate_spec(velocity_derate, joints=None, spine_mode: bool = False,
+                         joint_limits: Union[bool, int] = True,
+                         body_contacts: Union[bool, int] = False) -> Optional[_abi.UpkieVelocityDerate]:
+    """``UpkieVelocityDerate`` (``UpkieSim.set_velocity_derate``) from a dict with keys ``max_velocity`` and
+    ``derate`` (optional, default ``_abi.MOTEUS_MAX_VELOCITY_DERATE``), in rad/s (rev/s times ``2 pi``; see
+    ``UPKIE_VELOCITY_DERATE``). ``max_velocity`` is a limit ``v``, a ``(low, high)`` range from which every reset draws
+    each joint's limit, or a dict ``{joint: v or (low, high)}``; ``derate`` a band or a dict ``{joint: band}``.
+    ``joints`` (names, ``JOINT_NAMES``) are the joints that have a limit; None: the joints of a per-joint
+    ``max_velocity``, or all six. Raises ``UpkieException`` on an unknown key or joint, a limit or band that is not a
+    finite number > 0, ``low > high``, a joint without a limit, an empty joint list, ``spine_mode`` (whose spine applies
+    its own torque law), no joint limits and ``body_contacts`` (the limits run in the kernels of the observation
+    delay)."""
+    if velocity_derate is None:
+        return None
+    if not isinstance(velocity_derate, dict) or "max_velocity" not in velocity_derate:
+        raise UpkieException(f"velocity_derate: expected a dict with keys 'max_velocity' and 'derate', got "
+                             f"{velocity_derate!r}")
+    unknown = [k for k in velocity_derate if k not in ("max_velocity", "derate")]
+    if unknown:
+        raise UpkieException(f"velocity_derate: unknown key(s) {unknown}, expected 'max_velocity' and 'derate'")
+    mv = velocity_derate["max_velocity"]
+    per_joint = isinstance(mv, dict)
+    names = (list(mv) if per_joint else list(_abi.JOINT_NAMES)) if joints is None else list(joints)
+    bad = [j for j in names + (list(mv) if per_joint else []) if j not in _abi.JOINT_NAMES]
+    if bad:
+        raise UpkieException(f"velocity_derate: unknown joint(s) {bad}, expected names of {_abi.JOINT_NAMES}")
+    if not names:
+        raise UpkieException("velocity_derate_joints: at least one joint")
+    spec = _abi.UpkieVelocityDerate()
+    lo = np.ones(_abi.NJ, dtype=np.float32)
+    hi = np.ones(_abi.NJ, dtype=np.float32)
+    band = np.ones(_abi.NJ, dtype=np.float32)
+    d = velocity_derate.get("derate", _abi.MOTEUS_MAX_VELOCITY_DERATE)
+    if isinstance(d, dict):
+        bad = [j for j in d if j not in _abi.JOINT_NAMES]
+        if bad:
+            raise UpkieException(f"velocity_derate: derate: unknown joint(s) {bad}, expected names of "
+                                 f"{_abi.JOINT_NAMES}")
+    for j in names:
+        k = _abi.JOINT_NAMES.index(j)
+        if per_joint and j not in mv:
+            raise UpkieException(f"velocity_derate: {j} has no max_velocity")
+        lo[k], hi[k] = _positive_range(f"max_velocity.{j}" if per_joint else "max_velocity", mv[j] if per_joint else mv)
+        dj = d.get(j, _abi.MOTEUS_MAX_VELOCITY_DERATE) if isinstance(d, dict) else d
+        try:
+            band[k] = np.float32(dj)
+        except (TypeError, ValueError):
+            raise UpkieException(f"velocity_derate: derate: expected a number, got {dj!r}") from None
+        if not (np.isfinite(band[k]) and band[k] > 0):
+            raise UpkieException(f"velocity_derate: derate: expected a finite band > 0 rad/s, got {band[k]}")
+    if spine_mode:
+        raise UpkieException("velocity_derate: spine_mode applies the spine's own torque law; the limits are not "
+                             "available there")
+    if not joint_limits:
+        raise UpkieException("velocity_derate: needs joint_limits (the limits run in the kernels with joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("velocity_derate: body_contacts has no velocity-limit kernels")
+    spec.max_velocity_low[:] = [float(x) for x in lo]
+    spec.max_velocity_high[:] = [float(x) for x in hi]
+    spec.derate[:] = [float(x) for x in band]
+    spec.joint_mask = sum(1 << _abi.JOINT_NAMES.index(j) for j in set(names))
+    return spec
+
+
+def _set_velocity_derate(sim, spec: Optional[_abi.UpkieVelocityDerate]) -> None:
+    if spec is None:
+        sim.set_velocity_derate(None)
+    else:
+        sim.set_velocity_derate(list(zip(spec.max_velocity_low, spec.max_velocity_high)), list(spec.derate),
+                                [n for j, n in enumerate(_abi.JOINT_NAMES) if (spec.joint_mask >> j) & 1])
+
+
 def _set_servo_noise(sim, spec: Optional[_abi.UpkieServoNoise]) -> None:
     if spec is None:
         sim.set_servo_noise(None)
@@ -1048,6 +1151,14 @@ class B200VectorEnv(VectorEnv):
     physics, the torques, terminations and ``get_state`` see the true replies. The draws are keyed on the seed of
     ``reset(seed=s)``, which also restarts the draw counters of the envs it resets. ``set_servo_noise`` changes or
     (``None``) stops it.
+
+    ``velocity_derate`` (a dict ``{"max_velocity": ..., "derate": ...}`` in rad/s, see ``velocity_derate_spec``;
+    ``UPKIE_VELOCITY_DERATE`` holds the robot's configured 2 rev/s legs and 8 rev/s wheels, a rev/s being ``2 pi``
+    rad/s) limits the servos ``velocity_derate_joints`` (names, default those of ``max_velocity``) as the moteus
+    ``servo.max_velocity`` does: past a limit drawn per joint at every reset of the env, the torque that drives a joint
+    faster falls linearly to zero over the derate band, while a braking torque passes. The torque every env type
+    observes is the derated one. The draws are keyed on the seed of ``reset(seed=s)``, which also restarts the draw
+    counters of the envs it resets. ``set_velocity_derate`` changes or (``None``) stops it.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -1094,6 +1205,8 @@ class B200VectorEnv(VectorEnv):
         encoder_offset: Optional[Union[float, Tuple[float, float]]] = None,
         encoder_offset_joints: Optional[Sequence[str]] = None,
         servo_noise: Optional[Dict[str, Any]] = None,
+        velocity_derate: Optional[Dict[str, Any]] = None,
+        velocity_derate_joints: Optional[Sequence[str]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -1151,6 +1264,8 @@ class B200VectorEnv(VectorEnv):
                                        config.joint_limits, config.body_contacts)  # validated before any device
         noise_spec = servo_noise_spec(servo_noise, bool(config.spine_mode), config.joint_limits, config.body_contacts,
                                       sense_spec is not None, drop_spec is not None)  # validated before any device
+        vlim_spec = velocity_derate_spec(velocity_derate, velocity_derate_joints, bool(config.spine_mode),
+                                         config.joint_limits, config.body_contacts)  # validated before any device
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -1218,6 +1333,16 @@ class B200VectorEnv(VectorEnv):
             _set_encoder_offset(self.sim, enc_spec)  # before the first reset, which draws every env's offsets
         if noise_spec is not None:
             _set_servo_noise(self.sim, noise_spec)  # before the first reset, which draws every env's levels
+        if vlim_spec is not None:
+            _set_velocity_derate(self.sim, vlim_spec)  # before the first reset, which draws every env's limits
+
+    def set_velocity_derate(self, velocity_derate, joints=None) -> None:
+        """Limit the servos ``joints`` (names, None: those of ``max_velocity``) past a velocity drawn per env (a dict
+        in rad/s, see ``velocity_derate_spec``; ``UPKIE_VELOCITY_DERATE`` for the robot's configuration); ``None``
+        turns the limits off. New ranges take effect at each env's next reset; the joints it adds are limited at their
+        ``high`` bound until then, and those it drops have no limit from now on."""
+        _set_velocity_derate(self.sim, velocity_derate_spec(velocity_derate, joints, bool(self.config.spine_mode),
+                                                            self.config.joint_limits, self.config.body_contacts))
 
     def set_servo_noise(self, noise) -> None:
         """Add white noise to the servos' position and velocity replies at levels drawn per env (a dict, see
@@ -1480,6 +1605,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_servo_noise_state(count, sigma)
+            if self.sim.velocity_derate_spec is not None:
+                # so are the velocity limits
+                count, vmax = self.sim.get_velocity_derate_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_velocity_derate_state(count, vmax)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

@@ -481,6 +481,72 @@ class UpkieSim:
         self._check_tensor(sigma, (self.n, 2 * _abi.NJ), name="sigma")
         check(lib().upkie_b200_set_servo_noise_state(self._h, _ptr(count), _ptr(sigma), self._stream()))
 
+    def set_velocity_derate(self, max_velocity=None, derate=None, joints: Optional[Sequence[str]] = None) -> None:
+        """While limits are set, each servo of ``joints`` (names, None: all six) derates its torque past a velocity
+        limit, as the moteus ``servo.max_velocity`` does: every reset of an env draws one limit per joint,
+        ``v ~ U(low, high)`` in rad/s (keyed on the auto-reset seed and the env's counter, ``include/upkie_b200.h``),
+        and in every substep a joint with ``|qd| > v`` has the torque that drives it faster capped by
+        ``clip((v + derate - |qd|) / derate, 0, 1) * tau_max``; a braking torque passes unchanged. A speed in rev/s is
+        ``2 * pi`` times that in rad/s: the robot's 2 rev/s is 12.57 rad/s. ``max_velocity`` is a ``(low, high)`` pair of
+        bounds or a sequence of six per-joint ``(low, high)`` pairs (``JOINT_NAMES`` order), ``derate`` a band in
+        rad/s or six of them (None: ``MOTEUS_MAX_VELOCITY_DERATE``, 2 rev/s); ``max_velocity=None`` turns the limits
+        off. Setting limits draws nothing: each env keeps
+        the limits of the joints that stay limited until its next reset, and the joints a spec adds take ``high``
+        until then."""
+        if max_velocity is None:
+            check(lib().upkie_b200_set_velocity_derate(self._h, None))
+            self._velocity_derate = None
+            return
+        mv = np.asarray(max_velocity, dtype=np.float32)
+        if mv.shape == (2,):
+            lo, hi = np.full(_abi.NJ, mv[0], np.float32), np.full(_abi.NJ, mv[1], np.float32)
+        elif mv.shape == (_abi.NJ, 2):
+            lo, hi = mv[:, 0], mv[:, 1]
+        else:
+            raise UpkieException("set_velocity_derate: max_velocity expects (low, high) or six (low, high) pairs")
+        d = np.asarray(_abi.MOTEUS_MAX_VELOCITY_DERATE if derate is None else derate, dtype=np.float32).reshape(-1)
+        if d.shape == (1,):
+            d = np.repeat(d, _abi.NJ)
+        if d.shape != (_abi.NJ,):
+            raise UpkieException("set_velocity_derate: derate expects one band or six")
+        names = list(_abi.JOINT_NAMES) if joints is None else list(joints)
+        unknown = [j for j in names if j not in _abi.JOINT_NAMES]
+        if unknown:
+            raise UpkieException(f"set_velocity_derate: unknown joint(s) {unknown}")
+        mask = sum(1 << _abi.JOINT_NAMES.index(j) for j in set(names))
+        spec = _abi.UpkieVelocityDerate()
+        spec.max_velocity_low[:] = [float(x) for x in lo]
+        spec.max_velocity_high[:] = [float(x) for x in hi]
+        spec.derate[:] = [float(x) for x in d]
+        spec.joint_mask = mask
+        check(lib().upkie_b200_set_velocity_derate(self._h, C.byref(spec)))
+        self._velocity_derate = (tuple(zip(spec.max_velocity_low, spec.max_velocity_high)), tuple(spec.derate), mask)
+
+    @property
+    def velocity_derate_spec(self):
+        """``(max_velocity, derate, joint_mask)`` of the velocity limits in force (six ``(low, high)`` pairs and six
+        bands, rad/s), or None."""
+        return getattr(self, "_velocity_derate", None)
+
+    def get_velocity_derate_state(self):
+        """Per-env velocity-limit state ``(count[N], max_velocity[N, 6])``: the draw counters (int32 bits of uint32)
+        and each env's limit per joint in rad/s (0 for a joint without one)."""
+        if self.velocity_derate_spec is None:
+            raise UpkieException("no velocity limits are set (set_velocity_derate)")
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        vmax = torch.empty((self.n, _abi.NJ), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_velocity_derate_state(self._h, _ptr(count), _ptr(vmax), self._stream()))
+        return count, vmax
+
+    def set_velocity_derate_state(self, count: torch.Tensor, max_velocity: torch.Tensor) -> None:
+        """Set every env's draw counter and velocity limits (finite and > 0 on a limited joint, zero on the others): a
+        checkpoint, or limits configured on a robot (kept until each env's next reset)."""
+        if self.velocity_derate_spec is None:
+            raise UpkieException("no velocity limits are set (set_velocity_derate)")
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(max_velocity, (self.n, _abi.NJ), name="max_velocity")
+        check(lib().upkie_b200_set_velocity_derate_state(self._h, _ptr(count), _ptr(max_velocity), self._stream()))
+
     def get_servo_noise_mark(self) -> torch.Tensor:
         """Per-env mark ``[N]`` (uint8): 1 while the env reports its reset observation (``spine_obs`` and
         ``reset_obs`` then carry the reset cycle's noise), 0 after a step that did not reset it."""
@@ -970,6 +1036,10 @@ class UpkieSim:
             sd["servo_noise"] = self.servo_noise_spec
             sd["servo_noise_count"], sd["servo_noise_sigma"] = self.get_servo_noise_state()
             sd["servo_noise_mark"] = self.get_servo_noise_mark()
+        # the velocity limits: (max_velocity, derate, joint_mask) and the per-env state (absent without a spec)
+        if self.velocity_derate_spec is not None:
+            sd["velocity_derate"] = self.velocity_derate_spec
+            sd["velocity_derate_count"], sd["velocity_derate_max_velocity"] = self.get_velocity_derate_state()
         sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
@@ -1098,6 +1168,14 @@ class UpkieSim:
             self.set_encoder_offset(enc[0], enc[1], [n for j, n in enumerate(_abi.JOINT_NAMES) if (enc[2] >> j) & 1])
             self.set_encoder_offset_state(*(sd[k].to(dev).contiguous() for k in (
                 "encoder_offset_count", "encoder_offset_offset")))
+        # the velocity limits; a checkpoint without them (or written before they existed) turns them off
+        vlim = sd.get("velocity_derate")
+        if vlim is None:
+            self.set_velocity_derate(None)
+        else:
+            self.set_velocity_derate(vlim[0], vlim[1], [n for j, n in enumerate(_abi.JOINT_NAMES) if (vlim[2] >> j) & 1])
+            self.set_velocity_derate_state(*(sd[k].to(dev).contiguous() for k in (
+                "velocity_derate_count", "velocity_derate_max_velocity")))
         # the servo noise (off above); a checkpoint without it (or written before it existed) leaves it off
         noise = sd.get("servo_noise")
         if noise is not None:
