@@ -1067,6 +1067,81 @@ int upkie_b200_set_velocity_derate(void* handle, const UpkieVelocityDerate* spec
 int upkie_b200_get_velocity_derate_state(void* handle, uint32_t* count, float* max_velocity, void* stream);
 int upkie_b200_set_velocity_derate_state(void* handle, const uint32_t* count, const float* max_velocity, void* stream);
 
+/* ---- IMU attitude estimation (Pi3HatInterface.cpp:151-169, pi3hat/imu.h:84-95) ----------------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. On the robot the spine never sees the true
+ * tilt: it reads orientation_imu_in_ars from the pi3hat's attitude filter, which has its own gyro-bias estimate. While
+ * a spec is set every env runs an attitude filter on its simulated IMU, and every orientation-derived observation
+ * reports its estimate instead of the true orientation.
+ * Assumption: the pi3hat's filter is an unscented Kalman filter whose source is in neither this project nor its
+ * reference. The model implemented here is an explicit complementary filter with gyro-bias estimation (Mahony), chosen
+ * because it has the three error classes of such a filter (convergence after a start or a disturbance, a tilt error
+ * toward atan(a / g) under sustained horizontal acceleration, drift from a gyro bias not yet estimated) and is cheap
+ * enough to run in every spine cycle. It does not reproduce the UKF's gains or transients.
+ * - Per-env state (device pointers): count[N], gains[N][2] (kp in 1/s, ki in 1/s^2), quat[N][4] (w, x, y, z: the
+ *   estimated IMU-to-world rotation q) and bias[N][3] (b, rad/s, IMU frame).
+ * - Law: once per substep (one 1 kHz spine cycle at the default 200 Hz / 5 substeps), after that substep's physics,
+ *   with h = dt / nb_substeps. Inputs, in the true IMU frame (the misaligned one under an IMU misalignment):
+ *   w_m = R_i^T omega + the env's gyro bias, and a_m = R_i^T ((v_i - v_i') / h + 9.81 e_z) + the env's accelerometer
+ *   bias, with R_i the IMU-to-world rotation, v_i the world-frame IMU velocity after the substep and v_i' the one
+ *   after the previous substep (the step's observation update's at the first substep of a tick), as the observation
+ *   history differentiates it. The biases are the parameter table's columns, or the config's (ImuUncertainty). The
+ *   white IMU noise is not an input: it stays a per-step draw on the report (drawing it in every substep would cost
+ *   two more Philox blocks per substep). In float, in this order:
+ *     v = (2 (x z - y w), 2 (y z + x w), 1 - 2 (x x + y y))      R(q)^T e_z, the predicted "up" in the IMU frame
+ *     n = |a_m|; e = n > 1e-3 ? (a_m * (1 / n)) x v : 0
+ *     b_k = b_k - (ki * e_k) * h;  w_k = (w_m,k - b_k) + kp * e_k
+ *     t = 0.5 * |w| * h; if |w| > 0: c = cos t, s = sin t / |w| (t < 0.25: c = 1 - t^2 (1/2 - t^2 (1/24 - t^2 / 720)),
+ *     s = 0.5 h (1 - t^2 (1/6 - t^2 (1/120 - t^2 / 5040)))), r = q (x) (c, s w), q = r * (1 / |r|); q unchanged at |w| = 0.
+ * - Draw per reset: at every reset of env i (both fused auto-resets, upkie_b200_reset with or without a mask or host
+ *   rows) a per-env counter k goes up by 1, and Philox4x32-10 with key seed (upkie_b200_set_autoreset) and counters
+ *   (g, 2^51 | k << 4), g = env_offset + i, gives four words: kp, ki, roll and pitch, each
+ *   min(low + fl(fl(high - low) * u(w)), high), u(w) = (w >> 8) / 2^24 (the servo dropouts' map). Tag bit 51 alone
+ *   keeps these counters apart from every tag listed in the velocity-limit block above (63 ... 52) and from the cycle
+ *   counters below bit 52, which carry bits 59 | 58 or 55 | 54.
+ * - Initialisation: after the reset substep, the estimate is that of a base oriented R_b E (the estimate taken back to
+ *   the base through the nominal rotation_base_to_imu), R_b the observed (misaligned) base orientation of the
+ *   post-reset state and E = Ry(pitch) Rx(roll) the drawn error, a rotation in the base frame; b = 0.
+ *   upkie_b200_set_state re-initialises every env the same way with E = I, keeping gains and counts (the sensors see
+ *   the state set).
+ * - Where it appears: imu.orientation, base_orientation.pitch, base_orientation.rotation_base_to_world (the estimate
+ *   taken back to the base) and the gyropod and pendulum pitch: in step rows, upkie_b200_spine_obs, reset_obs, the
+ *   final observation and final spine observation, and the UPKIE_SP_IMU_QUAT / PITCH / ROT columns of every history
+ *   entry (each the estimate after its own substep). Under an observation delay of one tick the report is the estimate
+ *   of the cycle observed. A same-step auto-reset's final observation carries the terminal episode's estimate.
+ * - Not affected: every angular velocity (the gyro's true-frame rates), the accelerations, the linear velocity, the
+ *   servo rows and odometry, the physics, terminations and auto-resets (a fall stays the simulator's judgement), and
+ *   upkie_b200_get_state.
+ * Setting a spec draws nothing: an env of a handle that had no filter takes kp_high and ki_high, the true orientation
+ * and b = 0 until its next reset; a replacement keeps each env's state. NULL turns the filter off (the per-env state is
+ * freed once the device is idle). Either invalidates the last step's stash of terminal states
+ * (upkie_b200_final_spine_obs), whose layout follows the spec. get/set_attitude_filter_state: UPKIE_B200_EINVAL without
+ * a spec, and for a quaternion that is not unit within 1e-5, a value that is not finite, or gains outside the caps
+ * below. get/set_attitude_filter_report: report[N][4], the estimate each env's observation reports under an
+ * observation delay (that of the cycle its snapshot observed; a checkpoint carries it, as it carries the snapshot);
+ * set_attitude_filter_state leaves it, as setting the estimate leaves the snapshot; UPKIE_B200_EINVAL for a
+ * quaternion that is not unit within 1e-5.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: a bound that is not finite or low > high; kp_low < 0 or
+ * kp_high * h > 0.5 (the discrete correction must not overshoot); ki_low < 0 or ki_high > 10; a roll or pitch bound
+ * beyond pi/4 in magnitude; spine_mode, joint_limits == 0 and body_contacts (it runs in the observation-delay kernels);
+ * an observation delay of more than one tick (upkie_b200_set_observation_delay_ticks with max_ticks > 1, refused in
+ * both orders: the report of a deeper delay would need a ring of estimates). upkie_b200_set_config refuses
+ * joint_limits = 0, body_contacts and a dt / nb_substeps for which kp * h > 0.5 for the largest kp an env holds or
+ * the spec's kp_high while a spec is set; the in-kernel rollout transports reject a handle with one. The set call waits
+ * for the device. */
+typedef struct UpkieAttitudeFilter {
+  float kp_low, kp_high;       /* 1/s, proportional gain of the accelerometer correction */
+  float ki_low, ki_high;       /* 1/s^2, integral gain of the gyro-bias estimate */
+  float roll_low, roll_high;   /* rad, initial estimate error about the base x axis */
+  float pitch_low, pitch_high; /* rad, initial estimate error about the base y axis */
+} UpkieAttitudeFilter;
+int upkie_b200_set_attitude_filter(void* handle, const UpkieAttitudeFilter* spec);
+int upkie_b200_get_attitude_filter_state(void* handle, uint32_t* count, float* gains, float* quat, float* bias,
+                                         void* stream);
+int upkie_b200_set_attitude_filter_state(void* handle, const uint32_t* count, const float* gains, const float* quat,
+                                         const float* bias, void* stream);
+int upkie_b200_get_attitude_filter_report(void* handle, float* quat, void* stream);
+int upkie_b200_set_attitude_filter_report(void* handle, const float* quat, void* stream);
+
 /* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
  * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
  * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last

@@ -481,6 +481,23 @@ class UpkieVelocityDerate(C.Structure):
     ]
 
 
+class UpkieAttitudeFilter(C.Structure):
+    """``UpkieAttitudeFilter`` of include/upkie_b200.h: the ranges each reset draws an env's attitude-filter gains
+    (kp in 1/s, ki in 1/s^2) and initial estimate error (roll, pitch about the base axes, rad) from."""
+
+    _fields_ = [
+        ("kp_low", C.c_float), ("kp_high", C.c_float),
+        ("ki_low", C.c_float), ("ki_high", C.c_float),
+        ("roll_low", C.c_float), ("roll_high", C.c_float),
+        ("pitch_low", C.c_float), ("pitch_high", C.c_float),
+    ]
+
+
+ATTITUDE_FILTER_MAX_KP_H = 0.5  # kp_high * (dt / nb_substeps) at most: the discrete correction must not overshoot
+ATTITUDE_FILTER_MAX_KI = 10.0  # 1/s^2, the largest ki_high
+ATTITUDE_FILTER_MAX_ERROR = 0.78539816  # rad, the largest |roll| or |pitch| bound of the initial error (pi/4)
+
+
 MAX_HISTORY = 64  # UPKIE_MAX_HISTORY: the most entries an observation history reports
 MAX_HISTORY_CHANNELS = 16  # UPKIE_MAX_HISTORY_CHANNELS: the most spine columns it records
 

@@ -76,6 +76,11 @@ SYMBOLS = {
     "upkie_b200_set_velocity_derate": (C.c_int, [_vp, C.POINTER(_abi.UpkieVelocityDerate)]),
     "upkie_b200_get_velocity_derate_state": (C.c_int, [_vp, _vp, _vp, _vp]),
     "upkie_b200_set_velocity_derate_state": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_set_attitude_filter": (C.c_int, [_vp, C.POINTER(_abi.UpkieAttitudeFilter)]),
+    "upkie_b200_get_attitude_filter_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    "upkie_b200_set_attitude_filter_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
+    "upkie_b200_get_attitude_filter_report": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_attitude_filter_report": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_set_history": (C.c_int, [_vp, C.POINTER(_abi.UpkieHistory)]),
     "upkie_b200_get_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_history_entries": (C.c_int, [_vp, C.POINTER(C.c_int)]),

@@ -272,6 +272,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.encoder_offset = nullptr;
   P.servo_noise = nullptr;
   P.velocity_derate = nullptr;
+  P.attitude_filter = nullptr;
   return 0;
 }
 
@@ -479,6 +480,28 @@ inline const char* velocity_derate_spec_error(const UpkieVelocityDerate& s, cons
     return "set_velocity_derate: needs joint_limits != 0 (the limits run in the observation-delay kernels)";
   if (P.spine_mode) return "set_velocity_derate: spine_mode applies the spine's own torque law";
   if (P.body_contacts) return "set_velocity_derate: body_contacts has no velocity-limit kernels";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses an attitude-filter spec (upkie_b200_set_attitude_filter), null when it takes
+// it: every bound finite, low <= high, 0 <= kp with kp_high * h <= 0.5, 0 <= ki <= 10, and |roll|, |pitch| <= pi/4
+inline const char* attitude_filter_spec_error(const UpkieAttitudeFilter& s, const SimParams& P) {
+  const float b[8] = {s.kp_low, s.kp_high, s.ki_low, s.ki_high, s.roll_low, s.roll_high, s.pitch_low, s.pitch_high};
+  for (int k = 0; k < 8; ++k)
+    if (!std::isfinite(b[k])) return "set_attitude_filter: every bound must be finite";
+  for (int k = 0; k < 8; k += 2)
+    if (!(b[k] <= b[k + 1])) return "set_attitude_filter: low <= high required for kp, ki, roll and pitch";
+  if (!(s.kp_low >= 0.f)) return "set_attitude_filter: kp_low >= 0 required";
+  if (!(double(s.kp_high) * double(P.h) <= 0.5))
+    return "set_attitude_filter: kp_high * (dt / nb_substeps) <= 0.5 required (the correction must not overshoot)";
+  if (!(s.ki_low >= 0.f) || !(s.ki_high <= 10.f)) return "set_attitude_filter: 0 <= ki_low and ki_high <= 10 required";
+  for (int k = 4; k < 8; ++k)
+    if (!(b[k] >= -0.78539816f && b[k] <= 0.78539816f))
+      return "set_attitude_filter: roll and pitch bounds must be within [-pi/4, pi/4] radians";
+  if (P.joint_limits == 0)
+    return "set_attitude_filter: needs joint_limits != 0 (the filter runs in the observation-delay kernels)";
+  if (P.spine_mode) return "set_attitude_filter: spine_mode models its spine's own IMU";
+  if (P.body_contacts) return "set_attitude_filter: body_contacts has no attitude-filter kernels";
   return nullptr;
 }
 

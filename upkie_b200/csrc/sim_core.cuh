@@ -162,6 +162,10 @@ struct SimParams {
   // servo velocity limits (upkie_b200_set_velocity_derate): the handle's device block, null = off. Read by the step
   // kernels of FAM_SENSE (step_family.h) and k_reset only. Appended last.
   const struct VelocityDerate* velocity_derate;
+  // IMU attitude estimation (upkie_b200_set_attitude_filter): the handle's device block, null = off. Read by the step
+  // kernels of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs, k_history_fill and k_attitude_init only.
+  // Appended last.
+  const struct AttitudeFilter* attitude_filter;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -2596,6 +2600,189 @@ UPKIE_HD void velocity_derate_reset(const VelocityDerate& V, uint64_t seed, uint
   const Vmax6 o = velocity_derate_draw(spec, seed, g, k);
 #pragma unroll
   for (int j = 0; j < UPKIE_NJ; ++j) col[size_t(j) * stride] = o.v[j];
+}
+
+// ---- IMU attitude estimation (upkie_b200_set_attitude_filter, Pi3HatInterface.cpp:151-169) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h), [rows][stride] structure-of-arrays
+// like the state, env i in column i: count[i] = k, the number of the env's last draw; gains (kp, ki); quat, the
+// estimate q_i (w, x, y, z) of the IMU-to-world rotation; bias, the gyro-bias estimate b_i. `rep` is the estimate the
+// env's observation reports under an observation delay (that of the cycle observed), `vel` the world-frame IMU velocity
+// of the env's last substep (scratch of the step kernels), and qbi the quaternion of rotation_base_to_imu.
+struct AttitudeFilter {
+  UpkieAttitudeFilter spec;
+  float qbi[4];
+  uint32_t* count;
+  float* gains;
+  float* quat;
+  float* bias;
+  float* rep;
+  float* vel;
+  int stride;
+};
+
+// bit 51 of the high counter word alone, the per-reset draws, (k << 4) below bit 36: never set by sample_init_state
+// (below 2^34) or the noise (below bit 42); every other tag sets a bit above 51 (the reset randomisation 63, the pushes
+// 62, the action delay 61, the observation delay 60, the servo dropouts 59 and 59 | 58, the IMU misalignment 57, the
+// encoder offsets 56, the servo noise 55, 55 | 54 and 55 | 54 | 53, the velocity limits 52)
+constexpr uint64_t kAttitudeFilterTag = uint64_t(1) << 51;
+
+struct AttitudeDraw {
+  float kp, ki, roll, pitch;
+};
+
+// Draw k of the env of global index g: words 0 .. 3 of one block give kp, ki, roll and pitch, push_value's exact form
+// (the map of the servo dropouts)
+UPKIE_HD AttitudeDraw attitude_filter_draw(const UpkieAttitudeFilter& s, uint64_t seed, uint64_t g, uint32_t k) {
+  const Philox4 r = philox4x32_10(g, kAttitudeFilterTag | (uint64_t(k) << 4), seed);
+  return AttitudeDraw{push_value(r.v[0], s.kp_low, s.kp_high), push_value(r.v[1], s.ki_low, s.ki_high),
+                      push_value(r.v[2], s.roll_low, s.roll_high), push_value(r.v[3], s.pitch_low, s.pitch_high)};
+}
+
+// p (x) q, quaternions (w, x, y, z)
+UPKIE_HD void quat_mul(const float p[4], const float q[4], float r[4]) {
+  r[0] = p[0] * q[0] - p[1] * q[1] - p[2] * q[2] - p[3] * q[3];
+  r[1] = p[0] * q[1] + p[1] * q[0] + p[2] * q[3] - p[3] * q[2];
+  r[2] = p[0] * q[2] - p[1] * q[3] + p[2] * q[0] + p[3] * q[1];
+  r[3] = p[0] * q[3] + p[1] * q[2] - p[2] * q[1] + p[3] * q[0];
+}
+
+// One step of the filter (include/upkie_b200.h: the law, in this order): the estimate q and the bias estimate b of a
+// filter of gains kp, ki, updated in place over a substep h from the gyro rate w_m and the specific force a_m of the
+// IMU frame
+UPKIE_HD void attitude_filter_step(float q[4], float b[3], float kp, float ki, float h, const float wm[3],
+                                   const float am[3]) {
+  const float vx = 2.f * (q[1] * q[3] - q[2] * q[0]);
+  const float vy = 2.f * (q[2] * q[3] + q[1] * q[0]);
+  const float vz = 1.f - 2.f * (q[1] * q[1] + q[2] * q[2]);
+  float e[3] = {0.f, 0.f, 0.f};
+  const float n = sqrtf(am[0] * am[0] + am[1] * am[1] + am[2] * am[2]);
+  if (n > 1e-3f) {
+    const float inv = 1.f / n;
+    const float ux = am[0] * inv, uy = am[1] * inv, uz = am[2] * inv;
+    e[0] = uy * vz - uz * vy;
+    e[1] = uz * vx - ux * vz;
+    e[2] = ux * vy - uy * vx;
+  }
+  float w[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    b[k] = b[k] - (ki * e[k]) * h;
+    w[k] = (wm[k] - b[k]) + kp * e[k];
+  }
+  const float nw = sqrtf(w[0] * w[0] + w[1] * w[1] + w[2] * w[2]);
+  if (!(nw > 0.f)) return;
+  const float t = 0.5f * nw * h;
+  float c, s;
+  if (t < 0.25f) {
+    // the series of cos t and sin t / t (truncation below 1e-8 here), free of the approximate sin / cos of fast math
+    // at the small angles of one substep
+    const float t2 = t * t;
+    c = 1.f - t2 * (0.5f - t2 * (1.f / 24.f - t2 * (1.f / 720.f)));
+    s = 0.5f * h * (1.f - t2 * (1.f / 6.f - t2 * (1.f / 120.f - t2 * (1.f / 5040.f))));
+  } else {
+    c = cosf(t);
+    s = sinf(t) / nw;
+  }
+  const float d[4] = {c, s * w[0], s * w[1], s * w[2]};
+  float r[4];
+  quat_mul(q, d, r);
+  const float inv = 1.f / sqrtf(r[0] * r[0] + r[1] * r[1] + r[2] * r[2] + r[3] * r[3]);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) q[k] = r[k] * inv;
+}
+
+// The filter's inputs of the state S, whose orientation is the observed one (the IMU misalignment's view applied):
+// the gyro rate w_m and the specific force a_m of the IMU frame, from the IMU velocities v (after the substep) and vp
+// (after the previous one), with the env's gyro and accelerometer biases gb, ab
+UPKIE_HD void attitude_filter_inputs(const SimParams& P, const AttitudeFilter& A, const RobotState& S, const float v[3],
+                                     const float vp[3], const float gb[3], const float ab[3], float wm[3],
+                                     float am[3]) {
+  const float qbc[4] = {A.qbi[0], -A.qbi[1], -A.qbi[2], -A.qbi[3]};
+  float qi[4];
+  quat_mul(S.quat, qbc, qi);
+  float R[9];
+  quat_to_rot(qi, R);
+  float f[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) f[k] = (v[k] - vp[k]) * P.inv_h;
+  f[2] += 9.81f;
+  rot_tmul(R, S.angvel, wm);
+  rot_tmul(R, f, am);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    wm[k] += gb[k];
+    am[k] += ab[k];
+  }
+}
+
+// The env's IMU biases (the parameter table's columns, or the config's; zero without IMU uncertainty)
+UPKIE_HD void attitude_filter_biases(const SimParams& P, int env, float gb[3], float ab[3]) {
+  const bool table = env >= 0 && P.env_params != nullptr;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    gb[k] = 0.f;
+    ab[k] = 0.f;
+    if (P.any_imu_uncertainty) {
+      gb[k] = table ? env_param(P, env, UPKIE_EP_IMU_GYRO_BIAS + k) : P.imu_gyro_bias[k];
+      ab[k] = table ? env_param(P, env, UPKIE_EP_IMU_ACC_BIAS + k) : P.imu_acc_bias[k];
+    }
+  }
+}
+
+// The estimate of a base observed with orientation qb (the misalignment's view applied) and an estimate error
+// E = Ry(pitch) Rx(roll) in the base frame: qb (x) E (x) qbi^-1
+UPKIE_HD void attitude_filter_initial(const AttitudeFilter& A, const float qb[4], float roll, float pitch, float q[4]) {
+  const Quat4 E = imu_misalign_quat(roll, pitch, 0.f);
+  float t[4];
+  quat_mul(qb, E.q, t);
+  const float qbc[4] = {A.qbi[0], -A.qbi[1], -A.qbi[2], -A.qbi[3]};
+  quat_mul(t, qbc, q);
+}
+
+// The estimate q taken back to the base: q (x) qbi, the orientation every orientation-derived observation reports
+UPKIE_HD void attitude_filter_base(const AttitudeFilter& A, const float q[4], float qb[4]) { quat_mul(q, A.qbi, qb); }
+
+// The base pitch of the base orientation qb (base_pitch's arithmetic)
+UPKIE_HD float attitude_filter_pitch(const float qb[4]) {
+  return asinf(clampf(2.f * (qb[0] * qb[2] - qb[3] * qb[1]), -1.f, 1.f));
+}
+
+// Whether spine column `col` is orientation-derived (the estimate replaces it)
+UPKIE_HD constexpr bool attitude_filter_column(int col) {
+  return col == UPKIE_SP_PITCH || (col >= UPKIE_SP_ROT && col < UPKIE_SP_IMU_ANGVEL);
+}
+
+// The orientation-derived columns of a spine observation o, from the base orientation qb (spine_observation's
+// arithmetic, those columns only)
+UPKIE_HD void attitude_filter_observation(const SimParams& P, const float qb[4], float* o) {
+  RobotState T;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) T.quat[k] = qb[k];
+  o[UPKIE_SP_PITCH] = base_pitch(T);
+  const float zero[3] = {0.f, 0.f, 0.f};
+  for (int c = UPKIE_SP_ROT; c < UPKIE_SP_IMU_ANGVEL; ++c) o[c] = history_value(P, T, zero, c);
+}
+
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, stored, and the new episode's estimate of
+// the observed post-reset state S (misalignment view applied), stored as the estimate and the report, b = 0. The
+// block's fields are copied before the first store, as servo_dropout_reset.
+UPKIE_HD void attitude_filter_reset(const AttitudeFilter& A, uint64_t seed, uint64_t g, int i, const RobotState& S) {
+  const AttitudeFilter B = A;
+  const size_t stride = size_t(B.stride);
+  const uint32_t k = B.count[i] + 1u;
+  B.count[i] = k;
+  const AttitudeDraw d = attitude_filter_draw(B.spec, seed, g, k);
+  float q[4];
+  attitude_filter_initial(B, S.quat, d.roll, d.pitch, q);
+  B.gains[size_t(i)] = d.kp;
+  B.gains[stride + size_t(i)] = d.ki;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    B.quat[size_t(r) * stride + size_t(i)] = q[r];
+    B.rep[size_t(r) * stride + size_t(i)] = q[r];
+  }
+#pragma unroll
+  for (int r = 0; r < 3; ++r) B.bias[size_t(r) * stride + size_t(i)] = 0.f;
 }
 
 }  // namespace upkie_b200

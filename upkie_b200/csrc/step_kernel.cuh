@@ -290,6 +290,137 @@ __device__ __noinline__ void derate_reset_lane(const SimParams& P, uint64_t seed
   velocity_derate_reset(*P.velocity_derate, seed, g, i);
 }
 
+// The attitude filter (F.sense kernels, P.attitude_filter set). Out of line, as history_substep: the estimate, the
+// bias estimate and the last substep's IMU velocity stay in the env's columns of the device block, so that the substep
+// loop carries none of them. attitude_lane: one spine cycle of env i, the end of substep `sub` (S a copy of the state
+// after it, em the env's misalignment, env its column of the parameter table): the filter steps, from the IMU velocity
+// of the previous substep (the state's, which the last observation update stored, at sub = 0); `snap`: the new
+// estimate is also the report (the observation-delay snapshot of this cycle); `entry` (non-null): the history entry of
+// the cycle, whose orientation-derived columns it overwrites with the estimate.
+__device__ __forceinline__ void attitude_entry(const SimParams& P, const float q[4], float* entry, size_t hstride,
+                                               int hcount, uint32_t ticks) {
+  float qb[4];
+  attitude_filter_base(*P.attitude_filter, q, qb);
+  float o[UPKIE_SP_IMU_ANGVEL];
+  attitude_filter_observation(P, qb, o);
+  for (int c = 0; c < hcount; ++c) {
+    const int col = __ldg(P.history->columns + c);
+    if (!attitude_filter_column(col)) continue;
+    const float v = history_pick(o, col);
+    for (uint32_t e = 0; e < ticks; ++e) __stcg(entry + (size_t(e) * size_t(hcount) + size_t(c)) * hstride, v);
+  }
+}
+struct AttitudeKin {  // the fields of the state the filter reads: the substep loop passes these, not a state copy
+  float quat[4], linvel[3], angvel[3], prev_imu_vel[3];
+};
+__device__ __forceinline__ AttitudeKin attitude_kin(const RobotState& S) {
+  AttitudeKin k;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) k.quat[r] = S.quat[r];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    k.linvel[r] = S.linvel[r];
+    k.angvel[r] = S.angvel[r];
+    k.prev_imu_vel[r] = S.prev_imu_vel[r];
+  }
+  return k;
+}
+__device__ __noinline__ void attitude_lane(const SimParams& P, const AttitudeKin K, const Quat4 em, int i, int env,
+                                           int sub, bool snap, float* entry, size_t hstride, int hcount) {
+  RobotState S;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) S.quat[r] = K.quat[r];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    S.linvel[r] = K.linvel[r];
+    S.angvel[r] = K.angvel[r];
+    S.prev_imu_vel[r] = K.prev_imu_vel[r];
+  }
+  const AttitudeFilter& A = *P.attitude_filter;
+  const size_t stride = size_t(A.stride);
+  float* const vel = A.vel + size_t(i);
+  float* const quat = A.quat + size_t(i);
+  float* const bias = A.bias + size_t(i);
+  float v[3], vp[3];
+  imu_velocity(P, S, v);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    vp[k] = sub == 0 ? S.prev_imu_vel[k] : __ldcg(vel + size_t(k) * stride);
+    __stcg(vel + size_t(k) * stride, v[k]);
+  }
+  imu_misalign_view(S, em);
+  float gb[3], ab[3], wm[3], am[3];
+  attitude_filter_biases(P, env, gb, ab);
+  attitude_filter_inputs(P, A, S, v, vp, gb, ab, wm, am);
+  float q[4], b[3];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) q[r] = __ldcg(quat + size_t(r) * stride);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) b[r] = __ldcg(bias + size_t(r) * stride);
+  attitude_filter_step(q, b, __ldcg(A.gains + size_t(i)), __ldcg(A.gains + stride + size_t(i)), P.h, wm, am);
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    __stcg(quat + size_t(r) * stride, q[r]);
+    if (snap) __stcg(A.rep + size_t(r) * stride + size_t(i), q[r]);
+  }
+#pragma unroll
+  for (int r = 0; r < 3; ++r) __stcg(bias + size_t(r) * stride, b[r]);
+  if (entry) attitude_entry(P, q, entry, hstride, hcount, 1u);
+}
+// The estimate env i's observation reports (`rep`: under an observation delay, the snapshot's), loaded
+__device__ __forceinline__ void attitude_load(const SimParams& P, int i, bool rep, float q[4]) {
+  const AttitudeFilter& A = *P.attitude_filter;
+  const float* const col = (rep ? A.rep : A.quat) + size_t(i);
+  const size_t stride = size_t(A.stride);
+#pragma unroll
+  for (int r = 0; r < 4; ++r) q[r] = __ldcg(col + size_t(r) * stride);
+}
+// The observation-delay snapshot at the start of a tick: the report is the estimate in force
+__device__ __noinline__ void attitude_snap_lane(const SimParams& P, int i) {
+  const AttitudeFilter& A = *P.attitude_filter;
+  const size_t stride = size_t(A.stride);
+#pragma unroll
+  for (int r = 0; r < 4; ++r) __stcg(A.rep + size_t(r) * stride + size_t(i), __ldcg(A.quat + size_t(r) * stride + size_t(i)));
+}
+// The base pitch of the estimate env i's observation reports (the gyropod and pendulum rows)
+__device__ __noinline__ float attitude_pitch_lane(const SimParams& P, int i, bool rep) {
+  float q[4], qb[4];
+  attitude_load(P, i, rep, q);
+  attitude_filter_base(*P.attitude_filter, q, qb);
+  return attitude_filter_pitch(qb);
+}
+// A same-step auto-reset's terminal step: the pitch of the estimate it reports, and that estimate into the four rows
+// of the final-spine-observation stash after the state (and the parameter columns with reset randomisation) when
+// `stash`
+__device__ __noinline__ float attitude_final_lane(const SimParams& P, int n_pad, int i, bool rep, bool stash) {
+  float q[4], qb[4];
+  attitude_load(P, i, rep, q);
+  if (stash) {
+    float* const row = P.final_state + size_t(kFinalRows + (P.reset_rand ? kFinalParamCols : 0)) * size_t(n_pad);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) row[size_t(r) * size_t(n_pad) + size_t(i)] = q[r];
+  }
+  attitude_filter_base(*P.attitude_filter, q, qb);
+  return attitude_filter_pitch(qb);
+}
+// A reset of env i: its next draw and the new episode's estimate, from the true post-reset state S observed through
+// the new episode's misalignment em (out of line, as tilt_reset_lane)
+__device__ __noinline__ void attitude_reset_lane(const SimParams& P, const Quat4 qs, const Quat4 em, uint64_t seed,
+                                                 uint64_t g, int i) {
+  RobotState S;
+#pragma unroll
+  for (int r = 0; r < 4; ++r) S.quat[r] = qs.q[r];
+  imu_misalign_view(S, em);
+  attitude_filter_reset(*P.attitude_filter, seed, g, i, S);
+}
+// A history refilled by a reset: every entry's orientation-derived columns report the new estimate
+__device__ __noinline__ void attitude_fill_lane(const SimParams& P, int i, float* col, size_t stride, int count,
+                                                uint32_t ticks) {
+  float q[4];
+  attitude_load(P, i, false, q);
+  attitude_entry(P, q, col, stride, count, ticks);
+}
+
 // ---- one env tick of the robot `tid` --------------------------------------------------
 // `tile4` is this warp's staging tile (TILE >= 1): on entry it holds the warp's 32 action rows when
 // `full` (prefetched by the caller), during the substeps each lane's clamped row, and it is reused to transpose the
@@ -604,6 +735,13 @@ __device__ __forceinline__ void step_env(
       else if (live) em = tilt_reset_lane(P, seed, env_offset + uint64_t(i), i);
     }
   }
+  // IMU attitude estimation (F.sense kernels, P.attitude_filter set: a uniform branch). Each substep of a lane that does
+  // not reset steps the env's filter on the IMU of its cycle (attitude_lane, after the history entry, whose orientation
+  // columns it overwrites with the estimate); an observation-delay snapshot keeps the estimate of its cycle as the
+  // report. A reset draws and initialises after the tick (attitude_reset_lane, before the history refill); the
+  // same-step final observation and stash report the terminal episode's estimate, taken before it. The gyropod and
+  // pendulum rows report the estimate's pitch (the rates stay the true frame's). Without the feature nothing runs.
+  const bool filtering = F.sense && P.attitude_filter;
   auto sense_load = [&](int k) { return __ldcg(scol + size_t(k) * sstride); };
   auto sense_store = [&](int k, float v) { __stcg(scol + size_t(k) * sstride, v); };
   if (sensing && live && sdl == uint32_t(P.nb_substeps)) {  // the state at the start of the tick
@@ -612,6 +750,9 @@ __device__ __forceinline__ void step_env(
     obs_delay_snapshot(P, S, v, sense_load, sense_store);
     // the end of the last tick: every servo reports what the held rows latched then
     if (dropping) dropout_sense(P, ~0u, i, scol, sstride);
+    if constexpr (F.sense) {
+      if (filtering) attitude_snap_lane(P, i);  // and the estimate of that cycle
+    }
   }
   // spine-rate observation history (F.sense kernels, P.history set: a uniform branch). Each substep of a lane that does
   // not reset stores the selected spine columns of its state into ring entry (head + sub) % ticks, differentiating the
@@ -688,6 +829,13 @@ __device__ __forceinline__ void step_env(
         history_substep(P, S, hvel, hring + size_t((hhead + uint32_t(sub)) % hticks) * size_t(hcount) * hstride,
                         hstride, hcount, hacc, dcur, i, em, eo, seed, env_offset + uint64_t(i),
                         servo_noise_cycle(nz.tick, uint32_t(sub)));
+      if constexpr (F.sense) {
+        if (filtering && !resetting && live)
+          attitude_lane(P, attitude_kin(S), em, i, env_col, sub, sensing && uint32_t(sub) + sdl + 1u == uint32_t(P.nb_substeps),
+                        recording ? hring + size_t((hhead + uint32_t(sub)) % hticks) * size_t(hcount) * hstride
+                                  : nullptr,
+                        hstride, hcount);
+      }
     } else {
 #pragma unroll
       for (int k = 0; k < kPhaseSyncs; ++k) PhaseSync()();
@@ -741,6 +889,7 @@ __device__ __forceinline__ void step_env(
 
   bool fin_pending = false;  // F.sense, same-step reset: the terminal observation is stashed after the tick
   float fin_o6[6], fin_yaw = 0.f, fin_yaw_vel = 0.f;
+  float fin_pitch = 0.f;  // the attitude filter: the pitch of the terminal episode's reported estimate
   const Quat4 fin_e = em;  // the terminal episode's misalignment (a same-step reset draws the next one into em)
   const Offset6 fin_eo = eo;  // and its encoder offsets
   if (AUTORESET == AUTORESET_SAME_STEP) {
@@ -755,6 +904,8 @@ __device__ __forceinline__ void step_env(
         }
         fin_yaw = S.yaw;
         fin_yaw_vel = S.yaw_vel;
+        // the attitude filter: the terminal episode's reported estimate (and into the stash), before the reset
+        if (filtering) fin_pitch = attitude_final_lane(P, n_pad, i, sensing, P.final_state && live);
       }
       if (!(F.sense && sensing)) {
         // servo dropouts: the terminal step's observation and stash report the latched servos. The reset below keeps
@@ -780,6 +931,7 @@ __device__ __forceinline__ void step_env(
           if (tilting && imu_misalign_view(S, em) && MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
           // the encoder offsets: its reported positions (the reset below overwrites q whole, reset_pose)
           if (offsetting && encoder_offset_view(S, eo) && MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
+          if (filtering && MODE != MODE_SERVOS) o6[1] = fin_pitch;  // and the estimate's pitch
         }
         if (P.final_obs && live)
           store_final_obs<MODE, spine>(P, S, L, o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
@@ -834,12 +986,22 @@ __device__ __forceinline__ void step_env(
   }
 
   if (live) store_state(state, n_pad, i, S);
+  // the attitude filter: a reset's draw and the new episode's estimate, of the post-reset state (the true state, here
+  // in S) observed through the new episode's misalignment
+  if constexpr (F.sense) {
+    if (filtering && live && dreset)
+      attitude_reset_lane(P, Quat4{{S.quat[0], S.quat[1], S.quat[2], S.quat[3]}}, em, seed, env_offset + uint64_t(i), i);
+  }
   // the history: a reset fills the lane's ring from its post-reset state (the true state, here in S), and every lane's
   // head moves on by the tick's substeps
   if (recording && live) {
-    if (refill)
+    if (refill) {
       history_fill_lane(P, S, hring, hstride, hcount, hticks, em, eo, seed, env_offset + uint64_t(i), i,
                         (hhead + uint32_t(P.nb_substeps)) % hticks, servo_noise_reset_cycle(nk), nz.tick);
+      if constexpr (F.sense) {
+        if (filtering) attitude_fill_lane(P, i, hring, hstride, hcount, hticks);  // with the new estimate
+      }
+    }
     __stcg(P.history->head + i, (hhead + uint32_t(P.nb_substeps)) % hticks);
   }
   // the dropouts: a reset latches the lane's post-reset state (the true state, here in S) and draws its next p_i
@@ -871,6 +1033,9 @@ __device__ __forceinline__ void step_env(
       if constexpr (F.sense) fodo = offsetting && encoder_offset_view(S, fin_eo);  // and its reported positions
       if (MODE != MODE_SERVOS && (sdl != 0 || dcur != 0 || ftilt || fodo || fnoise))
         gyropod_obs(P, S, fin_o6);  // (a dropout patched the snapshot, or the orientation is the sensed one)
+      if constexpr (F.sense && MODE != MODE_SERVOS) {
+        if (filtering) fin_o6[1] = fin_pitch;  // the terminal episode's reported estimate
+      }
       if (P.final_obs && live)
         store_final_obs<MODE, spine>(P, S, L, fin_o6, F.extras ? &nz : nullptr, TILE && compact, i, env_col);
       if (P.final_state && live) store_final_state<spine>(P, S, L, n_pad, i);
@@ -923,6 +1088,11 @@ __device__ __forceinline__ void step_env(
   // odometry)
   if constexpr (F.sense) {
     if (offsetting && encoder_offset_view(S, eo) && MODE != MODE_SERVOS) gyropod_obs(P, S, o6);
+  }
+  // the attitude filter: the gyropod and pendulum rows report the pitch of the estimate (the snapshot's under an
+  // observation delay; a reset's new one)
+  if constexpr (F.sense && MODE != MODE_SERVOS) {
+    if (filtering) o6[1] = attitude_pitch_lane(P, i, sensing);
   }
   if (spine && live) {
     float lr[UPKIE_LAG_DIM];

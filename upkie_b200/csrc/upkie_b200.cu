@@ -19,7 +19,9 @@
 // encoder offsets: k_reset draws and shifts the leg targets, and the same three kernels read the servo positions
 // through them (encoder_offset_observed). Nor does the servo noise: k_reset draws, noises the leg targets, the latch
 // and the history refill, and the same three kernels read the servo replies through it (servo_noise_observed). The
-// servo velocity limits touch the torque law only: k_reset draws, and the step kernels' substeps derate.
+// servo velocity limits touch the torque law only: k_reset draws, and the step kernels' substeps derate. The attitude
+// filter has one, k_attitude_init (a new filter, set_state): k_reset draws and initialises, and k_spine_obs,
+// k_reset_obs and k_history_fill report the estimate (attitude_observed).
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -27,6 +29,7 @@
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -175,6 +178,16 @@ struct Handle {
   uint32_t* vlim_count = nullptr;
   float* vlim_max = nullptr;  // [UPKIE_NJ][n_pad], v_i
   uint32_t vlim_mask = 0;     // joint_mask of the spec in force
+  // IMU attitude estimation (upkie_b200_set_attitude_filter): the device block P.attitude_filter points to while a spec
+  // is set, and the per-env state it points to (allocated with the first spec, freed when it is turned off)
+  AttitudeFilter* att_dev = nullptr;
+  uint32_t* att_count = nullptr;
+  float* att_gains = nullptr;  // [2][n_pad] kp, ki
+  float* att_quat = nullptr;   // [4][n_pad] q_i
+  float* att_bias = nullptr;   // [3][n_pad] b_i
+  float* att_rep = nullptr;    // [4][n_pad] the estimate the observation reports under an observation delay
+  float* att_vel = nullptr;    // [3][n_pad] the step kernels' last-substep IMU velocity
+  UpkieAttitudeFilter att_spec{};  // the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -194,6 +207,8 @@ Handle* as_handle(void* h) {
 // `env_offset`), and the per-env state of every randomisation the handle runs restarts with them, in the per-lane
 // functions of the step kernels' fused resets. Those draws are keyed on the auto-reset's seed and env offset
 // (`rand_seed`, `rand_offset`), whatever init rows the reset takes.
+__device__ void attitude_history_observed(const SimParams& P, int i, const History& H);
+
 __global__ void __launch_bounds__(128)
 k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict__ state,
         const uint8_t* __restrict__ mask, const float* __restrict__ init_state, const float* __restrict__ eps_all,
@@ -286,6 +301,11 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
   // the misalignment's next draw, before the history: the new episode is observed through it
   Quat4 e{{1.f, 0.f, 0.f, 0.f}};
   if (P.imu_misalign) e = imu_misalign_reset(*P.imu_misalign, rand_seed, g, i);
+  if (P.attitude_filter) {  // the attitude filter's next draw and the new episode's estimate, before the history
+    RobotState V = S;
+    imu_misalign_view(V, e);
+    attitude_filter_reset(*P.attitude_filter, rand_seed, g, i, V);
+  }
   if (P.history) {  // a new episode's history starts from its post-reset columns
     const History& H = *P.history;
     if (P.servo_noise) {  // each entry with the noise of its cycle, the newest the reset observation's
@@ -306,11 +326,39 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
       encoder_offset_view(V, d);
       history_fill(H, P, V, i);
     }
+    attitude_history_observed(P, i, H);
   }
   if (P.servo_dropout) {  // a new p_i, the reset latched (its replies as the reset observation reports them)
     RobotState V = S;
     if (P.servo_noise) servo_noise_view(V, nd);
     servo_dropout_reset(*P.servo_dropout, rand_seed, g, i, V);
+  }
+}
+
+// The attitude filter: the orientation-derived columns of env i's spine observation o reported from its estimate (`q`:
+// rows [4][n_pad] of estimates, the block's own by default: the report under an observation delay, the estimate
+// otherwise), and those columns of every entry of its history
+__device__ void attitude_observed(const SimParams& P, int i, float* o, const float* q = nullptr, int n_pad = 0) {
+  if (!P.attitude_filter) return;
+  const AttitudeFilter& A = *P.attitude_filter;
+  size_t stride = size_t(n_pad);
+  if (!q) {
+    q = P.obs_delay ? A.rep : A.quat;
+    stride = size_t(A.stride);
+  }
+  float e[4], qb[4];
+  for (int r = 0; r < 4; ++r) e[r] = q[size_t(r) * stride + size_t(i)];
+  attitude_filter_base(A, e, qb);
+  attitude_filter_observation(P, qb, o);
+}
+__device__ void attitude_history_observed(const SimParams& P, int i, const History& H) {
+  if (!P.attitude_filter) return;
+  float o[UPKIE_SP_IMU_ANGVEL];
+  attitude_observed(P, i, o);
+  for (int c = 0; c < H.count; ++c) {
+    if (!attitude_filter_column(H.columns[c])) continue;
+    for (int en = 0; en < H.ticks; ++en)
+      H.ring[(size_t(en) * size_t(H.count) + size_t(c)) * size_t(H.stride) + size_t(i)] = o[H.columns[c]];
   }
 }
 
@@ -400,11 +448,13 @@ __global__ void k_history_fill(const __grid_constant__ SimParams P, const Histor
         [&](uint32_t e, int c, float v) {
           H->ring[(size_t(e) * size_t(H->count) + size_t(c)) * size_t(H->stride) + size_t(i)] = v;
         });
+    attitude_history_observed(P, i, *H);
     return;
   }
   imu_misalign_observed(P, i, S);
   encoder_offset_observed(P, i, S);
   history_fill(*H, P, S, i);
+  attitude_history_observed(P, i, *H);
 }
 
 // The spine observation rows of the states `state` (and in spine mode the lag records `lag`), with the noise keys of
@@ -414,7 +464,7 @@ __global__ void k_history_fill(const __grid_constant__ SimParams P, const Histor
 __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ state,
                             const float* __restrict__ lag, const uint32_t* __restrict__ mark, uint32_t gen,
                             const uint32_t* __restrict__ tick, uint64_t env_offset, float* __restrict__ out,
-                            uint64_t seed) {
+                            uint64_t seed, const float* __restrict__ att = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   if (mark && mark[i] != gen) return;
@@ -439,6 +489,7 @@ __global__ void k_spine_obs(const __grid_constant__ SimParams P, int n, int n_pa
     float tq[6];
     measured_torques(P, S, &nz, tq, i);
     spine_observation(P, S, o, tq);
+    attitude_observed(P, i, o, att, n_pad);  // (`att`: the stash's rows of the terminal estimates)
   }
   apply_imu_uncertainty(P, nz, o, i);
 #pragma unroll
@@ -476,11 +527,41 @@ __global__ void k_reset_obs(const __grid_constant__ SimParams P, int n, int n_pa
   }
   float o6[6];
   gyropod_obs(P, S, o6);
+  if (P.attitude_filter) {  // the pitch of the estimate the env reports
+    float o[UPKIE_SP_IMU_ANGVEL];
+    attitude_observed(P, i, o);
+    o6[1] = o[UPKIE_SP_PITCH];
+  }
   if (obs_dim == 6) {
     for (int k = 0; k < 6; ++k) out[size_t(i) * 6 + k] = o6[k];
   } else {
     out[size_t(i) * 4 + 0] = o6[1]; out[size_t(i) * 4 + 1] = o6[0];
     out[size_t(i) * 4 + 2] = o6[4]; out[size_t(i) * 4 + 3] = o6[3];
+  }
+}
+
+// The attitude filter of every env from its state (set_state, a first filter): the estimate of the observed (misaligned)
+// orientation without an error, stored as the estimate and the report, b = 0; `gains` (a first filter) also stores
+// kp, ki
+__global__ void k_attitude_init(const __grid_constant__ SimParams P, int n, int n_pad, const float* __restrict__ state,
+                                bool gains, float kp, float ki) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  RobotState S;
+  load_state(state, n_pad, i, S);
+  imu_misalign_observed(P, i, S);
+  const AttitudeFilter& A = *P.attitude_filter;
+  const size_t stride = size_t(A.stride);
+  float q[4];
+  attitude_filter_initial(A, S.quat, 0.f, 0.f, q);
+  for (int r = 0; r < 4; ++r) {
+    A.quat[size_t(r) * stride + size_t(i)] = q[r];
+    A.rep[size_t(r) * stride + size_t(i)] = q[r];
+  }
+  for (int r = 0; r < 3; ++r) A.bias[size_t(r) * stride + size_t(i)] = 0.f;
+  if (gains) {
+    A.gains[size_t(i)] = kp;
+    A.gains[stride + size_t(i)] = ki;
   }
 }
 
@@ -737,7 +818,9 @@ int prepare_final_state(Handle* h, int32_t flag, bool& stash) {
   if (!stash) return UPKIE_B200_OK;
   // reset randomisation: the pre-reset parameter-table columns go to kFinalParamCols more rows
   const bool params = h->P.reset_rand != nullptr;
-  const int rows = (h->lag ? kFinalRowsSpine : kFinalRows) + (params ? kFinalParamCols : 0);
+  // the attitude filter: the terminal estimates go to 4 more rows after those (no spine mode with a filter)
+  const int rows = (h->lag ? kFinalRowsSpine : kFinalRows) + (params ? kFinalParamCols : 0) +
+                   (h->P.attitude_filter ? 4 : 0);
   if (h->final_state && h->final_rows < rows) {
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaDeviceSynchronize());  // steps in flight may still write the smaller stash
@@ -1124,6 +1207,8 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->enc_dev); cudaFree(h->enc_count); cudaFree(h->enc_offset);
   cudaFree(h->noise_dev); cudaFree(h->noise_count); cudaFree(h->noise_sigma); cudaFree(h->noise_fresh);
   cudaFree(h->vlim_dev); cudaFree(h->vlim_count); cudaFree(h->vlim_max);
+  cudaFree(h->att_dev); cudaFree(h->att_count); cudaFree(h->att_gains); cudaFree(h->att_quat); cudaFree(h->att_bias);
+  cudaFree(h->att_rep); cudaFree(h->att_vel);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
   cudaFree(h->d_act); cudaFree(h->d_obs); cudaFree(h->d_rew); cudaFree(h->d_term); cudaFree(h->d_trunc);
   for (int k = 0; k < kHostStreams; ++k)
@@ -1187,6 +1272,23 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: velocity limits need joint_limits != 0");
   if (h->P.velocity_derate && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no velocity-limit kernels");
+  if (h->P.attitude_filter && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: the attitude filter needs joint_limits != 0");
+  if (h->P.attitude_filter && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no attitude-filter kernels");
+  if (h->P.attitude_filter) {
+    // the bound holds for the gains every env holds (a narrower spec keeps each env's gains until its next reset, and
+    // set_attitude_filter_state may set others) and for those the spec in force draws
+    CUDA_TRY(cudaSetDevice(h->device));
+    CUDA_TRY(cudaDeviceSynchronize());  // resets in flight may draw new gains
+    std::vector<float> kp(size_t(h->n));
+    CUDA_TRY(cudaMemcpy(kp.data(), h->att_gains, kp.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    float kp_max = h->att_spec.kp_high;
+    for (float k : kp) kp_max = std::max(kp_max, k);
+    if (!(double(kp_max) * double(P.h) <= 0.5))
+      return fail(UPKIE_B200_EINVAL, "set_config: the attitude filter's largest kp (held by an env or the spec's "
+                                     "kp_high) times dt / nb_substeps must stay <= 0.5");
+  }
   if (P.body_contacts && !h->body_rec) {  // switched on after creation: the record buffer is allocated now
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMalloc(&h->body_rec, size_t(UPKIE_BODY_REC_DIM) * h->n_pad * sizeof(float)));
@@ -1212,6 +1314,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.encoder_offset = h->P.encoder_offset;  // and the encoder offsets
   P.servo_noise = h->P.servo_noise;        // and the servo noise
   P.velocity_derate = h->P.velocity_derate;  // and the velocity limits
+  P.attitude_filter = h->P.attitude_filter;  // and the attitude filter
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -1643,7 +1746,8 @@ int upkie_b200_final_spine_obs(void* handle, float* out, void* stream) {
       P, h->n, h->n_pad, stash + size_t(kFinalStateRow) * h->n_pad,
       h->lag ? stash + size_t(kFinalLagRow) * h->n_pad : nullptr,
       reinterpret_cast<const uint32_t*>(stash + size_t(kFinalMarkRow) * h->n_pad), h->final_gen, h->tick,
-      h->env_offset, out, h->seed);
+      h->env_offset, out, h->seed,
+      h->P.attitude_filter ? stash + size_t(kFinalRows + (h->final_params ? kFinalParamCols : 0)) * h->n_pad : nullptr);
   CUDA_TRY(cudaGetLastError());
   return UPKIE_B200_OK;
 }
@@ -1685,6 +1789,12 @@ int upkie_b200_set_state(void* handle, const float* state, void* stream) {
   }
   // the servo dropouts latch the state set
   if (h->P.servo_dropout) CUDA_TRY(servo_dropout_latch(h, ~0u, static_cast<cudaStream_t>(stream)));
+  // the attitude filter starts from the state set, without an error (before the history, which reports it)
+  if (h->P.attitude_filter) {
+    k_attitude_init<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(h->P, h->n, h->n_pad, h->state,
+                                                                                 false, 0.f, 0.f);
+    CUDA_TRY(cudaGetLastError());
+  }
   // the observation history restarts from the state set
   if (h->P.history) {
     k_history_fill<<<grid_of(h->n), 128, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -2038,8 +2148,14 @@ int upkie_b200_set_observation_delay_ticks(void* handle, const UpkieObservationD
   if (h->P.servo_noise && h->P.servo_dropout)
     return fail(UPKIE_B200_EINVAL, "set_observation_delay: not with both servo noise and servo dropouts (a delayed "
                                    "snapshot does not record which of its replies were held)");
+  if (h->P.attitude_filter && max_ticks > 1)
+    return fail(UPKIE_B200_EINVAL, "set_observation_delay_ticks: not more than one tick with an attitude filter (the "
+                                   "report of a deeper delay would need a ring of estimates)");
   CUDA_TRY(cudaSetDevice(h->device));
   CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the block
+  // the attitude filter: the sensed rows start from the state (below), and the report from the estimate
+  if (h->P.attitude_filter && !h->P.obs_delay)
+    CUDA_TRY(cudaMemcpy(h->att_rep, h->att_quat, size_t(4) * h->n_pad * sizeof(float), cudaMemcpyDeviceToDevice));
   const bool allocated = h->sense_rows != nullptr;
   if (alloc_sense_state(h)) return UPKIE_B200_ECUDA;  // a first allocation fills the rows from the state
   if (resize_sense_history(h, int(max_ticks))) return UPKIE_B200_ECUDA;
@@ -2560,6 +2676,152 @@ int upkie_b200_set_velocity_derate_state(void* handle, const uint32_t* count, co
   }
   CUDA_TRY(cudaMemcpyAsync(h->vlim_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
   CUDA_TRY(ring_cols(max_velocity, UPKIE_NJ, h->n, h->n_pad, h->vlim_max, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_attitude_filter(void* handle, const UpkieAttitudeFilter* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  h->final_valid = false;  // the stash's layout follows the spec (the terminal estimates' rows)
+  if (!spec) {
+    if (h->P.attitude_filter) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the per-env state
+      h->P.attitude_filter = nullptr;
+      float** bufs[] = {&h->att_gains, &h->att_quat, &h->att_bias, &h->att_rep, &h->att_vel};
+      for (float** b : bufs) {
+        cudaFree(*b);
+        *b = nullptr;
+      }
+      cudaFree(h->att_count);
+      h->att_count = nullptr;
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = attitude_filter_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  if (h->P.obs_delay && h->sense_ticks > 1)
+    return fail(UPKIE_B200_EINVAL, "set_attitude_filter: not with an observation delay of more than one tick (its "
+                                   "report would need a ring of estimates)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
+  const bool first = !h->P.attitude_filter;
+  if (first) {
+    const size_t col = size_t(h->n_pad) * sizeof(float);
+    CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->att_count), size_t(h->n) * sizeof(uint32_t)},
+                           {reinterpret_cast<void**>(&h->att_gains), 2 * col},
+                           {reinterpret_cast<void**>(&h->att_quat), 4 * col},
+                           {reinterpret_cast<void**>(&h->att_bias), 3 * col},
+                           {reinterpret_cast<void**>(&h->att_rep), 4 * col},
+                           {reinterpret_cast<void**>(&h->att_vel), 3 * col}}));
+  }
+  if (!h->att_dev) CUDA_TRY(cudaMalloc(&h->att_dev, sizeof(AttitudeFilter)));
+  AttitudeFilter A;
+  std::memset(&A, 0, sizeof(A));
+  A.spec = *spec;
+  quat_from_rot(h->P.Rbi, A.qbi);
+  A.count = h->att_count;
+  A.gains = h->att_gains;
+  A.quat = h->att_quat;
+  A.bias = h->att_bias;
+  A.rep = h->att_rep;
+  A.vel = h->att_vel;
+  A.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->att_dev, &A, sizeof(A), cudaMemcpyHostToDevice));
+  h->P.attitude_filter = h->att_dev;
+  h->att_spec = *spec;
+  if (first) {  // every env: the upper gains, the true orientation and b = 0 until its next reset
+    k_attitude_init<<<grid_of(h->n), 128>>>(h->P, h->n, h->n_pad, h->state, true, spec->kp_high, spec->ki_high);
+    CUDA_TRY(cudaGetLastError());
+  }
+  CUDA_TRY(cudaDeviceSynchronize());
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_attitude_filter_state(void* handle, uint32_t* count, float* gains, float* quat, float* bias,
+                                         void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !gains || !quat || !bias)
+    return fail(UPKIE_B200_EINVAL, "get_attitude_filter_state: invalid argument");
+  if (!h->P.attitude_filter)
+    return fail(UPKIE_B200_EINVAL, "get_attitude_filter_state: no attitude filter is set (upkie_b200_set_attitude_filter)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemcpyAsync(count, h->att_count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_rows(h->att_gains, 2, h->n, h->n_pad, gains, s));
+  CUDA_TRY(ring_rows(h->att_quat, 4, h->n, h->n_pad, quat, s));
+  CUDA_TRY(ring_rows(h->att_bias, 3, h->n, h->n_pad, bias, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_attitude_filter_state(void* handle, const uint32_t* count, const float* gains, const float* quat,
+                                         const float* bias, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !gains || !quat || !bias)
+    return fail(UPKIE_B200_EINVAL, "set_attitude_filter_state: invalid argument");
+  if (!h->P.attitude_filter)
+    return fail(UPKIE_B200_EINVAL, "set_attitude_filter_state: no attitude filter is set (upkie_b200_set_attitude_filter)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // read back (after the caller's work on the stream) and checked here: finite values, unit quaternions, gains within
+  // the caps of a spec (not the spec in force: a narrower spec keeps each env's gains until its next reset)
+  const size_t n = size_t(h->n);
+  std::vector<float> g(n * 2), q(n * 4), b(n * 3);
+  CUDA_TRY(cudaMemcpyAsync(g.data(), gains, g.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaMemcpyAsync(q.data(), quat, q.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaMemcpyAsync(b.data(), bias, b.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (size_t i = 0; i < n; ++i) {
+    const float kp = g[2 * i], ki = g[2 * i + 1];
+    if (!std::isfinite(kp) || !std::isfinite(ki) || !(kp >= 0.f) || !(double(kp) * double(h->P.h) <= 0.5) ||
+        !(ki >= 0.f) || !(ki <= 10.f))
+      return fail(UPKIE_B200_EINVAL, "set_attitude_filter_state: every gain must be finite, 0 <= kp with "
+                                     "kp * (dt / nb_substeps) <= 0.5, and 0 <= ki <= 10");
+    double norm2 = 0.0;
+    for (int r = 0; r < 4; ++r) {
+      const float v = q[4 * i + r];
+      if (!std::isfinite(v)) return fail(UPKIE_B200_EINVAL, "set_attitude_filter_state: every value must be finite");
+      norm2 += double(v) * double(v);
+    }
+    if (!(std::fabs(std::sqrt(norm2) - 1.0) <= 1e-5))
+      return fail(UPKIE_B200_EINVAL, "set_attitude_filter_state: every quaternion must be unit (within 1e-5)");
+    for (int r = 0; r < 3; ++r)
+      if (!std::isfinite(b[3 * i + r]))
+        return fail(UPKIE_B200_EINVAL, "set_attitude_filter_state: every value must be finite");
+  }
+  CUDA_TRY(cudaMemcpyAsync(h->att_count, count, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_cols(gains, 2, h->n, h->n_pad, h->att_gains, s));
+  CUDA_TRY(ring_cols(quat, 4, h->n, h->n_pad, h->att_quat, s));
+  CUDA_TRY(ring_cols(bias, 3, h->n, h->n_pad, h->att_bias, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_attitude_filter_report(void* handle, float* quat, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !quat) return fail(UPKIE_B200_EINVAL, "get_attitude_filter_report: invalid argument");
+  if (!h->P.attitude_filter)
+    return fail(UPKIE_B200_EINVAL, "get_attitude_filter_report: no attitude filter is set (upkie_b200_set_attitude_filter)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(ring_rows(h->att_rep, 4, h->n, h->n_pad, quat, static_cast<cudaStream_t>(stream)));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_attitude_filter_report(void* handle, const float* quat, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !quat) return fail(UPKIE_B200_EINVAL, "set_attitude_filter_report: invalid argument");
+  if (!h->P.attitude_filter)
+    return fail(UPKIE_B200_EINVAL, "set_attitude_filter_report: no attitude filter is set (upkie_b200_set_attitude_filter)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  std::vector<float> q(size_t(h->n) * 4);
+  CUDA_TRY(cudaMemcpyAsync(q.data(), quat, q.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  for (int i = 0; i < h->n; ++i) {
+    double norm2 = 0.0;
+    for (int r = 0; r < 4; ++r) norm2 += double(q[4 * size_t(i) + r]) * double(q[4 * size_t(i) + r]);
+    if (!(std::fabs(std::sqrt(norm2) - 1.0) <= 1e-5))  // (NaN fails too)
+      return fail(UPKIE_B200_EINVAL, "set_attitude_filter_report: every quaternion must be unit (within 1e-5)");
+  }
+  CUDA_TRY(ring_cols(quat, 4, h->n, h->n_pad, h->att_rep, s));
   return UPKIE_B200_OK;
 }
 

@@ -804,6 +804,80 @@ def imu_misalignment_spec(misalignment, spine_mode: bool = False, joint_limits: 
     return _abi.UpkieImuMisalignment(*bounds)
 
 
+def attitude_filter_spec(attitude_filter, spine_mode: bool = False, joint_limits: Union[bool, int] = True,
+                         body_contacts: Union[bool, int] = False,
+                         dt: Optional[float] = None, nb_substeps: Optional[int] = None,
+                         obs_delay_ticks: int = 1) -> Optional[_abi.UpkieAttitudeFilter]:
+    """``UpkieAttitudeFilter`` (``UpkieSim.set_attitude_filter``) from a dict with keys ``kp`` (1/s, required),
+    ``ki`` (1/s^2), ``roll`` and ``pitch`` (rad, the initial estimate error about the base axes), each a fixed value
+    or a ``(low, high)`` range every reset draws the env's value from; a missing optional key is 0. Raises
+    ``UpkieException`` on an unknown key, a bound that is not a finite number, ``low > high``, ``kp < 0`` or
+    ``kp_high * dt / nb_substeps > 0.5`` (when ``dt`` and ``nb_substeps`` are given), ``ki < 0`` or ``ki > 10``,
+    ``|roll|`` or ``|pitch| > pi/4``, ``spine_mode`` (whose spine models its own IMU), no joint limits,
+    ``body_contacts`` (the filter runs in the kernels of the observation delay) and an observation delay of more than
+    one tick."""
+    if attitude_filter is None:
+        return None
+    if not isinstance(attitude_filter, dict) or "kp" not in attitude_filter:
+        raise UpkieException(f"attitude_filter: expected a dict with keys kp, ki, roll and pitch, got "
+                             f"{attitude_filter!r}")
+    unknown = sorted(set(attitude_filter) - {"kp", "ki", "roll", "pitch"})
+    if unknown:
+        raise UpkieException(f"attitude_filter: unknown key(s) {unknown}, expected kp, ki, roll and pitch")
+    bounds = {}
+    for key in ("kp", "ki", "roll", "pitch"):
+        r = attitude_filter.get(key, 0.0)
+        if isinstance(r, (int, float, np.integer, np.floating)):
+            lo, hi = r, r
+        else:
+            try:
+                lo, hi = r
+            except (TypeError, ValueError):
+                raise UpkieException(f"attitude_filter: {key}: expected a value or a (low, high) pair, got {r!r}") \
+                    from None
+        try:
+            lo, hi = np.float32(lo), np.float32(hi)
+        except (TypeError, ValueError):
+            raise UpkieException(f"attitude_filter: {key}: expected numbers, got ({lo!r}, {hi!r})") from None
+        if not (np.isfinite(lo) and np.isfinite(hi)):
+            raise UpkieException(f"attitude_filter: {key}: expected finite bounds, got ({lo}, {hi})")
+        if lo > hi:
+            raise UpkieException(f"attitude_filter: {key}: expected low <= high, got ({lo}, {hi})")
+        bounds[key] = (lo, hi)
+    if bounds["kp"][0] < 0:
+        raise UpkieException(f"attitude_filter: kp: expected gains >= 0, got {bounds['kp']}")
+    if dt is not None and nb_substeps is not None:
+        h = np.float32(np.float64(dt) / np.float64(nb_substeps))
+        if float(bounds["kp"][1]) * float(h) > _abi.ATTITUDE_FILTER_MAX_KP_H:
+            raise UpkieException(f"attitude_filter: kp: kp_high * (dt / nb_substeps) must stay <= "
+                                 f"{_abi.ATTITUDE_FILTER_MAX_KP_H}, got {bounds['kp'][1]} * {h}")
+    if bounds["ki"][0] < 0 or bounds["ki"][1] > np.float32(_abi.ATTITUDE_FILTER_MAX_KI):
+        raise UpkieException(f"attitude_filter: ki: expected 0 <= ki <= {_abi.ATTITUDE_FILTER_MAX_KI}, got "
+                             f"{bounds['ki']}")
+    for key in ("roll", "pitch"):
+        if max(abs(bounds[key][0]), abs(bounds[key][1])) > np.float32(_abi.ATTITUDE_FILTER_MAX_ERROR):
+            raise UpkieException(f"attitude_filter: {key}: expected errors within [-pi/4, pi/4] radians, got "
+                                 f"{bounds[key]}")
+    if spine_mode:
+        raise UpkieException("attitude_filter: spine_mode models its spine's own IMU; the filter is not available there")
+    if not joint_limits:
+        raise UpkieException("attitude_filter: needs joint_limits (the filter runs in the kernels with joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("attitude_filter: body_contacts has no attitude-filter kernels")
+    if obs_delay_ticks > 1:
+        raise UpkieException("attitude_filter: not with an observation delay of more than one tick (its report would "
+                             "need a ring of estimates)")
+    return _abi.UpkieAttitudeFilter(*(float(v) for key in ("kp", "ki", "roll", "pitch") for v in bounds[key]))
+
+
+def _set_attitude_filter(sim, spec: Optional[_abi.UpkieAttitudeFilter]) -> None:
+    if spec is None:
+        sim.set_attitude_filter(None)
+    else:
+        sim.set_attitude_filter((spec.kp_low, spec.kp_high), (spec.ki_low, spec.ki_high),
+                                (spec.roll_low, spec.roll_high), (spec.pitch_low, spec.pitch_high))
+
+
 _ENCODER_OFFSET_MAX = np.float32(0.5)  # the largest |bound|, radians (the C check compares float32 values)
 
 
@@ -1159,6 +1233,14 @@ class B200VectorEnv(VectorEnv):
     faster falls linearly to zero over the derate band, while a braking torque passes. The torque every env type
     observes is the derated one. The draws are keyed on the seed of ``reset(seed=s)``, which also restarts the draw
     counters of the envs it resets. ``set_velocity_derate`` changes or (``None``) stops it.
+
+    ``attitude_filter`` (a dict ``{"kp": ..., "ki": ..., "roll": ..., "pitch": ...}``, see ``attitude_filter_spec``)
+    makes every env report the orientation an attitude filter estimates from its simulated IMU, as the robot's spine
+    reads the pi3hat's filter: the IMU orientation, the base pitch and rotation, and the gyropod and pendulum pitch
+    carry the filter's convergence, its tilt error under acceleration and its drift from gyro bias, while the rates,
+    accelerations, physics and terminations do not. Every reset of an env draws its gains and an initial estimate error;
+    the draws are keyed on the seed of ``reset(seed=s)``, which also restarts the draw counters of the envs it resets.
+    ``set_attitude_filter`` changes or (``None``) stops it.
     """
 
     metadata: Dict[str, Any] = {"autoreset_mode": "disabled"}
@@ -1207,6 +1289,7 @@ class B200VectorEnv(VectorEnv):
         servo_noise: Optional[Dict[str, Any]] = None,
         velocity_derate: Optional[Dict[str, Any]] = None,
         velocity_derate_joints: Optional[Sequence[str]] = None,
+        attitude_filter: Optional[Dict[str, Any]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -1264,6 +1347,9 @@ class B200VectorEnv(VectorEnv):
                                        config.joint_limits, config.body_contacts)  # validated before any device
         noise_spec = servo_noise_spec(servo_noise, bool(config.spine_mode), config.joint_limits, config.body_contacts,
                                       sense_spec is not None, drop_spec is not None)  # validated before any device
+        att_spec = attitude_filter_spec(attitude_filter, bool(config.spine_mode), config.joint_limits,
+                                        config.body_contacts, 1.0 / frequency, config.nb_substeps,
+                                        self.max_delay_ticks if sense_spec is not None else 1)  # before any device
         vlim_spec = velocity_derate_spec(velocity_derate, velocity_derate_joints, bool(config.spine_mode),
                                          config.joint_limits, config.body_contacts)  # validated before any device
         # validated before any device is touched
@@ -1335,6 +1421,17 @@ class B200VectorEnv(VectorEnv):
             _set_servo_noise(self.sim, noise_spec)  # before the first reset, which draws every env's levels
         if vlim_spec is not None:
             _set_velocity_derate(self.sim, vlim_spec)  # before the first reset, which draws every env's limits
+        if att_spec is not None:
+            _set_attitude_filter(self.sim, att_spec)  # before the first reset, which draws every env's filter
+
+    def set_attitude_filter(self, attitude_filter) -> None:
+        """Report every env's orientation from an attitude filter on its IMU, with gains and an initial error drawn per
+        env (a dict, see ``attitude_filter_spec``); ``None`` turns the filter off. New ranges take effect at each env's
+        next reset; a first filter starts every env from its true orientation with the upper gains."""
+        sense = getattr(self.sim, "_observation_delay", None)
+        _set_attitude_filter(self.sim, attitude_filter_spec(
+            attitude_filter, bool(self.config.spine_mode), self.config.joint_limits, self.config.body_contacts,
+            float(self.config.dt), self.config.nb_substeps, self.max_delay_ticks if sense is not None else 1))
 
     def set_velocity_derate(self, velocity_derate, joints=None) -> None:
         """Limit the servos ``joints`` (names, None: those of ``max_velocity``) past a velocity drawn per env (a dict
@@ -1613,6 +1710,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_velocity_derate_state(count, vmax)
+            if self.sim.attitude_filter_spec is not None:
+                # and the attitude filter's draws
+                count, gains, quat, bias = self.sim.get_attitude_filter_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_attitude_filter_state(count, gains, quat, bias)
         rows = np.zeros((n, _abi.INIT_DIM), dtype=np.float32)
         for i in range(n):
             if mask is not None and not mask[i]:

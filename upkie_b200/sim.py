@@ -382,6 +382,74 @@ class UpkieSim:
         self._check_tensor(quat, (self.n, 4), name="quat")
         check(lib().upkie_b200_set_imu_misalignment_state(self._h, _ptr(count), _ptr(quat), self._stream()))
 
+    def set_attitude_filter(self, kp: Optional[Tuple[float, float]], ki: Tuple[float, float] = (0.0, 0.0),
+                            roll: Tuple[float, float] = (0.0, 0.0), pitch: Tuple[float, float] = (0.0, 0.0)) -> None:
+        """While ranges are set, each env runs an attitude filter on its simulated IMU (an explicit complementary filter
+        with gyro-bias estimation, once per substep; ``include/upkie_b200.h``), and every orientation-derived
+        observation (the IMU orientation, the base pitch and ``rotation_base_to_world``, the gyropod and pendulum
+        pitch) reports its estimate instead of the true orientation; the rates, accelerations, physics, terminations
+        and ``get_state`` are untouched. Every reset of an env draws its gains ``kp`` (1/s) and ``ki`` (1/s^2) and an
+        initial estimate error ``roll``, ``pitch`` (rad, about the base axes) from ``(low, high)`` ranges, keyed on the
+        auto-reset seed and the env's counter. ``kp=None`` turns the filter off. Setting ranges draws nothing: an env
+        of a handle without a filter starts from the true orientation with the upper gains until its next reset."""
+        if kp is None:
+            check(lib().upkie_b200_set_attitude_filter(self._h, None))
+            self._attitude_filter = None
+            return
+        spec = _abi.UpkieAttitudeFilter(*(float(v) for r in (kp, ki, roll, pitch) for v in r))
+        check(lib().upkie_b200_set_attitude_filter(self._h, C.byref(spec)))
+        self._attitude_filter = ((spec.kp_low, spec.kp_high), (spec.ki_low, spec.ki_high),
+                                 (spec.roll_low, spec.roll_high), (spec.pitch_low, spec.pitch_high))
+
+    @property
+    def attitude_filter_spec(self) -> Optional[Tuple[Tuple[float, float], ...]]:
+        """``((kp_low, kp_high), (ki_low, ki_high), (roll_low, roll_high), (pitch_low, pitch_high))`` in force, or
+        None."""
+        return getattr(self, "_attitude_filter", None)
+
+    def get_attitude_filter_state(self):
+        """Per-env attitude-filter state ``(count[N], gains[N, 2], quat[N, 4], bias[N, 3])``: the draw counters (int32
+        bits of uint32), the gains (kp, ki), the estimated IMU-to-world rotation (w, x, y, z) and the gyro-bias
+        estimate (rad/s, IMU frame)."""
+        if self.attitude_filter_spec is None:
+            raise UpkieException("no attitude filter is set (set_attitude_filter)")
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        gains = torch.empty((self.n, 2), dtype=torch.float32, device=self.device)
+        quat = torch.empty((self.n, 4), dtype=torch.float32, device=self.device)
+        bias = torch.empty((self.n, 3), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_attitude_filter_state(self._h, _ptr(count), _ptr(gains), _ptr(quat), _ptr(bias),
+                                                         self._stream()))
+        return count, gains, quat, bias
+
+    def set_attitude_filter_state(self, count: torch.Tensor, gains: torch.Tensor, quat: torch.Tensor,
+                                  bias: torch.Tensor) -> None:
+        """Set every env's draw counter, gains, estimate (unit within 1e-5) and bias estimate: a checkpoint."""
+        if self.attitude_filter_spec is None:
+            raise UpkieException("no attitude filter is set (set_attitude_filter)")
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(gains, (self.n, 2), name="gains")
+        self._check_tensor(quat, (self.n, 4), name="quat")
+        self._check_tensor(bias, (self.n, 3), name="bias")
+        check(lib().upkie_b200_set_attitude_filter_state(self._h, _ptr(count), _ptr(gains), _ptr(quat), _ptr(bias),
+                                                         self._stream()))
+
+    def get_attitude_filter_report(self) -> torch.Tensor:
+        """``[N, 4]`` the estimate (w, x, y, z, IMU to world) each env's observation reports under an observation delay:
+        that of the cycle its snapshot observed."""
+        if self.attitude_filter_spec is None:
+            raise UpkieException("no attitude filter is set (set_attitude_filter)")
+        out = torch.empty((self.n, 4), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_attitude_filter_report(self._h, _ptr(out), self._stream()))
+        return out
+
+    def set_attitude_filter_report(self, quat: torch.Tensor) -> None:
+        """Set every env's reported estimate (unit within 1e-5, see ``get_attitude_filter_report``): a checkpoint.
+        ``set_attitude_filter_state`` leaves it, as setting the estimate leaves an observation delay's snapshot."""
+        if self.attitude_filter_spec is None:
+            raise UpkieException("no attitude filter is set (set_attitude_filter)")
+        self._check_tensor(quat, (self.n, 4), name="quat")
+        check(lib().upkie_b200_set_attitude_filter_report(self._h, _ptr(quat), self._stream()))
+
     def set_encoder_offset(self, low: Optional[float], high: Optional[float] = None,
                            joints: Optional[Sequence[str]] = None) -> None:
         """While a range is set, each servo of ``joints`` (names, None: the four hip and knee joints) is zeroed off by
@@ -1040,6 +1108,12 @@ class UpkieSim:
         if self.velocity_derate_spec is not None:
             sd["velocity_derate"] = self.velocity_derate_spec
             sd["velocity_derate_count"], sd["velocity_derate_max_velocity"] = self.get_velocity_derate_state()
+        # the attitude filter: its ranges and the per-env state (absent without a spec)
+        if self.attitude_filter_spec is not None:
+            sd["attitude_filter"] = self.attitude_filter_spec
+            (sd["attitude_filter_count"], sd["attitude_filter_gains"], sd["attitude_filter_quat"],
+             sd["attitude_filter_bias"]) = self.get_attitude_filter_state()
+            sd["attitude_filter_report"] = self.get_attitude_filter_report()
         sd.update({
             "lag": self.get_lag() if self.config.spine_mode else None,  # spine mode: replies / IMU of the last cycles
             "state": self.get_state(), "episode": episode, "tick": tick, "pending_reset": pending, "error_flags": flags,
@@ -1052,6 +1126,9 @@ class UpkieSim:
 
     def load_state_dict(self, sd: dict) -> None:
         dev = self.device
+        # the attitude filter is off while the state and the observation delay are restored (set_state re-initialises
+        # its estimates, and a handle with a filter refuses a delay of more than one tick), and restored last
+        self.set_attitude_filter(None)
         self.set_state(sd["state"].to(dev))
         if sd.get("lag") is not None:
             self.set_lag(sd["lag"].to(dev))
@@ -1183,6 +1260,14 @@ class UpkieSim:
             self.set_servo_noise_state(*(sd[k].to(dev).contiguous() for k in ("servo_noise_count", "servo_noise_sigma")))
             if sd.get("servo_noise_mark") is not None:
                 self.set_servo_noise_mark(sd["servo_noise_mark"].to(dev).contiguous())
+        # the attitude filter (off above), after the state; a checkpoint without it (or written before it existed)
+        # leaves it off
+        att = sd.get("attitude_filter")
+        if att is not None:
+            self.set_attitude_filter(*att)
+            self.set_attitude_filter_state(*(sd[k].to(dev).contiguous() for k in (
+                "attitude_filter_count", "attitude_filter_gains", "attitude_filter_quat", "attitude_filter_bias")))
+            self.set_attitude_filter_report(sd["attitude_filter_report"].to(dev).contiguous())
         self.set_autoreset(*sd["autoreset"])
 
     def error_flags(self) -> torch.Tensor:
