@@ -810,9 +810,13 @@ UPKIE_HD void contact_solve_ten_rows(const SimParams& P, RobotState& S, const Le
   for (int k = 0; k < 4; ++k) S.lam_t[k] = lam[6 + k];
   f2 F[6];
   {
+    // F = sum_d lam_d J_d = (Pc x w, w) with w the wheels' total impulse: J itself need not outlive the Delassus matrix
     const f2 ln = mk2(lam[4], lam[5]), l1 = mk2(lam[6], lam[8]), l2 = mk2(lam[7], lam[9]);
+    f2 w[3];
 #pragma unroll
-    for (int i = 0; i < 6; ++i) F[i] = fma2(ln, J[0][i], fma2(l1, J[1][i], mul2(l2, J[2][i])));
+    for (int i = 0; i < 3; ++i) w[i] = fma2(ln, bc2(zb[i]), mul2(sw, fma2(l1, bc2(t1[i]), mul2(l2, bc2(t2[i])))));
+    cross3_2(Pc, w, &F[0]);
+    F[3] = w[0]; F[4] = w[1]; F[5] = w[2];
   }
   f2 u[3], nptop[6];
   legs_impulse_up_general(P, lc, F, mul2(dirH, mk2(lam[0], lam[2])), mul2(dirK, mk2(lam[1], lam[3])), u, nptop);
@@ -1521,8 +1525,13 @@ UPKIE_HD void physics_substep_paired(const SimParams& P, RobotState& S, const fl
     f2 F[6];
     {
       const f2 ln = mk2(lam[0], lam[1]), l1 = mk2(lam[2], lam[4]), l2 = mk2(lam[3], lam[5]);
+      // F = (Pc x w, w) in the same order as contact_solve_ten_rows, which must give a robot without a limit row the
+      // same bits as this solver
+      f2 w[3];
 #pragma unroll
-      for (int i = 0; i < 6; ++i) F[i] = fma2(ln, J[0][i], fma2(l1, J[1][i], mul2(l2, J[2][i])));
+      for (int i = 0; i < 3; ++i) w[i] = fma2(ln, bc2(zb[i]), mul2(sw, fma2(l1, bc2(t1[i]), mul2(l2, bc2(t2[i])))));
+      cross3_2(Pc, w, &F[0]);
+      F[3] = w[0]; F[4] = w[1]; F[5] = w[2];
     }
     f2 u[3], nptop[6];
     legs_impulse_up(P, lc, F, u, nptop);
