@@ -1142,6 +1142,51 @@ int upkie_b200_set_attitude_filter_state(void* handle, const uint32_t* count, co
 int upkie_b200_get_attitude_filter_report(void* handle, float* quat, void* stream);
 int upkie_b200_set_attitude_filter_report(void* handle, const float* quat, void* stream);
 
+/* ---- Servo torque-constant errors (pybullet_backend.py:457-459, moteus current loop) -----------------------------
+ * An addition to ABI 8: no existing layout, constant or signature changed. The reference applies every commanded
+ * torque exactly and reports it as measured. A moteus servo closes its loop on current and converts it to torque
+ * through a nominal torque constant, and it reports that same estimate; the torque its joint receives differs by the
+ * constant's error and the gearbox losses, from motor to motor. While a spec is set each joint of each env delivers a
+ * scale s_ij of the torque its servo commands and reports ("motor strength" in legged-robot RL, where (0.9, 1.1) is a
+ * usual range; no measured tolerance of the Upkie's servos is known to this project).
+ * - Draw per reset: at every reset of env i (both fused auto-resets, upkie_b200_reset with or without a mask or host
+ *   rows) a per-env counter k goes up by 1, and Philox4x32-10 with key seed (upkie_b200_set_autoreset) and counters
+ *   (g, 2^50 | k << 4 | b), b = 0, 1, g = env_offset + i, gives joint j word j % 4 of block b = j / 4:
+ *   s_ij = min(low_j + fl(fl(high_j - low_j) * u(w)), high_j), u(w) = (w >> 8) / 2^24 (the servo dropouts' map). Every
+ *   joint's word is drawn whatever the mask, and a joint outside joint_mask stores exactly 1, so that changing the mask
+ *   changes no other joint's draw. Tag bit 50 alone keeps these counters apart from every tag listed above (63 ... 51)
+ *   and from the cycle counters below bit 52, which carry bits 59 | 58 or 55 | 54.
+ * - Law: in every substep, t is the torque of the servo law as without a spec (PD law, joint friction and control
+ *   noise, clipped to +-maximum_torque, then the velocity limit's derate if one is set). The torque reply is t (what
+ *   the servo believes it applies; torque measurement noise added on top of it), and the physics integrates
+ *   fl(s_ij * t) (rounded once: never contracted into the substep's next add). External forces and pushes are added
+ *   after the scale, unscaled; the action delay's command is scaled like any other; the zero-torque substep of a reset
+ *   stays zero. Consequences of keeping the reference's law: the joint friction, folded into the command before the
+ *   clip (pybullet_backend.py:537-552), is scaled with it, and the velocity derate acts on the servo's side, so that
+ *   its cap is s_ij * f * tau_max in delivered torque.
+ * - Not affected: every observation but through the physics (the torque replies of step rows, upkie_b200_spine_obs,
+ *   history entries, final and reset observations, and the UPKIE_ST_TORQUE columns of upkie_b200_get_state all report
+ *   t), terminations and auto-resets, and the stash of terminal states (whose layout does not change).
+ * Setting a spec draws nothing: each env keeps the scales of the joints that stay in the mask until its next reset;
+ * the joints a spec adds to the mask (every joint of the first spec) hold 1 until then, and the joints it drops store
+ * 1. NULL turns the feature off (the per-env state is freed once the device is idle). Per-env state
+ * (get/set_torque_scale_state, for checkpoints and fixed scales; device pointers): count[N] and scale[N][6];
+ * UPKIE_B200_EINVAL without a spec, for a value of a joint of the mask in force that is not finite or outside (0, 2],
+ * and for a value other than exactly 1 of a joint outside it.
+ * Rejected with UPKIE_B200_EINVAL, the previous spec kept: a bound that is not finite, low <= 0, low > high or
+ * high > 2 on a joint of the mask, a joint_mask of zero or with bits above 5, reserved != 0, spine_mode (whose spine
+ * applies its own torque law), joint_limits == 0 and body_contacts (it runs in the observation-delay kernels).
+ * upkie_b200_set_config rejects joint_limits = 0 and body_contacts while a spec is set; the in-kernel rollout
+ * transports reject a handle with one. The set call waits for the device. */
+typedef struct UpkieTorqueScale {
+  float scale_low[6], scale_high[6]; /* dimensionless, range of each joint's delivered-torque scale (UPKIE_NJ order) */
+  uint32_t joint_mask;               /* bit j: joint j's delivered torque is scaled */
+  uint32_t reserved;                 /* 0 */
+} UpkieTorqueScale;
+int upkie_b200_set_torque_scale(void* handle, const UpkieTorqueScale* spec);
+int upkie_b200_get_torque_scale_state(void* handle, uint32_t* count, float* scale, void* stream);
+int upkie_b200_set_torque_scale_state(void* handle, const uint32_t* count, const float* scale, void* stream);
+
 /* ---- Spine-rate observation history (HistoryObserver.h, upkie/cpp/observers/) ----------------------------------
  * An addition to ABI 8: no existing layout, constant or signature changed. The step runs nb_substeps substeps per
  * tick, each one cycle of a 1 kHz spine at the default 200 Hz / 5 substeps. A history makes each env report the last

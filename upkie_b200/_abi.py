@@ -498,6 +498,22 @@ ATTITUDE_FILTER_MAX_KI = 10.0  # 1/s^2, the largest ki_high
 ATTITUDE_FILTER_MAX_ERROR = 0.78539816  # rad, the largest |roll| or |pitch| bound of the initial error (pi/4)
 
 
+class UpkieTorqueScale(C.Structure):
+    """``UpkieTorqueScale`` of include/upkie_b200.h: the range of each joint's delivered-torque scale, drawn per env at
+    every reset (dimensionless, UPKIE_NJ order): the physics integrates the scale times the torque the servo commands
+    and reports."""
+
+    _fields_ = [
+        ("scale_low", C.c_float * 6),
+        ("scale_high", C.c_float * 6),
+        ("joint_mask", C.c_uint32),
+        ("reserved", C.c_uint32),
+    ]
+
+
+TORQUE_SCALE_MAX = 2.0  # the largest scale_high (and scale a state may hold)
+
+
 MAX_HISTORY = 64  # UPKIE_MAX_HISTORY: the most entries an observation history reports
 MAX_HISTORY_CHANNELS = 16  # UPKIE_MAX_HISTORY_CHANNELS: the most spine columns it records
 

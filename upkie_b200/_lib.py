@@ -81,6 +81,9 @@ SYMBOLS = {
     "upkie_b200_set_attitude_filter_state": (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "upkie_b200_get_attitude_filter_report": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_set_attitude_filter_report": (C.c_int, [_vp, _vp, _vp]),
+    "upkie_b200_set_torque_scale": (C.c_int, [_vp, C.POINTER(_abi.UpkieTorqueScale)]),
+    "upkie_b200_get_torque_scale_state": (C.c_int, [_vp, _vp, _vp, _vp]),
+    "upkie_b200_set_torque_scale_state": (C.c_int, [_vp, _vp, _vp, _vp]),
     "upkie_b200_set_history": (C.c_int, [_vp, C.POINTER(_abi.UpkieHistory)]),
     "upkie_b200_get_history": (C.c_int, [_vp, _vp, _vp]),
     "upkie_b200_history_entries": (C.c_int, [_vp, C.POINTER(C.c_int)]),

@@ -273,6 +273,7 @@ inline int make_sim_params(const UpkieModel& m, const UpkieSimConfig& c, SimPara
   P.servo_noise = nullptr;
   P.velocity_derate = nullptr;
   P.attitude_filter = nullptr;
+  P.torque_scale = nullptr;
   return 0;
 }
 
@@ -480,6 +481,40 @@ inline const char* velocity_derate_spec_error(const UpkieVelocityDerate& s, cons
     return "set_velocity_derate: needs joint_limits != 0 (the limits run in the observation-delay kernels)";
   if (P.spine_mode) return "set_velocity_derate: spine_mode applies the spine's own torque law";
   if (P.body_contacts) return "set_velocity_derate: body_contacts has no velocity-limit kernels";
+  return nullptr;
+}
+
+// Why a handle with parameters P refuses a torque-scale spec (upkie_b200_set_torque_scale), null when it takes it: every
+// bound finite, and on a joint of the mask 0 < low <= high <= 2
+inline const char* torque_scale_spec_error(const UpkieTorqueScale& s, const SimParams& P) {
+  if (s.joint_mask == 0 || (s.joint_mask >> UPKIE_NJ) != 0)
+    return "set_torque_scale: joint_mask must select joints of bits 0 .. 5, at least one";
+  if (s.reserved != 0) return "set_torque_scale: reserved must be 0";
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!std::isfinite(s.scale_low[j]) || !std::isfinite(s.scale_high[j]))
+      return "set_torque_scale: every bound must be finite";
+    if (!((s.joint_mask >> j) & 1u)) continue;
+    if (!(s.scale_low[j] > 0.f && s.scale_low[j] <= s.scale_high[j] && s.scale_high[j] <= 2.f))
+      return "set_torque_scale: 0 < scale_low <= scale_high <= 2 required on every joint of the mask";
+  }
+  if (P.joint_limits == 0)
+    return "set_torque_scale: needs joint_limits != 0 (the scale runs in the observation-delay kernels)";
+  if (P.spine_mode) return "set_torque_scale: spine_mode applies the spine's own torque law";
+  if (P.body_contacts) return "set_torque_scale: body_contacts has no torque-scale kernels";
+  return nullptr;
+}
+
+// Why per-env torque scales v[n][UPKIE_NJ] are refused under the mask in force (upkie_b200_set_torque_scale_state),
+// null when they are taken: a scale in (0, 2] on every joint of the mask, exactly 1 on every other joint
+inline const char* torque_scale_state_error(uint32_t joint_mask, const float* v, size_t n) {
+  for (size_t k = 0; k < n * UPKIE_NJ; ++k) {
+    if ((joint_mask >> (k % UPKIE_NJ)) & 1u) {
+      if (!(v[k] > 0.f && v[k] <= 2.f))  // (NaN fails too)
+        return "set_torque_scale_state: every scale of a joint of joint_mask must be in (0, 2]";
+    } else if (v[k] != 1.f) {
+      return "set_torque_scale_state: a joint outside joint_mask must have a scale of exactly 1";
+    }
+  }
   return nullptr;
 }
 

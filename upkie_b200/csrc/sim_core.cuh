@@ -166,6 +166,9 @@ struct SimParams {
   // kernels of FAM_SENSE (step_family.h), k_reset, k_spine_obs, k_reset_obs, k_history_fill and k_attitude_init only.
   // Appended last.
   const struct AttitudeFilter* attitude_filter;
+  // servo torque-constant errors (upkie_b200_set_torque_scale): the handle's device block, null = off. Read by the step
+  // kernels of FAM_SENSE (step_family.h) and k_reset only. Appended last.
+  const struct TorqueScale* torque_scale;
 };
 
 // Column k of env i's row of the per-env parameter table (read where it is used, through the read-only cache: the
@@ -1058,6 +1061,41 @@ UPKIE_HD float velocity_derate_joint(const VelocityDerate& V, int i, int j, floa
                                 tau_max);
 }
 
+// ---- Servo torque-constant errors (upkie_b200_set_torque_scale, pybullet_backend.py:457-459) ----
+// The handle's device block: the spec and the per-env state (include/upkie_b200.h): count[i] = k, the number of the
+// env's last draw, and scale = s_i, each joint's delivered-torque scale (exactly 1 outside the mask), [UPKIE_NJ][stride]
+// structure-of-arrays like the state, env i in column i. The draws are at the end of this file.
+struct TorqueScale {
+  UpkieTorqueScale spec;
+  uint32_t* count;
+  float* scale;
+  int stride;
+};
+
+// An env's six scales, as the substeps of a tick hold them
+struct Scale6 {
+  float s[UPKIE_NJ];
+};
+
+// Env i's scales through load(j) (its column of the per-env state)
+template <typename Load>
+UPKIE_HD Scale6 torque_scale_load(Load load) {
+  Scale6 o;
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) o.s[j] = load(j);
+  return o;
+}
+
+// The torque a joint receives when its servo applies t under the scale s: fl(s * t), one rounding. On the device the
+// product is __fmul_rn, which fast-math contraction never folds into the substep's next add.
+UPKIE_HD float torque_scale_apply(float s, float t) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rn(s, t);
+#else
+  return s * t;
+#endif
+}
+
 // Derived observation quantities (pybullet_backend.py:333-490). Updates the
 // IMU finite-difference state exactly once per call, as get_spine_observation.
 UPKIE_HD void observe_update(const SimParams& P, RobotState& S) {
@@ -1200,12 +1238,15 @@ UPKIE_HD void servo_substep(const SimParams& P, RobotState& S, const float a[UPK
                             const NoiseCtx* nz = nullptr, int sub = 0, const ExtForces* ext = nullptr,
                             int limits = 0, BodyRecOut rec = BodyRecOut{nullptr, 0}, int env = -1,
                             const ExtPush* push = nullptr, const VelocityDerate* derate = nullptr,
-                            int derate_env = 0) {
+                            int derate_env = 0, const Scale6* tscale = nullptr) {
   // `env`: this robot's column of the per-env parameter table; env < 0 (the default, and a constant in the
   // instantiations that never run with a table) compiles the table reads out. Its values are read where they are used, under a uniform branch
   // on the table pointer; the arithmetic is the same for the config's values and the table's.
   // `derate` (non-null in every lane of a FAM_SENSE launch with velocity limits; a null constant elsewhere, which
   // compiles the law out): the servo velocity limits of env `derate_env`, read from its column in every substep.
+  // `tscale` (likewise, for a FAM_SENSE launch with torque scales): the env's six delivered-torque scales, loaded once
+  // per tick (exactly 1 outside the mask, and fl(1 t) = t). The reply S.torque stays the servo's t; the physics
+  // integrates fl(s t).
   const bool table = env >= 0 && P.env_params != nullptr;
   float tau[6];
   float noise[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -1227,7 +1268,7 @@ UPKIE_HD void servo_substep(const SimParams& P, RobotState& S, const float a[UPK
                            aj[UPKIE_ACT_VELOCITY], aj[UPKIE_ACT_KP_SCALE], aj[UPKIE_ACT_KD_SCALE],
                            aj[UPKIE_ACT_MAXIMUM_TORQUE], noise[j]);
     if (derate) t = velocity_derate_joint(*derate, derate_env, j, S.qd[j], t, P.tau_max[j]);
-    tau[j] = zero_torque ? 0.f : t;
+    tau[j] = zero_torque ? 0.f : (tscale ? torque_scale_apply(tscale->s[j], t) : t);
     if (!zero_torque) S.torque[j] = t;
   }
   if (limits != 0) {
@@ -2563,7 +2604,8 @@ UPKIE_HD void history_fill_noise(const History& H, const SimParams& P, const Rob
 // bit 52 of the high counter word, the per-reset draws of v_i, (k << 4) | b below bit 36: never set by
 // sample_init_state (below 2^34), the noise (below bit 42), the reset randomisation (bit 63), the pushes (62), the
 // action delay (61), the observation delay (60), the servo dropouts (59, and 59 | 58, below bit 52 otherwise), the IMU
-// misalignment (57), the encoder offsets (56) or the servo noise (55, 55 | 54 below bit 52, and 55 | 54 | 53)
+// misalignment (57), the encoder offsets (56), the servo noise (55, 55 | 54 below bit 52, and 55 | 54 | 53), the
+// attitude filter (51 alone) or the torque scales (50 alone)
 constexpr uint64_t kVelocityDerateTag = uint64_t(1) << 52;
 
 struct Vmax6 {
@@ -2602,6 +2644,46 @@ UPKIE_HD void velocity_derate_reset(const VelocityDerate& V, uint64_t seed, uint
   for (int j = 0; j < UPKIE_NJ; ++j) col[size_t(j) * stride] = o.v[j];
 }
 
+// ---- Servo torque-constant errors: the draws (upkie_b200_set_torque_scale; the block and the law above servo_substep) ----
+// bit 50 of the high counter word alone, the per-reset draws of s_i, (k << 4) | b below bit 36: never set by
+// sample_init_state (below 2^34) or the noise (below bit 42); every other tag sets a bit above 50 (the reset
+// randomisation 63, the pushes 62, the action delay 61, the observation delay 60, the servo dropouts 59 and 59 | 58, the
+// IMU misalignment 57, the encoder offsets 56, the servo noise 55, 55 | 54 and 55 | 54 | 53, the velocity limits 52,
+// the attitude filter 51)
+constexpr uint64_t kTorqueScaleTag = uint64_t(1) << 50;
+
+// Draw k of the env of global index g: word j % 4 of the block of counter j / 4 gives joint j's scale, push_value's
+// exact form (the map of the servo dropouts). Every joint's word is drawn whatever the mask, and a joint outside it
+// gets exactly 1, so that the mask changes no other joint's draw.
+UPKIE_HD Scale6 torque_scale_draw(const UpkieTorqueScale& s, uint64_t seed, uint64_t g, uint32_t k) {
+  Scale6 o;
+#pragma unroll
+  for (int b = 0; b < 2; ++b) {
+    const Philox4 r = philox4x32_10(g, kTorqueScaleTag | (uint64_t(k) << 4) | uint64_t(b), seed);
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const int j = 4 * b + w;
+      if (j < UPKIE_NJ)
+        o.s[j] = ((s.joint_mask >> j) & 1u) ? push_value(r.v[w], s.scale_low[j], s.scale_high[j]) : 1.f;
+    }
+  }
+  return o;
+}
+
+// A reset of env i (the step kernels' fused resets, k_reset): the next draw, stored. The block's fields are copied
+// before the first store, as servo_dropout_reset.
+UPKIE_HD void torque_scale_reset(const TorqueScale& T, uint64_t seed, uint64_t g, int i) {
+  const UpkieTorqueScale spec = T.spec;
+  uint32_t* const count = T.count;
+  float* const col = T.scale + size_t(i);
+  const size_t stride = size_t(T.stride);
+  const uint32_t k = count[i] + 1u;
+  count[i] = k;
+  const Scale6 o = torque_scale_draw(spec, seed, g, k);
+#pragma unroll
+  for (int j = 0; j < UPKIE_NJ; ++j) col[size_t(j) * stride] = o.s[j];
+}
+
 // ---- IMU attitude estimation (upkie_b200_set_attitude_filter, Pi3HatInterface.cpp:151-169) ----
 // The handle's device block: the spec and the per-env state (include/upkie_b200.h), [rows][stride] structure-of-arrays
 // like the state, env i in column i: count[i] = k, the number of the env's last draw; gains (kp, ki); quat, the
@@ -2623,7 +2705,8 @@ struct AttitudeFilter {
 // bit 51 of the high counter word alone, the per-reset draws, (k << 4) below bit 36: never set by sample_init_state
 // (below 2^34) or the noise (below bit 42); every other tag sets a bit above 51 (the reset randomisation 63, the pushes
 // 62, the action delay 61, the observation delay 60, the servo dropouts 59 and 59 | 58, the IMU misalignment 57, the
-// encoder offsets 56, the servo noise 55, 55 | 54 and 55 | 54 | 53, the velocity limits 52)
+// encoder offsets 56, the servo noise 55, 55 | 54 and 55 | 54 | 53, the velocity limits 52), except the torque
+// scales' bit 50 alone, below it
 constexpr uint64_t kAttitudeFilterTag = uint64_t(1) << 51;
 
 struct AttitudeDraw {

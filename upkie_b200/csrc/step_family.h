@@ -27,6 +27,7 @@ enum {
   FAM_BODY_DELAY = 9, // FAM_BODY_PUSH + action delay
   FAM_SENSE = 10,     // FAM_DELAY + observation delay + observation history + servo reply dropouts + IMU misalignment
                       // + encoder offsets + servo measurement noise + servo velocity limits + attitude filter
+                      // + servo torque scales
   kNumFamilies = 11
 };
 
@@ -105,6 +106,8 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "velocity limits have no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.attitude_filter)
     no = "the attitude filter has no in-kernel rollout transport (use upkie_b200_step with compact rows)";
+  else if (in_kernel && P.torque_scale)
+    no = "torque scales have no in-kernel rollout transport (use upkie_b200_step with compact rows)";
   else if (in_kernel && P.max_episode_steps > 0)
     no = "max_episode_steps has no in-kernel rollout transport: it does not carry truncated (use upkie_b200_step with "
          "compact rows)";
@@ -162,6 +165,12 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
     no = "the attitude filter needs joint_limits != 0";
   else if (P.attitude_filter && P.body_contacts)
     no = "the attitude filter has no body-contact kernels";
+  else if (P.torque_scale && P.spine_mode)
+    no = "torque scales: spine_mode applies the spine's own torque law";
+  else if (P.torque_scale && P.joint_limits == 0)
+    no = "torque scales need joint_limits != 0";
+  else if (P.torque_scale && P.body_contacts)
+    no = "torque scales have no body-contact kernels";
   if (no) {
     *why = no;
     return -1;
@@ -170,10 +179,10 @@ inline int step_family(const SimParams& P, bool ext, int mode, int transport, co
   // the observation-delay family carries the action delay and the pushes too (runtime-uniform branches on
   // P.action_delay and P.push), the observation history (P.history), the servo dropouts (P.servo_dropout), the IMU
   // misalignment (P.imu_misalign), the encoder offsets (P.encoder_offset), the servo noise (P.servo_noise) and the
-  // servo velocity limits (P.velocity_derate) and the attitude filter (P.attitude_filter), by the same rule; the set
-  // calls reject spine mode, no limits and body contacts
+  // servo velocity limits (P.velocity_derate), the attitude filter (P.attitude_filter) and the torque scales
+  // (P.torque_scale), by the same rule; the set calls reject spine mode, no limits and body contacts
   if (P.obs_delay || P.history || P.servo_dropout || P.imu_misalign || P.encoder_offset || P.servo_noise ||
-      P.velocity_derate || P.attitude_filter)
+      P.velocity_derate || P.attitude_filter || P.torque_scale)
     return FAM_SENSE;
   // the delay families carry the pushes too (a runtime-uniform branch on P.push); the set calls reject spine mode and
   // no limits

@@ -290,6 +290,19 @@ __device__ __noinline__ void derate_reset_lane(const SimParams& P, uint64_t seed
   velocity_derate_reset(*P.velocity_derate, seed, g, i);
 }
 
+// The torque scales (F.sense kernels, P.torque_scale set): env i's s_i, loaded once per lane (coherent loads, as
+// tilt_load_lane) and held through the tick's substeps, and a reset's next draw, stored (out of line, as
+// tilt_reset_lane)
+__device__ __forceinline__ Scale6 tscale_load_lane(const SimParams& P, int i) {
+  const TorqueScale& T = *P.torque_scale;
+  const float* const col = T.scale + size_t(i);
+  const size_t stride = size_t(T.stride);
+  return torque_scale_load([&](int j) { return __ldcg(col + size_t(j) * stride); });
+}
+__device__ __noinline__ void tscale_reset_lane(const SimParams& P, uint64_t seed, uint64_t g, int i) {
+  torque_scale_reset(*P.torque_scale, seed, g, i);
+}
+
 // The attitude filter (F.sense kernels, P.attitude_filter set). Out of line, as history_substep: the estimate, the
 // bias estimate and the last substep's IMU velocity stay in the env's columns of the device block, so that the substep
 // loop carries none of them. attitude_lane: one spine cycle of env i, the end of substep `sub` (S a copy of the state
@@ -648,6 +661,21 @@ __device__ __forceinline__ void step_env(
     vderate = P.velocity_derate;
     if (vderate && resetting && live) derate_reset_lane(P, seed, env_offset + uint64_t(i), i);
   }
+  // servo torque scales (F.sense kernels, P.torque_scale set: a uniform branch). `tsv` is the lane's s_i, loaded once
+  // and held through the substeps (holding them left the same stack frame as reading the column in every substep, and
+  // ran faster). The physics of every substep integrates fl(s t) for the servo's torque t (servo_substep), after the
+  // velocity derate and before external forces and pushes; the torque replies stay t. A next-step reset draws the next
+  // s_i here (its substeps are zero-torque, which stay zero), a same-step reset at the reset below, after the terminal
+  // step's physics. Null outside FAM_SENSE, which compiles the law out.
+  const TorqueScale* tscale = nullptr;
+  Scale6 tsv{{1.f, 1.f, 1.f, 1.f, 1.f, 1.f}};
+  if constexpr (F.sense) {
+    tscale = P.torque_scale;
+    if (tscale) {
+      if (!resetting) tsv = tscale_load_lane(P, i);
+      else if (live) tscale_reset_lane(P, seed, env_offset + uint64_t(i), i);
+    }
+  }
   // TILE >= 1: the row the substeps read (torque law, action delay, spine cycle) is the lane's own row of the warp's
   // tile, written here whole (9 x 16 B at a stride of 9 float4: conflict-free) whether the row came from the tile or
   // from global memory, instead of a 36-float register array that ptxas spills to the local-memory frame and reloads in
@@ -806,7 +834,7 @@ __device__ __forceinline__ void step_env(
         // second and third inlined copy of the substep that these kernels never run
         servo_substep(P, S, arow, resetting, eps, mu, WarpAny(), PhaseSync(), F.extras ? &nz : nullptr, sub,
                       (F.extras && ext) ? &xf : nullptr, F.limits ? (P.joint_limits == 2 ? 2 : 3) : 0, br, env_col,
-                      pushing ? &pu : nullptr, vderate, i);
+                      pushing ? &pu : nullptr, vderate, i, tscale ? &tsv : nullptr);
       }
       if (dropping && !resetting && live) {
         ServoReplies R;
@@ -962,6 +990,7 @@ __device__ __forceinline__ void step_env(
         if (offsetting && live) eo = offset_reset_lane(P, seed, env_offset + uint64_t(i), i);  // and delta_i
         if (noising && live) nk = noise_reset_lane(P, seed, env_offset + uint64_t(i), i);  // and sigma_i
         if (vderate && live) derate_reset_lane(P, seed, env_offset + uint64_t(i), i);       // and v_i
+        if (tscale && live) tscale_reset_lane(P, seed, env_offset + uint64_t(i), i);        // and s_i
       }
       const uint32_t ep = episode[i] + 1u;
       if (live) episode[i] = ep;

@@ -21,7 +21,8 @@
 // and the history refill, and the same three kernels read the servo replies through it (servo_noise_observed). The
 // servo velocity limits touch the torque law only: k_reset draws, and the step kernels' substeps derate. The attitude
 // filter has one, k_attitude_init (a new filter, set_state): k_reset draws and initialises, and k_spine_obs,
-// k_reset_obs and k_history_fill report the estimate (attitude_observed).
+// k_reset_obs and k_history_fill report the estimate (attitude_observed). The torque scales touch the physics only:
+// k_reset draws, and the step kernels' substeps scale the torque integrated.
 // MPC kernels live in mpc.cuh, the UpkieBaseVelocity epilogue (k_base_velocity_post) in base_velocity.cu.
 //
 // There is deliberately NO CPU path in this library: every entry point needs a
@@ -188,6 +189,12 @@ struct Handle {
   float* att_rep = nullptr;    // [4][n_pad] the estimate the observation reports under an observation delay
   float* att_vel = nullptr;    // [3][n_pad] the step kernels' last-substep IMU velocity
   UpkieAttitudeFilter att_spec{};  // the spec in force
+  // servo torque-constant errors (upkie_b200_set_torque_scale): the device block P.torque_scale points to while a spec
+  // is set, and the per-env state it points to (allocated with the first spec, freed when it is turned off)
+  TorqueScale* tsc_dev = nullptr;
+  uint32_t* tsc_count = nullptr;
+  float* tsc_scale = nullptr;  // [UPKIE_NJ][n_pad], s_i
+  uint32_t tsc_mask = 0;       // joint_mask of the spec in force
   cudaStream_t host_streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t host_events[64] = {};
   int host_kernel_streams = 1;
@@ -279,6 +286,7 @@ k_reset(const __grid_constant__ SimParams P, int n, int n_pad, float* __restrict
     servo_noise_leg_targets(S, nd);
   }
   if (P.velocity_derate) velocity_derate_reset(*P.velocity_derate, rand_seed, g, i);  // the new episode's v_i
+  if (P.torque_scale) torque_scale_reset(*P.torque_scale, rand_seed, g, i);           // and s_i
   Offset6 d{{0.f, 0.f, 0.f, 0.f, 0.f, 0.f}};
   if (P.encoder_offset) {
     d = encoder_offset_reset(*P.encoder_offset, rand_seed, g, i);
@@ -1207,6 +1215,7 @@ void upkie_b200_destroy(void* handle) {
   cudaFree(h->enc_dev); cudaFree(h->enc_count); cudaFree(h->enc_offset);
   cudaFree(h->noise_dev); cudaFree(h->noise_count); cudaFree(h->noise_sigma); cudaFree(h->noise_fresh);
   cudaFree(h->vlim_dev); cudaFree(h->vlim_count); cudaFree(h->vlim_max);
+  cudaFree(h->tsc_dev); cudaFree(h->tsc_count); cudaFree(h->tsc_scale);
   cudaFree(h->att_dev); cudaFree(h->att_count); cudaFree(h->att_gains); cudaFree(h->att_quat); cudaFree(h->att_bias);
   cudaFree(h->att_rep); cudaFree(h->att_vel);
   cudaFreeHost(h->h_fin); cudaFreeHost(h->h_act); cudaFreeHost(h->h_obs); cudaFreeHost(h->h_rew); cudaFreeHost(h->h_term); cudaFreeHost(h->h_trunc);
@@ -1276,6 +1285,10 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
     return fail(UPKIE_B200_EINVAL, "set_config: the attitude filter needs joint_limits != 0");
   if (h->P.attitude_filter && P.body_contacts)
     return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no attitude-filter kernels");
+  if (h->P.torque_scale && P.joint_limits == 0)
+    return fail(UPKIE_B200_EINVAL, "set_config: torque scales need joint_limits != 0");
+  if (h->P.torque_scale && P.body_contacts)
+    return fail(UPKIE_B200_EINVAL, "set_config: body_contacts has no torque-scale kernels");
   if (h->P.attitude_filter) {
     // the bound holds for the gains every env holds (a narrower spec keeps each env's gains until its next reset, and
     // set_attitude_filter_state may set others) and for those the spec in force draws
@@ -1315,6 +1328,7 @@ int upkie_b200_set_config(void* handle, const UpkieSimConfig* config) {
   P.servo_noise = h->P.servo_noise;        // and the servo noise
   P.velocity_derate = h->P.velocity_derate;  // and the velocity limits
   P.attitude_filter = h->P.attitude_filter;  // and the attitude filter
+  P.torque_scale = h->P.torque_scale;        // and the torque scales
   if (P.max_episode_steps > 0 && P.max_episode_steps != h->P.max_episode_steps) {
     // a limit switched on or changed: episodes are timed from this call. The counts were not kept (no limit) or
     // were kept against another limit; steps enqueued before the call finish first.
@@ -2822,6 +2836,82 @@ int upkie_b200_set_attitude_filter_report(void* handle, const float* quat, void*
       return fail(UPKIE_B200_EINVAL, "set_attitude_filter_report: every quaternion must be unit (within 1e-5)");
   }
   CUDA_TRY(ring_cols(quat, 4, h->n, h->n_pad, h->att_rep, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_torque_scale(void* handle, const UpkieTorqueScale* spec) {
+  Handle* h = as_handle(handle);
+  if (!h) return fail(UPKIE_B200_EINVAL, "invalid handle");
+  if (!spec) {
+    if (h->P.torque_scale) {
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may use the per-env state
+      h->P.torque_scale = nullptr;
+      cudaFree(h->tsc_count);
+      cudaFree(h->tsc_scale);
+      h->tsc_count = nullptr;
+      h->tsc_scale = nullptr;
+      h->tsc_mask = 0;
+    }
+    return UPKIE_B200_OK;
+  }
+  if (const char* why = torque_scale_spec_error(*spec, h->P)) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaSetDevice(h->device));
+  CUDA_TRY(cudaDeviceSynchronize());  // launches in flight may read the device block
+  // the joints the spec adds to the mask hold 1 until each env's next reset, and those it drops store 1: on a handle
+  // that had no spec every joint starts at 1, and a replacement resets the joints whose membership changes
+  uint32_t fill = (h->tsc_mask ^ spec->joint_mask) & ((1u << UPKIE_NJ) - 1u);
+  if (!h->P.torque_scale) {  // switched on: zero counters
+    CUDA_TRY(alloc_zeroed({{reinterpret_cast<void**>(&h->tsc_count), size_t(h->n) * sizeof(uint32_t)},
+                           {reinterpret_cast<void**>(&h->tsc_scale), size_t(UPKIE_NJ) * h->n_pad * sizeof(float)}}));
+    fill = (1u << UPKIE_NJ) - 1u;
+  }
+  for (int j = 0; j < UPKIE_NJ; ++j) {
+    if (!((fill >> j) & 1u)) continue;
+    k_fill<<<grid_of(h->n), 128>>>(h->n, h->tsc_scale + size_t(j) * h->n_pad, 1.f);
+    CUDA_TRY(cudaGetLastError());
+  }
+  if (!h->tsc_dev) CUDA_TRY(cudaMalloc(&h->tsc_dev, sizeof(TorqueScale)));
+  TorqueScale T;
+  std::memset(&T, 0, sizeof(T));
+  T.spec = *spec;
+  T.count = h->tsc_count;
+  T.scale = h->tsc_scale;
+  T.stride = h->n_pad;
+  CUDA_TRY(cudaMemcpy(h->tsc_dev, &T, sizeof(T), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaDeviceSynchronize());
+  h->P.torque_scale = h->tsc_dev;
+  h->tsc_mask = spec->joint_mask;
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_get_torque_scale_state(void* handle, uint32_t* count, float* scale, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !scale) return fail(UPKIE_B200_EINVAL, "get_torque_scale_state: invalid argument");
+  if (!h->P.torque_scale)
+    return fail(UPKIE_B200_EINVAL, "get_torque_scale_state: no torque scales are set (upkie_b200_set_torque_scale)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  CUDA_TRY(cudaMemcpyAsync(count, h->tsc_count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_rows(h->tsc_scale, UPKIE_NJ, h->n, h->n_pad, scale, s));
+  return UPKIE_B200_OK;
+}
+
+int upkie_b200_set_torque_scale_state(void* handle, const uint32_t* count, const float* scale, void* stream) {
+  Handle* h = as_handle(handle);
+  if (!h || !count || !scale) return fail(UPKIE_B200_EINVAL, "set_torque_scale_state: invalid argument");
+  if (!h->P.torque_scale)
+    return fail(UPKIE_B200_EINVAL, "set_torque_scale_state: no torque scales are set (upkie_b200_set_torque_scale)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // every joint of the mask in force must hold a scale in (0, 2], every other joint exactly 1: read back (after the
+  // caller's work on the stream) and checked here
+  std::vector<float> v(size_t(h->n) * UPKIE_NJ);
+  CUDA_TRY(cudaMemcpyAsync(v.data(), scale, v.size() * sizeof(float), cudaMemcpyDefault, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  if (const char* why = torque_scale_state_error(h->tsc_mask, v.data(), size_t(h->n))) return fail(UPKIE_B200_EINVAL, why);
+  CUDA_TRY(cudaMemcpyAsync(h->tsc_count, count, size_t(h->n) * sizeof(uint32_t), cudaMemcpyDeviceToDevice, s));
+  CUDA_TRY(ring_cols(scale, UPKIE_NJ, h->n, h->n_pad, h->tsc_scale, s));
   return UPKIE_B200_OK;
 }
 

@@ -1097,6 +1097,75 @@ def _set_velocity_derate(sim, spec: Optional[_abi.UpkieVelocityDerate]) -> None:
                                 [n for j, n in enumerate(_abi.JOINT_NAMES) if (spec.joint_mask >> j) & 1])
 
 
+def _scale_range(name: str, value):
+    """(low, high) float32 of one torque scale: a scale ``s`` or a ``(low, high)`` range, 0 < low <= high <= 2"""
+    if isinstance(value, (int, float, np.integer, np.floating)):
+        lo = hi = value
+    else:
+        try:
+            lo, hi = value
+        except (TypeError, ValueError):
+            raise UpkieException(f"torque_scale: {name}: expected a scale or a (low, high) pair, got {value!r}") \
+                from None
+    try:
+        lo, hi = np.float32(lo), np.float32(hi)
+    except (TypeError, ValueError):
+        raise UpkieException(f"torque_scale: {name}: expected numbers, got ({lo!r}, {hi!r})") from None
+    if not (np.isfinite(lo) and np.isfinite(hi)) or not lo > 0 or not hi <= _abi.TORQUE_SCALE_MAX:
+        raise UpkieException(f"torque_scale: {name}: expected finite scales in (0, {_abi.TORQUE_SCALE_MAX:g}], got "
+                             f"({lo}, {hi})")
+    if lo > hi:
+        raise UpkieException(f"torque_scale: {name}: expected low <= high, got ({lo}, {hi})")
+    return lo, hi
+
+
+def torque_scale_spec(torque_scale, joints=None, spine_mode: bool = False, joint_limits: Union[bool, int] = True,
+                      body_contacts: Union[bool, int] = False) -> Optional[_abi.UpkieTorqueScale]:
+    """``UpkieTorqueScale`` (``UpkieSim.set_torque_scale``) from a scale ``s``, a ``(low, high)`` range from which every
+    reset draws each joint's scale, or a dict ``{joint: s or (low, high)}`` (dimensionless; ``(0.9, 1.1)`` is a usual
+    "motor strength" range in legged-robot RL, not a measured figure of the Upkie's servos). ``joints`` (names,
+    ``JOINT_NAMES``) are the joints whose delivered torque is scaled; None: the joints of a dict, or all six. Raises
+    ``UpkieException`` on an unknown joint, a scale that is not a finite number in ``(0, 2]``, ``low > high``, a joint
+    without a scale, an empty joint list, ``spine_mode`` (whose spine applies its own torque law), no joint limits and
+    ``body_contacts`` (the scales run in the kernels of the observation delay)."""
+    if torque_scale is None:
+        return None
+    per_joint = isinstance(torque_scale, dict)
+    names = (list(torque_scale) if per_joint else list(_abi.JOINT_NAMES)) if joints is None else list(joints)
+    bad = [j for j in names + (list(torque_scale) if per_joint else []) if j not in _abi.JOINT_NAMES]
+    if bad:
+        raise UpkieException(f"torque_scale: unknown joint(s) {bad}, expected names of {_abi.JOINT_NAMES}")
+    if not names:
+        raise UpkieException("torque_scale_joints: at least one joint")
+    lo = np.ones(_abi.NJ, dtype=np.float32)
+    hi = np.ones(_abi.NJ, dtype=np.float32)
+    for j in names:
+        k = _abi.JOINT_NAMES.index(j)
+        if per_joint and j not in torque_scale:
+            raise UpkieException(f"torque_scale: {j} has no scale")
+        lo[k], hi[k] = _scale_range(j if per_joint else "scale", torque_scale[j] if per_joint else torque_scale)
+    if spine_mode:
+        raise UpkieException("torque_scale: spine_mode applies the spine's own torque law; the scales are not "
+                             "available there")
+    if not joint_limits:
+        raise UpkieException("torque_scale: needs joint_limits (the scales run in the kernels with joint-limit rows)")
+    if body_contacts:
+        raise UpkieException("torque_scale: body_contacts has no torque-scale kernels")
+    spec = _abi.UpkieTorqueScale()
+    spec.scale_low[:] = [float(x) for x in lo]
+    spec.scale_high[:] = [float(x) for x in hi]
+    spec.joint_mask = sum(1 << _abi.JOINT_NAMES.index(j) for j in set(names))
+    return spec
+
+
+def _set_torque_scale(sim, spec: Optional[_abi.UpkieTorqueScale]) -> None:
+    if spec is None:
+        sim.set_torque_scale(None)
+    else:
+        sim.set_torque_scale(list(zip(spec.scale_low, spec.scale_high)),
+                             [n for j, n in enumerate(_abi.JOINT_NAMES) if (spec.joint_mask >> j) & 1])
+
+
 def _set_servo_noise(sim, spec: Optional[_abi.UpkieServoNoise]) -> None:
     if spec is None:
         sim.set_servo_noise(None)
@@ -1234,6 +1303,14 @@ class B200VectorEnv(VectorEnv):
     observes is the derated one. The draws are keyed on the seed of ``reset(seed=s)``, which also restarts the draw
     counters of the envs it resets. ``set_velocity_derate`` changes or (``None``) stops it.
 
+    ``torque_scale`` (a scale, a ``(low, high)`` range or ``{joint: s or (low, high)}``, see ``torque_scale_spec``)
+    makes the servos ``torque_scale_joints`` (names, default those of a dict, or all six) deliver a scale of the torque
+    they command, drawn per joint at every reset of the env, as a servo whose torque constant is off: the physics
+    integrates the scaled torque, while the torque every env type observes stays the commanded one. ``(0.9, 1.1)`` is a
+    usual range in legged-robot RL, not a measured tolerance of the Upkie's servos. The draws are keyed on the seed of
+    ``reset(seed=s)``, which also restarts the draw counters of the envs it resets. ``set_torque_scale`` changes or
+    (``None``) stops it.
+
     ``attitude_filter`` (a dict ``{"kp": ..., "ki": ..., "roll": ..., "pitch": ...}``, see ``attitude_filter_spec``)
     makes every env report the orientation an attitude filter estimates from its simulated IMU, as the robot's spine
     reads the pi3hat's filter: the IMU orientation, the base pitch and rotation, and the gyropod and pendulum pitch
@@ -1290,6 +1367,8 @@ class B200VectorEnv(VectorEnv):
         velocity_derate: Optional[Dict[str, Any]] = None,
         velocity_derate_joints: Optional[Sequence[str]] = None,
         attitude_filter: Optional[Dict[str, Any]] = None,
+        torque_scale: Optional[Union[float, Tuple[float, float], Dict[str, Any]]] = None,
+        torque_scale_joints: Optional[Sequence[str]] = None,
     ):
         max_episode_steps = _check_max_episode_steps(max_episode_steps)
         rr_spec = reset_randomization_spec(reset_randomization)  # validated before any device is touched
@@ -1352,6 +1431,8 @@ class B200VectorEnv(VectorEnv):
                                         self.max_delay_ticks if sense_spec is not None else 1)  # before any device
         vlim_spec = velocity_derate_spec(velocity_derate, velocity_derate_joints, bool(config.spine_mode),
                                          config.joint_limits, config.body_contacts)  # validated before any device
+        tsc_spec = torque_scale_spec(torque_scale, torque_scale_joints, bool(config.spine_mode), config.joint_limits,
+                                     config.body_contacts)  # validated before any device is touched
         # validated before any device is touched
         env_params = env_params_table(self.num_envs, _abi.config_env_params(config), torque_control_kp,
                                       torque_control_kd, joint_properties) if per_env else None
@@ -1421,6 +1502,8 @@ class B200VectorEnv(VectorEnv):
             _set_servo_noise(self.sim, noise_spec)  # before the first reset, which draws every env's levels
         if vlim_spec is not None:
             _set_velocity_derate(self.sim, vlim_spec)  # before the first reset, which draws every env's limits
+        if tsc_spec is not None:
+            _set_torque_scale(self.sim, tsc_spec)  # before the first reset, which draws every env's scales
         if att_spec is not None:
             _set_attitude_filter(self.sim, att_spec)  # before the first reset, which draws every env's filter
 
@@ -1440,6 +1523,13 @@ class B200VectorEnv(VectorEnv):
         ``high`` bound until then, and those it drops have no limit from now on."""
         _set_velocity_derate(self.sim, velocity_derate_spec(velocity_derate, joints, bool(self.config.spine_mode),
                                                             self.config.joint_limits, self.config.body_contacts))
+
+    def set_torque_scale(self, torque_scale, joints=None) -> None:
+        """Scale the torque the servos ``joints`` (names, None: those of a dict, or all six) deliver by a factor drawn
+        per env (see ``torque_scale_spec``); ``None`` turns the scales off. New ranges take effect at each env's next
+        reset; the joints it adds hold a scale of 1 until then, and those it drops have none from now on."""
+        _set_torque_scale(self.sim, torque_scale_spec(torque_scale, joints, bool(self.config.spine_mode),
+                                                      self.config.joint_limits, self.config.body_contacts))
 
     def set_servo_noise(self, noise) -> None:
         """Add white noise to the servos' position and velocity replies at levels drawn per env (a dict, see
@@ -1710,6 +1800,14 @@ class B200VectorEnv(VectorEnv):
                 else:
                     count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
                 self.sim.set_velocity_derate_state(count, vmax)
+            if self.sim.torque_scale_spec is not None:
+                # so are the torque scales
+                count, scale = self.sim.get_torque_scale_state()
+                if mask is None:
+                    count.zero_()
+                else:
+                    count.masked_fill_(torch.from_numpy(mask).to(count.device).bool(), 0)
+                self.sim.set_torque_scale_state(count, scale)
             if self.sim.attitude_filter_spec is not None:
                 # and the attitude filter's draws
                 count, gains, quat, bias = self.sim.get_attitude_filter_state()

@@ -615,6 +615,63 @@ class UpkieSim:
         self._check_tensor(max_velocity, (self.n, _abi.NJ), name="max_velocity")
         check(lib().upkie_b200_set_velocity_derate_state(self._h, _ptr(count), _ptr(max_velocity), self._stream()))
 
+    def set_torque_scale(self, scale=None, joints: Optional[Sequence[str]] = None) -> None:
+        """While scales are set, each joint of ``joints`` (names, None: all six) receives a scale of the torque its servo
+        commands and reports, as a servo whose torque constant is off: every reset of an env draws one scale per joint,
+        ``s ~ U(low, high)`` (keyed on the auto-reset seed and the env's counter, ``include/upkie_b200.h``), and in every
+        substep the physics integrates ``s * t`` for the servo's torque ``t`` (after its clip and velocity derate),
+        while the torque replies and ``get_state`` keep ``t``. ``scale`` is a ``(low, high)`` pair of bounds or a
+        sequence of six per-joint ``(low, high)`` pairs (``JOINT_NAMES`` order), with ``0 < low <= high <= 2``;
+        ``(0.9, 1.1)`` is a usual "motor strength" range in legged-robot RL, not a measured figure of the Upkie's
+        servos. ``scale=None`` turns the scales off. Setting scales draws nothing: each env keeps the scales of the
+        joints that stay scaled until its next reset, and the joints a spec adds hold 1 until then."""
+        if scale is None:
+            check(lib().upkie_b200_set_torque_scale(self._h, None))
+            self._torque_scale = None
+            return
+        sc = np.asarray(scale, dtype=np.float32)
+        if sc.shape == (2,):
+            lo, hi = np.full(_abi.NJ, sc[0], np.float32), np.full(_abi.NJ, sc[1], np.float32)
+        elif sc.shape == (_abi.NJ, 2):
+            lo, hi = sc[:, 0], sc[:, 1]
+        else:
+            raise UpkieException("set_torque_scale: scale expects (low, high) or six (low, high) pairs")
+        names = list(_abi.JOINT_NAMES) if joints is None else list(joints)
+        unknown = [j for j in names if j not in _abi.JOINT_NAMES]
+        if unknown:
+            raise UpkieException(f"set_torque_scale: unknown joint(s) {unknown}")
+        mask = sum(1 << _abi.JOINT_NAMES.index(j) for j in set(names))
+        spec = _abi.UpkieTorqueScale()
+        spec.scale_low[:] = [float(x) for x in lo]
+        spec.scale_high[:] = [float(x) for x in hi]
+        spec.joint_mask = mask
+        check(lib().upkie_b200_set_torque_scale(self._h, C.byref(spec)))
+        self._torque_scale = (tuple(zip(spec.scale_low, spec.scale_high)), mask)
+
+    @property
+    def torque_scale_spec(self):
+        """``(scale, joint_mask)`` of the torque scales in force (six ``(low, high)`` pairs), or None."""
+        return getattr(self, "_torque_scale", None)
+
+    def get_torque_scale_state(self):
+        """Per-env torque-scale state ``(count[N], scale[N, 6])``: the draw counters (int32 bits of uint32) and each
+        env's scale per joint (exactly 1 for a joint without one)."""
+        if self.torque_scale_spec is None:
+            raise UpkieException("no torque scales are set (set_torque_scale)")
+        count = torch.empty(self.n, dtype=torch.int32, device=self.device)
+        scale = torch.empty((self.n, _abi.NJ), dtype=torch.float32, device=self.device)
+        check(lib().upkie_b200_get_torque_scale_state(self._h, _ptr(count), _ptr(scale), self._stream()))
+        return count, scale
+
+    def set_torque_scale_state(self, count: torch.Tensor, scale: torch.Tensor) -> None:
+        """Set every env's draw counter and torque scales (in ``(0, 2]`` on a scaled joint, exactly 1 on the others): a
+        checkpoint, or fixed scales (kept until each env's next reset)."""
+        if self.torque_scale_spec is None:
+            raise UpkieException("no torque scales are set (set_torque_scale)")
+        self._check_tensor(count, (self.n,), torch.int32, "count")
+        self._check_tensor(scale, (self.n, _abi.NJ), name="scale")
+        check(lib().upkie_b200_set_torque_scale_state(self._h, _ptr(count), _ptr(scale), self._stream()))
+
     def get_servo_noise_mark(self) -> torch.Tensor:
         """Per-env mark ``[N]`` (uint8): 1 while the env reports its reset observation (``spine_obs`` and
         ``reset_obs`` then carry the reset cycle's noise), 0 after a step that did not reset it."""
@@ -1108,6 +1165,10 @@ class UpkieSim:
         if self.velocity_derate_spec is not None:
             sd["velocity_derate"] = self.velocity_derate_spec
             sd["velocity_derate_count"], sd["velocity_derate_max_velocity"] = self.get_velocity_derate_state()
+        # the torque scales: (scale, joint_mask) and the per-env state (absent without a spec)
+        if self.torque_scale_spec is not None:
+            sd["torque_scale"] = self.torque_scale_spec
+            sd["torque_scale_count"], sd["torque_scale_scale"] = self.get_torque_scale_state()
         # the attitude filter: its ranges and the per-env state (absent without a spec)
         if self.attitude_filter_spec is not None:
             sd["attitude_filter"] = self.attitude_filter_spec
@@ -1253,6 +1314,13 @@ class UpkieSim:
             self.set_velocity_derate(vlim[0], vlim[1], [n for j, n in enumerate(_abi.JOINT_NAMES) if (vlim[2] >> j) & 1])
             self.set_velocity_derate_state(*(sd[k].to(dev).contiguous() for k in (
                 "velocity_derate_count", "velocity_derate_max_velocity")))
+        # the torque scales; a checkpoint without them (or written before they existed) turns them off
+        tsc = sd.get("torque_scale")
+        if tsc is None:
+            self.set_torque_scale(None)
+        else:
+            self.set_torque_scale(tsc[0], [n for j, n in enumerate(_abi.JOINT_NAMES) if (tsc[1] >> j) & 1])
+            self.set_torque_scale_state(*(sd[k].to(dev).contiguous() for k in ("torque_scale_count", "torque_scale_scale")))
         # the servo noise (off above); a checkpoint without it (or written before it existed) leaves it off
         noise = sd.get("servo_noise")
         if noise is not None:
